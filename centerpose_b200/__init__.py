@@ -1,4 +1,4 @@
-"""centerpose_b200 — B200-native (sm_100a) drop-in for the centerpose inference hot path.
+"""centerpose_b200 — Hopper-native (H100, sm_90a) drop-in for the centerpose inference hot path.
 
 Public surface mirrors the reference (tensorboy/centerpose):
   ``create_model`` / ``load_model`` / ``save_model``   (lib/models/model.py:63-131)

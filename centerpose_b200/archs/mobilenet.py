@@ -2,7 +2,7 @@
 ``lib/models/backbones/mobilenet/mobilenetv3.py:159-233``): parameter tree + lowering to fused ops.
 
 Channel padding.  The reference's channel counts (24, 40, 72, 120, 184, 200 ...) are not multiples of 16,
-the K / N granularity of the tcgen05 kernels, and a DCN's gathered operand tile is 64 channels wide.  The
+the K / N granularity of the wgmma kernels, and a DCN's gathered operand tile is 64 channels wide.  The
 lowering therefore carries every activation with ZERO-PADDED channels (:func:`padded`: next multiple of 16;
 24 / 40 / 160 -> 64 / 64 / 192 because those tensors feed the IDAUp DCNs) and zero-pads the folded weights
 and biases to match.  Padded channels stay exactly zero through ReLU, h-swish, the SE gate (x * s) and the

@@ -1,4 +1,4 @@
-"""In-tree build of the C-ABI shared library (nvcc, sm_100a only).
+"""In-tree build of the C-ABI shared library (nvcc, sm_90a only: the kernels use wgmma, Hopper's warpgroup MMA).
 
 ``python -m centerpose_b200.build`` or ``__graft_entry__.build()``.  nvcc cross-compiles
 without a GPU; the resulting ``centerpose_b200/lib/libcenterpose_b200.so`` is git-ignored
@@ -19,10 +19,11 @@ LIBDIR = os.path.join(HERE, "lib")
 LIBPATH = os.path.join(LIBDIR, "libcenterpose_b200.so")
 STAMP = os.path.join(LIBDIR, "build.stamp")
 
-NVCC_FLAGS = [
-    "-shared", "-Xcompiler", "-fPIC", "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
-]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ["-Xcompiler", "-fPIC", "-std=c++17", "-O3", "-lineinfo"] + ARCH
+# NVVM's -O3 pipeline for sm_90 takes tens of minutes on the CUDA-core kernels of net_simt.cu (seconds for other targets);
+# -O1 compiles them in under half a minute
+FILE_FLAGS = {"net_simt.cu": ["-Xcicc", "-O1"]}
 
 
 def _nvcc() -> str:
@@ -42,7 +43,7 @@ def _digest() -> str:
             [os.path.join(HERE, "..", "include", "centerpose_b200.h")]:
         with open(p, "rb") as f:
             h.update(p.encode()); h.update(f.read())
-    h.update(" ".join(NVCC_FLAGS).encode())
+    h.update(" ".join(NVCC_FLAGS).encode()); h.update(repr(sorted(FILE_FLAGS.items())).encode())
     return h.hexdigest()
 
 
@@ -57,8 +58,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     procs = []
     for src in _sources():
         obj = os.path.join(LIBDIR, os.path.basename(src)[:-3] + ".o")
-        cmd = [nvcc, "-c", "-Xcompiler", "-fPIC", "-std=c++17", "-O3", "-lineinfo",
-               "-gencode", "arch=compute_100a,code=sm_100a", "-o", obj, src]
+        cmd = [nvcc, "-c"] + NVCC_FLAGS + FILE_FLAGS.get(os.path.basename(src), []) + ["-o", obj, src]
         if verbose:
             cmd.insert(1, "-Xptxas"); cmd.insert(2, "-v")
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
@@ -69,7 +69,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             print(out)
         if pr.returncode != 0:
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIBPATH] + objs
+    link = [nvcc, "-shared"] + ARCH + ["-o", LIBPATH] + objs
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}")

@@ -1,4 +1,4 @@
-// Shared host/device helpers for the centerpose_b200 C-ABI library (sm_100a only).
+// Shared host/device helpers for the centerpose_b200 C-ABI library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -48,11 +48,11 @@ __device__ __forceinline__ float act_fn(float v, uint32_t act) {
   return act == CPB200_FLAG_HSWISH ? v * r / 6.f : r / 6.f;
 }
 // bf16-output variant: multiply by 1/6 instead of the IEEE division (differs from act_fn by <= 1 ulp of fp32,
-// far below the bf16 rounding that follows).  The division cost 20+ instructions per element and made the
-// MobileNetV3 expand convs and depthwise convs instruction-bound (profiles/r01_launches_mbv3_v1_summary.txt).
+// far below the bf16 rounding that follows).  The division costs 20+ instructions per element, enough to make the
+// MobileNetV3 expand convs and depthwise convs instruction-bound.
 // the multiply-by-1/6 form on its own: used wherever the result is re-split into 16-bit planes (the split tensor-core
-// epilogues and the element-wise kernels on planes).  The exact division cost 64 % on the h-swish 1x1 expand convs of
-// MobileNetV3 in fp16x2 (tools/prof_act.py: 316 vs 193 us); 1 ulp of fp32 is 2^-13 of the planes' own precision.
+// epilogues and the element-wise kernels on planes; tools/prof_act.py times both forms); 1 ulp of fp32 is 2^-13 of the
+// planes' own precision.
 __device__ __forceinline__ float act_fast(float v, uint32_t act) {
   if (act == CPB200_FLAG_RELU) return fmaxf(v, 0.f);
   if (act == 0u) return v;

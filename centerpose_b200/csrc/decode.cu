@@ -1,4 +1,4 @@
-// Fused multi_pose_decode for sm_100a: 3x3 max-pool NMS + per-channel top-K + gather +
+// Fused multi_pose_decode for sm_90a: 3x3 max-pool NMS + per-channel top-K + gather +
 // keypoint/candidate assignment in ONE launch.
 //
 // Replaces (reference file:line)  lib/models/decode.py:10-16 (_nms), :87-96 (_topk_channel),
@@ -165,7 +165,7 @@ __device__ void scan_vec(Smem &s, const float *__restrict__ map, int H, int W, b
 // Same algorithm as scan_vec with everything the general path pays per row folded away at compile time: lane = column
 // group, warp = row strip, no out-of-range threads, the row's left / right neighbours always come from the shuffle
 // (lane 0 / 31 see -inf), row addresses advance by a constant, the logistic is a template switch.  The general path
-// executes ~150 instructions per row per thread (ncu, profiles/r01_ncu_decode_prof_v3.txt), this one ~60.
+// executes ~2.5x the instructions per row per thread.
 template <bool SIG>
 __device__ void scan_w128(Smem &s, const float *__restrict__ map, int H, float floorv) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -720,7 +720,7 @@ extern "C" int cpb200_sigmoid_inplace(float *x, size_t n, void *stream) {
   if (!x && n) return cpb::fail(CPB200_ERR_ARG, "sigmoid: null pointer");
   if (n == 0) return CPB200_OK;
   int blocks = (int)((n + 1023) / 1024);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   sigmoid_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, n);
   return cpb::check_launch("sigmoid_kernel");
 }

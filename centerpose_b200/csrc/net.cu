@@ -46,7 +46,7 @@ extern "C" int cpb200_prepare_ops(cpb200_op *ops, int n) {
     if (ops[i].type == CPB200_OP_STEM && (ops[i].flags & CPB200_FLAG_TC)) {
       if (!cpb::stem_tc_eligible(ops[i])) return cpb::fail(CPB200_ERR_ARG, "op %d: shape not supported by the tensor-core stem", i);
     } else if (cpb::sp_eligible(ops[i])) {
-      // small-channel 3x3 conv: SIMT-fed tcgen05 kernel, nothing to prepare (csrc/net_tc_sp.cu)
+      // small-channel 3x3 conv: SIMT-fed wgmma kernel, nothing to prepare (csrc/net_tc_sp.cu)
     } else if (ops[i].flags & CPB200_FLAG_TC) {
       rc = cpb::tc_prepare_op(ops[i]);
       if (rc) return rc;

@@ -1,7 +1,7 @@
 // CUDA-core (SIMT) implementations of the fused network ops, fp32 accumulate, activations
 // fp32 or bf16 NHWC.  This is the "precise" path (act_dtype = fp32 reproduces the reference's
 // fp32 arithmetic up to summation order) and the fallback for layers whose shapes the
-// tcgen05 path (net_tc.cu) does not take.  Reference semantics per op:
+// wgmma path (net_tc.cu) does not take.  Reference semantics per op:
 //   CONV          torch.nn.Conv2d + folded eval BatchNorm2d (+ residual add) (+ ReLU)
 //                 e.g. pose_dla_dcn.py:43-57 (BasicBlock), :155-163 (Root: the torch.cat of
 //                 the children is never materialised — each child is one K-slab), :199-204
@@ -914,7 +914,7 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
     case CPB200_OP_CONVERT: {
       const long long n = (long long)op.B * op.H * op.W * op.cin[0];
       if (n % 4) return cpb::fail(CPB200_ERR_ARG, "convert: element count must be a multiple of 4");
-      const unsigned grid = (unsigned)std::min<long long>((n / 4 + 255) / 256, 148LL * 16);
+      const unsigned grid = (unsigned)std::min<long long>((n / 4 + 255) / 256, 132LL * 16);
       if (op.flags & CPB200_FLAG_TO_F32)
         convert_from_split_kernel<<<grid, 256, 0, st>>>(static_cast<const uint16_t *>(op.src[0]), static_cast<float *>(op.dst), n / 4, (size_t)n, fmt);
       else
@@ -925,7 +925,7 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
       if (op.cin[0] != 3 || op.cout != 16 || (op.H & 1) || (op.W & 1) || op.Ho != op.H / 2 || op.Wo != op.W / 2)
         return cpb::fail(CPB200_ERR_ARG, "s2d: needs a (B,3,H,W) input with even H, W and a 16-channel (B,H/2,W/2) output");
       const long long total = (long long)op.B * op.Ho * op.Wo;
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 16);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
       s2d_split_kernel<<<grid, 256, 0, st>>>(static_cast<const float *>(op.src[0]), static_cast<uint16_t *>(op.dst), op.B, op.H, op.W,
                                              (size_t)total * 16, fmt);
       return cpb::check_launch("s2d_split_kernel");
@@ -933,7 +933,7 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
     case CPB200_OP_MAXPOOL: {
       if (op.cin[0] % 4) return cpb::fail(CPB200_ERR_ARG, "maxpool: C %% 4 != 0");
       const long long total = (long long)op.B * op.Ho * op.Wo * (op.cin[0] / 4);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 32);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 32);
       maxpool_split_kernel<<<grid, 256, 0, st>>>(static_cast<const uint16_t *>(op.src[0]), static_cast<uint16_t *>(op.dst),
                                                  op.B, op.H, op.W, op.cin[0], op.Ho, op.Wo, op.kh, op.stride, op.pad_h, fmt);
       return cpb::check_launch("maxpool_split_kernel");
@@ -969,7 +969,7 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
 #define DW_TILED(KK, SS, PX)                                                                                   \
   if (op.kh == KK && op.stride == SS && op.pad_h == KK / 2) {                                                    \
     const long long tot = (long long)op.B * op.Ho * ((op.Wo + PX - 1) / PX) * (C / VEC);                         \
-    const unsigned g = (unsigned)std::min<long long>((tot + 255) / 256, 148LL * 32);                            \
+    const unsigned g = (unsigned)std::min<long long>((tot + 255) / 256, 132LL * 32);                            \
     dwconv_tiled_kernel<bf16, VEC, KK, SS, PX, SpC, SpM><<<g, 256, 0, st>>>(x, y, static_cast<const float *>(op.weight), \
         op.bias, tot, op.H, op.W, C, op.Ho, op.Wo, op.flags & CPB_ACT_MASK);                                    \
     return cpb::check_launch("dwconv_tiled_kernel");                                                            \
@@ -977,7 +977,7 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
       DW_TILED(3, 1, 4) DW_TILED(5, 1, 4) DW_TILED(3, 2, 2) DW_TILED(5, 2, 2)
 #undef DW_TILED
       const long long total = (long long)op.B * op.Ho * op.Wo * (C / VEC);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 32);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 32);
       dwconv_kernel<bf16, VEC, SpC, SpM><<<grid, 256, 0, st>>>(x, y, static_cast<const float *>(op.weight), op.bias, total,
           op.H, op.W, C, op.Ho, op.Wo, op.kh, op.stride, op.pad_h, op.flags & CPB_ACT_MASK);
       return cpb::check_launch("dwconv_kernel");
@@ -994,7 +994,7 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
       if (C % 4 || !op.res || (op.src_pitch[0] != 0 && op.src_pitch[0] != C)) return cpb::fail(CPB200_ERR_ARG, "scale_add (split): C %% 4 != 0, missing scale vector or sliced input");
       const size_t plane = (size_t)op.B * op.H * op.W * C;
       const long long per_image = (long long)op.H * op.W * (C / 4), total = per_image * op.B;
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 16);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
       scale_add_kernel<float, SpC, const float *, SpM><<<grid, 256, 0, st>>>(SpC{static_cast<const uint16_t *>(op.src[0]), plane, fmt},
           static_cast<const float *>(op.res), SpC{static_cast<const uint16_t *>(op.aux), plane, fmt},
           SpM{static_cast<uint16_t *>(op.dst), plane, fmt}, total, per_image, C / 4);
@@ -1008,7 +1008,7 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
         return cpb::fail(CPB200_ERR_ARG, "upsample_add (split): factor %d must be a power of two, C %% 4 == 0, whole-tensor input", f);
       const size_t plane_o = (size_t)op.B * op.Ho * op.Wo * C;
       const long long total = (long long)op.B * op.Ho * op.Wo * (C / 4);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 16);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
       upsample_add_kernel<float, SpC, SpM><<<grid, 256, 0, st>>>(SpC{static_cast<const uint16_t *>(op.src[0]), (size_t)op.B * op.H * op.W * C, fmt},
           SpC{static_cast<const uint16_t *>(op.aux), plane_o, fmt}, SpM{static_cast<uint16_t *>(op.dst), plane_o, fmt},
           total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, op.flags & CPB_ACT_MASK);
@@ -1099,7 +1099,7 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
     case CPB200_OP_MAXPOOL: {
       if (op.cin[0] % 4) return cpb::fail(CPB200_ERR_ARG, "maxpool: C %% 4 != 0");
       const long long total = (long long)op.B * op.Ho * op.Wo * (op.cin[0] / 4);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 32);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 32);
       maxpool_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T *>(op.src[0]), static_cast<T *>(op.dst),
                                               op.B, op.H, op.W, op.cin[0], op.Ho, op.Wo, op.kh, op.stride, op.pad_h);
       return cpb::check_launch("maxpool_kernel");
@@ -1135,7 +1135,7 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
 #define DW_TILED(KK, SS, PX)                                                                                   \
   if (op.kh == KK && op.stride == SS && op.pad_h == KK / 2) {                                                    \
     const long long tot = (long long)op.B * op.Ho * ((op.Wo + PX - 1) / PX) * (C / VEC);                         \
-    const unsigned g = (unsigned)std::min<long long>((tot + 255) / 256, 148LL * 32);                            \
+    const unsigned g = (unsigned)std::min<long long>((tot + 255) / 256, 132LL * 32);                            \
     dwconv_tiled_kernel<T, VEC, KK, SS, PX><<<g, 256, 0, st>>>(static_cast<const T *>(op.src[0]),                \
         static_cast<T *>(op.dst), static_cast<const float *>(op.weight), op.bias, tot, op.H, op.W, C, op.Ho,     \
         op.Wo, op.flags & CPB_ACT_MASK);                                                                        \
@@ -1144,7 +1144,7 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
       DW_TILED(3, 1, 4) DW_TILED(5, 1, 4) DW_TILED(3, 2, 2) DW_TILED(5, 2, 2)
 #undef DW_TILED
       const long long total = (long long)op.B * op.Ho * op.Wo * (C / VEC);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 32);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 32);
       dwconv_kernel<T, VEC><<<grid, 256, 0, st>>>(static_cast<const T *>(op.src[0]), static_cast<T *>(op.dst),
           static_cast<const float *>(op.weight), op.bias, total, op.H, op.W, C, op.Ho, op.Wo, op.kh, op.stride, op.pad_h,
           op.flags & CPB_ACT_MASK);
@@ -1161,7 +1161,7 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
       const int C = op.cin[0];
       if (C % 4 || !op.res) return cpb::fail(CPB200_ERR_ARG, "scale_add: C %% 4 != 0 or missing scale vector");
       const long long per_image = (long long)op.H * op.W * (C / 4), total = per_image * op.B;
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 16);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
       scale_add_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T *>(op.src[0]), static_cast<const T *>(op.res),
           static_cast<const T *>(op.aux), static_cast<T *>(op.dst), total, per_image, C / 4);
       return cpb::check_launch("scale_add_kernel");
@@ -1173,7 +1173,7 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
       if (f < 1 || (1 << sh) != f || op.Ho != op.H * f || op.Wo != op.W * f || op.cin[0] % 4)
         return cpb::fail(CPB200_ERR_ARG, "upsample_add: factor %d must be a power of two, C %% 4 == 0", f);
       const long long total = (long long)op.B * op.Ho * op.Wo * (op.cin[0] / 4);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 16);
+      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
       upsample_add_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T *>(op.src[0]), static_cast<const T *>(op.aux),
           static_cast<T *>(op.dst), total, op.H, op.W, op.cin[0] / 4, op.Ho, op.Wo, sh, op.flags & CPB_ACT_MASK);
       return cpb::check_launch("upsample_add_kernel");

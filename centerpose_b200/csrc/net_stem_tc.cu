@@ -4,17 +4,17 @@
 //
 // Why: on CUDA cores the 7x7x3 -> 16 stem costs 37 632 FMAs per output pixel (1.07 ms for 32 x 512^2,
 // 13 % of the DLA-34 step at half the fp32 FMA peak).  Here the im2col happens IN SHARED MEMORY: producer
-// threads build the K-major bf16 operand tile straight from a staged input patch, one tcgen05.mma chain
-// per 128-pixel tile does the arithmetic, and HBM only sees the image once and the output once.  (A first
+// threads build the K-major bf16 operand tile straight from a staged input patch, one wgmma chain
+// per 64-pixel half tile does the arithmetic, and HBM only sees the image once and the output once.  (A first
 // attempt that materialised a 32-channel im2col tensor in HBM was slower than the CUDA-core kernel.)
 //
 //   K index  k = (c * 7 + r) * 8 + s   (s = 0..7; the 8th column has a zero weight), 168 real + 24 zero = 192
 //            => every 16-byte chunk of an operand row is 8 CONSECUTIVE input pixels of one (channel, row).
-//   A tile   128 pixels (8 rows x 16 cols) x 192, three 64-wide slabs in the 128-byte-swizzled UMMA layout
+//   A tile   128 pixels (8 rows x 16 cols) x 192, three 64-wide slabs in the 128-byte-swizzled wgmma layout
 //            (chunk j of row m at (j ^ (m & 7)) * 16), written with st.shared.v4 + fence.proxy.async.
 //   B tile   weights, pre-swizzled by the host (plan.py::_pack_stem_tc), copied to shared memory once per CTA.
-//   warps    0-7 producers (two groups of 128, alternating tiles; thread m of a group builds row m),
-//            8 MMA issuer + TMEM owner, 9-12 epilogue.
+//   warps    0-7 two consumer warpgroups (rows 0-63 / 64-127: wgmma + epilogue), 8-15 producers (two groups of 128,
+//            alternating tiles; thread m of a group builds row m).
 #include "tc_common.cuh"
 
 namespace {
@@ -22,7 +22,8 @@ namespace {
 using namespace tc;
 
 constexpr int PGROUPS = 2;                     // producer groups of 128 threads, alternating tiles
-constexpr int ST_THREADS = (4 * PGROUPS + 5) * 32;
+constexpr int CONS = 256;                      // two consumer warpgroups
+constexpr int ST_THREADS = CONS + 128 * PGROUPS;
 constexpr int TH = 8, TW = 16;                 // output tile (M = 128)
 constexpr int KW8 = 8, KH = 7, CIN = 3;
 constexpr int NCHUNK = CIN * KH;               // 21 real 16-byte chunks per operand row
@@ -30,7 +31,6 @@ constexpr int SLABS = 3;                       // K = 192
 constexpr int A_SLAB_BYTES = 128 * 128;        // 128 rows x 128 B
 constexpr int A_STAGE_BYTES = SLABS * A_SLAB_BYTES;
 constexpr int NSTAGE = 3;
-constexpr int NACC = 4;
 
 struct StemArgs {
   const float *x;            // (B,3,H,W) fp32
@@ -56,23 +56,15 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stem_tc_kernel(const StemArgs a
   const uint32_t a_base = smem_base;
   const uint32_t b_base = smem_base + NSTAGE * A_STAGE_BYTES;
   float *patch0 = reinterpret_cast<float *>(smem_raw + (smem_base - smem_u32(smem_raw)) + NSTAGE * A_STAGE_BYTES + SLABS * B_SLAB_BYTES);
-  __shared__ __align__(8) uint64_t bars[2 * NSTAGE + 2 * NACC];
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t bars[2 * NSTAGE];
   __shared__ float s_bias[N];
   const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[NSTAGE]);
-  const uint32_t tfull0 = smem_u32(&bars[2 * NSTAGE]), tempty0 = smem_u32(&bars[2 * NSTAGE + NACC]);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t TMEM_COLS = (NACC * N) < 32 ? 32u : (uint32_t)(NACC * N);
 
-  // ---- one-time setup: barriers, TMEM, zeroed A stages (the 3 pad chunks stay zero), weights, bias ----
+  // ---- one-time setup: barriers, zeroed A stages (the 3 pad chunks stay zero), weights, bias ----
   if (threadIdx.x == 0) {
-    for (int s = 0; s < NSTAGE; ++s) { mbar_init(full0 + 8 * s, 128); mbar_init(empty0 + 8 * s, 1); }
-    for (int s = 0; s < NACC; ++s) { mbar_init(tfull0 + 8 * s, 1); mbar_init(tempty0 + 8 * s, 4); }
+    for (int s = 0; s < NSTAGE; ++s) { mbar_init(full0 + 8 * s, 128); mbar_init(empty0 + 8 * s, CONS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 4 * PGROUPS) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   for (int i = threadIdx.x; i < NSTAGE * A_STAGE_BYTES / 16; i += ST_THREADS)
     asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(a_base + i * 16), "r"(0u) : "memory");
@@ -82,10 +74,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stem_tc_kernel(const StemArgs a
   }
   for (int i = threadIdx.x; i < N; i += ST_THREADS) s_bias[i] = a.bias ? __ldg(a.bias + i) : 0.f;
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
   auto decode_tile = [&](int t, int &n, int &h0, int &w0) {
     const int tw = t % a.tiles_w; t /= a.tiles_w;
@@ -93,11 +82,11 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stem_tc_kernel(const StemArgs a
     h0 = th * TH; w0 = tw * TW;
   };
 
-  if (warp < 4 * PGROUPS) {
+  if (warp >= CONS / 32) {
     // =============================== producers: patch -> swizzled K-major operand rows ===============================
-    // One warp per scheduler is latency-bound on the LDS -> cvt -> STS chains (624 us for 32 x 512^2 with one group),
-    // so PGROUPS groups work on alternate tiles; stages are handed to the MMA warp in tile order.
-    const int grp = warp >> 2;
+    // One warp per scheduler is latency-bound on the LDS -> cvt -> STS chains, so PGROUPS groups work on alternate tiles;
+    // stages are handed to the consumers in tile order.
+    const int grp = (warp - CONS / 32) >> 2;
     const int m = threadIdx.x & 127;                       // operand row = tile pixel (ty, tx)
     const int ty = m >> 4, tx = m & 15;
     float *patch = patch0 + grp * (2 * CIN * PH * PP);
@@ -107,7 +96,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stem_tc_kernel(const StemArgs a
     constexpr int NLD = (CIN * PH * PW + 127) / 128;       // patch elements per producer thread
     float pre[NLD];
     // The patch of tile i+1 is requested from global memory BEFORE tile i's operand rows are built and parked in
-    // registers meanwhile: without this every tile paid a full exposed DRAM/L2 round trip (2.7 us per tile).
+    // registers meanwhile: without this every tile pays a full exposed DRAM/L2 round trip.
     auto fetch = [&](int t) {
       int n, h0, w0; decode_tile(t, n, h0, w0);
       const int hi0 = h0 * S - 3, wi0 = w0 * S - 3;
@@ -155,99 +144,64 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stem_tc_kernel(const StemArgs a
       // next tile's bar.sync, i.e. every producer has finished reading this buffer.
       pb ^= 1;
     }
-  } else if (warp == 4 * PGROUPS) {
-    // =============================== MMA issuer ===============================
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t accphase = 0;
-    for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-      mbar_wait(tempty0 + 8 * acc, accphase ^ 1);
-      mbar_wait(full0 + 8 * stage, phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d_tmem = tmem_base + acc * N;
-        const uint64_t ad0 = make_desc(a_base + stage * A_STAGE_BYTES, 128, 2);
-        const uint64_t bd0 = make_desc(b_base, 128, 2);
-#pragma unroll
-        for (int sl = 0; sl < SLABS; ++sl) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(d_tmem, ad0 + (uint32_t)(sl * (A_SLAB_BYTES >> 4) + 2 * k), bd0 + (uint32_t)(sl * (B_SLAB_BYTES >> 4) + 2 * k),
-                      idesc, (sl > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(empty0 + 8 * stage);
-        umma_commit(tfull0 + 8 * acc);
-      }
-      __syncwarp();
-      if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-      if (++acc == NACC) { acc = 0; accphase ^= 1; }
-    }
   } else {
-    // =============================== epilogue (4 warps) ===============================
-    const int q = warp & 3;                                // TMEM lane quadrant this warp may read
-    const int m = q * 32 + lane;
-    const int ty = m >> 4, tx = m & 15;
-    int acc = 0; uint32_t accphase = 0;
+    // =============================== consumers: wgmma + epilogue ===============================
+    const int wg = warp >> 2, tq = threadIdx.x & 127;
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    int stage = 0; uint32_t phase = 0;
     for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-      int n, h0, w0; decode_tile(t, n, h0, w0);
-      const int ho = h0 + ty, wo = w0 + tx;
-      const bool ok = ho < a.Ho && wo < a.Wo;
-      __nv_bfloat16 *o = a.y + (((size_t)n * a.Ho + ho) * a.Wo + wo) * N;
-      mbar_wait(tfull0 + 8 * acc, accphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * N;
+      mbar_wait(full0 + 8 * stage, phase);
+      const uint64_t ad0 = make_desc(a_base + stage * A_STAGE_BYTES + wg * 64 * 128, 128, 1);
+      const uint64_t bd0 = make_desc(b_base, 128, 1);
+      wg_fence();
 #pragma unroll
-      for (int c = 0; c < N / 16; ++c) {
-        uint32_t v[16];
-        tmem_ld16(taddr + c * 16, v);
-        tmem_ld_wait();
-        if (ok) {
-          uint4 o0, o1;
-          __nv_bfloat162 *ob0 = reinterpret_cast<__nv_bfloat162 *>(&o0), *ob1 = reinterpret_cast<__nv_bfloat162 *>(&o1);
+      for (int sl = 0; sl < SLABS; ++sl) {
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            ob0[j] = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(__uint_as_float(v[2 * j]) + s_bias[c * 16 + 2 * j], a.act),
-                                           cpb::act_out<__nv_bfloat16>(__uint_as_float(v[2 * j + 1]) + s_bias[c * 16 + 2 * j + 1], a.act));
-            ob1[j] = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(__uint_as_float(v[8 + 2 * j]) + s_bias[c * 16 + 8 + 2 * j], a.act),
-                                           cpb::act_out<__nv_bfloat16>(__uint_as_float(v[8 + 2 * j + 1]) + s_bias[c * 16 + 8 + 2 * j + 1], a.act));
-          }
-          { const uint32_t ow[8] = {o0.x, o0.y, o0.z, o0.w, o1.x, o1.y, o1.z, o1.w}; st_global_32B(o + c * 16, ow); }
-        }
+        for (int k = 0; k < 4; ++k)
+          wgmma_k16<N>(acc, ad0 + (uint32_t)(sl * (A_SLAB_BYTES >> 4) + 2 * k), bd0 + (uint32_t)(sl * (B_SLAB_BYTES >> 4) + 2 * k),
+                       (sl > 0 || k > 0) ? 1u : 0u, 1u);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-      if (++acc == NACC) { acc = 0; accphase ^= 1; }
+      wg_commit();
+      wg_wait<0>();
+      acc_fence(acc);
+      if (lane == 0) mbar_arrive(empty0 + 8 * stage);
+      if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+      int n, h0, w0; decode_tile(t, n, h0, w0);
+#pragma unroll
+      for (int j = 0; j < N / 4; ++j) {
+        const int m = wg * 64 + frag_row(tq, j), c = frag_col(tq, j);
+        const int ho = h0 + (m >> 4), wo = w0 + (m & 15);
+        if (ho >= a.Ho || wo >= a.Wo) continue;
+        store_pair16<1>(a.y, nullptr, (((size_t)n * a.Ho + ho) * a.Wo + wo) * N + c, 0, acc[2 * j] + s_bias[c], acc[2 * j + 1] + s_bias[c + 1],
+                        a.act, 0u);
+      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4 * PGROUPS) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Stride-1 variant (DLA-34 base_layer): fold only the VERTICAL taps into the K dimension and let the UMMA
+// Stride-1 variant (DLA-34 base_layer): fold only the VERTICAL taps into the K dimension and let the wgmma
 // descriptors do the horizontal ones.  Per tile (16 rows x 8 cols) the producers build, for every output row ty
 // and every input column x of the 14-wide halo, ONE 64-byte vector T[ty][x][k = c*7 + r] = in[c][ty + r][x]
 // (21 real values of 32) — 224 vectors instead of 128 x 21 chunks, ~8x less shared-memory traffic and cvt work.
 // Horizontal tap s is then the operand window starting s vectors later: descriptor start + s * 64 B, stride
 // between 8-row groups = 14 * 64 B (same shifted-window trick as csrc/net_tc3.cu; 64-byte swizzle on absolute
-// address bits).  7 taps x K=32 = 14 tcgen05.mma per tile.
+// address bits).  7 taps x K=32 = 14 wgmma per warpgroup and tile.
 constexpr int HT_H = 16, HT_W = 8;                       // output tile, M = 128, m = ty * 8 + tx
 constexpr int HP_W = HT_W + 6, HP_H = HT_H + 6;          // input patch 22 x 14 per channel
 constexpr int HVEC = HT_H * HP_W;                        // 224 operand vectors per tile = producer threads
 constexpr int HA_STAGE_BYTES = ((HVEC * 64 + 1023) / 1024) * 1024;
-constexpr int H_GROUPS = 3;                              // producer groups (7 warps each) on alternate tiles: tiles in flight
-constexpr int H_THREADS = H_GROUPS * HVEC + 5 * 32;      // producers + MMA warp + 4 epilogue warps
+constexpr int H_GROUPS = 1;                              // producer groups (7 warps each) on alternate tiles: the consumers' 64
+                                                         // accumulator registers leave room for one beside them
+constexpr int H_THREADS = CONS + H_GROUPS * HVEC;        // consumers + producers
 template <int N_, int P_> struct HStages { static constexpr int value = (P_ == 2 && N_ > 16) ? 4 : 6; };
 
 // P = 2 (split operands, CPB200_BF16X2 / CPB200_F16X2): every producer thread splits its 21 fp32 input values into a hi and a
 // lo 64-byte vector; a stage is [hi vectors | lo vectors], the weight image per horizontal tap [hi tile | lo tile]
-// (plan.py::_pack_stem_tc_h), so A_hi x [W_hi ; W_lo] is one N = 2N instruction into two accumulator halves and
-// A_lo x W_hi a second one; the epilogue adds the halves and stores the hi / lo planes of the output.
+// (plan.py::_pack_stem_tc_h); A_hi x W_hi goes to one accumulator array, A_hi x W_lo and
+// A_lo x W_hi to a second one; the epilogue adds them and stores the hi / lo planes of the output.
 template <int N, int P>
 __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs a) {
   constexpr int H_NSTAGE = HStages<N, P>::value;
@@ -255,28 +209,18 @@ __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs 
   constexpr int HA_STAGE = P * HA_PLANE_BYTES;
   constexpr int B_TILE_BYTES = N * 64;
   constexpr int B_TAP_BYTES = P * B_TILE_BYTES;
-  constexpr int ACC_COLS = P * N;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;
   const uint32_t b_base = smem_base + H_NSTAGE * HA_STAGE;
-  __shared__ __align__(8) uint64_t bars[2 * H_NSTAGE + 2 * NACC];
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t bars[2 * H_NSTAGE];
   __shared__ float s_bias[N];
   const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[H_NSTAGE]);
-  const uint32_t tfull0 = smem_u32(&bars[2 * H_NSTAGE]), tempty0 = smem_u32(&bars[2 * H_NSTAGE + NACC]);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int MMA_WARP = H_GROUPS * HVEC / 32;
-  constexpr uint32_t TMEM_COLS = (NACC * ACC_COLS) < 32 ? 32u : (uint32_t)(NACC * ACC_COLS);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < H_NSTAGE; ++s) { mbar_init(full0 + 8 * s, HVEC); mbar_init(empty0 + 8 * s, 1); }
-    for (int s = 0; s < NACC; ++s) { mbar_init(tfull0 + 8 * s, 1); mbar_init(tempty0 + 8 * s, 4); }
+    for (int s = 0; s < H_NSTAGE; ++s) { mbar_init(full0 + 8 * s, HVEC); mbar_init(empty0 + 8 * s, CONS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   for (int i = threadIdx.x; i < H_NSTAGE * HA_STAGE / 16; i += H_THREADS)      // pad values (k >= 21) stay zero
     asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(a_base + i * 16), "r"(0u) : "memory");
@@ -286,36 +230,24 @@ __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs 
   }
   for (int i = threadIdx.x; i < N; i += H_THREADS) s_bias[i] = a.bias ? __ldg(a.bias + i) : 0.f;
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
   auto decode_tile = [&](int t, int &n, int &h0, int &w0) {
     const int tw = t % a.tiles_w; t /= a.tiles_w;
     const int th = t % a.tiles_h; n = t / a.tiles_h;
     h0 = th * HT_H; w0 = tw * HT_W;
   };
-  auto sbo_desc = [](uint32_t saddr, uint32_t sbo_bytes) {      // K-major, 64-byte swizzle (layout type 4)
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(sbo_bytes >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)4 << 61;
-    return d;
-  };
 
-  if (warp < MMA_WARP) {
+  if (warp >= CONS / 32) {
     // =============================== producers: thread v = (ty, x) builds one 64-byte vector ===============================
     // The 21 values come straight from global memory (read-only path; the 7 threads that share an input element
     // hit L1) and the NEXT tile's values are requested before this tile's vector is converted and stored, so a
     // producer thread never waits on anything but the stage's empty barrier: no CTA-level barrier, no staging
     // buffer.  What bounds a producer is the global-load round trip of its NEXT tile (~1 us under load: three
-    // different producer designs all ran at ~1.1 us per tile with one tile in flight), so H_GROUPS independent
-    // groups take alternate tiles and hand their stages to the MMA warp in tile order.
-    const int grp = threadIdx.x / HVEC;
-    const int v = threadIdx.x - grp * HVEC;
+    // with one tile in flight), so H_GROUPS independent
+    // groups take alternate tiles and hand their stages to the consumers in tile order.
+    const int grp = (threadIdx.x - CONS) / HVEC;
+    const int v = (threadIdx.x - CONS) - grp * HVEC;
     const int tstep = gridDim.x * H_GROUPS;
     const int ty = v / HP_W, x = v % HP_W;
     float f[24];
@@ -380,102 +312,55 @@ __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs 
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       mbar_arrive(full0 + 8 * stage);
     }
-  } else if (warp == MMA_WARP) {
-    // =============================== MMA issuer ===============================
-    const uint32_t idesc = P == 1 ? ((1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24))
-                                  : idesc_m128(N, a.fmt);
-    const uint32_t idesc2 = idesc_m128(2 * N, a.fmt);
-    int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t accphase = 0;
-    for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-      mbar_wait(tempty0 + 8 * acc, accphase ^ 1);
-      mbar_wait(full0 + 8 * stage, phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-        const uint64_t ad0 = sbo_desc(a_base + stage * HA_STAGE, HP_W * 64);
-        const uint64_t bd0 = sbo_desc(b_base, 8 * 64);
-#pragma unroll
-        for (int s = 0; s < 7; ++s) {
-#pragma unroll
-          for (int k = 0; k < 2; ++k) {
-            const uint32_t first = (s > 0 || k > 0) ? 1u : 0u;
-            if constexpr (P == 2) {
-              umma_bf16(d_tmem, ad0 + (uint32_t)(s * 4 + 2 * k), bd0 + (uint32_t)(s * (B_TAP_BYTES >> 4) + 2 * k), idesc2, first);
-              umma_bf16(d_tmem + N, ad0 + (uint32_t)((HA_PLANE_BYTES >> 4) + s * 4 + 2 * k), bd0 + (uint32_t)(s * (B_TAP_BYTES >> 4) + 2 * k), idesc, 1u);
-            } else {
-              umma_bf16(d_tmem, ad0 + (uint32_t)(s * 4 + 2 * k), bd0 + (uint32_t)(s * (B_TAP_BYTES >> 4) + 2 * k), idesc, first);
-            }
-          }
-        }
-        umma_commit(empty0 + 8 * stage);
-        umma_commit(tfull0 + 8 * acc);
-      }
-      __syncwarp();
-      if (++stage == H_NSTAGE) { stage = 0; phase ^= 1; }
-      if (++acc == NACC) { acc = 0; accphase ^= 1; }
-    }
   } else {
-    // =============================== epilogue (4 warps) ===============================
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int ty = m >> 3, tx = m & 7;
-    int acc = 0; uint32_t accphase = 0;
+    // =============================== consumers: wgmma + epilogue ===============================
+    const int wg = warp >> 2, tq = threadIdx.x & 127;
+    const uint32_t bf = (P == 1 || a.fmt == 0) ? 1u : 0u;
+    float acc[N / 2], acc2[P == 2 ? N / 2 : 1];                 // hi x W_hi | hi x W_lo + lo x W_hi (split operands)
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (P == 2 ? N / 2 : 1); ++i) acc2[i] = 0.f;
+    int stage = 0; uint32_t phase = 0;
     for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-      int n, h0, w0; decode_tile(t, n, h0, w0);
-      const int ho = h0 + ty, wo = w0 + tx;
-      const bool ok = ho < a.Ho && wo < a.Wo;
-      __nv_bfloat16 *o = a.y + (((size_t)n * a.Ho + ho) * a.Wo + wo) * N;
-      mbar_wait(tfull0 + 8 * acc, accphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_COLS;
+      mbar_wait(full0 + 8 * stage, phase);
+      // this warpgroup's 64 rows = output rows 8 wg .. 8 wg + 7 = 8 halo rows of vectors further on
+      const uint64_t ad0 = desc_sbo(a_base + stage * HA_STAGE + wg * 8 * HP_W * 64, HP_W * 64, 2);
+      const uint64_t bd0 = desc_sbo(b_base, 8 * 64, 2);
+      wg_fence();
 #pragma unroll
-      for (int c = 0; c < N / 16; ++c) {
-        uint32_t v[16];
-        tmem_ld16(taddr + c * 16, v);
-        if constexpr (P == 2) {
-          uint32_t v2[16];
-          tmem_ld16(taddr + N + c * 16, v2);
-          tmem_ld_wait();
-          if (ok) {
-            uint32_t oh[8], ol[8];
+      for (int s = 0; s < 7; ++s) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float x0 = fmaf(__uint_as_float(v[2 * j]) + __uint_as_float(v2[2 * j]), a.acc_scale, s_bias[c * 16 + 2 * j]);
-              const float x1 = fmaf(__uint_as_float(v[2 * j + 1]) + __uint_as_float(v2[2 * j + 1]), a.acc_scale, s_bias[c * 16 + 2 * j + 1]);
-              split2(cpb::act_fast(x0, a.act), cpb::act_fast(x1, a.act), a.fmt, oh[j], ol[j]);
-            }
-            uint16_t *op_ = reinterpret_cast<uint16_t *>(o) + c * 16;
-            st_global_32B(op_, oh);
-            st_global_32B(op_ + a.y_plane, ol);
+        for (int k = 0; k < 2; ++k) {
+          const uint32_t first = (s > 0 || k > 0) ? 1u : 0u;
+          const uint64_t ad = ad0 + (uint32_t)(s * 4 + 2 * k), bd = bd0 + (uint32_t)(s * (B_TAP_BYTES >> 4) + 2 * k);
+          if constexpr (P == 2) {
+            wgmma_k16<N>(acc, ad, bd, first, bf);                                            // A_hi x W_hi
+            wgmma_k16<N>(acc2, ad, bd + (uint32_t)(B_TILE_BYTES >> 4), first, bf);           // A_hi x W_lo
+            wgmma_k16<N>(acc2, ad + (uint32_t)(HA_PLANE_BYTES >> 4), bd, 1u, bf);            // A_lo x W_hi
+          } else {
+            wgmma_k16<N>(acc, ad, bd, first, 1u);
           }
-          continue;
-        }
-        tmem_ld_wait();
-        if (ok) {
-          uint4 o0, o1;
-          __nv_bfloat162 *ob0 = reinterpret_cast<__nv_bfloat162 *>(&o0), *ob1 = reinterpret_cast<__nv_bfloat162 *>(&o1);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            ob0[j] = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(__uint_as_float(v[2 * j]) + s_bias[c * 16 + 2 * j], a.act),
-                                           cpb::act_out<__nv_bfloat16>(__uint_as_float(v[2 * j + 1]) + s_bias[c * 16 + 2 * j + 1], a.act));
-            ob1[j] = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(__uint_as_float(v[8 + 2 * j]) + s_bias[c * 16 + 8 + 2 * j], a.act),
-                                           cpb::act_out<__nv_bfloat16>(__uint_as_float(v[8 + 2 * j + 1]) + s_bias[c * 16 + 8 + 2 * j + 1], a.act));
-          }
-          { const uint32_t ow[8] = {o0.x, o0.y, o0.z, o0.w, o1.x, o1.y, o1.z, o1.w}; st_global_32B(o + c * 16, ow); }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-      if (++acc == NACC) { acc = 0; accphase ^= 1; }
+      wg_commit();
+      wg_wait<0>();
+      acc_fence(acc); acc_fence(acc2);
+      if (lane == 0) mbar_arrive(empty0 + 8 * stage);
+      if (++stage == H_NSTAGE) { stage = 0; phase ^= 1; }
+      int n, h0, w0; decode_tile(t, n, h0, w0);
+#pragma unroll
+      for (int j = 0; j < N / 4; ++j) {
+        const int m = wg * 64 + frag_row(tq, j), c = frag_col(tq, j);
+        const int ho = h0 + (m >> 3), wo = w0 + (m & 7);
+        if (ho >= a.Ho || wo >= a.Wo) continue;
+        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
+        if constexpr (P == 2) { v0 += acc2[2 * j]; v1 += acc2[2 * j + 1]; }
+        const float f0 = P == 2 ? fmaf(v0, a.acc_scale, s_bias[c]) : v0 + s_bias[c];
+        const float f1 = P == 2 ? fmaf(v1, a.acc_scale, s_bias[c + 1]) : v1 + s_bias[c + 1];
+        store_pair16<P>(a.y, nullptr, (((size_t)n * a.Ho + ho) * a.Wo + wo) * N + c, a.y_plane, f0, f1, a.act, a.fmt);
+      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 

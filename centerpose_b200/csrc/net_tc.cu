@@ -1,28 +1,29 @@
-// tcgen05 / TMEM / TMA implicit-GEMM convolution for sm_100a (bf16 NHWC activations, fp32
-// accumulate in tensor memory).
+// wgmma / TMA implicit-GEMM convolution for sm_90a (bf16 NHWC activations, fp32 accumulate in registers).
 //
-//   M tile  = 128 output pixels = a TH x TW rectangle of one image (8x16, or 16x8 for narrow maps)
-//   N tile  = BN output channels (16..256), one tcgen05.mma.cta_group::1.kind::f16 of shape 128 x BN x 16
+//   M tile  = 128 output pixels = a TH x TW rectangle of one image (8x16, or 16x8 for narrow maps); two consumer warpgroups
+//             own rows 0-63 and 64-127 (wgmma m64nNk16 each)
+//   N tile  = BN output channels (16..256)
 //   K loop  = filter taps x concatenated inputs x channel slabs of BK (64/32/16 = one swizzle atom)
 //
 // A operand: for tap (r,s) the 128 x BK slab is the input window
 //   x[n, h0*stride + r - pad : .. : stride, w0*stride + s - pad : .. : stride, c0 : c0+BK]
 // fetched by ONE 4-D TMA tiled load (box {BK, TW, TH, 1}, element strides {1,stride,stride,1});
 // TMA zero-fills out-of-bounds coordinates, which IS the convolution's zero padding, and lands the
-// box in shared memory as 128 rows of BK bf16 in the 128B/64B/32B-swizzled K-major layout the UMMA
+// box in shared memory as 128 rows of BK bf16 in the 128B/64B/32B-swizzled K-major layout the wgmma
 // shared-memory descriptor expects — no im2col buffer exists anywhere.
 // B operand: weights packed slab-major [tap][K-slab][Cout_pad][BK] bf16 (K-major), 3-D TMA box {BK, BN, 1}.
 // `Root` concatenations are K-slabs from up to four tensor maps (no torch.cat copy).
 //
-// Warp roles (192 threads, persistent CTAs, one per SM): warp 0 = TMA producer, warp 1 = MMA
-// issuer + TMEM owner, warps 2..5 = epilogue (tcgen05.ld -> +bias (+residual) -> ReLU -> bf16 ->
-// global).  Two to eight TMEM accumulator stages let the epilogue of tile i overlap the MMAs of tile i+1;
-// a STAGES-deep smem ring with full/empty mbarriers feeds the tensor core.
+// Warp roles (persistent CTAs, one per SM): warps 0-7 = two consumer warpgroups (wgmma issue, then the epilogue straight
+// from the accumulator registers: +bias (+residual) -> activation -> store), warp 8 = TMA producer (DCN: warps 8-15 gather
+// the A tile, one lane of warp 8 also issues the weight loads); a STAGES-deep smem ring
+// with full/empty mbarriers feeds the tensor cores, and a stage is released as soon as the MMAs of the NEXT stage are queued.
 //
 // Split-operand precisions (P = 2, CPB200_BF16X2 / CPB200_F16X2, see tc_common.cuh): a stage is
-// [A_hi | A_lo | W_hi | W_lo]; per K step the issuer emits A_hi x [W_hi ; W_lo] as one N = 2*BN instruction when
-// 2*BN <= 256 (two adjacent accumulator halves, added in the epilogue) plus A_lo x W_hi, or three N = BN instructions
-// for BN = 256.  The DCN gather blends the four corners of BOTH planes in fp32 and re-splits the sample.
+// [A_hi | A_lo | W_hi | W_lo]; per K step the consumers issue three N = BN products: A_hi x W_hi into one accumulator array,
+// A_hi x W_lo and A_lo x W_hi into a second one (added in the epilogue).  Separate arrays keep the wgmma of one K step
+// independent of each other, so ptxas does not serialise them.
+// The DCN gather blends the four corners of BOTH planes in fp32 and re-splits the sample.
 #include <type_traits>
 #include "tc_common.cuh"
 #include <mutex>
@@ -30,7 +31,8 @@
 
 namespace {
 
-constexpr int TC_THREADS = 320;        // TMA producer, MMA issuer, two epilogue groups of four warps (tiles alternate between them)
+constexpr int CONS_THREADS = 256;      // two consumer warpgroups
+constexpr int TC_THREADS = CONS_THREADS + 32;        // + TMA producer warp
 constexpr int TILE_M = 128;
 
 struct alignas(64) TcArgs {
@@ -42,16 +44,16 @@ struct alignas(64) TcArgs {
   int B, Ho, Wo;
   int TH, TW, tiles_h, tiles_w, n_tiles;
   int cout, cout_store;       // cout_store: channel pitch of dst/res
-  int BK, stages, total_tiles, nacc;
+  int BK, stages, total_tiles;
   void *dst;
   const void *res;
   const float *bias;
   unsigned flags;
-  unsigned swizzle_bits;      // UMMA layout_type for the chosen BK
+  unsigned swizzle_bits;      // wgmma layout type for the chosen BK
   // deformable conv (DCN) only: A tiles are gathered by producer warps instead of TMA
   const __nv_bfloat16 *dcn_src;   // (B,H,W,Cin) bf16
   const float *dcn_om;            // (B,H,W,27) fp32: 18 offsets (dy,dx per tap) | 9 mask logits
-  int H, W, om_pitch, dcn_prefetch;
+  int H, W, om_pitch;
   int Hd, Wd, sy, sx, oy, ox;     // strided output mapping (dense ConvTranspose2d parity sub-convs)
   int out_ch_off, out_ch_total;   // NCHW fp32 output: channel slice of dst
   // split-operand mode (P = 2)
@@ -64,50 +66,32 @@ struct alignas(64) TcArgs {
 
 using namespace tc;
 
-#ifndef CPB_DCN_GW
-#define CPB_DCN_GW 16                 // gather-producer warps: 8 (16 rows each, two half batches) or 16 (8 rows each)
-#endif
-constexpr int DCN_GW = CPB_DCN_GW;
+constexpr int DCN_GW = 8;                       // gather-producer warps
 constexpr int DCN_ROWS = 128 / DCN_GW;          // operand rows per gather warp
-constexpr int DCN_THREADS = (6 + DCN_GW) * 32;
+constexpr int DCN_THREADS = CONS_THREADS + DCN_GW * 32;   // 16 warps: 4 per scheduler partition leave 128 registers a thread
 
 struct __align__(16) DcnPrm { int off[4]; uint32_t wt[4]; };   // element offsets; corner weights: packed bf16x2 (w,w), or fp32 bits when P = 2
 
 template <int BN, bool DCN, int P>
 __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcArgs a) {
-  constexpr bool NCAT = (P == 2) && (2 * BN <= 256);       // hi*[hi;lo] as one N = 2*BN instruction
-  constexpr int ACC_COLS = NCAT ? 2 * BN : BN;             // TMEM columns per accumulator stage
+  static_assert(P == 1 || BN <= 128, "split operands: two BN-column accumulators per thread");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages x (A planes | B planes)] then barriers
+  // carve: [stages x (A planes | B planes)]
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_bytes = TILE_M * a.BK * 2, b_bytes = BN * a.BK * 2;
   const uint32_t stage_bytes = P * a_bytes + ((P * b_bytes + 1023u) & ~1023u);
-  __shared__ __align__(8) uint64_t bars[2 * 8 + 16];
-  __shared__ uint32_t s_tmem;
-  __shared__ float s_bias[2][2][BN];      // [epilogue group][tile parity within the group]
+  __shared__ __align__(8) uint64_t bars[2 * 8];
   __shared__ DcnPrm s_prm[DCN ? DCN_GW : 1][DCN ? 9 : 1][DCN ? DCN_ROWS : 1];
   const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[8]);
-  const uint32_t tfull0 = smem_u32(&bars[16]), tempty0 = smem_u32(&bars[24]);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t need_cols = (uint32_t)a.nacc * ACC_COLS;
-  const uint32_t TMEM_COLS = need_cols <= 32 ? 32u : need_cols <= 64 ? 64u : need_cols <= 128 ? 128u : need_cols <= 256 ? 256u : 512u;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == CONS_THREADS) {
     if (!DCN) for (int s = 0; s < a.nsrc; ++s) tmap_prefetch(&a.amap[s]);
     tmap_prefetch(&a.bmap);
-    for (int s = 0; s < a.stages; ++s) { mbar_init(full0 + 8 * s, DCN ? 1 + DCN_GW : 1); mbar_init(empty0 + 8 * s, 1); }
-    for (int s = 0; s < 8; ++s) { mbar_init(tfull0 + 8 * s, 1); mbar_init(tempty0 + 8 * s, 4); }
+    for (int s = 0; s < a.stages; ++s) { mbar_init(full0 + 8 * s, DCN ? 1 + DCN_GW : 1); mbar_init(empty0 + 8 * s, CONS_THREADS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
   const int taps = a.kh * a.kw;
   int kblocks_per_tap = 0;
@@ -121,7 +105,7 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
     h0 = th * a.TH; w0 = tw * a.TW;
   };
 
-  if (warp == 0) {
+  if (!DCN && warp == CONS_THREADS / 32) {
     // =============================== TMA producer ===============================
     if (elect_one()) {
       int stage = 0; uint32_t phase = 0;
@@ -135,13 +119,9 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
             for (int c0 = 0; c0 < a.cin[s]; c0 += a.BK) {
               mbar_wait(empty0 + 8 * stage, phase ^ 1);
               const uint32_t sa = smem_base + stage * stage_bytes, sb = sa + P * a_bytes;
-              if (DCN) {
-                mbar_expect_tx(full0 + 8 * stage, P * b_bytes);
-              } else {
-                mbar_expect_tx(full0 + 8 * stage, P * (a_bytes + b_bytes));
+              mbar_expect_tx(full0 + 8 * stage, P * (a_bytes + b_bytes));
 #pragma unroll
-                for (int pl = 0; pl < P; ++pl) tma_load_4d(sa + pl * a_bytes, &a.amap[s], full0 + 8 * stage, c0, wi, hi, n + pl * a.B);
-              }
+              for (int pl = 0; pl < P; ++pl) tma_load_4d(sa + pl * a_bytes, &a.amap[s], full0 + 8 * stage, c0, wi, hi, n + pl * a.B);
 #pragma unroll
               for (int pl = 0; pl < P; ++pl)
                 tma_load_3d(sb + pl * b_bytes, &a.bmap, full0 + 8 * stage, 0, nt * BN,
@@ -153,93 +133,42 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    // instruction descriptor: D=f32, A=B=bf16, both K-major, N = BN, M = 128
-    const uint32_t idesc = P == 1 ? ((1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TILE_M >> 4) << 24))
-                                  : idesc_m128(BN, a.fmt);
-    const uint32_t idesc2 = idesc_m128(NCAT ? 2 * BN : BN, a.fmt);
-    // ONE elected thread runs the whole issue loop in the form tools/mma_probe.py's `pipe2` mode shows to reach the back-to-back
-    // MMA rate (profiles/r02_mma_probe_pipe*.log): K steps unrolled at compile time, descriptor templates + a 14-bit start
-    // address, the accumulate flag in a register, and the next stage's full barrier polled before this stage's MMAs.
-    if (elect_one()) {
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t accphase = 0;
-      const uint32_t row_bytes = a.BK * 2;
-      const uint64_t dT = make_desc(0u, row_bytes, a.swizzle_bits);
-      const uint32_t base14 = (smem_base & 0x3FFFFu) >> 4, sstep = stage_bytes >> 4;
-      const uint32_t aplane = a_bytes >> 4, bplane = b_bytes >> 4, boff = (uint32_t)(P * a_bytes) >> 4;   // descriptor start-address units
-      auto run = [&](auto KS_) {
-        constexpr int KS = decltype(KS_)::value;
-        uint32_t peek = mbar_try_once(full0 + 8 * stage, phase);
-        for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-          mbar_wait(tempty0 + 8 * acc, accphase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-          uint32_t accf = 0u;                                    // 0 for the tile's very first MMA, 1 afterwards
-          for (int kb = 0; kb < kblocks; ++kb) {
-            if (!peek) mbar_wait(full0 + 8 * stage, phase);
-            tc_fence_after();
-            const uint64_t ad = dT + (base14 + (uint32_t)stage * sstep), bd = ad + boff;
-            const uint32_t empty = empty0 + 8 * stage;
-            if (++stage == a.stages) { stage = 0; phase ^= 1; }
-            peek = mbar_try_once(full0 + 8 * stage, phase);
-#pragma unroll
-            for (int k = 0; k < KS; ++k) {
-              const uint32_t first = k == 0 ? accf : 1u;
-              if constexpr (P == 1) {
-                umma_bf16(d_tmem, ad + 2 * k, bd + 2 * k, idesc, first);
-              } else {
-                if constexpr (NCAT) {
-                  umma_bf16(d_tmem, ad + 2 * k, bd + 2 * k, idesc2, first);                 // A_hi x [W_hi ; W_lo]
-                } else {
-                  umma_bf16(d_tmem, ad + 2 * k, bd + 2 * k, idesc, first);                  // A_hi x W_hi
-                  umma_bf16(d_tmem, ad + 2 * k, bd + bplane + 2 * k, idesc, 1u);            // A_hi x W_lo
-                }
-                // A_lo x W_hi joins the other small term in the second accumulator half (see net_tc3.cu: the fp32
-                // accumulator truncates per instruction in proportion to its magnitude)
-                umma_bf16(d_tmem + (NCAT ? BN : 0), ad + aplane + 2 * k, bd + 2 * k, idesc, 1u);
-              }
-            }
-            accf = 1u;
-            umma_commit(empty);                         // frees the smem slot when these MMAs retire
-            if (kb == kblocks - 1) umma_commit(tfull0 + 8 * acc);
-          }
-          if (++acc == a.nacc) { acc = 0; accphase ^= 1; }
-        }
-      };
-      const int ksteps = a.BK / 16;
-      if (ksteps == 4) run(std::integral_constant<int, 4>{});
-      else if (ksteps == 2) run(std::integral_constant<int, 2>{});
-      else run(std::integral_constant<int, 1>{});
-    }
-    __syncwarp();
-  } else if (DCN && warp >= 6) {
-    // =============================== DCN gather producers (warps 6..21) ===============================
+  } else if (DCN && warp >= CONS_THREADS / 32) {
+    // =============================== DCN gather producers ===============================
     // A[row = pixel][k = channel] of tap t is  sigmoid(mask_t) * bilinear(x, p + tap_t + offset_t)
     // (dcn_v2_im2col_cuda.cu:25-54,125-195), rounded to bf16 and stored straight into the 128B-swizzled
-    // K-major tile the UMMA descriptor reads (16-byte chunk j of row r lives at chunk j ^ (r & 7)).
-    // 16 gather warps x 8 rows (four warps per scheduler: the gather is latency-bound, more resident warps beat deeper
-    // per-thread pipelining; an 8 x 16 variant was 12 % slower).  Per tile each warp first turns the 27 offset/mask
-    // values of its pixels into (4 corner offsets, 4 corner weights) for all 9 taps (one round trip to global memory
-    // instead of one per tap); per stage every thread fetches 2 rows x 4 corners of one 16-byte chunk, and the loads
-    // of the NEXT unit of work are issued before this one's results are stored.
-    // P = 2 (split operands): corners come from both planes, are summed and blended in fp32 with fp32 weights
-    // (expf, not ex2.approx, for the mask), and the sample is re-split into the hi / lo A tiles; the unit of
-    // software pipelining is one row (8 loads in flight per thread, as for P = 1).
-    const int gw = warp - 6;                               // rows [DCN_ROWS*gw, DCN_ROWS*(gw+1))
+    // K-major tile the wgmma descriptor reads (16-byte chunk j of row r lives at chunk j ^ (r & 7)).
+    // Per tile each warp first turns the 27 offset/mask values of its pixels into (4 corner offsets, 4 corner weights) for
+    // all 9 taps (one round trip to global memory instead of one per tap); per stage every thread fetches the 4 corners of
+    // one 16-byte chunk of DCN_ROWS / 4 rows, and the loads of the NEXT unit of work are issued before this one's results
+    // are stored.  P = 2 (split operands): corners come from both planes, are summed and blended in fp32 with fp32 weights
+    // (expf, not ex2.approx, for the mask), and the sample is re-split into the hi / lo A tiles.
+    constexpr int NI = DCN_ROWS / 4;                       // rows per thread and stage
+    const int gw = warp - CONS_THREADS / 32;               // rows [DCN_ROWS*gw, DCN_ROWS*(gw+1))
+    // the weight tile of a stage: loaded by one lane of gather warp 0 once the stage is free (its expect_tx is the
+    // barrier's extra arrival)
+    auto load_b = [&](int stage_, int nt_, int tap, int c0) {
+      if (gw != 0 || lane != 0) return;
+      const uint32_t sb = smem_base + stage_ * stage_bytes + P * a_bytes;
+      mbar_expect_tx(full0 + 8 * stage_, P * b_bytes);
+#pragma unroll
+      for (int pl = 0; pl < P; ++pl)
+        tma_load_3d(sb + pl * b_bytes, &a.bmap, full0 + 8 * stage_, 0, nt_ * BN, pl * a.wplane + tap * kblocks_per_tap + c0 / a.BK);
+    };
     int stage = 0; uint32_t phase = 0;
     const int Cin = a.cin[0];
     const int slabs = Cin >> 6;
     const int nk = 9 * slabs;
     const int chunk = lane & 7, rsub = lane >> 3;
     const __nv_bfloat16 *srcc = a.dcn_src + chunk * 8;
-    static_assert(DCN_ROWS == 8, "gather layout: 16 warps x 8 rows");
-    const int px = lane & 7, tg = lane >> 3;               // pixel of the warp, tap group {0,1,2} {3,4} {5,6} {7,8}
+    const int px = lane & 7, tg = lane >> 3;               // pixel of the warp's group of 8, tap group {0,1,2} {3,4} {5,6} {7,8}
     const int tap0 = tg == 0 ? 0 : 1 + 2 * tg, ntap = tg == 0 ? 3 : 2;
     for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
       int n, h0, w0, nt; decode_tile(t, n, h0, w0, nt);
-      {
-        const int rp = gw * 8 + px;
+      __syncwarp();                                        // previous tile's readers are done with s_prm
+#pragma unroll 1
+      for (int pg = 0; pg < DCN_ROWS / 8; ++pg) {
+        const int rp = gw * DCN_ROWS + pg * 8 + px;
         const int ho = h0 + rp / a.TW, wo = w0 + rp % a.TW;
         const bool okp = ho < a.Ho && wo < a.Wo;
         const float *om = a.dcn_om + (((size_t)n * a.H + ho) * a.W + wo) * a.om_pitch;
@@ -250,7 +179,6 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
           const bool ld = okp && i < ntap;
           oh[i] = ld ? __ldg(om + 2 * tap) : 0.f; ow[i] = ld ? __ldg(om + 2 * tap + 1) : 0.f; ml[i] = ld ? __ldg(om + 18 + tap) : 0.f;
         }
-        __syncwarp();                                      // previous tile's readers are done with s_prm
 #pragma unroll
         for (int i = 0; i < 3; ++i) {
           if (i < ntap) {
@@ -277,18 +205,18 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
                 if (h_high <= a.H - 1 && w_high <= a.W - 1) { pr.off[3] = ((rowb + h_high) * a.W + w_high) * Cin * OS; pr.wt[3] = pk(lh * lw * mk); }
               }
             }
-            s_prm[gw][tap][px] = pr;
+            s_prm[gw][tap][pg * 8 + px] = pr;
           }
         }
-        __syncwarp();
       }
+      __syncwarp();
       if constexpr (P == 1) {
         uint4 v[2][4];
         uint32_t w[2][4];
-        auto issue = [&](int tap, int c0) {
+        auto issue = [&](int tap, int c0, int h) {           // rows (2h, 2h + 1) of this thread
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
-            const DcnPrm q = s_prm[gw][tap][i * 4 + rsub];
+            const DcnPrm q = s_prm[gw][tap][(2 * h + i) * 4 + rsub];
 #pragma unroll
             for (int c = 0; c < 4; ++c) {       // invalid corners: weight 0, offset 0 (a safe address)
               v[i][c] = __ldg(reinterpret_cast<const uint4 *>(srcc + (size_t)(unsigned)q.off[c] + c0));
@@ -296,33 +224,43 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
             }
           }
         };
-        int tap_n = 0, c0_n = 0;
-        issue(0, 0);
+        int tap_c = 0, c0_c = 0;
+        issue(0, 0, 0);
         for (int k = 0; k < nk; ++k) {
-          c0_n += 64;
+          int tap_n = tap_c, c0_n = c0_c + 64;
           if (c0_n >= Cin) { c0_n = 0; ++tap_n; }
           mbar_wait(empty0 + 8 * stage, phase ^ 1);
+          load_b(stage, nt, tap_c, c0_c);
           const uint32_t sa = smem_base + stage * stage_bytes;
 #pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            __nv_bfloat162 acc2[4];
+          for (int h = 0; h < NI / 2; ++h) {
+            uint4 o[2];
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const __nv_bfloat162 w2 = *reinterpret_cast<const __nv_bfloat162 *>(&w[i][c]);
-              const __nv_bfloat162 *vv = reinterpret_cast<const __nv_bfloat162 *>(&v[i][c]);
+            for (int i = 0; i < 2; ++i) {
+              __nv_bfloat162 acc2[4];
 #pragma unroll
-              for (int j = 0; j < 4; ++j) acc2[j] = (c == 0) ? __hmul2(w2, vv[j]) : __hfma2(w2, vv[j], acc2[j]);
+              for (int c = 0; c < 4; ++c) {
+                const __nv_bfloat162 w2 = *reinterpret_cast<const __nv_bfloat162 *>(&w[i][c]);
+                const __nv_bfloat162 *vv = reinterpret_cast<const __nv_bfloat162 *>(&v[i][c]);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc2[j] = (c == 0) ? __hmul2(w2, vv[j]) : __hfma2(w2, vv[j], acc2[j]);
+              }
+              o[i] = *reinterpret_cast<const uint4 *>(acc2);
             }
-            const uint4 o = *reinterpret_cast<const uint4 *>(acc2);
-            const int row = gw * 8 + i * 4 + rsub;
-            const uint32_t dst = sa + row * 128 + ((chunk ^ (row & 7)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(o.x), "r"(o.y), "r"(o.z), "r"(o.w) : "memory");
+            if (h + 1 < NI / 2) issue(tap_c, c0_c, h + 1);     // the next unit's corners fly across the stores / fence / wait
+            else if (k + 1 < nk) issue(tap_n, c0_n, 0);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const int row = gw * DCN_ROWS + (2 * h + i) * 4 + rsub;
+              const uint32_t dst = sa + row * 128 + ((chunk ^ (row & 7)) << 4);
+              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(o[i].x), "r"(o[i].y), "r"(o[i].z), "r"(o[i].w) : "memory");
+            }
           }
-          if (k + 1 < nk) issue(tap_n, c0_n);                // next stage's corners fly across the fence / arrive / wait
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
           __syncwarp();
-          if (lane == 0) mbar_arrive(full0 + 8 * stage);       // one arrival per gather warp (512 per-thread arrivals serialise on one word)
+          if (lane == 0) mbar_arrive(full0 + 8 * stage);       // one arrival per gather warp
           if (++stage == a.stages) { stage = 0; phase ^= 1; }
+          tap_c = tap_n; c0_c = c0_n;
         }
       } else {
         uint4 vh[4], vl[4];
@@ -347,15 +285,10 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
           int tap_n = tap_c, c0_n = c0_c + 64;
           if (c0_n >= Cin) { c0_n = 0; ++tap_n; }
           mbar_wait(empty0 + 8 * stage, phase ^ 1);
-          if (a.dcn_prefetch & 1) {                              // timing knob (CPB200_TC_DBG=1): no gather work at all
-            __syncwarp();
-            if (lane == 0) mbar_arrive(full0 + 8 * stage);
-            if (++stage == a.stages) { stage = 0; phase ^= 1; }
-            continue;
-          }
+          load_b(stage, nt, tap_c, c0_c);
           const uint32_t sa = smem_base + stage * stage_bytes;
 #pragma unroll
-          for (int i = 0; i < 2; ++i) {
+          for (int i = 0; i < NI; ++i) {
             float f[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) f[j] = 0.f;
@@ -363,8 +296,7 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
             if (a.fmt) {
               // fp16 planes: sample = sum_c w_c * hi_c (fp32 FMAs on the unpacked hi plane) + sum_c w_c * lo_c.  The second sum is
               // 2^-11 of the first, so packed fp16 FMAs on the lo plane as stored (weights rounded to fp16: error 2^-11 of
-              // 2^-11) leave the sample good to 2^-22 — and save the lo plane's unpack and the hi + lo adds (a third of the
-              // gather's arithmetic instructions; the gather's instruction count is what bounds the DCN, r02_dcn_whatif.md).
+              // 2^-11) leave the sample good to 2^-22 — and save the lo plane's unpack and the hi + lo adds.
               __half2 s2[4];
 #pragma unroll
               for (int j = 0; j < 4; ++j) s2[j] = __float2half2_rn(0.f);
@@ -381,7 +313,7 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
                 }
               }
               // the registers are free again: the next unit's corners fly while this one is split and stored
-              if (i == 0) issue(tap_c, c0_c, 1);
+              if (i + 1 < NI) issue(tap_c, c0_c, i + 1);
               else if (k + 1 < nk) issue(tap_n, c0_n, 0);
 #pragma unroll
               for (int j = 0; j < 4; ++j) {                  // |blend| <= max|x|: no saturation needed
@@ -401,180 +333,100 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
                   f[2 * j] = fmaf(wq[c], x.x, f[2 * j]); f[2 * j + 1] = fmaf(wq[c], x.y, f[2 * j + 1]);
                 }
               }
-              if (i == 0) issue(tap_c, c0_c, 1);
+              if (i + 1 < NI) issue(tap_c, c0_c, i + 1);
               else if (k + 1 < nk) issue(tap_n, c0_n, 0);
 #pragma unroll
               for (int j = 0; j < 4; ++j) split2_bounded(f[2 * j], f[2 * j + 1], 0u, oh[j], ol[j]);
             }
-            const int row = gw * 8 + i * 4 + rsub;
+            const int row = gw * DCN_ROWS + i * 4 + rsub;
             const uint32_t dst = sa + row * 128 + ((chunk ^ (row & 7)) << 4);
             asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(oh[0]), "r"(oh[1]), "r"(oh[2]), "r"(oh[3]) : "memory");
             asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst + a_bytes), "r"(ol[0]), "r"(ol[1]), "r"(ol[2]), "r"(ol[3]) : "memory");
           }
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
           __syncwarp();
-          if (lane == 0) mbar_arrive(full0 + 8 * stage);       // one arrival per gather warp (512 per-thread arrivals serialise on one word)
+          if (lane == 0) mbar_arrive(full0 + 8 * stage);       // one arrival per gather warp
           if (++stage == a.stages) { stage = 0; phase ^= 1; }
           tap_c = tap_n; c0_c = c0_n;
         }
       }
     }
-  } else {
-    // =============================== epilogue (warps 2..5 and, without the DCN gather warps, 6..9) ===============================
-    // Two groups on alternate tiles (the accumulator stages alternate with them: nacc is even).  The 1x1 convs have ONE K stage
-    // per tile, so their time is the epilogue's: one group read out a 128 x 128 split tile in ~6 us against ~1 us of loads + MMAs.
-    const int grp = (!DCN && warp >= 6) ? 1 : 0;
-    const int ngrp = DCN ? 1 : 2;
-    const int q = warp & 3;                              // TMEM lane quadrant this warp may read
-    const int row = q * 32 + lane;
-    const int et = threadIdx.x - 64 - grp * 128;         // 0..127
+  } else if (warp < CONS_THREADS / 32) {
+    // =============================== consumers: wgmma + epilogue ===============================
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const uint32_t bf = (P == 1 || a.fmt == 0) ? 1u : 0u;
+    const uint32_t row_bytes = a.BK * 2;
+    const uint64_t dT = make_desc(0u, row_bytes, a.swizzle_bits);
+    const uint32_t base14 = (smem_base & 0x3FFFFu) >> 4, sstep = stage_bytes >> 4;
+    const uint32_t aoff = (uint32_t)wg * ((64u * row_bytes) >> 4);           // this warpgroup's 64 rows of A
+    const uint32_t aplane = a_bytes >> 4, bplane = b_bytes >> 4, boff = (uint32_t)(P * a_bytes) >> 4;
+    const int ksteps = a.BK / 16;
     const uint32_t act = a.flags & CPB_ACT_MASK;
     const bool out_f32 = a.flags & CPB200_FLAG_OUT_F32;
     const bool out_nchw = a.flags & CPB200_FLAG_OUT_NCHW_F32;
-    int acc = 0; uint32_t accphase = 0;
-    int it = 0, par = 0;
-    for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x, ++it) {
-      if ((it % ngrp) != grp) {                          // the other group's tile: just keep the accumulator ring in step
-        if (++acc == a.nacc) { acc = 0; accphase ^= 1; }
-        continue;
+    float acc[BN / 2], acc2[P == 2 ? BN / 2 : 1];                 // hi x W_hi | hi x W_lo + lo x W_hi (split operands)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (P == 2 ? BN / 2 : 1); ++i) acc2[i] = 0.f;
+    int stage = 0; uint32_t phase = 0;
+    for (int tt = blockIdx.x; tt < a.total_tiles; tt += gridDim.x) {
+      int prev = -1;                                       // stage whose MMAs may still be running
+      for (int kb = 0; kb < kblocks; ++kb) {
+        mbar_wait(full0 + 8 * stage, phase);
+        const uint64_t sd = dT + (base14 + (uint32_t)stage * sstep);
+        const uint64_t ad = sd + aoff, bd = sd + boff;
+        wg_fence();
+        for (int k = 0; k < ksteps; ++k) {
+          const uint32_t first = (kb > 0 || k > 0) ? 1u : 0u;
+          if constexpr (P == 1) {
+            wgmma_k16<BN>(acc, ad + 2 * k, bd + 2 * k, first, 1u);
+          } else {
+            wgmma_k16<BN>(acc, ad + 2 * k, bd + 2 * k, first, bf);                     // A_hi x W_hi
+            wgmma_k16<BN>(acc2, ad + 2 * k, bd + bplane + 2 * k, first, bf);           // A_hi x W_lo
+            // A_lo x W_hi joins the other small term (see net_tc3.cu: the fp32 accumulator truncates per instruction in
+            // proportion to its magnitude)
+            wgmma_k16<BN>(acc2, ad + aplane + 2 * k, bd + 2 * k, 1u, bf);
+          }
+        }
+        wg_commit();
+        wg_wait<1>();                                      // the previous stage's MMAs have retired: release it
+        if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
+        prev = stage;
+        if (++stage == a.stages) { stage = 0; phase ^= 1; }
       }
-      int n, h0, w0, nt; decode_tile(t, n, h0, w0, nt);
+      wg_wait<0>();
+      acc_fence(acc); acc_fence(acc2);
+      if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
+      int n, h0, w0, nt; decode_tile(tt, n, h0, w0, nt);
       const int n0 = nt * BN;
-      float *sb = s_bias[grp][par];
-      par ^= 1;
-      for (int i = et; i < BN; i += 128) sb[i] = (a.bias && n0 + i < a.cout) ? __ldg(a.bias + n0 + i) : 0.f;
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
-      mbar_wait(tfull0 + 8 * acc, accphase);
-      tc_fence_after();
-      const int th = row / a.TW, tw = row % a.TW;
-      const int ho = h0 + th, wo = w0 + tw;
-      const bool ok = ho < a.Ho && wo < a.Wo;
-      const size_t pix = ((size_t)n * a.Hd + (ho * a.sy + a.oy)) * a.Wd + (wo * a.sx + a.ox);
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_COLS;
-      // two 16-column chunks per round: all their accumulator reads are in flight before the one wait (with a single chunk
-      // per wait the 1x1 convs — one K stage per tile — were bound by the epilogue's load -> wait -> convert -> store chain)
-      constexpr int NCH = BN / 16, CSTEP = (NCH >= 2 && !DCN) ? 2 : 1;      // the 704-thread DCN variant has 80 registers per thread
-#pragma unroll 1
-      for (int c2 = (a.dcn_prefetch & 2) ? NCH : 0; c2 < NCH; c2 += CSTEP) {
-        uint32_t va[CSTEP][16], vb[NCAT ? CSTEP : 1][16];
 #pragma unroll
-        for (int hc = 0; hc < CSTEP; ++hc) {
-          tmem_ld16(taddr + (c2 + hc) * 16, va[hc]);
-          if constexpr (NCAT) tmem_ld16(taddr + BN + (c2 + hc) * 16, vb[hc]);
+      for (int j = 0; j < BN / 4; ++j) {                   // pairs of adjacent columns of this thread's fragment
+        const int row = wg * 64 + frag_row(t, j), nb = n0 + frag_col(t, j);
+        const int ho = h0 + row / a.TW, wo = w0 + row % a.TW;
+        if (ho >= a.Ho || wo >= a.Wo || nb >= a.cout) continue;
+        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
+        if constexpr (P == 2) { v0 += acc2[2 * j]; v1 += acc2[2 * j + 1]; }
+        const bool has1 = nb + 1 < a.cout;
+        const float b0 = a.bias ? __ldg(a.bias + nb) : 0.f, b1 = (a.bias && has1) ? __ldg(a.bias + nb + 1) : 0.f;
+        const float f0 = P == 2 ? fmaf(v0, a.acc_scale, b0) : v0 + b0, f1 = P == 2 ? fmaf(v1, a.acc_scale, b1) : v1 + b1;
+        const size_t pix = ((size_t)n * a.Hd + (ho * a.sy + a.oy)) * a.Wd + (wo * a.sx + a.ox);
+        if (out_nchw) {
+          // head outputs: NCHW fp32 channel slice of dst
+          float *o = static_cast<float *>(a.dst) +
+                     (((size_t)n * a.out_ch_total + a.out_ch_off + nb) * a.Hd + (ho * a.sy + a.oy)) * a.Wd + (wo * a.sx + a.ox);
+          const size_t plane = (size_t)a.Hd * a.Wd;
+          o[0] = P == 2 ? cpb::act_fn(f0, act) : cpb::act_out<__nv_bfloat16>(f0, act);
+          if (has1) o[plane] = P == 2 ? cpb::act_fn(f1, act) : cpb::act_out<__nv_bfloat16>(f1, act);
+        } else if (out_f32) {
+          float *o = static_cast<float *>(a.dst) + pix * a.cout_store + nb;
+          o[0] = cpb::act_out<__nv_bfloat16>(f0, act);
+          if (has1) o[1] = cpb::act_out<__nv_bfloat16>(f1, act);
+        } else {
+          store_pair16<P>(a.dst, a.res, pix * a.cout_store + nb, a.dst_plane, f0, f1, act, a.fmt);
         }
-        tmem_ld_wait();
-#pragma unroll
-       for (int hc = 0; hc < CSTEP; ++hc) {
-        const int c = c2 + hc;
-        uint32_t (&v)[16] = va[hc];
-        if constexpr (NCAT) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(vb[hc][j]));
-        }
-        const int nb = n0 + c * 16;
-        if (ok && nb < a.cout) {
-          float f[16];
-          if constexpr (P == 2) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] = fmaf(__uint_as_float(v[j]), a.acc_scale, sb[c * 16 + j]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]) + sb[c * 16 + j];
-          }
-          if (out_nchw) {
-            // head outputs: lanes are consecutive pixels of a tile row -> coalesced fp32 stores per channel
-            float *o = static_cast<float *>(a.dst) +
-                       (((size_t)n * a.out_ch_total + a.out_ch_off + nb) * a.Hd + (ho * a.sy + a.oy)) * a.Wd + (wo * a.sx + a.ox);
-            const size_t plane = (size_t)a.Hd * a.Wd;
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (nb + j < a.cout) o[j * plane] = P == 2 ? cpb::act_fn(f[j], act) : cpb::act_out<__nv_bfloat16>(f[j], act);
-          } else if (out_f32) {
-            float *o = static_cast<float *>(a.dst) + pix * a.cout_store + nb;
-            if (nb + 16 <= a.cout && (a.cout_store & 3) == 0) {
-              if (act) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] = cpb::act_out<__nv_bfloat16>(f[j], act);
-              }
-              if ((a.cout_store & 7) == 0) {            // 32-byte rows: two sector-sized stores
-#pragma unroll
-                for (int j = 0; j < 16; j += 8) {
-                  const uint32_t ow[8] = {__float_as_uint(f[j]), __float_as_uint(f[j + 1]), __float_as_uint(f[j + 2]), __float_as_uint(f[j + 3]),
-                                          __float_as_uint(f[j + 4]), __float_as_uint(f[j + 5]), __float_as_uint(f[j + 6]), __float_as_uint(f[j + 7])};
-                  st_global_32B(o + j, ow);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4 *>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (nb + j < a.cout) o[j] = cpb::act_out<__nv_bfloat16>(f[j], act);
-            }
-          } else if constexpr (P == 2) {
-            // split output: hi plane at dst, lo plane dst_plane elements later; the residual is read the same way
-            uint16_t *o = static_cast<uint16_t *>(a.dst) + pix * a.cout_store + nb;
-            if (a.res) {
-              const uint16_t *rh = static_cast<const uint16_t *>(a.res) + pix * a.cout_store + nb;
-              const uint4 h0 = __ldg(reinterpret_cast<const uint4 *>(rh)), h1 = __ldg(reinterpret_cast<const uint4 *>(rh) + 1);
-              const uint4 l0 = __ldg(reinterpret_cast<const uint4 *>(rh + a.dst_plane)), l1 = __ldg(reinterpret_cast<const uint4 *>(rh + a.dst_plane) + 1);
-              const uint32_t hw_[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-              const uint32_t lw_[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float2 x = join2(hw_[j], lw_[j], a.fmt);
-                f[2 * j] += x.x; f[2 * j + 1] += x.y;
-              }
-            }
-            uint32_t oh[8], ol[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              split2(cpb::act_fast(f[2 * j], act), cpb::act_fast(f[2 * j + 1], act), a.fmt, oh[j], ol[j]);
-            st_global_32B(o, oh);                       // 32-byte stores: see net_tc3.cu's epilogue
-            st_global_32B(o + a.dst_plane, ol);
-          } else {
-            __nv_bfloat16 *o = static_cast<__nv_bfloat16 *>(a.dst) + pix * a.cout_store + nb;
-            if (a.res) {
-              const uint4 *rp = reinterpret_cast<const uint4 *>(static_cast<const __nv_bfloat16 *>(a.res) + pix * a.cout_store + nb);
-              uint4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
-              const __nv_bfloat162 *rb0 = reinterpret_cast<const __nv_bfloat162 *>(&r0);
-              const __nv_bfloat162 *rb1 = reinterpret_cast<const __nv_bfloat162 *>(&r1);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                float2 x0 = __bfloat1622float2(rb0[j]), x1 = __bfloat1622float2(rb1[j]);
-                f[2 * j] += x0.x; f[2 * j + 1] += x0.y; f[8 + 2 * j] += x1.x; f[8 + 2 * j + 1] += x1.y;
-              }
-            }
-            if (act) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = cpb::act_out<__nv_bfloat16>(f[j], act);
-            }
-            uint4 o0, o1;
-            __nv_bfloat162 *ob0 = reinterpret_cast<__nv_bfloat162 *>(&o0), *ob1 = reinterpret_cast<__nv_bfloat162 *>(&o1);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              ob0[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
-              ob1[j] = __floats2bfloat162_rn(f[8 + 2 * j], f[8 + 2 * j + 1]);
-            }
-            const uint32_t ow[8] = {o0.x, o0.y, o0.z, o0.w, o1.x, o1.y, o1.z, o1.w};
-            st_global_32B(o, ow);
-          }
-        }
-       }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-      if (++acc == a.nacc) { acc = 0; accphase ^= 1; }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
@@ -620,10 +472,10 @@ int cur_device() {
 int num_sms() {
   static std::atomic<int> n[MAX_DEVICES];          // zero-initialised; per device (a process may drive several GPUs)
   const int dev = cur_device();
-  if (dev < 0 || dev >= MAX_DEVICES) return 148;
+  if (dev < 0 || dev >= MAX_DEVICES) return 132;
   int v = n[dev].load(std::memory_order_relaxed);
   if (!v) {
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     n[dev].store(v, std::memory_order_relaxed);
   }
   return v;
@@ -680,27 +532,25 @@ int tc_prepare_op(cpb200_op &op) {
   }
   a.nsrc = op.nsrc; a.BK = bk;
   const CUtensorMapSwizzle sw = bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-  a.swizzle_bits = bk == 64 ? 2u : bk == 32 ? 4u : 6u;
+  a.swizzle_bits = bk == 64 ? 1u : bk == 32 ? 2u : 3u;
   a.kh = op.kh; a.kw = op.kw; a.stride = op.stride; a.pad_h = op.pad_h; a.pad_w = op.pad_w;
   a.B = op.B; a.Ho = op.Ho; a.Wo = op.Wo;
   a.TW = op.Wo >= 16 ? 16 : 8; a.TH = TILE_M / a.TW;
   a.tiles_h = (op.Ho + a.TH - 1) / a.TH; a.tiles_w = (op.Wo + a.TW - 1) / a.TW;
   int BN = 16;
   while (BN < op.cout && BN < 256) BN <<= 1;
-  if (P == 2 && BN > 128) BN = 128;            // split operands: two accumulator halves of BN columns each (2 * BN <= 256); also lets two
-                                               // DCN stages of [A_hi|A_lo|W_hi|W_lo] fit beside 39 KB of sampling parameters
+  if (P == 2 && BN > 128) BN = 128;            // split operands: two accumulator halves of BN columns each (2 * BN <= 256)
+  // DCN: the gather warps leave 120 registers per thread, so a consumer holds at most 64 accumulator registers
+  if (dcn && BN > 128 / P) BN = 128 / P;
   t->BN = BN; t->dcn = dcn;
   a.dcn_src = static_cast<const __nv_bfloat16 *>(op.src[0]); a.dcn_om = static_cast<const float *>(op.aux);
   a.H = op.H; a.W = op.W; a.om_pitch = op.aux_pitch > 0 ? op.aux_pitch : 27;
-  a.dcn_prefetch = 0;   // (an L1 prefetch two stages ahead was measured slower, dcn64 312 -> 355 us, and removed)
   a.Hd = op.Hd; a.Wd = op.Wd; a.sy = op.out_sy; a.sx = op.out_sx; a.oy = op.out_oy; a.ox = op.out_ox;
   a.n_tiles = (op.cout + BN - 1) / BN;
   a.cout = op.cout; a.cout_store = op.cout;
   if (!(op.flags & (CPB200_FLAG_OUT_F32 | CPB200_FLAG_OUT_NCHW_F32)) && (op.cout % 16)) { delete t; return fail(CPB200_ERR_ARG, "tc: 16-bit output needs cout %% 16 == 0"); }
   a.out_ch_off = op.out_ch_off; a.out_ch_total = op.out_ch_total;
   a.total_tiles = op.B * a.tiles_h * a.tiles_w * a.n_tiles;
-  const int acc_cols = (P == 2 && 2 * BN <= 256) ? 2 * BN : BN;
-  a.nacc = 512 / acc_cols > 8 ? 8 : 512 / acc_cols;      // TMEM accumulator stages
   a.dst = op.dst; a.res = op.res; a.bias = op.bias; a.flags = op.flags;
   a.dst_plane = (long long)op.B * op.Hd * op.Wd * op.cout;
   a.src_plane = (long long)op.B * op.H * op.W * op.cin[0];
@@ -708,10 +558,10 @@ int tc_prepare_op(cpb200_op &op) {
     return fail(CPB200_ERR_ARG, "tc: split-precision DCN input must stay below 4 GiB (32-bit gather offsets)"); }
   a.wplane = op.kh * op.kw * (cin_total / bk);
   const size_t a_bytes = (size_t)P * TILE_M * bk * 2, b_bytes = ((size_t)P * BN * bk * 2 + 1023) / 1024 * 1024;
-  const size_t budget = dcn ? 176 * 1024 : 200 * 1024;     // the DCN variant keeps 39 KB of sampling parameters in static smem
+  const size_t budget = dcn ? 176 * 1024 : 200 * 1024;     // the DCN variant keeps 37 KB of sampling parameters in static smem
   int stages = (int)(budget / (a_bytes + b_bytes));
   if (stages > 8) stages = 8;
-  if (dcn && stages > 4) stages = 4;      // leave the rest of the 228 KB to L1: the 9 taps x 4 corners re-read one ~30 KB footprint
+  if (dcn && stages > 4) stages = 4;      // leave the rest of the 256 KB to L1: the 9 taps x 4 corners re-read one ~30 KB footprint
   if (stages < 2) { delete t; return fail(CPB200_ERR_ARG, "tc: tile does not fit shared memory"); }
   a.stages = stages;
   t->smem = stages * (a_bytes + b_bytes) + 1024;
@@ -762,15 +612,14 @@ int tc_run_op(const cpb200_op &op, cudaStream_t st) {
   TcArgs args = t->args;
   args.dst = op.dst; args.res = op.res; args.bias = op.bias;
   args.dcn_om = static_cast<const float *>(op.aux);
-  if (const char *e = getenv("CPB200_TC_DBG")) args.dcn_prefetch = atoi(e);      // timing experiments (results are garbage)
 #define TC_CASE(N, D)                                                                                  \
   case N: return t->P == 2 ? launch_tc<N, D, 2>(*t, args, st) : launch_tc<N, D, 1>(*t, args, st);
   if (t->dcn) {
     switch (t->BN) {
-      TC_CASE(32, true) TC_CASE(64, true) TC_CASE(128, true)
-      case 256: if (t->P == 1) return launch_tc<256, true, 1>(*t, args, st); break;
+      TC_CASE(16, true) TC_CASE(32, true) TC_CASE(64, true)
+      case 128: if (t->P == 1) return launch_tc<128, true, 1>(*t, args, st); break;
     }
-    return fail(CPB200_ERR_STATE, "tc: DCN supports cout 32/64/128/256 tiles only");
+    return fail(CPB200_ERR_STATE, "tc: DCN supports cout tiles of 16..128 (bf16) / 16..64 (split) only");
   }
   switch (t->BN) {
     TC_CASE(16, false) TC_CASE(32, false) TC_CASE(64, false) TC_CASE(128, false)

@@ -1,36 +1,27 @@
-// tcgen05 3x3 / stride-1 / pad-1 convolution with HALO REUSE (bf16 NHWC, fp32 accumulate in TMEM).
+// wgmma 3x3 / stride-1 / pad-1 convolution with HALO REUSE (bf16 NHWC, fp32 accumulate in registers).
 //
 // The tap-per-stage kernel (net_tc.cu) fetches nine shifted 128-pixel windows per tile and channel
 // slab: 9 x 128 row requests through L2 for data that overlaps 89 %.  Here ONE (16+2) x (8+2) halo
 // box per slab is brought in by TMA (180 pixel rows) and all nine taps read it in place through
-// shifted UMMA shared-memory descriptors:
+// shifted wgmma shared-memory descriptors:
 //     tile = 16 rows x 8 columns of output pixels  ->  A row m = (th, tw) = (m / 8, m % 8);
 //     every 8-row core-matrix group of the A operand is therefore one tile row, so tap (r, s) is
 //         start address = halo + ((r * 10 + s) * pixel_bytes)      (+ 32 B per K step of 16)
 //         stride between 8-row groups (SBO) = 10 * pixel_bytes     (one halo row of pixels)
 // which is NOT a multiple of the 1024-byte swizzle repeat; it works because the hardware applies the
-// 128B/64B/32B swizzle XOR to absolute shared-memory address bits — measured with
-// cpb200_probe_halo (csrc/probe.cu, tools/halo_probe.py: exact with descriptor base_offset = 0).
-// TMA's out-of-bounds zero fill provides the conv padding for the halo border.
+// 128B/64B/32B swizzle XOR to absolute shared-memory address bits.  The second consumer warpgroup's 64 rows
+// start 8 halo rows later.  TMA's out-of-bounds zero fill provides the conv padding for the halo border.
 //
 // Weights: slab-major [tap][K-slab][Cout_pad][BK] bf16 via 3-D TMA; when the whole filter bank fits beside the halo
 // ring it is loaded ONCE per CTA and stays resident (e.g. 64->64: 72 KB), otherwise it streams
-// through its own ring.  Warps: 0 = halo producer, 1 = MMA issuer + TMEM owner, 2..5 and 7..10 = two epilogue
-// groups on alternate tiles, 6 = weight producer; persistent CTAs, up to eight TMEM accumulator stages.
-//
-// Tried and dropped (round 1, see profiles/r01_group_interleave_experiment.log): interleaving the taps of G
-// tiles in the issue loop so that consecutive tcgen05.mma instructions target different accumulators (and
-// every weight stage serves G tiles).  It beat its own G = 1 baseline (conv 128->128: 60 -> 46 us) but the
-// extra bookkeeping in the single issuing lane made that baseline slower than this straight-line version
-// (64->64: 59 us here, 67 us grouped), i.e. the issuer is bound by instructions issued, not by the
-// accumulator dependency chain.
+// through its own ring.  Warps: 0-7 = two consumer warpgroups (wgmma + epilogue), 8 = halo producer, 9 = weight
+// producer; persistent CTAs.
 //
 // Split-operand precisions (P = 2, act_dtype CPB200_BF16X2 / CPB200_F16X2; tc_common.cuh): activations and weights arrive
 // as hi / lo 16-bit planes.  The halo ring is plane-granular (the planes of a slab are two consecutive stages, TMA batch
-// coordinate n and n + B); a weight stage holds the hi tile immediately followed by the lo tile, so for 2*BN <= 256 the
-// products A_hi*[W_hi ; W_lo] are ONE tcgen05.mma of N = 2*BN into two adjacent accumulator halves (the issuing thread
-// is the bottleneck for N <= 128, ~90 cycles per instruction whatever N) and A_lo*W_hi a second one into the first
-// half; the epilogue adds the halves, scales by acc_scale, and writes hi / lo planes.  BN = 256: three N = 256 MMAs.
+// coordinate n and n + B); a weight stage holds the hi tile immediately followed by the lo tile.  A_hi*W_hi goes to one
+// accumulator array, A_hi*W_lo and A_lo*W_hi to a second one; the epilogue adds them, scales by acc_scale, and writes
+// hi / lo planes.
 #include <type_traits>
 #include "tc_common.cuh"
 #include <cstdlib>
@@ -39,16 +30,17 @@ using namespace tc;
 
 namespace {
 
-constexpr int C3_THREADS = 352;     // warps: 0 halo producer, 1 MMA, 2-5 epilogue group 0, 6 weight producer, 7-10 epilogue group 1
-constexpr int TW = 8, TH = 16, HW_ = TW + 2, HH_ = TH + 2;
+constexpr int C3_CONS = 256;                  // two consumer warpgroups
+constexpr int C3_THREADS = C3_CONS + 64;      // + halo producer warp + weight producer warp
+constexpr int TW = 8, TH = 16;
 constexpr int MAX_NA = 16, MAX_NB = 8;
 
 struct alignas(64) C3Args {
-  CUtensorMap amap, bmap, dmap;    // dmap: the OUTPUT tensor (TMA-store epilogue), box {32 channels, TW, TH, 1}, 64-byte swizzle
+  CUtensorMap amap, bmap;
   int cin, slabs, BK;
   int B, Ho, Wo, tiles_h, tiles_w, n_tiles, total_tiles;
   int cout, cout_store;
-  int na, nb, b_resident, nacc;
+  int na, nb, b_resident;
   int kh, kw, taps, hw;        // filter size, kh*kw, halo width in pixels (TW + kw - 1)
   unsigned a_stage_bytes, b_stage_bytes, a_tx_bytes, b_tx_bytes;
   void *dst;
@@ -59,134 +51,59 @@ struct alignas(64) C3Args {
   unsigned fmt;                // 0 = bf16 planes, 1 = fp16 planes
   float acc_scale;             // accumulator multiplier (inverse of the host's power-of-two weight scale)
   long long dst_plane;         // elements between the hi and lo planes of dst / res
-  unsigned dbg;                // timing experiments only (CPB200_C3_DBG): see profiles/r02_head3x3_whatif.md
   unsigned b_tile_bytes;       // bytes of one weight tile (BN x BK x 2); a P = 2 weight stage is [hi tile | lo tile]
-  // CTA pairs (mcast = 1 -> conv3x3_tc_kernel<BN, P, 2>): the two CTAs of a cluster walk the same (pixel-tile pair, N tile)
-  // sequence; every weight operand is split between them (bmap box = BN/2 rows)
-  int mcast, n_pix_tiles;
-  // TMA-store epilogue: byte offset of the staging area (2 epilogue groups x P planes x 128 rows x 64 B) behind the rings
-  int tstore; unsigned stg_off;
 };
 
-__device__ __forceinline__ uint64_t desc_sbo(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
-  return d;
-}
-
-// CG = 2: CTA PAIRS (cluster of two, cta_group::2).  One tcgen05.mma then covers 256 output pixels — the two pixel tiles of
-// the pair, each CTA's own halo as its half of A — against weights of which each CTA holds only HALF the rows (its half of
-// B), and is issued by the leader CTA alone.  Per SM that halves the instructions the single issuing thread has to emit
-// (~90 cycles each, the bound for N <= 128) and the shared-memory bytes the tensor core reads and TMA writes for B
-// (ncu on the 64->256 head conv, profiles/r02_ncu_head3x3_fp16x2_cg1.txt: tensor pipe 54 % busy with nothing else
-// saturated and the weight stages full: issue / smem-read bound).  Used for the streamed-weight convs with enough tiles.
-template <int BN, int P, int CG>
+template <int BN, int P>
 __global__ void __launch_bounds__(C3_THREADS, 1) conv3x3_tc_kernel(const __grid_constant__ C3Args a) {
-  constexpr bool NCAT = (P == 2) && (2 * BN <= 256);       // hi*[hi;lo] as one N = 2*BN instruction
-  static_assert(CG == 1 || P == 1 || NCAT, "CTA pairs with split operands use the N-concatenated form");
-  constexpr int ACC_COLS = NCAT ? 2 * BN : BN;             // TMEM columns per accumulator stage
+  static_assert(P == 1 || BN <= 128, "split operands: two BN-column accumulators per thread");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base, b_base = smem_base + a.na * a.a_stage_bytes;
-  __shared__ __align__(8) uint64_t bars[2 * MAX_NA + 2 * MAX_NB + 1 + 16];
-  __shared__ uint32_t s_tmem;
-  __shared__ float s_bias[2][2][BN];      // [epilogue group][tile parity within the group]
+  __shared__ __align__(8) uint64_t bars[2 * MAX_NA + 2 * MAX_NB + 1];
   const uint32_t afull0 = smem_u32(&bars[0]), aempty0 = smem_u32(&bars[MAX_NA]);
   const uint32_t bfull0 = smem_u32(&bars[2 * MAX_NA]), bempty0 = smem_u32(&bars[2 * MAX_NA + MAX_NB]);
   const uint32_t ball = smem_u32(&bars[2 * MAX_NA + 2 * MAX_NB]);
-  const uint32_t tfull0 = ball + 8, tempty0 = ball + 8 + 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr bool mc = CG == 2;
-  // Two accumulator stages only (ACC_COLS = 256): tile t+2 reuses the stage tile t is being read out of, so ONE read-out must
-  // fit into ONE tile's MMA time whatever the number of epilogue groups — alternating tiles between the groups does not help.
-  // Both groups then share every tile, each reading half of its column chunks.  History: with 16-byte direct stores this
-  // measured slower for split operands (424 -> 456 us on the 64->256 head conv: eight warps' stores at once on the L1 path);
-  // with the TMA-store epilogue it is the faster form for both (fp16x2 385 -> 345 us, bf16 137 -> 122 us).
-  const bool esplit = a.nacc == 2 && BN >= 32;
-  const uint32_t crank = mc ? cluster_ctarank() : 0u;
-  const bool leader = crank == 0;
-  const uint32_t need_cols = (uint32_t)a.nacc * ACC_COLS;
-  const uint32_t TMEM_COLS = need_cols <= 32 ? 32u : need_cols <= 64 ? 64u : need_cols <= 128 ? 128u : need_cols <= 256 ? 256u : 512u;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == C3_CONS) {
     tmap_prefetch(&a.amap); tmap_prefetch(&a.bmap);
-    if (a.tstore) tmap_prefetch(&a.dmap);
-    for (int s = 0; s < MAX_NA; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, 1); }
-    for (int s = 0; s < MAX_NB; ++s) { mbar_init(bfull0 + 8 * s, 1); mbar_init(bempty0 + 8 * s, 1); }
+    for (int s = 0; s < MAX_NA; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, C3_CONS / 32); }
+    for (int s = 0; s < MAX_NB; ++s) { mbar_init(bfull0 + 8 * s, 1); mbar_init(bempty0 + 8 * s, C3_CONS / 32); }
     mbar_init(ball, 1);
-    // accumulator-empty barriers: 4 epilogue warps per tile, 8 when both groups share every tile (esplit); CTA pairs: the
-    // leader's barriers collect the epilogue warps of BOTH CTAs
-    for (int s = 0; s < 8; ++s) { mbar_init(tfull0 + 8 * s, 1); mbar_init(tempty0 + 8 * s, (mc ? 2 : 1) * (esplit ? 8 : 4)); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    if constexpr (mc) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (mc) cluster_sync_all();       // the peer's barriers and tensor memory exist before anything is signalled across
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
   const uint32_t pix_bytes = a.BK * 2;
 
-  // it-th tile of this CTA.  Plain: tiles blockIdx.x + it * gridDim.x of (pixel tile, N tile) pairs, N fastest.  CTA pairs: the two
-  // CTAs of a cluster take the two pixel tiles of pair pp = u / n_tiles with the SAME N tile nt = u % n_tiles, u = cluster + it *
-  // clusters; an odd tail pair re-computes the last pixel tile on rank 1 without storing it (valid = false)
-  auto tile_at = [&](int it, int &n, int &h0, int &w0, int &nt, bool &valid) -> bool {
-    int pt;
-    if (!mc) {
-      int t = blockIdx.x + it * gridDim.x;
-      if (t >= a.total_tiles) return false;
-      nt = t % a.n_tiles; pt = t / a.n_tiles; valid = true;
-    } else {
-      const int u = (int)(blockIdx.x >> 1) + it * (int)(gridDim.x >> 1);
-      if (u >= ((a.n_pix_tiles + 1) >> 1) * a.n_tiles) return false;
-      nt = u % a.n_tiles; pt = 2 * (u / a.n_tiles) + (int)crank;
-      valid = pt < a.n_pix_tiles;
-      if (!valid) pt = a.n_pix_tiles - 1;
-    }
+  auto tile_at = [&](int it, int &n, int &h0, int &w0, int &nt) -> bool {
+    int t = blockIdx.x + it * gridDim.x;
+    if (t >= a.total_tiles) return false;
+    nt = t % a.n_tiles; int pt = t / a.n_tiles;
     const int tw = pt % a.tiles_w; pt /= a.tiles_w;
     const int th = pt % a.tiles_h; n = pt / a.tiles_h;
     h0 = th * TH; w0 = tw * TW;
     return true;
   };
 
-  if (warp == 0) {
+  if (warp == C3_CONS / 32) {
     // =============================== halo producer ===============================
-    if (elect_one() && !(a.dbg & 16u)) {
+    if (elect_one()) {
       int sa = 0; uint32_t pha = 0;
-      int n, h0, w0, nt; bool valid;
-      for (int it = 0; tile_at(it, n, h0, w0, nt, valid); ++it) {
+      int n, h0, w0, nt;
+      for (int it = 0; tile_at(it, n, h0, w0, nt); ++it) {
         for (int sl = 0; sl < a.slabs; ++sl) {
 #pragma unroll
           for (int pl = 0; pl < P; ++pl) {                 // plane-granular stages: hi then lo (batch coordinate n + B)
             mbar_wait(aempty0 + 8 * sa, pha ^ 1);
-            if constexpr (mc) {
-              // both halos of the pair complete on the LEADER's barrier (its MMA thread is the only consumer)
-              if (leader) mbar_expect_tx(afull0 + 8 * sa, 2 * a.a_tx_bytes);
-              tma_load_4d_cg2(a_base + sa * a.a_stage_bytes, &a.amap, afull0 + 8 * sa, sl * a.BK, w0 - (a.kw >> 1), h0 - (a.kh >> 1), n + pl * a.B);
-            } else if (a.dbg & 1u) {
-              mbar_arrive(afull0 + 8 * sa);
-            } else {
-              mbar_expect_tx(afull0 + 8 * sa, a.a_tx_bytes);
-              tma_load_4d(a_base + sa * a.a_stage_bytes, &a.amap, afull0 + 8 * sa, sl * a.BK, w0 - (a.kw >> 1), h0 - (a.kh >> 1), n + pl * a.B);
-            }
+            mbar_expect_tx(afull0 + 8 * sa, a.a_tx_bytes);
+            tma_load_4d(a_base + sa * a.a_stage_bytes, &a.amap, afull0 + 8 * sa, sl * a.BK, w0 - (a.kw >> 1), h0 - (a.kh >> 1), n + pl * a.B);
             if (++sa == a.na) { sa = 0; pha ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 6) {
+  } else if (warp == C3_CONS / 32 + 1) {
     // =============================== weight producer ===============================
     if (elect_one()) {
       const int wplane = a.taps * a.slabs;                 // weight blocks per plane
@@ -198,502 +115,125 @@ __global__ void __launch_bounds__(C3_THREADS, 1) conv3x3_tc_kernel(const __grid_
             for (int pl = 0; pl < P; ++pl)
               tma_load_3d(b_base + (sl * a.taps + tap) * a.b_stage_bytes + pl * a.b_tile_bytes, &a.bmap, ball, 0, 0,
                           pl * wplane + tap * a.slabs + sl);
-      } else if (!(a.dbg & 16u)) {
+      } else {
         int sb = 0; uint32_t phb = 0;
-        int n, h0, w0, nt; bool valid;
-        for (int it = 0; tile_at(it, n, h0, w0, nt, valid); ++it) {
+        int n, h0, w0, nt;
+        for (int it = 0; tile_at(it, n, h0, w0, nt); ++it) {
           for (int sl = 0; sl < a.slabs; ++sl)
             for (int tap = 0; tap < a.taps; ++tap) {
               mbar_wait(bempty0 + 8 * sb, phb ^ 1);
-              if constexpr (mc) {
-                // Each CTA holds HALF of every B operand (bmap box = BN/2 rows), all loads complete on the leader's barrier:
-                //   P = 1: rows [rank*BN/2, +BN/2) of the weight tile;
-                //   P = 2: region Y (BN rows) = the hi plane's tile on rank 0, the lo plane's on rank 1 -> the two halves of the
-                //          2*BN-row operand [W_hi ; W_lo] of A_hi x [W_hi ; W_lo];  region X (BN/2 rows) = rows [rank*BN/2, +BN/2)
-                //          of the hi plane -> this CTA's half of W_hi for A_lo x W_hi.
-                const uint32_t half = a.b_tile_bytes >> 1;
-                const uint32_t sbase = b_base + sb * a.b_stage_bytes;
-                const int blk = tap * a.slabs + sl;
-                if constexpr (P == 1) {
-                  if (leader) mbar_expect_tx(bfull0 + 8 * sb, a.b_tile_bytes);
-                  tma_load_3d_cg2(sbase, &a.bmap, bfull0 + 8 * sb, 0, nt * BN + (int)crank * (BN / 2), blk);
-                } else {
-                  if (leader) mbar_expect_tx(bfull0 + 8 * sb, 3 * a.b_tile_bytes);
-                  const int plane_blk = (int)crank * wplane + blk;
-                  tma_load_3d_cg2(sbase, &a.bmap, bfull0 + 8 * sb, 0, nt * BN, plane_blk);
-                  tma_load_3d_cg2(sbase + half, &a.bmap, bfull0 + 8 * sb, 0, nt * BN + BN / 2, plane_blk);
-                  tma_load_3d_cg2(sbase + 2 * half, &a.bmap, bfull0 + 8 * sb, 0, nt * BN + (int)crank * (BN / 2), blk);
-                }
-              } else if (a.dbg & 1u) {
-                mbar_arrive(bfull0 + 8 * sb);
-              } else {
-                mbar_expect_tx(bfull0 + 8 * sb, P * a.b_tile_bytes);
+              mbar_expect_tx(bfull0 + 8 * sb, P * a.b_tile_bytes);
 #pragma unroll
-                for (int pl = 0; pl < P; ++pl)
-                  tma_load_3d(b_base + sb * a.b_stage_bytes + pl * a.b_tile_bytes, &a.bmap, bfull0 + 8 * sb, 0, nt * BN,
-                              pl * wplane + tap * a.slabs + sl);
-              }
+              for (int pl = 0; pl < P; ++pl)
+                tma_load_3d(b_base + sb * a.b_stage_bytes + pl * a.b_tile_bytes, &a.bmap, bfull0 + 8 * sb, 0, nt * BN,
+                            pl * wplane + tap * a.slabs + sl);
               if (++sb == a.nb) { sb = 0; phb ^= 1; }
             }
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    // P = 1: idesc = bf16 x bf16, N = BN.  P = 2: idescN (N = BN) and idesc2 (N = 2*BN, NCAT only), format from a.fmt.
-    const uint32_t idesc = P == 1 ? ((1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24))
-                                  : idesc_m128(BN, a.fmt);
-    const uint32_t idesc2 = idesc_m128(NCAT ? 2 * BN : BN, a.fmt);
-    int sa = 0; uint32_t pha = 0; int sb = 0; uint32_t phb = 0; int acc = 0; uint32_t accphase = 0;
-    if (a.b_resident) { mbar_wait(ball, 0); tc_fence_after(); }
+  } else if (warp < C3_CONS / 32) {
+    // =============================== consumers: wgmma + epilogue ===============================
+    // Per slab the halo plane(s) are waited for once, then every tap issues its products.  Streamed weights: one weight stage
+    // per (slab, tap), released once the MMAs of the next one are queued; resident weights: nothing to wait for but the halo.
+    // The halo stages of a slab are released after its last tap.  The small cross term A_lo x W_hi joins A_hi x W_lo in the
+    // SECOND accumulator: the tensor core's fp32 accumulator truncates (round toward zero) at every instruction, an error
+    // proportional to the accumulator's magnitude — the large hi x hi sum must see as few additions as possible.
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const uint32_t bf = (P == 1 || a.fmt == 0) ? 1u : 0u;
     const int ksteps = a.BK / 16;
-    const uint32_t bstep = a.b_stage_bytes >> 4, pstep = pix_bytes >> 4, btile = a.b_tile_bytes >> 4;
-    int n_, h0_, w0_, nt_; bool valid_;
-    if constexpr (mc) {
-      // ---- CTA pair: the leader issues 256-row MMAs for both CTAs (streamed weights only) ----
-      if (leader) {
-        const uint32_t abf = (P == 1 || a.fmt == 0) ? 1u : 0u;
-        const uint32_t idN = idesc_mn(256, BN, abf), id2N = idesc_mn(256, NCAT ? 2 * BN : BN, abf);
-        for (int it = 0; tile_at(it, n_, h0_, w0_, nt_, valid_); ++it) {
-          mbar_wait(tempty0 + 8 * acc, accphase ^ 1);          // the epilogue warps of BOTH CTAs have drained this accumulator
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-          for (int sl = 0; sl < a.slabs; ++sl) {
-            const int sa_h = sa; const uint32_t pha_h = pha;
-            if (++sa == a.na) { sa = 0; pha ^= 1; }
-            int sa_l = sa_h; uint32_t pha_l = pha_h;
-            if constexpr (P == 2) {
-              sa_l = sa; pha_l = pha;
-              if (++sa == a.na) { sa = 0; pha ^= 1; }
-            }
-            mbar_wait(afull0 + 8 * sa_h, pha_h);               // both CTAs' halos of this slab (and plane) have landed
-            if constexpr (P == 2) mbar_wait(afull0 + 8 * sa_l, pha_l);
-            tc_fence_after();
-            const uint32_t halo_h = a_base + sa_h * a.a_stage_bytes, halo_l = a_base + sa_l * a.a_stage_bytes;
-            for (int tap = 0; tap < a.taps; ++tap) {
-              mbar_wait(bfull0 + 8 * sb, phb);
-              tc_fence_after();
-              if (elect_one()) {
-                const int r = tap / a.kw, s = tap - a.kw * r;
-                const uint32_t toff = (r * a.hw + s) * pix_bytes;
-                const uint64_t adh = desc_sbo(halo_h + toff, a.hw * pix_bytes, a.swizzle_bits);
-                const uint64_t adl = desc_sbo(halo_l + toff, a.hw * pix_bytes, a.swizzle_bits);
-                const uint64_t bdy = desc_sbo(b_base + sb * a.b_stage_bytes, 8 * pix_bytes, a.swizzle_bits);
-                for (int k = 0; k < ksteps; ++k) {
-                  const uint32_t first = (sl > 0 || tap > 0 || k > 0) ? 1u : 0u;
-                  if constexpr (P == 1) {
-                    umma_f16_cg2(d_tmem, adh + 2 * k, bdy + 2 * k, idN, first);
-                  } else {
-                    umma_f16_cg2(d_tmem, adh + 2 * k, bdy + 2 * k, id2N, first);                 // A_hi x [W_hi ; W_lo]
-                    umma_f16_cg2(d_tmem + BN, adl + 2 * k, bdy + btile + 2 * k, idN, 1u);       // A_lo x W_hi -> small-term half
-                  }
-                }
-                umma_commit_cg2(bempty0 + 8 * sb, (uint16_t)3);
-              }
-              __syncwarp();
-              if (++sb == a.nb) { sb = 0; phb ^= 1; }
-            }
-            if (elect_one()) {
-              umma_commit_cg2(aempty0 + 8 * sa_h, (uint16_t)3);
-              if constexpr (P == 2) umma_commit_cg2(aempty0 + 8 * sa_l, (uint16_t)3);
-              if (sl == a.slabs - 1) umma_commit_cg2(tfull0 + 8 * acc, (uint16_t)3);
-            }
-            __syncwarp();
-          }
-          if (++acc == a.nacc) { acc = 0; accphase ^= 1; }
-        }
-      }
-    } else if (!a.b_resident) {
-      // ---- streamed weights: ONE elected thread runs the whole issue loop, written the way tools/mma_probe.py's `pipe2`
-      // mode shows to run at the back-to-back MMA rate (profiles/r02_mma_probe_pipe*.log: 422 ns per 4-K-step split stage
-      // against 530-630 ns for a loop with a run-time K trip count and the barrier wait directly in front of the MMAs):
-      // K steps unrolled at compile time, descriptors = templates + a 14-bit start address, the accumulate flag a register
-      // (no per-instruction compare chain), and the NEXT stage's full barrier polled once before this stage's MMAs so that
-      // its round trip overlaps queued tensor work.
-      if (elect_one()) {
-        const uint64_t dA = desc_sbo(0u, a.hw * pix_bytes, a.swizzle_bits), dB = desc_sbo(0u, 8 * pix_bytes, a.swizzle_bits);
-        const uint32_t a_lo14 = (a_base & 0x3FFFFu) >> 4, b_lo14 = (b_base & 0x3FFFFu) >> 4;
-        const uint32_t astep = a.a_stage_bytes >> 4, rowstep = (uint32_t)a.hw * pstep;
-        auto run = [&](auto KS_) {
-          constexpr int KS = decltype(KS_)::value;
-          const bool dbg_noacc = a.dbg & 4u, dbg_nofull = a.dbg & 16u;
-          uint32_t peek = mbar_try_once(bfull0 + 8 * sb, phb);
-          for (int it = 0; tile_at(it, n_, h0_, w0_, nt_, valid_); ++it) {
-            if (!dbg_noacc) mbar_wait(tempty0 + 8 * acc, accphase ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-            uint32_t accf = 0u;                                  // 0 for the tile's very first MMA, 1 afterwards
-            for (int sl = 0; sl < a.slabs; ++sl) {
-              const int sa_h = sa; const uint32_t pha_h = pha;
-              if (++sa == a.na) { sa = 0; pha ^= 1; }
-              int sa_l = sa_h; uint32_t pha_l = pha_h;
-              if constexpr (P == 2) {
-                sa_l = sa; pha_l = pha;
-                if (++sa == a.na) { sa = 0; pha ^= 1; }
-              }
-              if (!dbg_nofull) {
-                mbar_wait(afull0 + 8 * sa_h, pha_h);
-                if constexpr (P == 2) mbar_wait(afull0 + 8 * sa_l, pha_l);
-              }
-              const uint64_t ah0 = dA + (a_lo14 + (uint32_t)sa_h * astep), al0 = dA + (a_lo14 + (uint32_t)sa_l * astep);
-              uint32_t roff = 0u;
-              for (int r = 0; r < a.kh; ++r, roff += rowstep) {
-                uint32_t toff = roff;
-                for (int q2 = 0; q2 < a.kw; ++q2, toff += pstep) {
-                  if (!peek && !dbg_nofull) mbar_wait(bfull0 + 8 * sb, phb);
-                  tc_fence_after();
-                  const uint64_t bd = dB + (b_lo14 + (uint32_t)sb * bstep);
-                  const uint64_t adh = ah0 + toff, adl = al0 + toff;
-                  const uint32_t bempty = bempty0 + 8 * sb;
-                  if (++sb == a.nb) { sb = 0; phb ^= 1; }
-                  peek = mbar_try_once(bfull0 + 8 * sb, phb);        // next stage (possibly of the next tile): poll early
-#pragma unroll
-                  for (int k = 0; k < KS; ++k) {
-                    const uint32_t first = k == 0 ? accf : 1u;
-                    if constexpr (P == 1) {
-                      umma_bf16(d_tmem, adh + 2 * k, bd + 2 * k, idesc, first);
-                    } else {
-                      if constexpr (NCAT) {
-                        umma_bf16(d_tmem, adh + 2 * k, bd + 2 * k, idesc2, first);
-                      } else {
-                        umma_bf16(d_tmem, adh + 2 * k, bd + 2 * k, idesc, first);
-                        umma_bf16(d_tmem, adh + 2 * k, bd + btile + 2 * k, idesc, 1u);
-                      }
-                      umma_bf16(d_tmem + (NCAT ? BN : 0), adl + 2 * k, bd + 2 * k, idesc, 1u);   // small terms share the second half
-                    }
-                  }
-                  accf = 1u;
-                  umma_commit(bempty);
-                }
-              }
-              umma_commit(aempty0 + 8 * sa_h);
-              if constexpr (P == 2) umma_commit(aempty0 + 8 * sa_l);
-              if (sl == a.slabs - 1 && !dbg_noacc) umma_commit(tfull0 + 8 * acc);
-            }
-            if (++acc == a.nacc) { acc = 0; accphase ^= 1; }
-          }
-          if (dbg_noacc) { umma_commit(tfull0); mbar_wait(tfull0, 0); }
-        };
-        if (ksteps == 4) run(std::integral_constant<int, 4>{});
-        else if (ksteps == 2) run(std::integral_constant<int, 2>{});
-        else run(std::integral_constant<int, 1>{});
-      }
-      __syncwarp();
-    } else {
-      // ---- resident weights (the whole filter bank sits in shared memory): same loop style, nothing to wait for inside a
-      // slab but the halo itself; split operands run a hi-plane stage (A_hi x [W_hi ; W_lo]) and then a lo-plane stage
-      // (A_lo x W_hi).  The small cross term joins A_hi x W_lo in the SECOND accumulator half: the tensor core's fp32
-      // accumulator truncates (round toward zero) at every instruction, an error proportional to the accumulator's
-      // magnitude — the large hi x hi sum must see as few additions as possible.
-      if (elect_one()) {
-        const uint64_t dA = desc_sbo(0u, a.hw * pix_bytes, a.swizzle_bits), dB = desc_sbo(0u, 8 * pix_bytes, a.swizzle_bits);
-        const uint32_t a_lo14 = (a_base & 0x3FFFFu) >> 4, b_lo14 = (b_base & 0x3FFFFu) >> 4;
-        const uint32_t astep = a.a_stage_bytes >> 4, rowstep = (uint32_t)a.hw * pstep;
-        auto run = [&](auto KS_) {
-          constexpr int KS = decltype(KS_)::value;
-          uint32_t peek = mbar_try_once(afull0 + 8 * sa, pha);
-          for (int it = 0; tile_at(it, n_, h0_, w0_, nt_, valid_); ++it) {
-            mbar_wait(tempty0 + 8 * acc, accphase ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-            uint32_t accf = 0u;                                  // 0 for the tile's very first MMA, 1 afterwards
-            for (int sl = 0; sl < a.slabs; ++sl) {
-              const uint64_t bd0 = dB + (b_lo14 + (uint32_t)(sl * a.taps) * bstep);
-#pragma unroll
-              for (int pl = 0; pl < P; ++pl) {
-                if (!peek) mbar_wait(afull0 + 8 * sa, pha);
-                tc_fence_after();
-                const uint64_t ad0 = dA + (a_lo14 + (uint32_t)sa * astep);
-                const uint32_t aempty = aempty0 + 8 * sa;
-                if (++sa == a.na) { sa = 0; pha ^= 1; }
-                peek = mbar_try_once(afull0 + 8 * sa, pha);          // next halo stage: poll early
-                uint64_t bd = bd0;
-                uint32_t roff = 0u;
-                for (int r = 0; r < a.kh; ++r, roff += rowstep) {
-                  uint64_t ad = ad0 + roff;
-                  for (int q2 = 0; q2 < a.kw; ++q2, ad += pstep, bd += bstep) {
-#pragma unroll
-                    for (int k = 0; k < KS; ++k) {
-                      const uint32_t first = k == 0 ? accf : 1u;
-                      if constexpr (P == 1) {
-                        umma_bf16(d_tmem, ad + 2 * k, bd + 2 * k, idesc, first);
-                      } else if (pl == 0) {
-                        if constexpr (NCAT) {
-                          umma_bf16(d_tmem, ad + 2 * k, bd + 2 * k, idesc2, first);
-                        } else {
-                          umma_bf16(d_tmem, ad + 2 * k, bd + 2 * k, idesc, first);
-                          umma_bf16(d_tmem, ad + 2 * k, bd + btile + 2 * k, idesc, 1u);
-                        }
-                      } else {
-                        umma_bf16(d_tmem + (NCAT ? BN : 0), ad + 2 * k, bd + 2 * k, idesc, 1u);
-                      }
-                    }
-                    if (pl == 0) accf = 1u;
-                  }
-                }
-                umma_commit(aempty);
-                if (pl == P - 1 && sl == a.slabs - 1) umma_commit(tfull0 + 8 * acc);
-              }
-            }
-            if (++acc == a.nacc) { acc = 0; accphase ^= 1; }
-          }
-        };
-        if (ksteps == 4) run(std::integral_constant<int, 4>{});
-        else if (ksteps == 2) run(std::integral_constant<int, 2>{});
-        else run(std::integral_constant<int, 1>{});
-      }
-      __syncwarp();
-    }
-  } else {
-    // =============================== epilogue (two groups of four warps) ===============================
-    // >= 4 accumulator stages: the groups take alternate tiles (a read-out may then last two tiles' MMA time).
-    // 2 accumulator stages (esplit): both groups read out every tile, half of the column chunks each.
-    const int grp = warp >= 7 ? 1 : 0;
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int et = grp ? (int)threadIdx.x - 224 : (int)threadIdx.x - 64;
+    const uint64_t dA = desc_sbo(0u, a.hw * pix_bytes, a.swizzle_bits), dB = desc_sbo(0u, 8 * pix_bytes, a.swizzle_bits);
+    const uint32_t pstep = pix_bytes >> 4;
+    const uint32_t a_lo14 = ((a_base & 0x3FFFFu) >> 4) + (uint32_t)wg * 8u * (uint32_t)a.hw * pstep;   // 8 halo rows per warpgroup
+    const uint32_t b_lo14 = (b_base & 0x3FFFFu) >> 4;
+    const uint32_t astep = a.a_stage_bytes >> 4, bstep = a.b_stage_bytes >> 4, rowstep = (uint32_t)a.hw * pstep;
+    const uint32_t btile = a.b_tile_bytes >> 4;                                  // W_lo follows W_hi in a weight stage
     const uint32_t act = a.flags & CPB_ACT_MASK;
     const bool out_f32 = a.flags & CPB200_FLAG_OUT_F32;
-    int acc = esplit ? 0 : grp; uint32_t accphase = 0;
-    int par = 0;                                            // tile parity within this group (bias double buffer)
-    bool bias_loaded = false;
-    int n, h0, w0, nt; bool valid;
-    const int c_first = esplit ? grp * (BN / 32) : 0, c_last = esplit ? c_first + BN / 32 : BN / 16;
-    const int tstep = esplit ? 1 : 2;
-    for (int it = esplit ? 0 : grp; !(a.dbg & 4u) && tile_at(it, n, h0, w0, nt, valid); it += tstep) {
+    float acc[BN / 2], acc2[P == 2 ? BN / 2 : 1];                 // hi x W_hi | hi x W_lo + lo x W_hi (split operands)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (P == 2 ? BN / 2 : 1); ++i) acc2[i] = 0.f;
+    int sa = 0; uint32_t pha = 0; int sb = 0; uint32_t phb = 0;
+    if (a.b_resident) mbar_wait(ball, 0);
+    int n, h0, w0, nt;
+    for (int it = 0; tile_at(it, n, h0, w0, nt); ++it) {
+      uint32_t accf = 0u;                                  // 0 for the tile's very first MMA, 1 afterwards
+      int prev_b = -1;                                     // streamed weight stage whose MMAs may still be running
+      for (int sl = 0; sl < a.slabs; ++sl) {
+        const int sa_h = sa; const uint32_t pha_h = pha;
+        if (++sa == a.na) { sa = 0; pha ^= 1; }
+        int sa_l = sa_h; uint32_t pha_l = pha_h;
+        if constexpr (P == 2) {
+          sa_l = sa; pha_l = pha;
+          if (++sa == a.na) { sa = 0; pha ^= 1; }
+        }
+        mbar_wait(afull0 + 8 * sa_h, pha_h);
+        if constexpr (P == 2) mbar_wait(afull0 + 8 * sa_l, pha_l);
+        const uint64_t ah0 = dA + (a_lo14 + (uint32_t)sa_h * astep), al0 = dA + (a_lo14 + (uint32_t)sa_l * astep);
+        for (int tap = 0; tap < a.taps; ++tap) {
+          const int r = tap / a.kw, q2 = tap - r * a.kw;
+          const uint32_t toff = (uint32_t)r * rowstep + (uint32_t)q2 * pstep;
+          uint64_t bd;
+          if (a.b_resident) {
+            bd = dB + (b_lo14 + (uint32_t)(sl * a.taps + tap) * bstep);
+          } else {
+            mbar_wait(bfull0 + 8 * sb, phb);
+            bd = dB + (b_lo14 + (uint32_t)sb * bstep);
+          }
+          const uint64_t adh = ah0 + toff, adl = al0 + toff;
+          wg_fence();
+          for (int k = 0; k < ksteps; ++k) {
+            const uint32_t first = k == 0 ? accf : 1u;
+            if constexpr (P == 1) {
+              wgmma_k16<BN>(acc, adh + 2 * k, bd + 2 * k, first, 1u);
+            } else {
+              wgmma_k16<BN>(acc, adh + 2 * k, bd + 2 * k, first, bf);
+              wgmma_k16<BN>(acc2, adh + 2 * k, bd + btile + 2 * k, first, bf);
+              wgmma_k16<BN>(acc2, adl + 2 * k, bd + 2 * k, 1u, bf);           // small terms share one accumulator
+            }
+          }
+          accf = 1u;
+          wg_commit();
+          wg_wait<1>();
+          if (!a.b_resident) {
+            if (prev_b >= 0 && lane == 0) mbar_arrive(bempty0 + 8 * prev_b);
+            prev_b = sb;
+            if (++sb == a.nb) { sb = 0; phb ^= 1; }
+          }
+        }
+        wg_wait<0>();
+        if (lane == 0) {
+          if (prev_b >= 0) mbar_arrive(bempty0 + 8 * prev_b);
+          mbar_arrive(aempty0 + 8 * sa_h);
+          if constexpr (P == 2) mbar_arrive(aempty0 + 8 * sa_l);
+        }
+        prev_b = -1;
+      }
+      acc_fence(acc); acc_fence(acc2);
+      // ---- epilogue: straight from the accumulator registers ----
       const int n0 = nt * BN;
-      float *sbias = s_bias[grp][par];
-      if (a.n_tiles > 1 || !bias_loaded) {      // one N tile: the bias never changes — load it once
-        for (int i = et; i < BN; i += 128) {
-          const float bv = (a.bias && n0 + i < a.cout) ? __ldg(a.bias + n0 + i) : 0.f;
-          sbias[i] = bv;
-          if (a.n_tiles == 1) s_bias[grp][par ^ 1][i] = bv;
+#pragma unroll
+      for (int j = 0; j < BN / 4; ++j) {
+        const int row = wg * 64 + frag_row(t, j), nb = n0 + frag_col(t, j);
+        const int ho = h0 + (row >> 3), wo = w0 + (row & 7);
+        if (ho >= a.Ho || wo >= a.Wo || nb >= a.cout) continue;
+        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
+        if constexpr (P == 2) { v0 += acc2[2 * j]; v1 += acc2[2 * j + 1]; }
+        const bool has1 = nb + 1 < a.cout;
+        const float b0 = a.bias ? __ldg(a.bias + nb) : 0.f, b1 = (a.bias && has1) ? __ldg(a.bias + nb + 1) : 0.f;
+        const float f0 = P == 2 ? fmaf(v0, a.acc_scale, b0) : v0 + b0, f1 = P == 2 ? fmaf(v1, a.acc_scale, b1) : v1 + b1;
+        const size_t pix = ((size_t)n * a.Ho + ho) * a.Wo + wo;
+        if (out_f32) {
+          float *o = static_cast<float *>(a.dst) + pix * a.cout_store + nb;
+          o[0] = cpb::act_out<__nv_bfloat16>(f0, act);
+          if (has1) o[1] = cpb::act_out<__nv_bfloat16>(f1, act);
+        } else {
+          store_pair16<P>(a.dst, a.res, pix * a.cout_store + nb, a.dst_plane, f0, f1, act, a.fmt);
         }
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
-        bias_loaded = true;
       }
-      mbar_wait(tfull0 + 8 * acc, accphase);
-      tc_fence_after();
-      const int ho = h0 + (row >> 3), wo = w0 + (row & 7);
-      const bool ok = valid && ho < a.Ho && wo < a.Wo;
-      const size_t pix = ((size_t)n * a.Ho + ho) * a.Wo + wo;
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_COLS;
-      if (a.tstore) {
-        // ---- TMA-store epilogue.  Every thread owns one pixel row, so direct global stores touch 32 lines per warp
-        // instruction and their L1 wavefronts compete with the MMAs' operand reads for the shared-memory data path
-        // (profiles/r02_head3x3_whatif.md).  Here 32 channels at a time go to a staging tile in shared memory (16-byte
-        // st.shared in the 64-byte-swizzle pattern: conflict-free, 4 wavefronts per 512 B) and ONE thread of the group
-        // hands the tile (both planes) to the copy engine; rows / channels outside the tensor are clipped by TMA.
-        const uint32_t stg = smem_base + a.stg_off + (uint32_t)grp * (uint32_t)(P * 8192);
-        const uint32_t srow = stg + (uint32_t)row * 64u, sx = ((uint32_t)row >> 1) & 3u;
-#pragma unroll 1
-        for (int c = (a.dbg & 2u) ? c_last : c_first; c < c_last; c += 2) {
-          if (n0 + c * 16 >= a.cout) break;                       // uniform over the group
-          uint32_t wh[2][8], wl[2][8];
-          // all accumulator reads of the round (2 chunks x both halves) are issued before the one wait
-          uint32_t va[2][16], vb[NCAT ? 2 : 1][16];
-          tmem_ld16(taddr + c * 16, va[0]);
-          tmem_ld16(taddr + (c + 1) * 16, va[1]);
-          if constexpr (NCAT) {
-            tmem_ld16(taddr + BN + c * 16, vb[0]);
-            tmem_ld16(taddr + BN + (c + 1) * 16, vb[1]);
-          }
-          tmem_ld_wait();
-#pragma unroll
-          for (int hc = 0; hc < 2; ++hc) {
-            uint32_t (&v)[16] = va[hc];
-            if constexpr (NCAT) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(vb[hc][j]));
-            }
-            const int nb = n0 + (c + hc) * 16;
-            float f[16];
-            if constexpr (P == 2) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = fmaf(__uint_as_float(v[j]), a.acc_scale, sbias[(c + hc) * 16 + j]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]) + sbias[(c + hc) * 16 + j];
-            }
-            if (a.res && ok && nb < a.cout) {
-              if constexpr (P == 2) {
-                const uint16_t *rh = static_cast<const uint16_t *>(a.res) + pix * a.cout_store + nb;
-                uint32_t hw_[8], lw_[8];                          // 32-byte sector loads, like the stores
-                ld_global_nc_32B(rh, hw_); ld_global_nc_32B(rh + a.dst_plane, lw_);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float2 x = join2(hw_[j], lw_[j], a.fmt);
-                  f[2 * j] += x.x; f[2 * j + 1] += x.y;
-                }
-              } else {
-                uint32_t rw[8];
-                ld_global_nc_32B(static_cast<const __nv_bfloat16 *>(a.res) + pix * a.cout_store + nb, rw);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float2 x = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&rw[j]));
-                  f[2 * j] += x.x; f[2 * j + 1] += x.y;
-                }
-              }
-            }
-            if constexpr (P == 2) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                split2(cpb::act_fast(f[2 * j], act), cpb::act_fast(f[2 * j + 1], act), a.fmt, wh[hc][j], wl[hc][j]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const __nv_bfloat162 b2 = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(f[2 * j], act), cpb::act_out<__nv_bfloat16>(f[2 * j + 1], act));
-                wh[hc][j] = *reinterpret_cast<const uint32_t *>(&b2);
-              }
-            }
-          }
-          if (a.dbg & 32u) {                                       // timing knob: accumulators read and converted, nothing stored
-            if (wh[0][0] == 0x12345678u && wl[1][7] == 0x9abcdef0u) asm volatile("st.shared.b32 [%0], %1;" ::"r"(srow), "r"(wh[1][3]) : "memory");
-            continue;
-          }
-          // the copy engine has finished READING the staging tile of the previous round
-          if (et == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-          asm volatile("bar.sync %0, 128;" ::"r"(3 + grp) : "memory");
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint32_t d = srow + (((uint32_t)j ^ sx) << 4);
-            const uint32_t *w_ = &wh[j >> 1][(j & 1) * 4];
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(d), "r"(w_[0]), "r"(w_[1]), "r"(w_[2]), "r"(w_[3]) : "memory");
-            if constexpr (P == 2) {
-              const uint32_t *l_ = &wl[j >> 1][(j & 1) * 4];
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(d + 8192u), "r"(l_[0]), "r"(l_[1]), "r"(l_[2]), "r"(l_[3]) : "memory");
-            }
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          asm volatile("bar.sync %0, 128;" ::"r"(3 + grp) : "memory");
-          if (et == 0 && valid) {
-            tma_store_4d(&a.dmap, stg, n0 + c * 16, w0, h0, n);
-            if constexpr (P == 2) tma_store_4d(&a.dmap, stg + 8192u, n0 + c * 16, w0, h0, n + a.B);
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          }
-        }
-      } else {
-      // direct stores (fp32 outputs, BN = 16, resident-weight convs without room for the staging tile): two chunks per round,
-      // their accumulator reads in flight before the one wait
-      constexpr int CSTEP = BN >= 32 ? 2 : 1;
-#pragma unroll 1
-      for (int c2 = (a.dbg & 2u) ? c_last : c_first; c2 < c_last; c2 += CSTEP) {
-        uint32_t va[CSTEP][16], vb[NCAT ? CSTEP : 1][16];
-#pragma unroll
-        for (int hc = 0; hc < CSTEP; ++hc) {
-          tmem_ld16(taddr + (c2 + hc) * 16, va[hc]);
-          if constexpr (NCAT) tmem_ld16(taddr + BN + (c2 + hc) * 16, vb[hc]);
-        }
-        tmem_ld_wait();
-#pragma unroll
-       for (int hc = 0; hc < CSTEP; ++hc) {
-        const int c = c2 + hc;
-        uint32_t (&v)[16] = va[hc];
-        if constexpr (NCAT) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(vb[hc][j]));
-        }
-        const int nb = n0 + c * 16;
-        if (ok && nb < a.cout) {
-          float f[16];
-          if constexpr (P == 2) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] = fmaf(__uint_as_float(v[j]), a.acc_scale, sbias[c * 16 + j]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]) + sbias[c * 16 + j];
-          }
-          if (out_f32) {
-            float *o = static_cast<float *>(a.dst) + pix * a.cout_store + nb;
-            if (nb + 16 <= a.cout && (a.cout_store & 3) == 0) {
-              if (act) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] = cpb::act_out<__nv_bfloat16>(f[j], act);
-              }
-              if ((a.cout_store & 7) == 0) {            // 32-byte rows: two sector-sized stores
-#pragma unroll
-                for (int j = 0; j < 16; j += 8) {
-                  const uint32_t ow[8] = {__float_as_uint(f[j]), __float_as_uint(f[j + 1]), __float_as_uint(f[j + 2]), __float_as_uint(f[j + 3]),
-                                          __float_as_uint(f[j + 4]), __float_as_uint(f[j + 5]), __float_as_uint(f[j + 6]), __float_as_uint(f[j + 7])};
-                  st_global_32B(o + j, ow);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4 *>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (nb + j < a.cout) o[j] = cpb::act_out<__nv_bfloat16>(f[j], act);
-            }
-          } else if constexpr (P == 2) {
-            // split output: hi plane at dst, lo plane dst_plane elements later; the residual is read the same way
-            uint16_t *o = static_cast<uint16_t *>(a.dst) + pix * a.cout_store + nb;
-            if (a.res) {
-              const uint16_t *rh = static_cast<const uint16_t *>(a.res) + pix * a.cout_store + nb;
-              const uint4 h0 = __ldg(reinterpret_cast<const uint4 *>(rh)), h1 = __ldg(reinterpret_cast<const uint4 *>(rh) + 1);
-              const uint4 l0 = __ldg(reinterpret_cast<const uint4 *>(rh + a.dst_plane)), l1 = __ldg(reinterpret_cast<const uint4 *>(rh + a.dst_plane) + 1);
-              const uint32_t hw_[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-              const uint32_t lw_[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float2 x = join2(hw_[j], lw_[j], a.fmt);
-                f[2 * j] += x.x; f[2 * j + 1] += x.y;
-              }
-            }
-            uint32_t oh[8], ol[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              split2(cpb::act_fast(f[2 * j], act), cpb::act_fast(f[2 * j + 1], act), a.fmt, oh[j], ol[j]);
-            st_global_32B(o, oh);                       // one 32-byte sector per thread and plane: every thread owns a pixel row,
-            st_global_32B(o + a.dst_plane, ol);         // so a warp store touches 32 lines — halve the number of such stores
-          } else {
-            __nv_bfloat16 *o = static_cast<__nv_bfloat16 *>(a.dst) + pix * a.cout_store + nb;
-            if (a.res) {
-              const uint4 *rp = reinterpret_cast<const uint4 *>(static_cast<const __nv_bfloat16 *>(a.res) + pix * a.cout_store + nb);
-              uint4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
-              const __nv_bfloat162 *rb0 = reinterpret_cast<const __nv_bfloat162 *>(&r0);
-              const __nv_bfloat162 *rb1 = reinterpret_cast<const __nv_bfloat162 *>(&r1);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                float2 x0 = __bfloat1622float2(rb0[j]), x1 = __bfloat1622float2(rb1[j]);
-                f[2 * j] += x0.x; f[2 * j + 1] += x0.y; f[8 + 2 * j] += x1.x; f[8 + 2 * j + 1] += x1.y;
-              }
-            }
-            if (act) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = cpb::act_out<__nv_bfloat16>(f[j], act);
-            }
-            uint4 o0, o1;
-            __nv_bfloat162 *ob0 = reinterpret_cast<__nv_bfloat162 *>(&o0), *ob1 = reinterpret_cast<__nv_bfloat162 *>(&o1);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              ob0[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
-              ob1[j] = __floats2bfloat162_rn(f[8 + 2 * j], f[8 + 2 * j + 1]);
-            }
-            const uint32_t ow[8] = {o0.x, o0.y, o0.z, o0.w, o1.x, o1.y, o1.z, o1.w};
-            st_global_32B(o, ow);
-          }
-        }
-       }
-      }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { if constexpr (mc) mbar_arrive_leader(tempty0 + 8 * acc); else mbar_arrive(tempty0 + 8 * acc); }
-      acc += tstep; par ^= 1;
-      if (acc >= a.nacc) { acc -= a.nacc; accphase ^= 1; }
     }
-    if (a.tstore && et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");     // staging is read out before the CTA ends
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (mc) cluster_sync_all();       // no CTA leaves while its peer may still signal its barriers / use its tensor memory
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (mc) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
@@ -701,29 +241,13 @@ struct C3Op {
   C3Args args;
   int BN, P, grid;
   size_t smem;
-  void *dst_mapped = nullptr;   // the output pointer args.dmap was encoded for
-  int B = 0, Ho = 0, Wo = 0, cout = 0;
 };
 
 template <int BN, int P>
 int launch_c3(const C3Op &t, const C3Args &args, cudaStream_t st) {
-  if constexpr (BN >= 32 && (P == 1 || 2 * BN <= 256)) {
-    if (args.mcast) {                                   // CTA pairs (cta_group::2): cluster of two
-      static SmemAttrCache cache2;
-      if (int rc = ensure_smem(conv3x3_tc_kernel<BN, P, 2>, t.smem, cache2)) return rc;
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3((unsigned)t.grid); cfg.blockDim = dim3(C3_THREADS); cfg.dynamicSmemBytes = t.smem; cfg.stream = st;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr; cfg.numAttrs = 1;
-      CPB_CUDA(cudaLaunchKernelEx(&cfg, conv3x3_tc_kernel<BN, P, 2>, args));
-      return cpb::check_launch("conv3x3_tc_kernel");
-    }
-  }
   static SmemAttrCache cache;
-  if (int rc = ensure_smem(conv3x3_tc_kernel<BN, P, 1>, t.smem, cache)) return rc;
-  conv3x3_tc_kernel<BN, P, 1><<<t.grid, C3_THREADS, t.smem, st>>>(args);
+  if (int rc = ensure_smem(conv3x3_tc_kernel<BN, P>, t.smem, cache)) return rc;
+  conv3x3_tc_kernel<BN, P><<<t.grid, C3_THREADS, t.smem, st>>>(args);
   return cpb::check_launch("conv3x3_tc_kernel");
 }
 
@@ -752,7 +276,7 @@ void *c3_prepare(const cpb200_op &op, int *rc) {
   C3Args &a = t->args;
   memset(&a, 0, sizeof(a));
   const int P = op.act_dtype == CPB200_BF16 ? 1 : 2;
-  t->P = P; t->B = op.B; t->Ho = op.Ho; t->Wo = op.Wo; t->cout = op.cout;
+  t->P = P;
   a.fmt = op.act_dtype == CPB200_F16X2 ? 1u : 0u;
   a.acc_scale = (op.acc_scale != 0.f ? op.acc_scale : 1.f);
   a.dst_plane = (long long)op.B * op.Ho * op.Wo * op.cout;
@@ -760,19 +284,16 @@ void *c3_prepare(const cpb200_op &op, int *rc) {
   const int bk = (cin % 64 == 0) ? 64 : (cin % 32 == 0) ? 32 : 16;
   a.cin = cin; a.BK = bk; a.slabs = cin / bk;
   const CUtensorMapSwizzle sw = bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-  a.swizzle_bits = bk == 64 ? 2u : bk == 32 ? 4u : 6u;
+  a.swizzle_bits = bk == 64 ? 1u : bk == 32 ? 2u : 3u;
   a.B = op.B; a.Ho = op.Ho; a.Wo = op.Wo;
   a.tiles_h = (op.Ho + TH - 1) / TH; a.tiles_w = (op.Wo + TW - 1) / TW;
   int BN = 16;
   while (BN < op.cout && BN < 256) BN <<= 1;
-  if (const char *e = getenv("CPB200_C3_BN")) { int v = atoi(e); if (v >= BN && v <= 256 && (v & (v - 1)) == 0) BN = v; }   // experiments
   if (P == 2 && BN > 128) BN = 128;       // split operands: [hi x hi | hi x lo + lo x hi] accumulator halves need 2 * BN <= 256 columns
   t->BN = BN;
   a.n_tiles = (op.cout + BN - 1) / BN;
   a.cout = op.cout; a.cout_store = op.cout;
   a.total_tiles = op.B * a.tiles_h * a.tiles_w * a.n_tiles;
-  const int acc_cols = (P == 2 && 2 * BN <= 256) ? 2 * BN : BN;
-  a.nacc = 512 / acc_cols > 8 ? 8 : 512 / acc_cols;      // TMEM accumulator stages (hides the MMA<->epilogue hand-off latency)
   a.dst = op.dst; a.res = op.res; a.bias = op.bias; a.flags = op.flags;
   a.kh = op.kh; a.kw = op.kw; a.taps = op.kh * op.kw; a.hw = TW + op.kw - 1;
   const int hh = TH + op.kh - 1;
@@ -781,12 +302,10 @@ void *c3_prepare(const cpb200_op &op, int *rc) {
   a.b_tx_bytes = BN * bk * 2;
   a.b_tile_bytes = a.b_tx_bytes;
   a.b_stage_bytes = ((unsigned)P * a.b_tx_bytes + 1023u) & ~1023u;      // P = 2: [hi tile | lo tile]
-  // dynamic shared memory: 227 KB per CTA minus the static part (barriers, up to 4 KB of bias) and the alignment slack
-  const size_t budget = (P == 2 ? 220 : 200) * 1024;
+  // dynamic shared memory: 227 KB per CTA minus the barriers and the alignment slack
+  const size_t budget = 220 * 1024;
   a.na = 3;
   if (a.a_stage_bytes <= 12 * 1024) a.na = (a.a_stage_bytes <= 6 * 1024) ? 16 : 8;   // small halos: deeper ring hides TMA latency
-  if (const char *e = getenv("CPB200_C3_DBG")) a.dbg = (unsigned)atoi(e);      // timing experiments (results are garbage)
-  if (const char *e = getenv("CPB200_C3_NA")) { int v = atoi(e); if (v >= 2 && v <= MAX_NA) a.na = v; }
   if (P == 2 && a.na < 4) a.na = 4;                         // two slabs' worth of planes in flight
   const size_t resident_bytes = (size_t)a.taps * a.slabs * a.b_stage_bytes;
   int na_res = a.na;
@@ -809,57 +328,7 @@ void *c3_prepare(const cpb200_op &op, int *rc) {
   }
   const int nsm = num_sms();
   t->grid = a.total_tiles < nsm ? a.total_tiles : nsm;
-  a.n_pix_tiles = op.B * a.tiles_h * a.tiles_w;
-  // streamed weights + enough tiles to keep every pair of SMs busy: CTA pairs (cta_group::2), each CTA holding half of B
-  a.mcast = 0;
-  {
-    // Opt-in (CPB200_C3_CG2=1): correct (tests/test_split_gpu.py::test_conv_cta_pair_path) but not faster than single CTAs —
-    // measured 422 vs 420 us on the 64->256 head conv: the streamed convs were bound by the issuing thread's per-stage
-    // overhead and by the accumulator read-out, neither of which a CTA pair shortens (profiles/r02_head3x3_whatif.md)
-    const char *e = getenv("CPB200_C3_CG2");
-    const bool want = e && e[0] == '1';
-    if (want && !a.b_resident && BN >= 32 && nsm >= 2 && a.n_pix_tiles >= nsm) {
-      a.mcast = 1;
-      t->grid = nsm & ~1;
-      // per-CTA weight stage: P = 1: half a tile;  P = 2: [this CTA's plane tile (BN rows) | its half of the hi tile (BN/2 rows)]
-      a.b_stage_bytes = (((unsigned)(P == 2 ? 3 : 1) * a.b_tile_bytes) / 2 + 1023u) & ~1023u;
-      int nb = (int)((budget - a.na * (size_t)a.a_stage_bytes) / a.b_stage_bytes);
-      if (nb > MAX_NB) nb = MAX_NB;
-      a.nb = nb;
-      t->smem = a.na * (size_t)a.a_stage_bytes + nb * (size_t)a.b_stage_bytes + 1024;
-    }
-  }
   const CUtensorMapDataType dt = a.fmt ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  // TMA-store epilogue (16-bit NHWC outputs): staging = 2 epilogue groups x P planes x (128 rows x 64 B) behind the rings.  It is
-  // taken from what the 227 KB leave after the static part; a streamed-weight ring gives up one stage for it if it has more
-  // than two, resident weights keep the direct 32-byte stores when the staging does not fit.
-  a.tstore = 0;
-  {
-    const char *e = getenv("CPB200_C3_TSTORE");
-    const size_t stg_bytes = (size_t)2 * P * 8192;
-    const size_t max_dyn = 232448 - (1536 + 16 * (size_t)BN);
-    const bool want = !(e && e[0] == '0') && !(op.flags & CPB200_FLAG_OUT_F32) && BN >= 32 && !a.mcast && op.cout % 8 == 0 &&
-                      (reinterpret_cast<uintptr_t>(op.dst) & 15) == 0;
-    if (want) {
-      if (t->smem + stg_bytes > max_dyn && !a.b_resident && a.nb > 2) {
-        --a.nb;
-        t->smem = a.na * (size_t)a.a_stage_bytes + a.nb * (size_t)a.b_stage_bytes + 1024;
-      }
-      if (t->smem + stg_bytes <= max_dyn) {
-        a.tstore = 1;
-        a.stg_off = (unsigned)(t->smem - 1024);
-        t->smem += stg_bytes;
-        const cuuint64_t dims[4] = {(cuuint64_t)op.cout, (cuuint64_t)op.Wo, (cuuint64_t)op.Ho, (cuuint64_t)op.B * P};
-        const cuuint64_t strides[3] = {(cuuint64_t)op.cout * 2, (cuuint64_t)op.Wo * op.cout * 2, (cuuint64_t)op.Ho * op.Wo * op.cout * 2};
-        const cuuint32_t box[4] = {32, (cuuint32_t)TW, (cuuint32_t)TH, 1};
-        const cuuint32_t es[4] = {1, 1, 1, 1};
-        CUresult r = enc(&a.dmap, dt, 4, op.dst, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                         CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { delete t; *rc = fail(CPB200_ERR_CUDA, "tc3: cuTensorMapEncodeTiled(dst) failed: %d", (int)r); return nullptr; }
-        t->dst_mapped = op.dst;
-      }
-    }
-  }
   {
     // split activations: the lo plane follows the hi plane, i.e. a batch of 2B images
     const cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.B * P};
@@ -875,7 +344,7 @@ void *c3_prepare(const cpb200_op &op, int *rc) {
     const int cout_pad = (op.cout + 15) / 16 * 16;
     const cuuint64_t dims[3] = {(cuuint64_t)bk, (cuuint64_t)cout_pad, (cuuint64_t)a.taps * (cuuint64_t)a.slabs * P};
     const cuuint64_t strides[2] = {(cuuint64_t)bk * 2, (cuuint64_t)cout_pad * bk * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)(a.mcast ? BN / 2 : BN), 1};      // mcast: each CTA loads half the rows
+    const cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)BN, 1};
     const cuuint32_t es[3] = {1, 1, 1};
     CUresult r = enc(&a.bmap, dt, 3, const_cast<void *>(op.weight), dims, strides, box, es,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -891,20 +360,6 @@ int c3_run(const void *h, const cpb200_op &op, cudaStream_t st) {
   const C3Op *t = static_cast<const C3Op *>(h);
   C3Args args = t->args;
   args.dst = op.dst; args.res = op.res; args.bias = op.bias;
-  if (args.tstore && op.dst != t->dst_mapped) {
-    // the caller re-bound the output (cpb200_prepare_ops contract: dst is read live): re-encode the store map for this run
-    if ((reinterpret_cast<uintptr_t>(op.dst) & 15) != 0) return fail(CPB200_ERR_ARG, "tc3: re-bound dst must be 16-byte aligned");
-    EncodeTiledFn enc = get_encode();
-    const int P = t->P;
-    const cuuint64_t dims[4] = {(cuuint64_t)t->cout, (cuuint64_t)t->Wo, (cuuint64_t)t->Ho, (cuuint64_t)t->B * P};
-    const cuuint64_t strides[3] = {(cuuint64_t)t->cout * 2, (cuuint64_t)t->Wo * t->cout * 2, (cuuint64_t)t->Ho * t->Wo * t->cout * 2};
-    const cuuint32_t box[4] = {32, (cuuint32_t)TW, (cuuint32_t)TH, 1};
-    const cuuint32_t es[4] = {1, 1, 1, 1};
-    if (!enc || enc(&args.dmap, args.fmt ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, op.dst, dims, strides, box, es,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return fail(CPB200_ERR_CUDA, "tc3: cuTensorMapEncodeTiled(dst) failed");
-  }
 #define C3_CASE(N)                                                                                   \
   case N: return t->P == 2 ? launch_c3<N, 2>(*t, args, st) : launch_c3<N, 1>(*t, args, st);
   switch (t->BN) {

@@ -1,14 +1,11 @@
-// Small-channel 3x3 convolutions (Cin = 16 or 32, stride 1 or 2, pad 1) on tcgen05 with SIMT-fed operands.
+// Small-channel 3x3 convolutions (Cin = 16 or 32, stride 1 or 2, pad 1) on wgmma with SIMT-fed operands.
 //
-// Why not TMA here: a tiled TMA box is fetched row by row, one request per (pixel row of the box) — measured
-// ~2.5-3 ns per request per SM whatever its width.  With 16 or 32 channels a request is only 32 / 64 bytes, so
-// the halo-reuse kernel (csrc/net_tc3.cu, 180 requests per tile) and the tap-per-stage kernel (csrc/net_tc.cu,
-// 9 x 128 requests per tile for stride 2) spend 0.5-3.7 us per 128-pixel tile waiting for the copy engine:
-// DLA-34 level0 (16->16 @512^2) 437 us and level1 (16->32 /2) 410 us against a ~100 us HBM floor.  Here producer
-// THREADS fetch the halo with coalesced 16-byte loads (a tile row is one contiguous 320..1088-byte segment of the
-// NHWC tensor) and store it straight into the swizzled K-major layout the UMMA descriptors read — the same
-// scheme as the stem (csrc/net_stem_tc.cu): next tile's loads in flight while this tile is stored, several
-// producer groups on alternate tiles, no CTA-wide barrier.
+// Why not TMA here: a tiled TMA box is fetched row by row, one request per (pixel row of the box).  With 16 or 32
+// channels a request is only 32 / 64 bytes, so the halo-reuse kernel (csrc/net_tc3.cu, 180 requests per tile) and the
+// tap-per-stage kernel (csrc/net_tc.cu, 9 x 128 requests per tile for stride 2) would spend most of a tile waiting for
+// the copy engine.  Here producer THREADS fetch the halo with coalesced 16-byte loads (a tile row is one contiguous
+// 320..1088-byte segment of the NHWC tensor) and store it straight into the swizzled K-major layout the wgmma descriptors
+// read — the same scheme as the stem (csrc/net_stem_tc.cu): next tile's loads in flight while this tile is stored.
 //
 //   halo     stride 1: 18 x 10 pixels, row R = hy*10 + hx;  tap (r,s) = window starting (r*10 + s) rows later,
 //            8-row-group stride 10 rows (as in net_tc3.cu).
@@ -19,10 +16,11 @@
 //            (chunk bit(s) [4..] ^= address bits [7..]); stage bases are 1024-aligned.
 //   weights  the ordinary tensor-core packing [tap][1 slab][N][C] bf16 (plan.py::_pack_conv_tc, bk = C), swizzled while being
 //            copied to shared memory once per CTA.
+//   warps    0-7 two consumer warpgroups (rows 0-63 / 64-127 of the tile: wgmma + epilogue), 8-15 producers.
 //   split    P = 2 (CPB200_BF16X2 / CPB200_F16X2, tc_common.cuh): the stage ring is plane-granular — a tile occupies two
 //            consecutive stages (hi halo, lo halo), fetched as two units of the producers' load pipeline; weights sit in
-//            shared memory as [tap][hi tile | lo tile], so A_hi x [W_hi ; W_lo] is ONE tcgen05.mma of N = 2N (N <= 64
-//            here) into two accumulator halves and A_lo x W_hi a second one; the epilogue adds the halves, applies
+//            shared memory as [tap][hi tile | lo tile]; A_hi x W_hi goes to one accumulator array, A_hi x W_lo and
+//            A_lo x W_hi to a second one; the epilogue adds them, applies
 //            acc_scale / bias / residual / activation in fp32 and stores the hi and lo planes.
 #include "tc_common.cuh"
 
@@ -33,10 +31,9 @@ namespace {
 using namespace tc;
 
 constexpr int SP_TH = 16, SP_TW = 8;
-constexpr int SP_GROUPS = 2;
-constexpr int SP_PT = 256;                                // producer threads per group
-constexpr int SP_THREADS = SP_GROUPS * SP_PT + 5 * 32;    // + MMA warp + 4 epilogue warps
-constexpr int SP_NACC = 4;
+constexpr int SP_CONS = 256;                              // two consumer warpgroups
+constexpr int SP_PT = 256;                                // producer threads
+constexpr int SP_THREADS = SP_CONS + SP_PT;
 
 struct SpArgs {
   const __nv_bfloat16 *x;      // (B,H,W,C)            [P = 2: hi plane, lo plane x_plane elements later; 16-bit either format]
@@ -65,7 +62,7 @@ struct SpGeom {
   static constexpr int NCHUNK = HH * HW * CH;             // 16-byte chunks fetched per tile
   static constexpr int NLD = (NCHUNK + SP_PT - 1) / SP_PT;
   static constexpr uint32_t SWMASK = (C == 16) ? 1u : 3u;
-  static constexpr uint32_t LAYOUT = (C == 16) ? 6u : 4u; // UMMA layout type: 32-byte / 64-byte swizzle
+  static constexpr uint32_t LAYOUT = (C == 16) ? 3u : 2u; // wgmma layout type: 32-byte / 64-byte swizzle
   static constexpr int NSTAGE = (STAGE_BYTES <= 12 * 1024) ? 6 : (STAGE_BYTES <= 20 * 1024 ? 5 : 4);
   // split mode: plane-granular stages, as many as fit beside the two weight planes (at most 8, at least 3)
   template <int N_>
@@ -86,28 +83,18 @@ __global__ void __launch_bounds__(SP_THREADS, 1) conv_sp_kernel(const SpArgs a) 
   static_assert(NSTAGE >= 3 && NSTAGE <= 8, "stage ring does not fit");
   constexpr int B_TILE_BYTES = N * G::PIX_B;               // one plane of one tap
   constexpr int B_TAP_BYTES = P * B_TILE_BYTES;            // [hi tile | lo tile]
-  constexpr int ACC_COLS = P * N;                          // P = 2: two accumulator halves (hi x hi + lo x hi | hi x lo)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;
   const uint32_t b_base = smem_base + NSTAGE * G::STAGE_BYTES;
-  __shared__ __align__(8) uint64_t bars[2 * 8 + 2 * SP_NACC];
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t bars[2 * 8];
   __shared__ float s_bias[N];
   const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[8]);
-  const uint32_t tfull0 = smem_u32(&bars[16]), tempty0 = smem_u32(&bars[16 + SP_NACC]);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int MMA_WARP = SP_GROUPS * SP_PT / 32;
-  constexpr uint32_t TMEM_COLS = (SP_NACC * ACC_COLS) < 32 ? 32u : (uint32_t)(SP_NACC * ACC_COLS);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < NSTAGE; ++s) { mbar_init(full0 + 8 * s, SP_PT); mbar_init(empty0 + 8 * s, 1); }
-    for (int s = 0; s < SP_NACC; ++s) { mbar_init(tfull0 + 8 * s, 1); mbar_init(tempty0 + 8 * s, 4); }
+    for (int s = 0; s < NSTAGE; ++s) { mbar_init(full0 + 8 * s, SP_PT); mbar_init(empty0 + 8 * s, SP_CONS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   // rows the producers never write (plane padding of the stride-2 layout) must hold finite values: zero everything once
   for (int i = threadIdx.x; i < NSTAGE * G::STAGE_BYTES / 16; i += SP_THREADS)
@@ -122,30 +109,17 @@ __global__ void __launch_bounds__(SP_THREADS, 1) conv_sp_kernel(const SpArgs a) 
   }
   for (int i = threadIdx.x; i < N; i += SP_THREADS) s_bias[i] = a.bias ? __ldg(a.bias + i) : 0.f;
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
   auto decode_tile = [&](int t, int &n, int &h0, int &w0) {
     const int tw = t % a.tiles_w; t /= a.tiles_w;
     const int th = t % a.tiles_h; n = t / a.tiles_h;
     h0 = th * SP_TH; w0 = tw * SP_TW;
   };
-  auto sbo_desc = [](uint32_t saddr, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(sbo_bytes >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)G::LAYOUT << 61;
-    return d;
-  };
 
-  if (warp < MMA_WARP) {
+  if (warp >= SP_CONS / 32) {
     // =============================== producers ===============================
-    const int grp = threadIdx.x / SP_PT;
-    const int p = threadIdx.x - grp * SP_PT;
+    const int p = threadIdx.x - SP_CONS;
     // chunk i = (hy*HW + hx)*CH + j of the halo: source offset (elements, relative to the halo origin) is tile
     // dependent only through (hi0, wi0); destination offset inside a stage is fixed -> precomputed.
     uint32_t doff[G::NLD];
@@ -178,14 +152,11 @@ __global__ void __launch_bounds__(SP_THREADS, 1) conv_sp_kernel(const SpArgs a) 
         pre[q] = ok ? __ldg(reinterpret_cast<const uint4 *>(xin + ((size_t)hi * a.W + wi) * C) + j) : make_uint4(0u, 0u, 0u, 0u);
       }
     };
-    const int tstep = gridDim.x * SP_GROUPS;
-    const int t_first = blockIdx.x + grp * gridDim.x;
-    int it = grp;
-    if (t_first < a.total_tiles) fetch(t_first, 0);
-    for (int t = t_first; t < a.total_tiles; t += tstep, it += SP_GROUPS) {
+    int vs = 0;
+    if ((int)blockIdx.x < a.total_tiles) fetch(blockIdx.x, 0);
+    for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
 #pragma unroll
-      for (int pl = 0; pl < P; ++pl) {                       // a tile = P consecutive plane stages
-        const int vs = it * P + pl;
+      for (int pl = 0; pl < P; ++pl, ++vs) {                 // a tile = P consecutive plane stages
         const int stage = vs % NSTAGE;
         const uint32_t phase = (uint32_t)(vs / NSTAGE) & 1u;
         mbar_wait(empty0 + 8 * stage, phase ^ 1);
@@ -195,140 +166,69 @@ __global__ void __launch_bounds__(SP_THREADS, 1) conv_sp_kernel(const SpArgs a) 
           if (hyx[q] >= 0)
             asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sa + doff[q]), "r"(pre[q].x), "r"(pre[q].y), "r"(pre[q].z),
                          "r"(pre[q].w) : "memory");
-        // the next unit's loads fly while the MMA warp consumes this one
+        // the next unit's loads fly while the consumers work on this one
         if (pl + 1 < P) fetch(t, pl + 1);
-        else if (t + tstep < a.total_tiles) fetch(t + tstep, 0);
+        else if (t + (int)gridDim.x < a.total_tiles) fetch(t + gridDim.x, 0);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         mbar_arrive(full0 + 8 * stage);
       }
     }
-  } else if (warp == MMA_WARP) {
-    // =============================== MMA issuer ===============================
-    const uint32_t idesc = P == 1 ? ((1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24))
-                                  : idesc_m128(N, a.fmt);
-    const uint32_t idesc2 = idesc_m128(2 * N, a.fmt);       // P = 2: A_hi x [W_hi ; W_lo]
-    int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t accphase = 0;
+  } else {
+    // =============================== consumers: wgmma + epilogue ===============================
+    const int wg = warp >> 2, tq = threadIdx.x & 127;
+    const uint32_t bf = (P == 1 || a.fmt == 0) ? 1u : 0u;
+    float acc[N / 2], acc2[P == 2 ? N / 2 : 1];                 // hi x W_hi | hi x W_lo + lo x W_hi (split operands)
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (P == 2 ? N / 2 : 1); ++i) acc2[i] = 0.f;
+    int stage = 0; uint32_t phase = 0;
     for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-      mbar_wait(tempty0 + 8 * acc, accphase ^ 1);
 #pragma unroll
       for (int pl = 0; pl < P; ++pl) {
         mbar_wait(full0 + 8 * stage, phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-          const uint64_t ad0 = sbo_desc(a_base + stage * G::STAGE_BYTES, G::PLANE_W * G::PIX_B);
-          const uint64_t bd0 = sbo_desc(b_base, 8 * G::PIX_B);
+        // this warpgroup's 64 rows = 8 output rows of the tile = 8 operand row groups further on
+        const uint64_t ad0 = desc_sbo(a_base + stage * G::STAGE_BYTES + wg * 8 * G::PLANE_W * G::PIX_B, G::PLANE_W * G::PIX_B, G::LAYOUT);
+        const uint64_t bd0 = desc_sbo(b_base, 8 * G::PIX_B, G::LAYOUT);
+        wg_fence();
 #pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {
-            const int r = tap / 3, s = tap % 3;
-            const int row0 = (S == 1) ? (r * G::PLANE_W + s)
-                                      : (((r & 1) * 2 + (s & 1)) * G::PLANE_ROWS + (r >> 1) * G::PLANE_W + (s >> 1));
+        for (int tap = 0; tap < 9; ++tap) {
+          const int r = tap / 3, s = tap % 3;
+          const int row0 = (S == 1) ? (r * G::PLANE_W + s)
+                                    : (((r & 1) * 2 + (s & 1)) * G::PLANE_ROWS + (r >> 1) * G::PLANE_W + (s >> 1));
 #pragma unroll
-            for (int k = 0; k < C / 16; ++k)
-              umma_bf16(d_tmem + (pl ? N : 0), ad0 + (uint32_t)(row0 * (G::PIX_B >> 4) + 2 * k), bd0 + (uint32_t)(tap * (B_TAP_BYTES >> 4) + 2 * k),
-                        (P == 2 && pl == 0) ? idesc2 : idesc, (pl > 0 || tap > 0 || k > 0) ? 1u : 0u);   // lo x hi -> second half
+          for (int k = 0; k < C / 16; ++k) {
+            const uint64_t ad = ad0 + (uint32_t)(row0 * (G::PIX_B >> 4) + 2 * k), bd = bd0 + (uint32_t)(tap * (B_TAP_BYTES >> 4) + 2 * k);
+            const uint32_t first = (pl > 0 || tap > 0 || k > 0) ? 1u : 0u;
+            if constexpr (P == 1) wgmma_k16<N>(acc, ad, bd, first, 1u);
+            else if (pl == 0) {
+              wgmma_k16<N>(acc, ad, bd, first, bf);                              // A_hi x W_hi
+              wgmma_k16<N>(acc2, ad, bd + (uint32_t)(B_TILE_BYTES >> 4), first, bf);   // A_hi x W_lo
+            } else {
+              wgmma_k16<N>(acc2, ad, bd, 1u, bf);                                // A_lo x W_hi
+            }
           }
-          umma_commit(empty0 + 8 * stage);
-          if (pl == P - 1) umma_commit(tfull0 + 8 * acc);
         }
-        __syncwarp();
+        wg_commit();
+        wg_wait<0>();
+        if (lane == 0) mbar_arrive(empty0 + 8 * stage);
         if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
       }
-      if (++acc == SP_NACC) { acc = 0; accphase ^= 1; }
-    }
-  } else {
-    // =============================== epilogue (4 warps) ===============================
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int ty = m >> 3, tx = m & 7;
-    int acc = 0; uint32_t accphase = 0;
-    for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
+      acc_fence(acc); acc_fence(acc2);
       int n, h0, w0; decode_tile(t, n, h0, w0);
-      const int ho = h0 + ty, wo = w0 + tx;
-      const bool ok = ho < a.Ho && wo < a.Wo;
-      const size_t pix = ((size_t)n * a.Ho + ho) * a.Wo + wo;
-      __nv_bfloat16 *o = a.y + pix * N;
-      uint4 rr[P == 1 ? N / 8 : 1];
-      if (P == 1 && a.res && ok) {
 #pragma unroll
-        for (int c = 0; c < N / 8; ++c) rr[c] = __ldg(reinterpret_cast<const uint4 *>(a.res + pix * N) + c);
+      for (int j = 0; j < N / 4; ++j) {
+        const int m = wg * 64 + frag_row(tq, j), c = frag_col(tq, j);
+        const int ho = h0 + (m >> 3), wo = w0 + (m & 7);
+        if (ho >= a.Ho || wo >= a.Wo) continue;
+        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
+        if constexpr (P == 2) { v0 += acc2[2 * j]; v1 += acc2[2 * j + 1]; }
+        const float f0 = P == 2 ? fmaf(v0, a.acc_scale, s_bias[c]) : v0 + s_bias[c];
+        const float f1 = P == 2 ? fmaf(v1, a.acc_scale, s_bias[c + 1]) : v1 + s_bias[c + 1];
+        const size_t pix = ((size_t)n * a.Ho + ho) * a.Wo + wo;
+        store_pair16<P>(a.y, a.res, pix * N + c, a.y_plane, f0, f1, a.act, a.fmt);
       }
-      mbar_wait(tfull0 + 8 * acc, accphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * ACC_COLS;
-#pragma unroll
-      for (int c = 0; c < N / 16; ++c) {
-        uint32_t v[16];
-        tmem_ld16(taddr + c * 16, v);
-        if constexpr (P == 2) {
-          uint32_t v2[16];
-          tmem_ld16(taddr + N + c * 16, v2);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(v2[j]));
-        } else {
-          tmem_ld_wait();
-        }
-        if (ok) {
-          float f[16];
-          if constexpr (P == 2) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] = fmaf(__uint_as_float(v[j]), a.acc_scale, s_bias[c * 16 + j]);
-            uint16_t *oh_ = reinterpret_cast<uint16_t *>(o) + c * 16;
-            if (a.res) {
-              const uint16_t *rh = reinterpret_cast<const uint16_t *>(a.res) + pix * N + c * 16;
-              const uint4 h0 = __ldg(reinterpret_cast<const uint4 *>(rh)), h1 = __ldg(reinterpret_cast<const uint4 *>(rh) + 1);
-              const uint4 l0 = __ldg(reinterpret_cast<const uint4 *>(rh + a.y_plane)), l1 = __ldg(reinterpret_cast<const uint4 *>(rh + a.y_plane) + 1);
-              const uint32_t hw_[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-              const uint32_t lw_[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float2 x = join2(hw_[j], lw_[j], a.fmt);
-                f[2 * j] += x.x; f[2 * j + 1] += x.y;
-              }
-            }
-            uint32_t oh[8], ol[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              split2(cpb::act_fast(f[2 * j], a.act), cpb::act_fast(f[2 * j + 1], a.act), a.fmt, oh[j], ol[j]);
-            st_global_32B(oh_, oh);
-            st_global_32B(oh_ + a.y_plane, ol);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]) + s_bias[c * 16 + j];
-            if (a.res) {
-              const __nv_bfloat162 *rb0 = reinterpret_cast<const __nv_bfloat162 *>(&rr[2 * c]);
-              const __nv_bfloat162 *rb1 = reinterpret_cast<const __nv_bfloat162 *>(&rr[2 * c + 1]);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float2 x0 = __bfloat1622float2(rb0[j]), x1 = __bfloat1622float2(rb1[j]);
-                f[2 * j] += x0.x; f[2 * j + 1] += x0.y; f[8 + 2 * j] += x1.x; f[8 + 2 * j + 1] += x1.y;
-              }
-            }
-            uint4 o0, o1;
-            __nv_bfloat162 *ob0 = reinterpret_cast<__nv_bfloat162 *>(&o0), *ob1 = reinterpret_cast<__nv_bfloat162 *>(&o1);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              ob0[j] = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(f[2 * j], a.act), cpb::act_out<__nv_bfloat16>(f[2 * j + 1], a.act));
-              ob1[j] = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(f[8 + 2 * j], a.act), cpb::act_out<__nv_bfloat16>(f[8 + 2 * j + 1], a.act));
-            }
-            const uint32_t ow[8] = {o0.x, o0.y, o0.z, o0.w, o1.x, o1.y, o1.z, o1.w};
-            st_global_32B(o + c * 16, ow);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-      if (++acc == SP_NACC) { acc = 0; accphase ^= 1; }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 

@@ -161,7 +161,7 @@ extern "C" int cpb200_flip_merge(const float *hm, const float *wh, const float *
     a.perm[j] = (signed char)flip_perm[j];
   }
   const long long total = (long long)P * (num_classes + 2 + 2 * J + (hm_hp ? J : 0)) * H * W;
-  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 16);
+  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
   flip_merge_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
   return cpb::check_launch("flip_merge_kernel");
 }

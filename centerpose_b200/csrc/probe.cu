@@ -1,30 +1,18 @@
-// Hardware probes (diagnostics, not on the product path): empirical checks of UMMA descriptor
-// behaviour that the available documentation does not settle.
+// Hardware probes (diagnostics, not on the product path): empirical checks of wgmma descriptor behaviour that the
+// available documentation does not settle, and TMA box throughput for the box shapes the conv kernels use.
 //
-// cpb200_probe_halo: can ONE (TH+2)x(TW+2) halo tile in shared memory (TMA, 128B swizzle, 128-byte
-// pixel rows) serve all nine taps of a 3x3 conv through shifted UMMA descriptors?  With TW = 8 every
-// 8-row core-matrix group of the A operand is one tile row, so tap (r,s) is
-//   start = base + (r*(TW+2) + s)*128 B,  SBO = (TW+2)*128 B  (not a multiple of the 1024-B swizzle
-// repeat).  Works iff the hardware applies the swizzle XOR to absolute smem address bits.
-#include "common.cuh"
-#include <cuda.h>
+// cpb200_probe_halo: can ONE (TH+2)x(TW+2) halo tile in shared memory (TMA, 128B swizzle, 128-byte pixel rows) serve all
+// nine taps of a 3x3 conv through shifted wgmma descriptors?  With TW = 8 every 8-row core-matrix group of the A operand is
+// one tile row, so tap (r,s) is
+//   start = base + (r*(TW+2) + s)*128 B,  SBO = (TW+2)*128 B  (not a multiple of the 1024-B swizzle repeat),
+// and the second warpgroup's 64 rows start 8 halo rows later.  Works iff the hardware applies the swizzle XOR to absolute
+// shared-memory address bits; variant 0 leaves the descriptor's base_offset at 0 (what csrc/net_tc3.cu does), variant 1
+// sets it to (start >> 7) & 7.
+#include "tc_common.cuh"
 
 namespace {
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  } while (!done);
-}
+using namespace tc;
 
 struct alignas(64) ProbeArgs {
   CUtensorMap xmap;    // (C=64, W=TW+2, H=TH+2, N=1) bf16
@@ -35,78 +23,50 @@ struct alignas(64) ProbeArgs {
 
 constexpr int TW = 8, TH = 16, HALO_W = TW + 2, HALO_H = TH + 2;
 
-__global__ void __launch_bounds__(128, 1) probe_halo_kernel(const __grid_constant__ ProbeArgs a) {
+__global__ void __launch_bounds__(256, 1) probe_halo_kernel(const __grid_constant__ ProbeArgs a) {
   extern __shared__ __align__(1024) uint8_t raw[];
   const uint32_t base = (smem_u32(raw) + 1023u) & ~1023u;
   const uint32_t xs = base;                                   // halo tile: 180 rows x 128 B = 23040 B
   const uint32_t ws = base + 24 * 1024;                       // 9 x (64 x 128 B) = 73728 B
-  __shared__ __align__(8) uint64_t bars[2];
-  __shared__ uint32_t s_tmem;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __shared__ __align__(8) uint64_t bar_;
+  const uint32_t bar = smem_u32(&bar_);
   if (threadIdx.x == 0) {
-    mbar_init(smem_u32(&bars[0]), 1); mbar_init(smem_u32(&bars[1]), 1);
+    mbar_init(bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(64) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = s_tmem;
   if (threadIdx.x == 0) {
-    const uint32_t bar = smem_u32(&bars[0]);
     mbar_expect_tx(bar, HALO_W * HALO_H * 128 + 9 * 64 * 128);
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                 ::"r"(xs), "l"(reinterpret_cast<uint64_t>(&a.xmap)), "r"(bar), "r"(0), "r"(0), "r"(0), "r"(0) : "memory");
-    for (int t = 0; t < 9; ++t)
-      asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-                   ::"r"(ws + t * 8192), "l"(reinterpret_cast<uint64_t>(&a.wmap)), "r"(bar), "r"(0), "r"(0), "r"(t) : "memory");
-    mbar_wait(bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    for (int t = 0; t < 9; ++t) {
-      const int r = t / 3, s = t % 3;
-      for (int k = 0; k < 4; ++k) {
-        const uint32_t astart = xs + (r * HALO_W + s) * 128 + k * 32;
-        uint64_t ad = 0;
-        ad |= (uint64_t)((astart & 0x3FFFF) >> 4);
-        ad |= (uint64_t)1 << 16;
-        ad |= (uint64_t)((HALO_W * 128) >> 4) << 32;             // SBO = one halo row of pixels
-        ad |= (uint64_t)1 << 46;
-        if (a.variant == 1) ad |= (uint64_t)((astart >> 7) & 7) << 49;
-        ad |= (uint64_t)2 << 61;
-        const uint32_t bstart = ws + t * 8192 + k * 32;
-        uint64_t bd = 0;
-        bd |= (uint64_t)((bstart & 0x3FFFF) >> 4);
-        bd |= (uint64_t)1 << 16;
-        bd |= (uint64_t)(1024 >> 4) << 32;
-        bd |= (uint64_t)1 << 46;
-        bd |= (uint64_t)2 << 61;
-        const uint32_t acc = (t > 0 || k > 0) ? 1u : 0u;
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                     ::"r"(tmem), "l"(ad), "l"(bd), "r"(idesc), "r"(acc) : "memory");
-      }
+    tma_load_4d(xs, &a.xmap, bar, 0, 0, 0, 0);
+    for (int t = 0; t < 9; ++t) tma_load_3d(ws + t * 8192, &a.wmap, bar, 0, 0, t);
+  }
+  mbar_wait(bar, 0);
+  const int wg = threadIdx.x >> 7, tq = threadIdx.x & 127;
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  wg_fence();
+#pragma unroll
+  for (int t = 0; t < 9; ++t) {
+    const int r = t / 3, s = t % 3;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t astart = xs + (r * HALO_W + s + wg * 8 * HALO_W) * 128 + k * 32;
+      uint64_t ad = desc_sbo(astart, HALO_W * 128, 1);        // SBO = one halo row of pixels
+      if (a.variant == 1) ad |= (uint64_t)((astart >> 7) & 7) << 49;
+      const uint64_t bd = make_desc(ws + t * 8192 + k * 32, 128, 1);
+      wgmma_k16<64>(acc, ad, bd, (t > 0 || k > 0) ? 1u : 0u, 1u);
     }
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bars[1])) : "memory");
   }
-  mbar_wait(smem_u32(&bars[1]), 0);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const int row = warp * 32 + lane;
-  for (int c = 0; c < 4; ++c) {
-    uint32_t v[16];
-    const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + c * 16;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                   "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                 : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    for (int j = 0; j < 16; ++j) a.out[row * 64 + c * 16 + j] = __uint_as_float(v[j]);
+  wg_commit();
+  wg_wait<0>();
+  acc_fence(acc);
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int row = wg * 64 + frag_row(tq, j), col = frag_col(tq, j);
+    a.out[row * 64 + col] = acc[2 * j];
+    a.out[row * 64 + col + 1] = acc[2 * j + 1];
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(64) : "memory");
 }
 
 // ---- TMA box-throughput probe: every CTA streams boxes of one shape through an N-deep smem ring ----
@@ -147,9 +107,6 @@ __global__ void __launch_bounds__(64, 1) probe_tma_kernel(const __grid_constant_
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 }  // namespace
 
 // x: (1, 18, 10, 64) bf16 NHWC;  w: (9, 64, 64) bf16 [tap][cout][cin];  out: (128, 64) fp32, row = th*8 + tw
@@ -184,9 +141,11 @@ extern "C" int cpb200_probe_halo(const void *x, const void *w, float *out, int v
   a.out = out; a.variant = variant;
   const size_t smem = 24 * 1024 + 9 * 8192 + 1024;
   CPB_CUDA(cudaFuncSetAttribute(probe_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  probe_halo_kernel<<<1, 128, smem, static_cast<cudaStream_t>(stream)>>>(a);
+  probe_halo_kernel<<<1, 256, smem, static_cast<cudaStream_t>(stream)>>>(a);
   return cpb::check_launch("probe_halo_kernel");
 }
+
+
 
 // Streams (C,W,H,N) bf16 through TMA boxes {C, box_w, box_h, 1} stepping (step_w, step_h); returns after enqueue.
 extern "C" int cpb200_probe_tma(const void *x, int C, int W, int H, int N, int box_w, int box_h, int step_w, int step_h,
@@ -212,7 +171,7 @@ extern "C" int cpb200_probe_tma(const void *x, int C, int W, int H, int N, int b
   const size_t smem = (size_t)stages * a.stage_bytes + 1024;
   if (stages > 16 || smem > 200 * 1024) return cpb::fail(CPB200_ERR_ARG, "probe: ring too large");
   CPB_CUDA(cudaFuncSetAttribute(probe_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int dev = 0, nsm = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  int dev = 0, nsm = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   probe_tma_kernel<<<nsm, 64, smem, static_cast<cudaStream_t>(stream)>>>(a);
   return cpb::check_launch("probe_tma_kernel");
 }

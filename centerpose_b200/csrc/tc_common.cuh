@@ -1,16 +1,15 @@
-// PTX wrappers shared by the tcgen05 / TMA kernels (sm_100a).
+// PTX wrappers shared by the wgmma / TMA kernels (sm_90a).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
+#include "wgmma.cuh"
 
 namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// One thread of a converged warp (PTX elect.sync).  Unlike `lane == 0`, ptxas knows the guarded region is
-// single-threaded and emits the uniform-datapath instructions (UTCHMMA, UTMALDG, UTCBAR) directly instead of
-// wrapping each one in an ELECT / BRA.U.ANY loop (~3x fewer issue cycles per tcgen05.mma).
+// One thread of a converged warp (PTX elect.sync).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -36,28 +35,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "=r"(done) : "r"(bar), "r"(parity) : "memory");
   } while (!done);
 }
-// TMA store of a 4-D box from shared memory (bulk async group; the caller commits / waits)
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap *map, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-// 256-bit read-only global load (sm_100: LDG.E.256.CONSTANT): one 32-byte sector per thread
-__device__ __forceinline__ void ld_global_nc_32B(const void *p, uint32_t (&w)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
-}
-// 256-bit global store (sm_100: STG.E.256): one full 32-byte sector per thread
-__device__ __forceinline__ void st_global_32B(void *p, const uint32_t (&w)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-               "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
-}
-// one poll (the hardware may suspend the thread for a bounded time inside the instruction)
-__device__ __forceinline__ uint32_t mbar_try_once(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-               : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  return done;
-}
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2, int c3) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
@@ -68,104 +45,49 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *map
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// ---- 2-CTA cluster helpers: TMA multicast of a box into the same shared-memory offset of every CTA in `mask` (each
-// destination CTA's mbarrier at the same offset receives the bytes), and a tcgen05.commit that arrives on that barrier in
-// every CTA of `mask` ----
-__device__ __forceinline__ void tma_load_3d_mcast(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5, %6}], [%2], %3;"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "h"(mask), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void umma_commit_mcast(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-// ---- cta_group::2 (CTA pair) forms.  A 2-CTA tcgen05.mma of shape 256 x N x 16 is issued by one thread of the LEADER CTA
-// (even rank); each CTA supplies its own 128 rows of A and N/2 rows of B (same shared-memory offsets in both CTAs) and
-// receives 128 rows of D in its own tensor memory.  Loads of either CTA signal the leader's mbarrier (peer bit of the
-// shared::cluster address cleared); commits arrive on the same-offset mbarrier of every CTA in the mask.
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;
-__device__ __forceinline__ void umma_f16_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_cg2(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_cg2(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_cg2(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-// arrive on the LEADER CTA's barrier at the same offset as `bar` (works from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar & PEER_BIT_MASK) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void tmap_prefetch(const CUtensorMap *map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t *v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory descriptor, K-major operand, rows of `row_bytes` (= swizzle span), 8-row
-// core-matrix groups packed back to back (what a TMA box with inner extent = swizzle span writes).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t row_bytes, uint32_t layout_type) {
+// ---- warpgroup MMA ----
+// Shared-memory matrix descriptor, K-major operand in a 128B / 64B / 32B-swizzled layout (layout 1 / 2 / 3): start address,
+// stride between 8-row core-matrix groups (SBO); the leading offset is unused for swizzled K-major operands.  The swizzle
+// XOR is applied to absolute shared-memory address bits, so a start address may sit anywhere inside a swizzle atom (+32 B
+// per K step of 16, whole 16..128-byte pixel rows for the shifted halo windows of the 3x3 / 7x7 kernels).
+__device__ __forceinline__ uint64_t desc_sbo(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);                 // start address, bits [0,14)
   d |= (uint64_t)1 << 16;                                  // leading byte offset (unused for swizzled K-major)
-  d |= (uint64_t)((8u * row_bytes) >> 4) << 32;            // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                                  // descriptor version 1 (sm_100)
-  d |= (uint64_t)layout_type << 61;                        // 2 = SW128, 4 = SW64, 6 = SW32
+  d |= (uint64_t)(sbo_bytes >> 4) << 32;                   // stride byte offset between 8-row groups
+  d |= (uint64_t)layout_type << 62;                        // 1 = SW128, 2 = SW64, 3 = SW32
   return d;
 }
-
+// rows of `row_bytes` (= swizzle span), 8-row groups packed back to back (what a TMA box with inner extent = swizzle span writes)
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t row_bytes, uint32_t layout_type) {
+  return desc_sbo(saddr, 8u * row_bytes, layout_type);
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Fragment order of a 64 x N accumulator: register i of thread t (0..127 of the warpgroup) holds
+//   row (t / 32) * 16 + (t % 32) / 4 + 8 * ((i / 2) % 2),  column 8 * (i / 4) + 2 * (t % 4) + i % 2.
+// The epilogues walk it as pairs of adjacent columns: pair j = registers (2j, 2j+1).
+__device__ __forceinline__ int frag_row(int t, int j) { return (t >> 5) * 16 + ((t & 31) >> 2) + 8 * (j & 1); }
+__device__ __forceinline__ int frag_col(int t, int j) { return 8 * (j >> 1) + 2 * (t & 3); }
 
 // ------------------------------------------------------------------------------------------------------------
 // Split-operand ("x2") arithmetic: every fp32 value v is carried as two 16-bit planes hi = rn16(v),
 // lo = rn16(v - hi); a product a*b is evaluated on the tensor core as a_hi*b_hi + a_hi*b_lo + a_lo*b_hi with fp32
-// accumulation in TMEM (the dropped a_lo*b_lo term is <= 2^-16 / 2^-22 of the product for bf16 / fp16 planes).
+// accumulation (the dropped a_lo*b_lo term is <= 2^-16 / 2^-22 of the product for bf16 / fp16 planes).
 // fmt: 0 = bf16 planes (8+8 significand bits, fp32 range), 1 = fp16 planes (11+11 bits, |v| <= 65504 — the epilogues
 // saturate; weights are pre-scaled by a power of two on the host so that their lo parts stay normal numbers).
-__device__ __forceinline__ uint32_t idesc_m128(uint32_t n, uint32_t fmt) {
-  // D = f32, A/B format (0 = f16, 1 = bf16), both K-major, N = n, M = 128
-  const uint32_t ab = fmt ? 0u : 1u;
-  return (1u << 4) | (ab << 7) | (ab << 10) | ((n >> 3) << 17) | ((128u >> 4) << 24);
-}
-__device__ __forceinline__ uint32_t idesc_mn(uint32_t m, uint32_t n, uint32_t ab_bf16) {
-  // D = f32, A/B format (0 = f16, 1 = bf16), both K-major; M = 128 (one CTA) or 256 (CTA pair)
-  return (1u << 4) | (ab_bf16 << 7) | (ab_bf16 << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
 __device__ __forceinline__ void split2(float a, float b, uint32_t fmt, uint32_t &hi, uint32_t &lo) {
   if (fmt) {
     a = fminf(fmaxf(a, -65504.f), 65504.f); b = fminf(fmaxf(b, -65504.f), 65504.f);
@@ -201,6 +123,32 @@ __device__ __forceinline__ float2 unpack2(uint32_t v, uint32_t fmt) {
 __device__ __forceinline__ float2 join2(uint32_t hi, uint32_t lo, uint32_t fmt) {
   const float2 h = unpack2(hi, fmt), l = unpack2(lo, fmt);
   return make_float2(h.x + l.x, h.y + l.y);
+}
+
+// 16-bit NHWC output of one pixel, channels (nb, nb + 1): f0 / f1 already carry bias and accumulator scale; adds the
+// residual (same layout as the output), applies the activation, stores (P = 2: hi plane at e, lo plane `plane` later).
+template <int P>
+__device__ __forceinline__ void store_pair16(void *dst, const void *res, size_t e, long long plane, float f0, float f1, uint32_t act,
+                                             uint32_t fmt) {
+  if constexpr (P == 2) {
+    uint16_t *o = static_cast<uint16_t *>(dst) + e;
+    if (res) {
+      const uint16_t *r = static_cast<const uint16_t *>(res) + e;
+      const float2 x = join2(__ldg(reinterpret_cast<const unsigned int *>(r)), __ldg(reinterpret_cast<const unsigned int *>(r + plane)), fmt);
+      f0 += x.x; f1 += x.y;
+    }
+    uint32_t hi, lo;
+    split2(cpb::act_fast(f0, act), cpb::act_fast(f1, act), fmt, hi, lo);
+    *reinterpret_cast<uint32_t *>(o) = hi;
+    *reinterpret_cast<uint32_t *>(o + plane) = lo;
+  } else {
+    __nv_bfloat16 *o = static_cast<__nv_bfloat16 *>(dst) + e;
+    if (res) {
+      const float2 x = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162 *>(static_cast<const __nv_bfloat16 *>(res) + e)));
+      f0 += x.x; f1 += x.y;
+    }
+    *reinterpret_cast<__nv_bfloat162 *>(o) = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(f0, act), cpb::act_out<__nv_bfloat16>(f1, act));
+  }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,

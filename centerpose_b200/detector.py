@@ -270,10 +270,10 @@ class MultiPoseDetector(BaseDetector):
         return results.tolist()
 
     def debug(self, debugger, images, dets, output, scale=1):
-        raise NotImplementedError("visual debugging (lib/utils/debugger.py) is outside the B200 hot path")
+        raise NotImplementedError("visual debugging (lib/utils/debugger.py) is outside the GPU hot path")
 
     def show_results(self, debugger, image, results):
-        raise NotImplementedError("visualisation (lib/utils/debugger.py) is outside the B200 hot path")
+        raise NotImplementedError("visualisation (lib/utils/debugger.py) is outside the GPU hot path")
 
     # -- additive: batched / device-resident paths ------------------------------------------------
     def merge_outputs_device(self, detections, nms=None, return_keep=False):

@@ -103,11 +103,11 @@ class BackBoneWithHead(nn.Module):
 
     def set_precision(self, precision: str, tc=None):
         """Arithmetic of the forward pass (the reference is fp32 end to end):
-          'fp16x2'  tcgen05 tensor cores on split operands — every activation / weight is a pair of fp16 planes
+          'fp16x2'  wgmma tensor cores on split operands — every activation / weight is a pair of fp16 planes
                     (hi + lo, 22 significand bits), a*b = a_hi*b_hi + a_hi*b_lo + a_lo*b_hi with fp32 accumulation:
-                    fp32-faithful (head maps within ~4e-6 relative L2 of the reference's fp32 result) at tensor-core
+                    fp32-faithful (DLA-34 512x512 head maps within 1.8e-5 relative L2 of the reference's fp32 result) at tensor-core
                     speed; activations must stay within the fp16 range (|v| <= 65504, saturating);
-          'bf16x2'  same with bf16 planes: full fp32 range, 16 significand bits (~6e-5 relative L2);
+          'bf16x2'  same with bf16 planes: full fp32 range, 16 significand bits;
           'bf16'    plain bf16 operands (fastest; ~2e-2 relative L2 through the ~100 layers);
           'fp32'    CUDA-core kernels, fp32 activations (reference arithmetic up to summation order; slow).
         tc=False keeps bf16 activations but forces the CUDA-core kernels — a debugging aid."""
@@ -141,10 +141,9 @@ class BackBoneWithHead(nn.Module):
             hc = self.head_conv
             fuse = pb.use_tc and hc % 16 == 0 and hc <= 128 and os.environ.get("CPB200_FUSE_HEADS", "1") != "0"
             if fuse:
-                # Narrow heads (ResNet-50 / HRNet: head_conv 64): ONE 3x3 conv produces all six hidden maps.  A
-                # tcgen05.mma costs the issuing thread the same ~90 cycles whether N is 64 or 256 (measured: the
-                # 256->64 head conv takes 190 us at N = 64, 194 at 128, 204 at 256), so six N=64 convs are issue-bound
-                # at 6x the instruction count of one N=384 conv; the feature map is also read once instead of six times.
+                # Narrow heads (ResNet-50 / HRNet: head_conv 64): ONE 3x3 conv produces all six hidden maps: wide N tiles
+                # issue fewer MMA instructions per output than six N=64 convs, and the feature map is read once instead of
+                # six times.
                 w_cat = torch.cat([w0_of(name) for name, _ in HEADS], dim=0)
                 b_cat = torch.cat([P(f"{name}.0.bias").float() for name, _ in HEADS], dim=0)
                 hid = pb.conv([feat], w_cat, b_cat, stride=1, pad=1, relu=True)

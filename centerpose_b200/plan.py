@@ -33,12 +33,12 @@ PRECISIONS = {"fp32": F32, "bf16": BF16, "bf16x2": BF16X2, "fp16x2": F16X2}
 BN_EPS = 1e-5
 
 
-# The tcgen05 fp32 accumulator rounds TOWARD ZERO at every instruction.  For dot products of random-sign operands this
-# shrinks the result by a factor that is linear in the number of K = 16 accumulation steps — measured on B200 with iid
-# Gaussian and post-ReLU operands (tools/rz_probe.py, profiles/r02_rz_probe.log): -1.6e-8 per step with fp16 planes
-# (K = 256 .. 4608, residual 0.6x the coherent part), -1.2e-8 with bf16 planes.  Uncorrected it is the dominant error of
-# the split precisions through a deep network because it is COHERENT: ~40 layers of DLA-34 add up to 7e-5, which the 16
-# chained DCNs amplify to 3e-4 at the heads (profiles/r02_layer_err_*.log).  The host therefore folds the expected
+# The wgmma fp32 accumulator rounds TOWARD ZERO at every instruction.  For dot products of random-sign operands this
+# shrinks the result by a factor that is linear in the number of K = 16 accumulation steps — measured on an H100 SXM
+# (400 W power limit) with iid Gaussian and post-ReLU operands (CPB200_RZ_COMP=0 python tools/rz_probe.py): -1.6e-8 per
+# step with fp16 planes (K = 256 .. 4608), -1.0e-8 .. -1.5e-8 with bf16 planes.  Uncorrected it is the dominant error of
+# the split precisions through a deep network because it is COHERENT: it adds up over the ~40 layers of DLA-34 and the
+# chained DCNs amplify it towards the heads (tools/layer_err.py shows it per layer).  The host therefore folds the expected
 # factor 1 + beta * K/16 into cpb200_op.acc_scale (a multiplication the epilogue performs anyway).  CPB200_RZ_COMP
 # overrides beta (0 disables); all-positive dot products shrink ~6x more and stay under-corrected.
 RZ_BETA = {"fp16x2": 1.6e-8, "bf16x2": 1.2e-8}
@@ -155,14 +155,14 @@ class PlanBuilder:
         self.device = device
         self.precision = precision
         self.act_dtype = PRECISIONS[precision]
-        # split-operand precisions: activations are hi/lo 16-bit planes, every conv runs on tcgen05 as three products
+        # split-operand precisions: activations are hi/lo 16-bit planes, every conv runs on wgmma as three products
         self.split = precision in ("bf16x2", "fp16x2")
         self.torch16 = torch.float16 if precision == "fp16x2" else torch.bfloat16
         self.torch_act = torch.float32 if precision == "fp32" else self.torch16
         self.ops: List[_PendingOp] = []
         self.keep: List[torch.Tensor] = []      # weights / biases kept alive
         self.syms: List[Sym] = []
-        # tensor-core (tcgen05) path: 16-bit operands only; CPB200_TC=0 forces the SIMT kernels (bf16: debugging)
+        # tensor-core (wgmma) path: 16-bit operands only; CPB200_TC=0 forces the SIMT kernels (bf16: debugging)
         if tc is None:
             tc = os.environ.get("CPB200_TC", "1") != "0"
         if self.split and not tc:
@@ -267,10 +267,9 @@ class PlanBuilder:
         return self._dev(p)
 
     def _pack_conv_tc(self, w: torch.Tensor, bk: int):
-        """(Co,Ci,kh,kw) fp32 -> tcgen05 layout [kh*kw][Ci/bk][Co_pad16][bk] bf16 (K-major B operand, slab-major:
+        """(Co,Ci,kh,kw) fp32 -> wgmma layout [kh*kw][Ci/bk][Co_pad16][bk] bf16 (K-major B operand, slab-major:
         the rows of one (tap, K-slab) block are contiguous, so a TMA weight box is one dense run of memory instead of
-        Co rows strided by Ci).  bk = the kernels' K-slab width.  (No measurable speed difference against the
-        strided [tap][Co][Ci] layout on B200 — kept because it lets one box span several slabs.)"""
+        Co rows strided by Ci).  bk = the kernels' K-slab width."""
         co, ci, kh, kw = w.shape
         assert ci % bk == 0
         cop = (co + 15) // 16 * 16

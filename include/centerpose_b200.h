@@ -1,5 +1,5 @@
 /*
- * centerpose_b200 — C ABI of the B200-native (sm_100a) centerpose inference hot path.
+ * centerpose_b200 — C ABI of the H100-native (sm_90a) centerpose inference hot path.
  *
  * The reference (tensorboy/centerpose) has no FFI for this path: its seams are Python
  * callables (SURVEY.md §8b).  Every entry point below names the reference interface it
@@ -28,7 +28,7 @@ extern "C" {
 #define CPB200_OK 0
 #define CPB200_ERR_ARG 1      /* bad argument (shape, null pointer, unsupported size) */
 #define CPB200_ERR_CUDA 2     /* CUDA runtime / launch failure */
-#define CPB200_ERR_STATE 3    /* library not usable (no sm_100 device, driver entry point missing) */
+#define CPB200_ERR_STATE 3    /* library not usable (no sm_90 device, driver entry point missing) */
 
 #define CPB200_DECODE_MAX_K 128
 #define CPB200_DECODE_MAX_J 32
@@ -145,7 +145,7 @@ enum cpb200_op_type {
   CPB200_OP_CONV = 1,        /* k x k conv (+bias)(+residual)(+ReLU); up to 4 channel-concatenated inputs */
   CPB200_OP_STEM = 2,        /* NCHW fp32 image -> NHWC, small-Cin direct conv (+bias+activation); with CPB200_FLAG_TC
                                 (7x7, Cin 3, stride 1/2, cout 16/64, bf16) the im2col is built in shared memory and
-                                the arithmetic runs on tcgen05 (weight = pre-swizzled operand image, plan.py)   */
+                                the arithmetic runs on wgmma (weight = pre-swizzled operand image, plan.py)     */
   CPB200_OP_MAXPOOL = 3,     /* k x k / stride s / pad p max-pool, NHWC                                     */
   CPB200_OP_DWDECONV_ADD = 4,/* depthwise ConvTranspose2d(k=2f,s=f,p=f/2) (+ skip add), NHWC  (IDAUp up_*) */
   CPB200_OP_DCN = 5,         /* modulated deformable 3x3 conv (DCNv2 forward) (+bias)(+ReLU)                */
@@ -173,7 +173,7 @@ enum cpb200_op_type {
 #define CPB200_FLAG_RELU 1u          /* ReLU in the epilogue                                     */
 #define CPB200_FLAG_OUT_NCHW_F32 2u  /* write fp32 NCHW into dst (channel slice out_ch_off..)    */
 #define CPB200_FLAG_OUT_F32 4u       /* write fp32 NHWC regardless of act_dtype (DCN offsets)    */
-#define CPB200_FLAG_TC 8u            /* run on the tcgen05 tensor-core path (bf16 only)          */
+#define CPB200_FLAG_TC 8u            /* run on the wgmma tensor-core path (16-bit operands)       */
 #define CPB200_FLAG_HSWISH 16u       /* x * relu6(x + 3) / 6 in the epilogue (mobilenetv3.py:84-87)   */
 #define CPB200_FLAG_HSIGMOID 32u     /* relu6(x + 3) / 6 in the epilogue     (mobilenetv3.py:90-93)   */
 #define CPB200_FLAG_TO_F32 64u       /* CPB200_OP_CONVERT direction: split planes -> fp32                    */
@@ -221,7 +221,7 @@ int cpb200_run_ops(const cpb200_op *ops, int n, void *stream);
 size_t cpb200_sizeof_op(void);
 
 /* Hardware probe (diagnostics only, not on the product path): one smem halo tile serving all nine
- * taps of a 3x3 conv through shifted UMMA descriptors.  x (1,18,10,64) bf16 NHWC, w (9,64,64) bf16
+ * taps of a 3x3 conv through shifted wgmma descriptors.  x (1,18,10,64) bf16 NHWC, w (9,64,64) bf16
  * [tap][cout][cin], out (128,64) fp32 with row = th*8 + tw.  variant 0/1 = descriptor base_offset 0 /
  * (start>>7)&7.  See centerpose_b200/csrc/probe.cu and tools/halo_probe.py. */
 int cpb200_probe_halo(const void *x, const void *w, float *out, int variant, void *stream);

@@ -72,7 +72,7 @@ TC_CASES = [
 
 @pytest.mark.parametrize("cins,cout,k,stride,H,W,res,relu,out", TC_CASES)
 def test_conv_tensor_core_path(cins, cout, k, stride, H, W, res, relu, out):
-    """tcgen05 implicit-GEMM conv vs torch fp32 on the same bf16-rounded inputs/weights.
+    """wgmma implicit-GEMM conv vs torch fp32 on the same bf16-rounded inputs/weights.
     Tolerance: |err| <= 1e-2 * max|ref| (bf16 output rounding 2^-9 + fp32 accumulation order)."""
     B = 3
     g = torch.Generator().manual_seed(sum(cins) * 7 + cout + k + stride)
@@ -224,7 +224,7 @@ def test_dcn_op_matches_oracle(precision, ci, co, H, W):
 
 @pytest.mark.parametrize("ci,co,H,W", [(64, 64, 16, 16), (128, 64, 24, 40), (256, 256, 16, 16), (512, 256, 8, 8), (64, 128, 33, 20)])
 def test_dcn_tensor_core_path(ci, co, H, W):
-    """tcgen05 DCN (gather producers write the swizzled A tile) vs the oracle on bf16-rounded data.
+    """wgmma DCN (gather producers write the swizzled A tile) vs the oracle on bf16-rounded data.
     Offsets are large (gain 1.5: many samples out of bounds).  Tolerance: relative L2 <= 1e-2 and
     |err| <= 3e-2 max|ref| (bf16 A-operand rounding after the fp32 bilinear blend, bf16 output)."""
     from oracle import dcn_ref
@@ -244,7 +244,7 @@ def test_dcn_tensor_core_path(ci, co, H, W):
 
 
 def test_dcn_tensor_core_zero_offset_identity():
-    """DCNv2/test.py:31-66 on the tcgen05 DCN: zero offsets, mask 0.5, identity weights => 2*out == in
+    """DCNv2/test.py:31-66 on the wgmma DCN: zero offsets, mask 0.5, identity weights => 2*out == in
     (exact: 0.5*x is representable in bf16)."""
     B, C, H, W = 2, 64, 24, 16
     x = torch.randint(-8, 9, (B, C, H, W), generator=torch.Generator().manual_seed(0)).float()
@@ -276,7 +276,7 @@ def test_dcn_zero_offset_identity():
 @pytest.mark.parametrize("co,stride,H,W", [(16, 1, 48, 40), (16, 1, 21, 37), (64, 2, 64, 96), (64, 2, 38, 50), (16, 2, 32, 32),
                                            (64, 1, 16, 24)])
 def test_stem_tensor_core_kernel(co, stride, H, W):
-    """csrc/net_stem_tc.cu: 7x7 Cin-3 stem with the im2col built in shared memory + tcgen05, vs torch fp32 on
+    """csrc/net_stem_tc.cu: 7x7 Cin-3 stem with the im2col built in shared memory + wgmma, vs torch fp32 on
     bf16-rounded image and weights (partial tiles, both strides, both output widths)."""
     B = 3
     g = torch.Generator().manual_seed(4)
@@ -295,7 +295,7 @@ def test_stem_tensor_core_kernel(co, stride, H, W):
 
 
 def test_stem_im2col_path():
-    """7x7 stem lowered to im2col-W (32 ch) + 7x1 tcgen05 halo conv vs torch fp32 on bf16-rounded data."""
+    """7x7 stem lowered to im2col-W (32 ch) + 7x1 wgmma halo conv vs torch fp32 on bf16-rounded data."""
     B, H, W = 2, 48, 40
     g = torch.Generator().manual_seed(4)
     x = torch.randn(B, 3, H, W, generator=g).bfloat16().float()
@@ -375,7 +375,7 @@ def test_dla34_forward_vs_oracle_both_precisions():
     ref = torch.cat(dla_ref.forward(sd, x), dim=1)
     got = torch.cat(m(x.to(DEV)), dim=1).cpu()
     _net_close(got.numpy(), ref.numpy())
-    for tc in (False, True):            # bf16 activations: CUDA-core kernels, then tcgen05 kernels
+    for tc in (False, True):            # bf16 activations: CUDA-core kernels, then wgmma kernels
         m.set_precision("bf16", tc=tc)
         got16 = torch.cat(m(x.to(DEV)), dim=1).cpu()
         rel = ((got16 - ref).norm() / ref.norm()).item()
@@ -420,7 +420,7 @@ def test_res50_matches_reference_golden_and_oracle():
 @pytest.mark.parametrize("tag", ["128", "256x320"])
 def test_hrnet_matches_reference_golden_and_oracle(tag):
     """BASELINE config 4 backbone: HRNet-W32 (pose_higher_hrnet.py) + heads.  128x128 drives the lowest-resolution
-    branches (4x4, 8x8) through the CUDA-core fallbacks; 256x320 keeps every conv on the tcgen05 kernels."""
+    branches (4x4, 8x8) through the CUDA-core fallbacks; 256x320 keeps every conv on the wgmma kernels."""
     from oracle import dla_ref
     from oracle.init_recipe import synth_images
     g = np.load(os.path.join(GOLD, f"hrnet32_{tag}.npz"))

@@ -1,5 +1,5 @@
 """GPU parity tests of the split-operand precisions ('fp16x2', 'bf16x2': every value carried as hi + lo 16-bit planes,
-products evaluated as hi*hi + hi*lo + lo*hi on tcgen05 with fp32 accumulation) — the tensor-core path that is meant to
+products evaluated as hi*hi + hi*lo + lo*hi on wgmma with fp32 accumulation) — the tensor-core path that is meant to
 reproduce the reference's fp32 arithmetic (lib/models/model.py:57-59 runs cuDNN fp32 convs and the fp32-only DCNv2,
 DCNv2/src/cuda/dcn_v2_cuda.cu:58).
 
@@ -165,7 +165,7 @@ def test_split_roundtrip_maxpool_upadd_stem(precision):
 @pytest.mark.parametrize("ci,co,H,W,gain", [(64, 64, 16, 16, 1.5), (128, 64, 24, 40, 1.5), (256, 256, 16, 16, 0.3), (512, 256, 8, 8, 0.3),
                                             (64, 128, 33, 20, 1.5)])
 def test_dcn_split(precision, ci, co, H, W, gain):
-    """tcgen05 DCN on split operands (both planes gathered, fp32 blend, sample re-split) vs the float64 oracle.  Offsets
+    """wgmma DCN on split operands (both planes gathered, fp32 blend, sample re-split) vs the float64 oracle.  Offsets
     with gain 1.5 put many samples out of bounds.  The sampling positions come from the split-precision offset conv, so
     the comparison includes its error: tolerance 4x the single-op bound."""
     from oracle import dcn_ref
@@ -187,7 +187,7 @@ def test_dcn_split(precision, ci, co, H, W, gain):
 
 
 def test_dcn_split_zero_offset_identity():
-    """DCNv2/test.py:31-66 on the split tcgen05 DCN: zero offsets, mask 0.5, identity weights => 2*out == in, up to the
+    """DCNv2/test.py:31-66 on the split wgmma DCN: zero offsets, mask 0.5, identity weights => 2*out == in, up to the
     accumulator-bias compensation factor 1 + beta * 36 = 1 + 6e-7 the host folds into acc_scale (plan.rz_compensation);
     exact with CPB200_RZ_COMP=0 (checked too)."""
     B, C, H, W = 2, 64, 24, 16
@@ -331,11 +331,11 @@ def test_split_batch_consistency_and_rebinding():
 
 @pytest.mark.parametrize("precision", ["bf16", "fp16x2", "bf16x2"])
 @pytest.mark.parametrize("B,ci,co,H,W,res", [(5, 64, 256, 64, 64, False),      # head conv shape: two N tiles, streamed weights
-                                              (11, 128, 128, 48, 40, True),     # 165 pixel tiles: odd pair count (ghost tile), partial tiles
+                                              (11, 128, 128, 48, 40, True),     # 165 pixel tiles, partial tiles
                                               (10, 256, 256, 32, 32, True)])    # four K slabs
-def test_conv_cta_pair_path(precision, B, ci, co, H, W, res):
-    """3x3 convs big enough (>= 148 pixel tiles, streamed weights) to take the cta_group::2 kernel: CTA pairs, 256-row
-    MMAs issued by the leader CTA, every weight operand split between the two CTAs (csrc/net_tc3.cu, CG = 2)."""
+def test_conv_streamed_weights_path(precision, B, ci, co, H, W, res):
+    """3x3 convs whose filter bank does not stay resident in shared memory (csrc/net_tc3.cu streams it through a weight
+    ring): several N tiles, several K slabs, partial tiles, more pixel tiles than SMs."""
     g = torch.Generator().manual_seed(B * 7 + ci + co)
     x = torch.randn(B, ci, H, W, generator=g)
     w = torch.randn(co, ci, 3, 3, generator=g) / (ci * 9) ** 0.5
@@ -349,7 +349,6 @@ def test_conv_cta_pair_path(precision, B, ci, co, H, W, res):
         ref = ref + r.double()
     ref = F.relu(ref)
     from centerpose_b200.plan import PlanBuilder
-    os.environ["CPB200_C3_CG2"] = "1"            # read by cpb200_prepare_ops (inside _run)
     pb = PlanBuilder(B, 1, 1, precision, torch.device(DEV))
     if precision == "bf16":
         sx = pb.external(x.permute(0, 2, 3, 1).contiguous().to(DEV, torch.bfloat16))
@@ -357,23 +356,20 @@ def test_conv_cta_pair_path(precision, B, ci, co, H, W, res):
     else:
         sx = pb.external(_nhwc(x)); sr = pb.external(_nhwc(r)) if res else None
     y = pb.conv([sx], w.to(DEV), b.to(DEV), stride=1, pad=1, relu=True, res=sr)
-    try:
-        got = _nchw(_run(pb, y))
-    finally:
-        os.environ.pop("CPB200_C3_CG2", None)
+    got = _nchw(_run(pb, y))
     err = (got - ref).abs().max().item(); scale = ref.abs().max().item()
     tol = 1e-2 if precision == "bf16" else OP_TOL[precision]
     assert err <= tol * scale, (precision, err, scale, err / scale)
 
 
 @pytest.mark.parametrize("precision", ["fp16x2", "bf16"])
-def test_halo_conv_output_rebinding_and_direct_store_epilogue(precision):
-    """The halo conv's TMA-store epilogue encodes a tensor map for the output at prepare time; `dst` is nevertheless read live
-    (include/centerpose_b200.h, cpb200_prepare_ops): re-binding it after the first run must write the new buffer (the map is
-    re-encoded) and leave the old one untouched.  CPB200_C3_TSTORE=0 (direct 32-byte stores) must give the same bits."""
+def test_halo_conv_output_rebinding(precision):
+    """`dst` of a prepared halo conv is read live (include/centerpose_b200.h, cpb200_prepare_ops): re-binding it after the
+    first run must write the new buffer and leave the old one untouched, and a freshly prepared plan must give the same
+    bits."""
     from centerpose_b200.plan import PlanBuilder
     g = torch.Generator().manual_seed(77)
-    B, ci, co, H, W = 2, 64, 128, 24, 40                     # partial tiles in both directions (TMA clips them)
+    B, ci, co, H, W = 2, 64, 128, 24, 40                     # partial tiles in both directions
     x = torch.randn(B, ci, H, W, generator=g)
     w = torch.randn(co, ci, 3, 3, generator=g) / (ci * 9) ** 0.5
     b = torch.randn(co, generator=g)
@@ -403,11 +399,7 @@ def test_halo_conv_output_rebinding_and_direct_store_epilogue(precision):
     assert bool((y.buf == 0x55).all()), "the old output buffer was written after re-binding"
     n_used = raw_first.numel() if precision != "bf16" else B * H * W * co * 2
     assert torch.equal(new[:n_used], raw_first[:n_used])
-    # the direct-store epilogue gives the same bits
-    os.environ["CPB200_C3_TSTORE"] = "0"
-    try:
-        pb2, y2, plan2 = build()
-        plan2.run(st); torch.cuda.synchronize()
-        assert torch.equal(y2.buf[:n_used], raw_first[:n_used])
-    finally:
-        os.environ.pop("CPB200_C3_TSTORE", None)
+    # a second, independently prepared plan gives the same bits
+    pb2, y2, plan2 = build()
+    plan2.run(st); torch.cuda.synchronize()
+    assert torch.equal(y2.buf[:n_used], raw_first[:n_used])

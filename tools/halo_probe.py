@@ -1,4 +1,4 @@
-"""Run the UMMA halo-descriptor probe (see csrc/probe.cu) and report which variant is exact."""
+"""Run the wgmma halo-descriptor probe (see csrc/probe.cu) and report which variant is exact."""
 import ctypes
 import json
 import os

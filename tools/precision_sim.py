@@ -1,7 +1,7 @@
 """CPU emulation of the split-operand tensor-core arithmetic (design aid, not product / not a test).
 
 Runs the oracle's DLA-34 forward with every conv / DCN GEMM replaced by the arithmetic a split-precision
-tcgen05 path would perform — operands decomposed into 16-bit planes, the cross products accumulated in fp32 —
+wgmma path would perform — operands decomposed into 16-bit planes, the cross products accumulated in fp32 —
 and reports the head-map error and the decoded-row agreement against the reference golden (dla34_512.npz).
 
     python tools/precision_sim.py [mode ...]     modes: fp32 bf16 bf16x2 fp16x2 bf16x3

@@ -1,4 +1,4 @@
-"""Hardware characterisation (GPU): how much does the tcgen05 fp32 accumulator's round-toward-zero behaviour shrink a
+"""Hardware characterisation (GPU): how much does the wgmma fp32 accumulator's round-toward-zero behaviour shrink a
 K-long dot product of split operands?  For iid random-sign data the error of the tensor-core result has a component
 proportional to the exact result (a coherent shrink factor) — the part that adds up linearly through a deep network.
 Prints, per K and operand statistics, the projection coefficient  <got - ref, ref> / <ref, ref>  and the residual.

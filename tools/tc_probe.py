@@ -1,4 +1,4 @@
-"""Diagnostic probe of the tcgen05 conv path: integer-valued inputs/weights and fp32 output, so
+"""Diagnostic probe of the wgmma conv path: integer-valued inputs/weights and fp32 output, so
 every result is exactly representable and any mismatch is a real defect (layout, descriptor,
 pipeline).  Each case runs in a subprocess with a timeout so that a hung kernel cannot take the
 whole GPU call down.  Usage: python tools/tc_probe.py [case_index]"""

@@ -33,4 +33,4 @@ for (C, W, H, N, bw, bh, sw, sh, st) in CASES:
     nt = ((W + sw - 1) // sw) * ((H + sh - 1) // sh) * N
     box_bytes = C * 2 * bw * bh
     print(f"TMAPROBE C={C} map={W}x{H} box={bw}x{bh} step={sw}x{sh} stages={st}: rc={rc} {ms*1e3:8.1f} us "
-          f"{nt * box_bytes / ms / 1e6:8.1f} GB/s(box bytes) {ms * 1e6 / (nt / 148):7.1f} ns/box/SM rows/box={bw*bh}")
+          f"{nt * box_bytes / ms / 1e6:8.1f} GB/s(box bytes) {ms * 1e6 / (nt / torch.cuda.get_device_properties(0).multi_processor_count):7.1f} ns/box/SM rows/box={bw*bh}")
