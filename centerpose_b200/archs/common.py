@@ -61,6 +61,24 @@ def bilinear_up(c, f):
     return m
 
 
+def scatter_columns(w: torch.Tensor, slabs) -> torch.Tensor:
+    """Input columns of a conv weight (Co, sum(real), kh, kw) laid out over a channel concatenation that is never
+    materialised: ``slabs`` is a list of ``(Sym, real)`` pairs, each a zero-padded activation (``Sym.C`` channels, the
+    first ``real`` of them live).  Returns (Co, sum(Sym.C), kh, kw) with every slab's columns at its padded offset and
+    zeros in the gaps."""
+    co, ci, kh, kw = w.shape
+    assert ci == sum(r for _, r in slabs), (ci, [(s.C, r) for s, r in slabs])
+    if all(s.C == r for s, r in slabs):
+        return w
+    out = torch.zeros(co, sum(s.C for s, _ in slabs), kh, kw, dtype=w.dtype, device=w.device)
+    src = dst = 0
+    for s, r in slabs:
+        out[:, dst:dst + r] = w[:, src:src + r]
+        src += r
+        dst += s.C
+    return out
+
+
 class StateView:
     """Read access to a (prefix-stripped) state_dict on the target device."""
 

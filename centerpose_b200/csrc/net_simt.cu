@@ -13,6 +13,8 @@
 //                 + dcn_v2_cuda.cu:123-163: sigmoid(mask) * bilinear sample, then the GEMM —
 //                 fused here: the sampled im2col tile lives in shared memory only (the
 //                 reference round-trips a (B, 9C, HW) fp32 `columns` buffer through HBM).
+//   AVGPOOL2      hardnet.py:141 nn.AvgPool2d(2, 2)
+//   RESIZE_BILINEAR  hardnet.py:95-100 F.interpolate(bilinear, align_corners=True)
 #include "common.cuh"
 #include <cuda_fp16.h>
 #include <cstdlib>
@@ -578,6 +580,79 @@ __global__ void __launch_bounds__(256) upsample_add_kernel(PI x, PI skip, PO y,
   }
 }
 
+// ---- 2x2 / stride-2 average pool, floor mode, NHWC   (HarDNet nn.AvgPool2d(2, 2), hardnet.py:141) ----
+// Thread = 4 channels of one output pixel.  The taps are summed in row-major order and scaled by 1/4 (exact), the
+// order of PyTorch's CPU kernel.  Odd trailing rows / columns are never read.
+template <typename T, typename PI = const T *, typename PO = T *>
+__global__ void __launch_bounds__(256) avgpool2_kernel(PI x, PO y, long long total, int H, int W, int C4, int Ho, int Wo) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c4 = (int)(i % C4);
+    long long p = i / C4;
+    const int wo = (int)(p % Wo); p /= Wo;
+    const int ho = (int)(p % Ho);
+    const int b = (int)(p / Ho);
+    const size_t q00 = (((size_t)b * H + 2 * ho) * W + 2 * wo) * C4 + c4, row = (size_t)W * C4;   // in 4-channel groups
+    const float4 a = io_ld4(x + q00 * 4), c = io_ld4(x + (q00 + C4) * 4);
+    const float4 d = io_ld4(x + (q00 + row) * 4), e = io_ld4(x + (q00 + row + C4) * 4);
+    io_st4(y + (size_t)i * 4, make_float4((((a.x + c.x) + d.x) + e.x) * 0.25f, (((a.y + c.y) + d.y) + e.y) * 0.25f,
+                                          (((a.z + c.z) + d.z) + e.z) * 0.25f, (((a.w + c.w) + d.w) + e.w) * 0.25f));
+  }
+}
+
+// ---- bilinear resize, align_corners=True, NHWC   (HarDNet TransitionUp's F.interpolate, hardnet.py:95-100) ----
+// Thread = 4 channels of one output pixel.  Source coordinates and weights follow PyTorch's fp32 arithmetic
+// (scale = (in-1)/(out-1) from the host, src = scale*dst, i1 = i0 + (i0 < in-1), l0 = 1 - l1); the result is the
+// vertical blend of the two horizontal blends.
+template <typename T, typename PI = const T *, typename PO = T *>
+__global__ void __launch_bounds__(256) resize_bilinear_kernel(PI x, PO y, long long total, int H, int W, int C4, int Ho, int Wo,
+                                                              float scale_h, float scale_w) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c4 = (int)(i % C4);
+    long long p = i / C4;
+    const int wo = (int)(p % Wo); p /= Wo;
+    const int ho = (int)(p % Ho);
+    const int b = (int)(p / Ho);
+    const float fy = scale_h * (float)ho, fx = scale_w * (float)wo;
+    const int y0 = (int)fy, x0 = (int)fx;
+    const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
+    const float ly1 = fy - (float)y0, ly0 = 1.f - ly1, lx1 = fx - (float)x0, lx0 = 1.f - lx1;
+    const size_t r0 = ((size_t)b * H + y0) * W, r1 = ((size_t)b * H + y1) * W;
+    const float4 a = io_ld4(x + ((r0 + x0) * C4 + c4) * 4), c = io_ld4(x + ((r0 + x1) * C4 + c4) * 4);
+    const float4 d = io_ld4(x + ((r1 + x0) * C4 + c4) * 4), e = io_ld4(x + ((r1 + x1) * C4 + c4) * 4);
+    io_st4(y + (size_t)i * 4, make_float4(ly0 * (lx0 * a.x + lx1 * c.x) + ly1 * (lx0 * d.x + lx1 * e.x),
+                                          ly0 * (lx0 * a.y + lx1 * c.y) + ly1 * (lx0 * d.y + lx1 * e.y),
+                                          ly0 * (lx0 * a.z + lx1 * c.z) + ly1 * (lx0 * d.z + lx1 * e.z),
+                                          ly0 * (lx0 * a.w + lx1 * c.w) + ly1 * (lx0 * d.w + lx1 * e.w)));
+  }
+}
+
+// CPB200_OP_AVGPOOL2 / CPB200_OP_RESIZE_BILINEAR for every activation dtype: PI / PO are plain pointers (fp32, bf16) or
+// the split-plane handles (bf16x2, fp16x2), so the split formats never leave their planes.
+template <typename T, typename PI, typename PO>
+int launch_resample(const cpb200_op &op, PI x, PO y, cudaStream_t st) {
+  const bool pool = op.type == CPB200_OP_AVGPOOL2;
+  const char *name = pool ? "avgpool2" : "resize_bilinear";
+  const int C = op.cin[0];
+  if (op.nsrc != 1 || C % 4 || op.cout != C || (op.src_pitch[0] != 0 && op.src_pitch[0] != C))
+    return cpb::fail(CPB200_ERR_ARG, "%s: needs one dense input with C %% 4 == 0 and cout == C (nsrc %d, C %d, cout %d, src_pitch %d)",
+                     name, op.nsrc, C, op.cout, op.src_pitch[0]);
+  if (pool && (op.H < 2 || op.W < 2 || op.Ho != op.H / 2 || op.Wo != op.W / 2))
+    return cpb::fail(CPB200_ERR_ARG, "avgpool2: %dx%d -> %dx%d is not a 2x2 / stride-2 floor-mode pool (needs H, W >= 2)",
+                     op.H, op.W, op.Ho, op.Wo);
+  if (!pool && (op.Ho < 1 || op.Wo < 1))
+    return cpb::fail(CPB200_ERR_ARG, "resize_bilinear: output size %dx%d", op.Ho, op.Wo);
+  const long long total = (long long)op.B * op.Ho * op.Wo * (C / 4);
+  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
+  if (pool) {
+    avgpool2_kernel<T, PI, PO><<<grid, 256, 0, st>>>(x, y, total, op.H, op.W, C / 4, op.Ho, op.Wo);
+    return cpb::check_launch("avgpool2_kernel");
+  }
+  const float sh = op.Ho > 1 ? (float)(op.H - 1) / (float)(op.Ho - 1) : 0.f;
+  const float sw = op.Wo > 1 ? (float)(op.W - 1) / (float)(op.Wo - 1) : 0.f;
+  resize_bilinear_kernel<T, PI, PO><<<grid, 256, 0, st>>>(x, y, total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, sw);
+  return cpb::check_launch("resize_bilinear_kernel");
+}
+
 // ---- depthwise k x k conv (stride s, pad k/2) + bias + activation, NHWC   (mobilenetv3.py:124-127 conv2/bn2) ----
 // y[b,ho,wo,c] = act(bias[c] + sum_{r,q} x[b, ho*s-p+r, wo*s-p+q, c] * w[r,q,c]).  Thread = VEC channels of one
 // output pixel (VEC * sizeof(T) = 16 bytes); consecutive threads walk the channels of a pixel, so every tap is
@@ -1014,6 +1089,12 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
           total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, op.flags & CPB_ACT_MASK);
       return cpb::check_launch("upsample_add_kernel");
     }
+    case CPB200_OP_AVGPOOL2:
+    case CPB200_OP_RESIZE_BILINEAR: {
+      const int C = op.cin[0];
+      return launch_resample<float, SpC, SpM>(op, SpC{static_cast<const uint16_t *>(op.src[0]), (size_t)op.B * op.H * op.W * C, fmt},
+                                              SpM{static_cast<uint16_t *>(op.dst), (size_t)op.B * op.Ho * op.Wo * C, fmt}, st);
+    }
     default:
       return cpb::fail(CPB200_ERR_ARG, "op type %d has no split-precision kernel (the host must route it through fp32)", op.type);
   }
@@ -1178,6 +1259,9 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
           static_cast<T *>(op.dst), total, op.H, op.W, op.cin[0] / 4, op.Ho, op.Wo, sh, op.flags & CPB_ACT_MASK);
       return cpb::check_launch("upsample_add_kernel");
     }
+    case CPB200_OP_AVGPOOL2:
+    case CPB200_OP_RESIZE_BILINEAR:
+      return launch_resample<T, const T *, T *>(op, static_cast<const T *>(op.src[0]), static_cast<T *>(op.dst), st);
     default: return cpb::fail(CPB200_ERR_ARG, "unknown op type %d", op.type);
   }
 }

@@ -15,7 +15,7 @@ import torch
 from torch import nn
 
 from .archs import dla as _dla
-from .archs.common import StateView, attach, conv
+from .archs.common import StateView, attach, conv, scatter_columns
 from .plan import PlanBuilder
 
 HEADS = (("hm", 1), ("wh", 2), ("hps", 34), ("reg", 2), ("hm_hp", 17), ("hp_offset", 2))
@@ -36,12 +36,18 @@ def _hrnet_arch():
     return _hr
 
 
+def _hardnet_arch():
+    from .archs import hardnet as _hd
+    return _hd
+
+
 _backbone_factory = {
     # arch name -> (module with build_params(cfg)/lower(), feature channels or None = ask the module)   model.py:24-38
     "dla": lambda n: (_dla, 64) if n == 34 else None,
     "res": lambda n: (_res_arch(), 256) if n == 50 else None,
     "hrnet": lambda n: (_hrnet_arch(), None),
     "mobilenetv3": lambda n: (_mobilenet_arch(), 24),
+    "hardnet": lambda n: (_hardnet_arch(), 48) if n == 0 else None,
 }
 
 
@@ -70,7 +76,7 @@ class BackBoneWithHead(nn.Module):
         arch_name = arch[:arch.find("_")] if "_" in arch else arch
         if arch_name not in _backbone_factory or _backbone_factory[arch_name](num_layers) is None:
             raise KeyError(f"centerpose_b200: backbone {arch!r} is not implemented "
-                           f"(available: dla_34, res_50, hrnet, mobilenetv3)")
+                           f"(available: dla_34, res_50, hrnet, mobilenetv3, hardnet)")
         self._arch_mod, feat_c = _backbone_factory[arch_name](num_layers)
         if feat_c is None:
             feat_c = self._arch_mod.feature_channels(cfg)
@@ -131,9 +137,16 @@ class BackBoneWithHead(nn.Module):
             x = pb.input(3)
             feat = self._arch_mod.lower(pb, StateView(sd, "backbone_model.", host), x)
             P = StateView(sd, "head_model.", host)
+            # lower() returns one activation, or a list of (activation, real channels) slabs standing for their channel
+            # concatenation (archs/hardnet.py): the head's 3x3 convs then take the slabs as their inputs
+            slabs = list(feat) if isinstance(feat, (list, tuple)) else None
+            srcs = [s for s, _ in slabs] if slabs is not None else [feat]
+            fmap = srcs[0]
 
             def w0_of(name):
                 w0 = P(f"{name}.0.weight").float()
+                if slabs is not None:
+                    return scatter_columns(w0, slabs)
                 if feat.C > w0.shape[1]:                 # backbone carries zero-padded channels (archs/mobilenet.py)
                     w0 = torch.nn.functional.pad(w0, (0, 0, 0, 0, 0, feat.C - w0.shape[1]))
                 return w0
@@ -146,17 +159,17 @@ class BackBoneWithHead(nn.Module):
                 # six times.
                 w_cat = torch.cat([w0_of(name) for name, _ in HEADS], dim=0)
                 b_cat = torch.cat([P(f"{name}.0.bias").float() for name, _ in HEADS], dim=0)
-                hid = pb.conv([feat], w_cat, b_cat, stride=1, pad=1, relu=True)
+                hid = pb.conv(srcs, w_cat, b_cat, stride=1, pad=1, relu=True)
             for i, (name, c) in enumerate(HEADS):
-                dst = pb.output(c, feat.H, feat.W, name)
+                dst = pb.output(c, fmap.H, fmap.W, name)
                 if fuse:
                     t = pb.channel_slice(hid, i * hc, hc)
                 else:
-                    t = pb.conv([feat], w0_of(name), P(f"{name}.0.bias").float(), stride=1, pad=1, relu=True)
+                    t = pb.conv(srcs, w0_of(name), P(f"{name}.0.bias").float(), stride=1, pad=1, relu=True)
                 pb.conv([t], P(f"{name}.2.weight").float(), P(f"{name}.2.bias").float(),
                         stride=1, pad=0, relu=False, out="nchw", dst=dst)
             plan = pb.build()
-            plan.out_shape = (feat.H, feat.W)
+            plan.out_shape = (fmap.H, fmap.W)
             if len(self._plans) > 8:
                 self._plans.clear()
             self._plans[key] = plan

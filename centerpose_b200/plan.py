@@ -26,6 +26,7 @@ from . import _lib
 
 OP_CONV, OP_STEM, OP_MAXPOOL, OP_DWDECONV_ADD, OP_DCN, OP_IM2COL_W, OP_UPSAMPLE_ADD = 1, 2, 3, 4, 5, 6, 7
 OP_DWCONV, OP_AVGPOOL, OP_SCALE_ADD, OP_CONVERT, OP_S2D = 8, 9, 10, 11, 12
+OP_AVGPOOL2, OP_RESIZE_BILINEAR = 13, 14
 FLAG_RELU, FLAG_OUT_NCHW_F32, FLAG_OUT_F32, FLAG_TC, FLAG_HSWISH, FLAG_HSIGMOID, FLAG_TO_F32 = 1, 2, 4, 8, 16, 32, 64
 _ACT_FLAG = {None: 0, "relu": FLAG_RELU, "hswish": FLAG_HSWISH, "hsigmoid": FLAG_HSIGMOID}
 F32, BF16, BF16X2, F16X2 = 0, 1, 2, 3
@@ -550,6 +551,24 @@ class PlanBuilder:
             self._emit(op, [x], y, [skip])
             return y
         return self._f32_op(op, [x], x.C, x.H * f, x.W * f, [skip])
+
+    def avgpool2(self, x: Sym):
+        """2x2 / stride-2 average pool, floor mode   (hardnet.py:141 nn.AvgPool2d(2, 2))."""
+        op = _PendingOp(type=OP_AVGPOOL2, flags=0, k=(2, 2), stride=2, pad=(0, 0), weight=None, bias=None, cout=x.C)
+        if self._native_split(x):
+            y = self._sym(x.C, x.H // 2, x.W // 2, "act")
+            self._emit(op, [x], y)
+            return y
+        return self._f32_op(op, [x], x.C, x.H // 2, x.W // 2)
+
+    def resize_bilinear(self, x: Sym, Ho: int, Wo: int):
+        """bilinear resize to (Ho, Wo) with align_corners=True   (hardnet.py:95-100, TransitionUp)."""
+        op = _PendingOp(type=OP_RESIZE_BILINEAR, flags=0, k=(1, 1), stride=1, pad=(0, 0), weight=None, bias=None, cout=x.C)
+        if self._native_split(x):
+            y = self._sym(x.C, Ho, Wo, "act")
+            self._emit(op, [x], y)
+            return y
+        return self._f32_op(op, [x], x.C, Ho, Wo)
 
     def dcn(self, x: Sym, w, b, om_w, om_b, relu=True):
         """DCN module (dcn_v2.py:117-127) with BN already folded into (w, b)."""

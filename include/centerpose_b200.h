@@ -161,11 +161,19 @@ enum cpb200_op_type {
   CPB200_OP_CONVERT = 11,    /* NHWC activation (B,H,W,cin[0]) between fp32 and the split 16-bit pair layout named by
                                 act_dtype (CPB200_BF16X2 / CPB200_F16X2): fp32 -> planes, or planes -> fp32 with
                                 CPB200_FLAG_TO_F32.  Lets ops without a native split kernel run on fp32 in between.   */
-  CPB200_OP_S2D = 12         /* space-to-depth of the network input for stride-2 stems in split precisions: NCHW fp32
+  CPB200_OP_S2D = 12,        /* space-to-depth of the network input for stride-2 stems in split precisions: NCHW fp32
                                 (B,3,H,W) (H, W even) -> split NHWC planes (B,H/2,W/2,16), channel (py*2+px)*3 + c =
                                 x[c][2h+py][2w+px], channels 12..15 zero.  A k x k / stride-2 / pad k/2 stem
                                 (msra_resnet.py:116-117 7x7, pose_higher_hrnet.py:283-284 3x3) is then a stride-1
                                 (k+1)/2+1-tap conv over 16 channels on the tensor-core path; src[0] is read live.   */
+  CPB200_OP_AVGPOOL2 = 13,   /* 2x2 / stride-2 average pool, NHWC, floor mode, no padding: (B,H,W,C) -> (B,H/2,W/2,C)
+                                with Ho == H/2, Wo == W/2, H, W >= 2, C % 4 == 0, one dense input
+                                (HarDNet nn.AvgPool2d(2, 2), hardnet.py:141).  All four activation dtypes.          */
+  CPB200_OP_RESIZE_BILINEAR = 14 /* bilinear resize with align_corners=True, NHWC: (B,H,W,C) -> (B,Ho,Wo,C), Ho, Wo >= 1,
+                                C % 4 == 0, one dense input (HarDNet TransitionUp, hardnet.py:95-100).  PyTorch's
+                                arithmetic in fp32: scale = (in-1)/(out-1) (0 when out == 1), src = scale*dst,
+                                i0 = (int)src, i1 = i0 + (i0 < in-1), l1 = src - i0, l0 = 1 - l1; the vertical blend
+                                of the two horizontal blends.  All four activation dtypes.                          */
 };
 /* A dense ConvTranspose2d(k4,s2,p1) (msra_resnet.py:168-193) is lowered by the host into four
  * 2x2 CONV ops, one per output parity, using pad_h/pad_w and the strided-output fields below. */
