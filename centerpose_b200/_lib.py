@@ -44,9 +44,16 @@ def lib() -> ctypes.CDLL:
     L.cpb200_pre_process.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_double), ctypes.c_void_p,
                                      ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
                                      ctypes.c_int, ctypes.c_void_p]
+    L.cpb200_pre_process_batch.restype = ctypes.c_int
+    L.cpb200_pre_process_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                           ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
+                                           ctypes.c_int, ctypes.c_void_p]
     L.cpb200_soft_nms_39.restype = ctypes.c_int
     L.cpb200_soft_nms_39.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                      ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+    L.cpb200_soft_nms_39_batch.restype = ctypes.c_int
+    L.cpb200_soft_nms_39_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
+                                           ctypes.c_float, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
     _lib = L
     return L
 

@@ -1,7 +1,8 @@
 // Device versions of two host-side steps around the decode (SURVEY.md §8 "next" rows 2 and 3):
 //   cpb200_flip_merge   flip-test averaging of the head maps  (lib/detectors/multi_pose.py:45-53 with
 //                       flip_tensor / flip_lr / flip_lr_off of lib/models/utils.py:27-47) in ONE pass,
-//   cpb200_soft_nms_39  the pose soft-NMS of lib/external/nms.pyx:172-275 on a device array.
+//   cpb200_soft_nms_39  the pose soft-NMS of lib/external/nms.pyx:172-275 on a device array (_batch: one CTA per image),
+// and the warp / normalise part of pre_process (cpb200_pre_process, _batch: one launch for many images).
 #include "common.cuh"
 
 namespace {
@@ -49,8 +50,10 @@ __global__ void __launch_bounds__(256) flip_merge_kernel(const FlipArgs a) {
 constexpr int NMS_T = 128;
 constexpr int NMS_COLS = 56, NMS_MOVE = 39;
 
+// One CTA per image: CTA b works on the (N0, 56) rows at boxes + b * N0 * 56 and writes keep_count[b].
 __global__ void __launch_bounds__(NMS_T) soft_nms_kernel(float *boxes, int N0, float sigma, float Nt, float threshold, int method,
                                                          int *keep_count) {
+  boxes += (size_t)blockIdx.x * N0 * NMS_COLS;
   extern __shared__ float sb[];                       // N0 x 56, then N0 pre-decay scores
   float *s_orig = sb + N0 * NMS_COLS;
   float *s_hit = s_orig + N0;                         // 1.0 when the row overlapped box i in this step (only those are
@@ -142,7 +145,23 @@ __global__ void __launch_bounds__(NMS_T) soft_nms_kernel(float *boxes, int N0, f
     __syncthreads();
   }
   for (int i = tid; i < N0 * NMS_COLS; i += NMS_T) boxes[i] = sb[i];
-  if (tid == 0 && keep_count) *keep_count = s_n;
+  if (tid == 0 && keep_count) keep_count[blockIdx.x] = s_n;
+}
+
+int soft_nms_launch(float *boxes, int B, int N, float sigma, float Nt, float threshold, int method, int *keep_counts,
+                    void *stream, const char *what) {
+  if (B < 0 || N < 0 || (!boxes && B > 0 && N > 0)) return cpb::fail(CPB200_ERR_ARG, "%s: bad arguments", what);
+  if (B == 0) return CPB200_OK;
+  if (N == 0) {
+    if (keep_counts) CPB_CUDA(cudaMemsetAsync(keep_counts, 0, (size_t)B * sizeof(int), static_cast<cudaStream_t>(stream)));
+    return CPB200_OK;
+  }
+  if (B > 65535) return cpb::fail(CPB200_ERR_ARG, "%s: B = %d images exceed one launch (max 65535)", what, B);
+  const size_t smem = (size_t)N * (NMS_COLS + 2) * sizeof(float);
+  if (smem > 200 * 1024) return cpb::fail(CPB200_ERR_ARG, "%s: N = %d rows do not fit shared memory (max 882)", what, N);
+  if (smem > 48 * 1024) CPB_CUDA(cudaFuncSetAttribute(soft_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  soft_nms_kernel<<<B, NMS_T, smem, static_cast<cudaStream_t>(stream)>>>(boxes, N, sigma, Nt, threshold, method, keep_counts);
+  return cpb::check_launch("soft_nms_kernel");
 }
 
 }  // namespace
@@ -168,16 +187,12 @@ extern "C" int cpb200_flip_merge(const float *hm, const float *wh, const float *
 
 extern "C" int cpb200_soft_nms_39(float *boxes, int N, float sigma, float Nt, float threshold, int method, int *keep_count,
                                   void *stream) {
-  if (N < 0 || (!boxes && N > 0)) return cpb::fail(CPB200_ERR_ARG, "soft_nms_39: bad arguments");
-  if (N == 0) {
-    if (keep_count) CPB_CUDA(cudaMemsetAsync(keep_count, 0, sizeof(int), static_cast<cudaStream_t>(stream)));
-    return CPB200_OK;
-  }
-  const size_t smem = (size_t)N * (NMS_COLS + 2) * sizeof(float);
-  if (smem > 200 * 1024) return cpb::fail(CPB200_ERR_ARG, "soft_nms_39: N = %d rows do not fit shared memory (max 882)", N);
-  if (smem > 48 * 1024) CPB_CUDA(cudaFuncSetAttribute(soft_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  soft_nms_kernel<<<1, NMS_T, smem, static_cast<cudaStream_t>(stream)>>>(boxes, N, sigma, Nt, threshold, method, keep_count);
-  return cpb::check_launch("soft_nms_kernel");
+  return soft_nms_launch(boxes, 1, N, sigma, Nt, threshold, method, keep_count, stream, "soft_nms_39");
+}
+
+extern "C" int cpb200_soft_nms_39_batch(float *boxes, int B, int N, float sigma, float Nt, float threshold, int method,
+                                        int *keep_counts, void *stream) {
+  return soft_nms_launch(boxes, B, N, sigma, Nt, threshold, method, keep_counts, stream, "soft_nms_39_batch");
 }
 
 // ---- device pre_process: warpAffine (bilinear, constant-0 border) + normalise + HWC->CHW (+ mirrored copy) ----
@@ -189,39 +204,71 @@ extern "C" int cpb200_soft_nms_39(float *boxes, int N, float sigma, float Nt, fl
 // evaluated in double and rounded to float like numpy does for `(inp / 255. - mean) / std`.astype(float32).
 namespace {
 
+static_assert(sizeof(cpb200_pre_image) == 64, "cpb200_pre_image layout is part of the C ABI");
+
 struct PreArgs {
-  const unsigned char *img;   // (h, w, 3) uint8
-  float *out;                 // (1 or 2, 3, OH, OW) fp32
-  int h, w, OH, OW, flip;
-  double m[6];                // inverse map (dst -> src), as computed by cv2
+  const unsigned char *imgs;       // packed (h, w, 3) uint8 images
+  const cpb200_pre_image *table;   // B entries on the device, or NULL: `one` describes the only image
+  cpb200_pre_image one;
+  float *out;                      // (B or 2B, 3, OH, OW) fp32
+  int OH, OW, flip;
   float mean[3], stdv[3];
 };
 
+// grid (pixel blocks, image): blockIdx.y selects the image, its forward matrix is inverted by every thread
 __global__ void __launch_bounds__(256) pre_process_kernel(const PreArgs a) {
+  const int b = blockIdx.y;
+  long long off; int h, w; double t[6];
+  if (a.table) {
+    const cpb200_pre_image *p = a.table + b;
+    off = p->offset; h = p->h; w = p->w;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) t[k] = p->trans_input[k];
+  } else {
+    off = a.one.offset; h = a.one.h; w = a.one.w;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) t[k] = a.one.trans_input[k];
+  }
+  // cv2::warpAffine without WARP_INVERSE_MAP inverts the matrix like this (imgwarp.cpp), in double on the host; the
+  // explicit round-to-nearest operations keep nvcc from contracting them into FMAs, so the inverse is the host's bit for bit
+  double D = __dsub_rn(__dmul_rn(t[0], t[4]), __dmul_rn(t[1], t[3]));
+  D = D != 0 ? __ddiv_rn(1.0, D) : 0;
+  const double m0 = __dmul_rn(t[4], D), m4 = __dmul_rn(t[0], D), m1 = __dmul_rn(t[1], -D), m3 = __dmul_rn(t[3], -D);
+  const double m2 = __dsub_rn(__dmul_rn(-m0, t[2]), __dmul_rn(m1, t[5]));
+  const double m5 = __dsub_rn(__dmul_rn(-m3, t[2]), __dmul_rn(m4, t[5]));
+  const unsigned char *img = a.imgs + off;
+  float *out = a.out + (size_t)(a.flip ? 2 * b : b) * 3 * a.OH * a.OW;
   const int total = a.OH * a.OW;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int x = i % a.OW, y = i / a.OW;
-    const long long adelta = llrint(a.m[0] * (double)x * 1024.0), bdelta = llrint(a.m[3] * (double)x * 1024.0);
-    const long long X0 = llrint((a.m[1] * (double)y + a.m[2]) * 1024.0) + 16, Y0 = llrint((a.m[4] * (double)y + a.m[5]) * 1024.0) + 16;
+    const long long adelta = llrint(m0 * (double)x * 1024.0), bdelta = llrint(m3 * (double)x * 1024.0);
+    const long long X0 = llrint((m1 * (double)y + m2) * 1024.0) + 16, Y0 = llrint((m4 * (double)y + m5) * 1024.0) + 16;
     const long long X = (X0 + adelta) >> 5, Y = (Y0 + bdelta) >> 5;
     long long sxl = X >> 5, syl = Y >> 5;
     sxl = sxl < -32768 ? -32768 : (sxl > 32767 ? 32767 : sxl);       // saturate_cast<short>
     syl = syl < -32768 ? -32768 : (syl > 32767 ? 32767 : syl);
     const int sx = (int)sxl, sy = (int)syl, fx = (int)(X & 31), fy = (int)(Y & 31);
     const int w0 = (32 - fx) * (32 - fy) * 32, w1 = fx * (32 - fy) * 32, w2 = (32 - fx) * fy * 32, w3 = fx * fy * 32;
-    const bool y0 = sy >= 0 && sy < a.h, y1 = sy + 1 >= 0 && sy + 1 < a.h, x0 = sx >= 0 && sx < a.w, x1 = sx + 1 >= 0 && sx + 1 < a.w;
-    const unsigned char *p00 = a.img + ((size_t)sy * a.w + sx) * 3;
+    const bool y0 = sy >= 0 && sy < h, y1 = sy + 1 >= 0 && sy + 1 < h, x0 = sx >= 0 && sx < w, x1 = sx + 1 >= 0 && sx + 1 < w;
+    const unsigned char *p00 = img + ((long long)sy * w + sx) * 3;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const int v00 = (y0 && x0) ? p00[c] : 0, v01 = (y0 && x1) ? p00[3 + c] : 0;
-      const int v10 = (y1 && x0) ? p00[(size_t)a.w * 3 + c] : 0, v11 = (y1 && x1) ? p00[(size_t)a.w * 3 + 3 + c] : 0;
+      const int v10 = (y1 && x0) ? p00[(size_t)w * 3 + c] : 0, v11 = (y1 && x1) ? p00[(size_t)w * 3 + 3 + c] : 0;
       int u = (v00 * w0 + v01 * w1 + v10 * w2 + v11 * w3 + (1 << 14)) >> 15;
       u = u < 0 ? 0 : (u > 255 ? 255 : u);
       const float f = (float)(((double)u / 255.0 - (double)a.mean[c]) / (double)a.stdv[c]);
-      a.out[((size_t)c * a.OH + y) * a.OW + x] = f;
-      if (a.flip) a.out[((size_t)(3 + c) * a.OH + y) * a.OW + (a.OW - 1 - x)] = f;
+      out[((size_t)c * a.OH + y) * a.OW + x] = f;
+      if (a.flip) out[((size_t)(3 + c) * a.OH + y) * a.OW + (a.OW - 1 - x)] = f;
     }
   }
+}
+
+int pre_process_launch(PreArgs &a, int B, const float *mean, const float *stdv, void *stream) {
+  for (int c = 0; c < 3; ++c) { a.mean[c] = mean[c]; a.stdv[c] = stdv[c]; }
+  const dim3 grid((unsigned)((a.OH * a.OW + 255) / 256), (unsigned)B);
+  pre_process_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  return cpb::check_launch("pre_process_kernel");
 }
 
 }  // namespace
@@ -230,20 +277,20 @@ extern "C" int cpb200_pre_process(const unsigned char *img, int h, int w, const 
                                   const float *mean, const float *stdv, int flip, void *stream) {
   if (!img || !trans_input || !out || !mean || !stdv || h <= 0 || w <= 0 || out_h <= 0 || out_w <= 0)
     return cpb::fail(CPB200_ERR_ARG, "pre_process: bad arguments");
-  PreArgs a;
-  a.img = img; a.out = out; a.h = h; a.w = w; a.OH = out_h; a.OW = out_w; a.flip = flip ? 1 : 0;
-  // cv2::warpAffine without WARP_INVERSE_MAP inverts the matrix like this (imgwarp.cpp)
-  double M[6];
-  for (int i = 0; i < 6; ++i) M[i] = trans_input[i];
-  double D = M[0] * M[4] - M[1] * M[3];
-  D = D != 0 ? 1. / D : 0;
-  const double A11 = M[4] * D, A22 = M[0] * D;
-  M[0] = A11; M[1] *= -D; M[3] *= -D; M[4] = A22;
-  const double b1 = -M[0] * M[2] - M[1] * M[5], b2 = -M[3] * M[2] - M[4] * M[5];
-  M[2] = b1; M[5] = b2;
-  for (int i = 0; i < 6; ++i) a.m[i] = M[i];
-  for (int c = 0; c < 3; ++c) { a.mean[c] = mean[c]; a.stdv[c] = stdv[c]; }
-  const int total = out_h * out_w;
-  pre_process_kernel<<<(total + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
-  return cpb::check_launch("pre_process_kernel");
+  PreArgs a = {};
+  a.imgs = img; a.table = nullptr; a.out = out; a.OH = out_h; a.OW = out_w; a.flip = flip ? 1 : 0;
+  a.one.offset = 0; a.one.h = h; a.one.w = w;
+  for (int i = 0; i < 6; ++i) a.one.trans_input[i] = trans_input[i];
+  return pre_process_launch(a, 1, mean, stdv, stream);
+}
+
+extern "C" int cpb200_pre_process_batch(const unsigned char *imgs, const cpb200_pre_image *table, int B, float *out, int out_h,
+                                        int out_w, const float *mean, const float *stdv, int flip, void *stream) {
+  if (!imgs || !table || !out || !mean || !stdv || B <= 0 || out_h <= 0 || out_w <= 0)
+    return cpb::fail(CPB200_ERR_ARG, "pre_process_batch: bad arguments");
+  if (B > 65535) return cpb::fail(CPB200_ERR_ARG, "pre_process_batch: B = %d images exceed one launch (max 65535)", B);
+  if ((long long)out_h * out_w > (1LL << 30)) return cpb::fail(CPB200_ERR_ARG, "pre_process_batch: output too large");
+  PreArgs a = {};
+  a.imgs = imgs; a.table = table; a.out = out; a.OH = out_h; a.OW = out_w; a.flip = flip ? 1 : 0;
+  return pre_process_launch(a, B, mean, stdv, stream);
 }

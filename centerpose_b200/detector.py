@@ -9,7 +9,9 @@ Differences that are additive only:
     sigmoid'ed ``hm`` / ``hm_hp`` like the reference's in-place ``sigmoid_``;
   * flip-test averaging (``multi_pose.py:45-53``) is done on the device — the reference's
     ``flip_lr`` / ``flip_lr_off`` round-trip through numpy (``lib/models/utils.py:30-47``);
-  * ``run_batch`` (new): many pre-processed images per call — the reference API is single-image.
+  * ``run_batch`` (new): many pre-processed images per call — the reference API is single-image;
+  * ``run_images`` (new): ``run()`` for a list of raw images, batched on the device, with the reference's
+    test-time flip / multi-scale / soft-NMS settings.
 """
 from __future__ import annotations
 
@@ -19,7 +21,7 @@ import cv2
 import numpy as np
 import torch
 
-from .decode import flip_merge, multi_pose_decode, sigmoid_
+from .decode import affine_for_meta, flip_merge, multi_pose_decode, sigmoid_
 from .image import get_affine_transform, multi_pose_post_process
 from .model import create_model, load_model
 from .soft_nms import soft_nms_39, soft_nms_39_cuda
@@ -54,10 +56,9 @@ class BaseDetector(object):
         # additive: cfg.B200.DEVICE_PREPROCESS (default on) — warp / normalise / transpose on the GPU (same values)
         self.device_preprocess = bool((b200 or {}).get("DEVICE_PREPROCESS", True)) if isinstance(b200, dict) else True
 
-    def pre_process(self, image, scale, meta=None):
-        """base_detector.py:32-62 — resize, centre-crop affine warp to the network input, normalise,
-        HWC->CHW, optional mirrored copy; returns the (1 or 2,3,H,W) tensor and the c/s/out-size meta."""
-        height, width = image.shape[0:2]
+    def _pre_process_geometry(self, height, width, scale):
+        """base_detector.py:33-47,59-61 — the resized size, network input size, forward ``trans_input`` and the
+        c/s/out-size meta of an image of (height, width) at one test scale."""
         new_height, new_width = int(height * scale), int(width * scale)
         if self.cfg.TEST.FIX_RES:
             inp_height, inp_width = self.cfg.MODEL.INPUT_H, self.cfg.MODEL.INPUT_W
@@ -71,6 +72,13 @@ class BaseDetector(object):
         trans_input = get_affine_transform(c, s, 0, [inp_width, inp_height])
         meta = {"c": c, "s": s, "out_height": inp_height // self.cfg.MODEL.DOWN_RATIO,
                 "out_width": inp_width // self.cfg.MODEL.DOWN_RATIO}
+        return new_height, new_width, inp_height, inp_width, trans_input, meta
+
+    def pre_process(self, image, scale, meta=None):
+        """base_detector.py:32-62 — resize, centre-crop affine warp to the network input, normalise,
+        HWC->CHW, optional mirrored copy; returns the (1 or 2,3,H,W) tensor and the c/s/out-size meta."""
+        height, width = image.shape[0:2]
+        new_height, new_width, inp_height, inp_width, trans_input, meta = self._pre_process_geometry(height, width, scale)
         if self.device_preprocess and image.dtype == np.uint8 and image.ndim == 3 and image.shape[2] == 3:
             # warp + normalise + HWC->CHW (+ mirrored copy) in one CUDA kernel, bit-exact with the cv2 / numpy lines
             # below (csrc/post.cu); a scale != 1 keeps cv2.resize on the host, as in the reference
@@ -167,6 +175,23 @@ class BaseDetector(object):
         out = {"results": {1: results}}
         out.update(clock)
         return out
+
+
+def group_by_shape(keys, max_batch):
+    """``keys[i]`` is the (scale index, input H, input W) of work item i.  Returns ``[(key, [item indices])]``: items
+    with equal keys in input order, split into runs of at most ``max_batch``; groups are ordered by each key's first
+    item.  Every item appears exactly once, so its results can be put back at its input position."""
+    if int(max_batch) < 1:
+        raise ValueError("max_batch must be >= 1, got %r" % (max_batch,))
+    by_key = {}
+    for i, k in enumerate(keys):
+        by_key.setdefault(tuple(k), []).append(i)
+    return [(k, idx[j:j + int(max_batch)]) for k, idx in by_key.items() for j in range(0, len(idx), int(max_batch))]
+
+
+# one entry of cpb200_pre_process_batch's device table (struct cpb200_pre_image, include/centerpose_b200.h)
+_PRE_IMAGE = np.dtype([("offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("trans_input", "<f8", (6,))])
+assert _PRE_IMAGE.itemsize == 64
 
 
 def _swap_pairs(C, pairs, device):
@@ -323,19 +348,101 @@ class MultiPoseDetector(BaseDetector):
     @torch.no_grad()
     def run_multiscale_fused(self, image):
         """Additive: the multi-scale test of ``run()`` (base_detector.py:99-127 with ``TEST_SCALES [1, 2]``-style
-        configs, experiments/hrnet_w32_512.yaml:142) kept on the device end to end: per scale pre_process -> network ->
-        decode with the back-projection fused, then ONE soft-NMS kernel over the concatenated rows.  Returns the merged
-        ``(N, 56)`` rows (numpy) in original-image pixels, like ``run()['results'][1]``."""
-        from .decode import affine_for_meta
-        per_scale = []
-        for scale in self.scales:
-            images, meta = self.pre_process(image, scale, None)
-            images = images.to(torch.device("cuda"), non_blocking=True)
-            if self.cfg.TEST.FLIP_TEST:
-                raise NotImplementedError("run_multiscale_fused: use run() for FLIP_TEST")
-            aff = affine_for_meta([meta], scale).to(images.device, non_blocking=True)
-            per_scale.append(self._decode_heads(self.model(images), affine=aff)[0])
-        return self.merge_outputs_device(per_scale).cpu().numpy()
+        configs, experiments/hrnet_w32_512.yaml:142) kept on the device end to end; ``run_images([image])[0]``.
+        Returns the merged ``(N, 56)`` rows (numpy) in original-image pixels, like ``run()['results'][1]``."""
+        return self.run_images([image])[0]
+
+    @torch.no_grad()
+    def run_images(self, images, max_batch=32):
+        """Additive: ``run()`` for many images at once, with the reference's test-time settings (``FLIP_TEST``,
+        ``TEST_SCALES``, ``FIX_RES``, ``NMS``; what tools/evaluate.py runs).  ``images`` is a list of BGR uint8 HWC
+        arrays or image paths.  Returns one float32 ``(N_i, 56)`` array per image, in input order, equal to
+        ``run(image)['results'][1]``: all rows, suppressed ones at the tail, as the reference's ``merge_outputs``.
+
+        Per test scale every image gets ``pre_process``'s geometry (a scale != 1 keeps ``cv2.resize`` on the host).
+        Images with the same (scale, input size) are batched, at most ``max_batch`` per forward (2x that many
+        network images with ``FLIP_TEST``): one pinned upload, one ``cpb200_pre_process_batch``, the forward, the
+        flip merge and the decode with the back-projection fused.  The per-scale rows are then concatenated per image
+        and, with ``TEST.NMS`` or several scales, go through one ``cpb200_soft_nms_39_batch`` for all images.  The
+        only host wait is the final device-to-host copy."""
+        import ctypes
+        from . import _lib
+        from .soft_nms import soft_nms_39_cuda_batch
+        if int(max_batch) < 1:
+            raise ValueError("run_images: max_batch must be >= 1, got %r" % (max_batch,))
+        loaded = []
+        for n, src in enumerate(images):
+            if not isinstance(src, (np.ndarray, str)):
+                raise ValueError("run_images: image %d is a %s, expected a BGR uint8 HWC array or a path"
+                                 % (n, type(src).__name__))
+            image = self._load(src)[0]
+            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+                raise ValueError("run_images: image %d must be uint8 (H, W, 3), got %s %s" % (n, image.dtype, image.shape))
+            loaded.append(image)
+        if not loaded:
+            return []
+        cfg = self.cfg
+        dev = torch.device("cuda")
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        flip = bool(cfg.TEST.FLIP_TEST)
+        K, S = int(cfg.TEST.TOPK), len(self.scales)
+        mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
+        std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
+        items, keys = [], []                     # one item per (image, scale)
+        for i, image in enumerate(loaded):
+            height, width = image.shape[0:2]
+            for si, scale in enumerate(self.scales):
+                new_h, new_w, inp_h, inp_w, trans_input, meta = self._pre_process_geometry(height, width, scale)
+                resized = image if (new_w, new_h) == (width, height) else cv2.resize(image, (new_w, new_h))
+                items.append((i, np.ascontiguousarray(resized), trans_input, meta))
+                keys.append((si, inp_h, inp_w))
+        rows = torch.empty((len(loaded), S * K, 56), dtype=torch.float32, device=dev)
+        for (si, inp_h, inp_w), idx in group_by_shape(keys, max_batch):
+            B = len(idx)
+            # one pinned buffer, one upload: [table (B x 64 B) | affine (B x 6 fp32) | image index (B int64) | pixels]
+            o_aff = B * _PRE_IMAGE.itemsize
+            o_idx = o_aff + B * 24 + (8 - B * 24 % 8) % 8
+            o_img = o_idx + B * 8
+            o_img += (16 - o_img % 16) % 16
+            sizes = [items[j][1].nbytes for j in idx]
+            host = torch.empty(o_img + sum(sizes), dtype=torch.uint8, pin_memory=True)
+            hv = host.numpy()
+            table = np.zeros(B, _PRE_IMAGE)
+            pos = 0
+            for n, j in enumerate(idx):
+                img = items[j][1]
+                table[n] = (pos, img.shape[0], img.shape[1], np.asarray(items[j][2], np.float64).reshape(6))
+                hv[o_img + pos:o_img + pos + img.nbytes] = img.reshape(-1)
+                pos += img.nbytes
+            hv[:o_aff] = table.view(np.uint8)
+            hv[o_aff:o_aff + B * 24] = affine_for_meta([items[j][3] for j in idx], self.scales[si]).numpy().view(np.uint8).reshape(-1)
+            hv[o_idx:o_idx + B * 8] = np.array([items[j][0] for j in idx], np.int64).view(np.uint8)
+            buf = host.to(dev, non_blocking=True)
+            aff = buf[o_aff:o_aff + B * 24].view(torch.float32).view(B, 6)
+            dst = buf[o_idx:o_idx + B * 8].view(torch.int64)
+            inp = torch.empty((2 * B if flip else B, 3, inp_h, inp_w), dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                st = _lib.lib().cpb200_pre_process_batch(buf.data_ptr() + o_img, buf.data_ptr(), B, inp.data_ptr(),
+                                                         inp_h, inp_w, mean, std, 1 if flip else 0, stream)
+            _lib.check(st, "pre_process_batch")
+            outputs = self.model(inp)
+            if flip:
+                # process()'s gating (multi_pose.py:35-53) on B [image, mirror] pairs
+                hm, wh, hps, reg, hm_hp, hp_offset = outputs
+                sigmoid_(hm)
+                if cfg.LOSS.HM_HP and not cfg.LOSS.MSE_LOSS:
+                    sigmoid_(hm_hp)
+                hm, wh, hps, hm_hp = flip_merge(hm, wh, hps, hm_hp if cfg.LOSS.HM_HP else None, self.flip_idx)
+                reg = reg[0::2].contiguous() if cfg.LOSS.REG_OFFSET else None
+                hp_offset = hp_offset[0::2].contiguous() if cfg.LOSS.REG_HP_OFFSET else None
+                dets = multi_pose_decode(hm, wh, hps, reg=reg, hm_hp=hm_hp, hp_offset=hp_offset, K=K, affine=aff)
+            else:
+                dets = self._decode_heads(outputs, affine=aff)
+            rows[dst, si * K:(si + 1) * K] = dets
+        if cfg.TEST.NMS or S > 1:
+            soft_nms_39_cuda_batch(rows, Nt=0.5, method=2)
+        out = rows.cpu().numpy()
+        return [out[i] for i in range(len(loaded))]
 
 
 detector_factory = {"multi_pose": MultiPoseDetector}     # detector_factory.py:5-7

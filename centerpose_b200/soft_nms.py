@@ -8,7 +8,8 @@ moved, the 17 keypoint-score columns 39..55 never move (``nms.pyx:214-217``); a 
 falls below ``threshold`` gets columns 0..4 overwritten by the last live row and columns 5..38
 swapped with it (``:257-268``); all arithmetic is C ``float``.
 N <= 100 x scales, O(N^2) on the host exactly as in the reference.  The device version is ``cpb200_soft_nms_39``
-(``csrc/post.cu``; ``detector.merge_outputs_device`` / ``run_batch_fused(nms=True)`` use it); this port serves
+(``csrc/post.cu``; ``detector.merge_outputs_device`` / ``run_batch_fused(nms=True)`` use it, ``run_images`` its batched
+form ``cpb200_soft_nms_39_batch``); this port serves
 ``merge_outputs``, whose inputs are host arrays as in the reference."""
 from __future__ import annotations
 
@@ -69,3 +70,21 @@ def soft_nms_39_cuda(boxes, sigma: float = 0.5, Nt: float = 0.3, threshold: floa
                                            int(method), keep.data_ptr(), torch.cuda.current_stream(boxes.device).cuda_stream)
     _lib.check(st, "soft_nms_39")
     return int(keep.item())
+
+
+def soft_nms_39_cuda_batch(boxes, sigma: float = 0.5, Nt: float = 0.3, threshold: float = 0.001, method: int = 0):
+    """``soft_nms_39_cuda`` for B images in one launch (``cpb200_soft_nms_39_batch``): ``boxes`` is a contiguous CUDA
+    float32 ``(B, N, 56)`` tensor, each image's rows mutated in place exactly like the host version.  Returns the
+    ``(B,)`` int32 CUDA tensor of kept-row counts; nothing waits for the device."""
+    import torch
+    from . import _lib
+    if not (boxes.is_cuda and boxes.dtype == torch.float32 and boxes.dim() == 3 and boxes.shape[2] == 56
+            and boxes.is_contiguous()):
+        raise ValueError("soft_nms_39_cuda_batch expects a contiguous CUDA float32 (B, N, 56) tensor")
+    keep = torch.empty(boxes.shape[0], dtype=torch.int32, device=boxes.device)
+    with torch.cuda.device(boxes.device):
+        st = _lib.lib().cpb200_soft_nms_39_batch(boxes.data_ptr(), boxes.shape[0], boxes.shape[1], float(sigma), float(Nt),
+                                                 float(threshold), int(method), keep.data_ptr(),
+                                                 torch.cuda.current_stream(boxes.device).cuda_stream)
+    _lib.check(st, "soft_nms_39_batch")
+    return keep

@@ -105,12 +105,32 @@ int cpb200_flip_merge(const float *hm, const float *wh, const float *hps, const 
 int cpb200_pre_process(const unsigned char *img, int h, int w, const double *trans_input, float *out, int out_h, int out_w,
                        const float *mean, const float *stdv, int flip, void *stream);
 
+/* One image of cpb200_pre_process_batch (64 bytes, lives in caller-owned DEVICE memory). */
+typedef struct cpb200_pre_image {
+  int64_t offset;            /* byte offset of the image's first pixel in `imgs` */
+  int32_t h, w;              /* image size; HWC uint8 BGR, rows packed (pitch 3*w bytes) */
+  double trans_input[6];     /* the forward 2x3 matrix of get_affine_transform(c, s, 0, [out_w, out_h]), row-major */
+} cpb200_pre_image;
+
+/* cpb200_pre_process for B images in one launch (grid over image x pixel); cpb200_pre_process is its B = 1 case and
+ * every image comes out bit-identical to it.  `imgs` is one device buffer holding all images, `table` a DEVICE array
+ * of B cpb200_pre_image; all images share the output size (out_h, out_w).  out is (B,3,out_h,out_w), or with
+ * flip != 0 (2B,3,out_h,out_w) ordered [img_0, mirror_0, img_1, mirror_1, ...] (the pair layout cpb200_flip_merge
+ * reads).  mean / stdv are HOST arrays of 3 floats.  1 <= B <= 65535. */
+int cpb200_pre_process_batch(const unsigned char *imgs, const cpb200_pre_image *table, int B, float *out, int out_h,
+                             int out_w, const float *mean, const float *stdv, int flip, void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)
  * receives the number of surviving rows.  One CTA; N*232 bytes of shared memory (N <= 882). */
 int cpb200_soft_nms_39(float *boxes, int N, float sigma, float Nt, float threshold, int method, int *keep_count,
                        void *stream);
+
+/* The same for B images at once: boxes is (B,N,56), one CTA per image, keep_counts (device, B ints, may be NULL)
+ * receives each image's surviving rows.  cpb200_soft_nms_39 is its B = 1 case.  N <= 882, B <= 65535. */
+int cpb200_soft_nms_39_batch(float *boxes, int B, int N, float sigma, float Nt, float threshold, int method,
+                             int *keep_counts, void *stream);
 
 
 /* ------------------------------------------------------------------------------------
