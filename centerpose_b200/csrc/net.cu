@@ -3,6 +3,7 @@
 
 namespace cpb {
 int run_op_simt_dispatch(const cpb200_op &op, cudaStream_t st);
+bool simt_runs_split(int type);
 int tc_prepare_op(cpb200_op &op);
 int tc_release_op(cpb200_op &op);
 int tc_run_op(const cpb200_op &op, cudaStream_t st);
@@ -21,10 +22,7 @@ static int validate(const cpb200_op &op, int i) {
   if (!op.dst) return cpb::fail(CPB200_ERR_ARG, "op %d: null dst", i);
   if (op.act_dtype < CPB200_F32 || op.act_dtype > CPB200_F16X2)
     return cpb::fail(CPB200_ERR_ARG, "op %d: bad act_dtype", i);
-  if ((op.act_dtype == CPB200_BF16X2 || op.act_dtype == CPB200_F16X2) && !(op.flags & CPB200_FLAG_TC) &&
-      op.type != CPB200_OP_CONVERT && op.type != CPB200_OP_MAXPOOL && op.type != CPB200_OP_DWDECONV_ADD &&
-      op.type != CPB200_OP_DWCONV && op.type != CPB200_OP_AVGPOOL && op.type != CPB200_OP_SCALE_ADD && op.type != CPB200_OP_UPSAMPLE_ADD &&
-      op.type != CPB200_OP_S2D && op.type != CPB200_OP_AVGPOOL2 && op.type != CPB200_OP_RESIZE_BILINEAR)
+  if ((op.act_dtype == CPB200_BF16X2 || op.act_dtype == CPB200_F16X2) && !(op.flags & CPB200_FLAG_TC) && !cpb::simt_runs_split(op.type))
     return cpb::fail(CPB200_ERR_ARG, "op %d: split-precision activations need the tensor-core path (or an element-wise op / CONVERT)", i);
   if ((op.type == CPB200_OP_CONV || op.type == CPB200_OP_DCN || op.type == CPB200_OP_STEM) && !op.weight)
     return cpb::fail(CPB200_ERR_ARG, "op %d: null weight", i);

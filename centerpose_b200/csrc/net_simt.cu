@@ -1,6 +1,6 @@
 // CUDA-core (SIMT) implementations of the fused network ops, fp32 accumulate, activations
-// fp32 or bf16 NHWC.  This is the "precise" path (act_dtype = fp32 reproduces the reference's
-// fp32 arithmetic up to summation order) and the fallback for layers whose shapes the
+// fp32 or bf16 NHWC (the element-wise ops also split planes).  This is the "precise" path (act_dtype = fp32
+// reproduces the reference's fp32 arithmetic up to summation order) and the fallback for layers whose shapes the
 // wgmma path (net_tc.cu) does not take.  Reference semantics per op:
 //   CONV          torch.nn.Conv2d + folded eval BatchNorm2d (+ residual add) (+ ReLU)
 //                 e.g. pose_dla_dcn.py:43-57 (BasicBlock), :155-163 (Root: the torch.cat of
@@ -17,8 +17,8 @@
 //   RESIZE_BILINEAR  hardnet.py:95-100 F.interpolate(bilinear, align_corners=True)
 #include "common.cuh"
 #include <cuda_fp16.h>
-#include <cstdlib>
 #include <algorithm>
+#include <type_traits>
 
 namespace {
 
@@ -86,14 +86,16 @@ struct Sp16 {
 
 // Pointer-like handles of split activations, so the element-wise kernels below take fp32, bf16 or split tensors on
 // either side through the same source: `p + n` advances both planes, io_ld4 joins hi + lo, io_st4 re-splits.
+// `p + n` is force-inlined: outlined (NVVM -O1), it returns the handle through the stack and stores through it become
+// generic instead of global.
 struct SpC {
   const uint16_t *p; size_t plane; uint32_t fmt;
-  __host__ __device__ SpC operator+(size_t n) const { return SpC{p + n, plane, fmt}; }
+  __host__ __device__ __forceinline__ SpC operator+(size_t n) const { return SpC{p + n, plane, fmt}; }
   __host__ __device__ explicit operator bool() const { return p != nullptr; }
 };
 struct SpM {
   uint16_t *p; size_t plane; uint32_t fmt;
-  __host__ __device__ SpM operator+(size_t n) const { return SpM{p + n, plane, fmt}; }
+  __host__ __device__ __forceinline__ SpM operator+(size_t n) const { return SpM{p + n, plane, fmt}; }
 };
 __device__ __forceinline__ float4 io_ld4(const float *p) { return Act<float>::ld4(p); }
 __device__ __forceinline__ float4 io_ld4(const bf16 *p) { return Act<bf16>::ld4(p); }
@@ -101,6 +103,61 @@ __device__ __forceinline__ float4 io_ld4(SpC p) { return Sp16::ld4(p.p, p.plane,
 __device__ __forceinline__ void io_st4(float *p, float4 v) { Act<float>::st4(p, v); }
 __device__ __forceinline__ void io_st4(bf16 *p, float4 v) { Act<bf16>::st4(p, v); }
 __device__ __forceinline__ void io_st4(SpM p, float4 v) { Sp16::st4(p.p, p.plane, p.fmt, v); }
+// N = 4 or 8 consecutive values as float4 members, not an array: NVVM's -O1 pipeline does not unroll loops, so an
+// array indexed in a loop would live in local memory.  The 8-element accesses are one 16-byte access per plane.
+template <int N> struct Vf;
+template <> struct Vf<4> { float4 a; };
+template <> struct Vf<8> { float4 a, b; };
+__device__ __forceinline__ float4 bf16x4(uint32_t lo, uint32_t hi) {
+  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&lo));
+  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&hi));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float4 sp16x4(uint32_t h0, uint32_t h1, uint32_t l0, uint32_t l1, uint32_t fmt) {
+  const float2 a = Sp16::up(h0, fmt), b = Sp16::up(h1, fmt), c = Sp16::up(l0, fmt), d = Sp16::up(l1, fmt);
+  return make_float4(a.x + c.x, a.y + c.y, b.x + d.x, b.y + d.y);
+}
+__device__ __forceinline__ Vf<8> io_ld8(const bf16 *p) {
+  const uint4 r = __ldg(reinterpret_cast<const uint4 *>(p));
+  return {bf16x4(r.x, r.y), bf16x4(r.z, r.w)};
+}
+__device__ __forceinline__ Vf<8> io_ld8(SpC p) {
+  const uint4 h = __ldg(reinterpret_cast<const uint4 *>(p.p)), l = __ldg(reinterpret_cast<const uint4 *>(p.p + p.plane));
+  return {sp16x4(h.x, h.y, l.x, l.y, p.fmt), sp16x4(h.z, h.w, l.z, l.w, p.fmt)};
+}
+template <int N, typename P> __device__ __forceinline__ Vf<N> io_ldv(P p) {
+  if constexpr (N == 4) return {io_ld4(p)};
+  else return io_ld8(p);
+}
+template <typename P> __device__ __forceinline__ void io_stv(P p, Vf<4> v) { io_st4(p, v.a); }
+__device__ __forceinline__ void io_stv(bf16 *p, Vf<8> v) {
+  const __nv_bfloat162 a = __floats2bfloat162_rn(v.a.x, v.a.y), b = __floats2bfloat162_rn(v.a.z, v.a.w);
+  const __nv_bfloat162 c = __floats2bfloat162_rn(v.b.x, v.b.y), d = __floats2bfloat162_rn(v.b.z, v.b.w);
+  *reinterpret_cast<uint4 *>(p) = make_uint4(*reinterpret_cast<const uint32_t *>(&a), *reinterpret_cast<const uint32_t *>(&b),
+                                             *reinterpret_cast<const uint32_t *>(&c), *reinterpret_cast<const uint32_t *>(&d));
+}
+__device__ __forceinline__ void io_stv(SpM p, Vf<8> v) {
+  uint4 h, l;
+  Sp16::split2(v.a.x, v.a.y, p.fmt, h.x, l.x); Sp16::split2(v.a.z, v.a.w, p.fmt, h.y, l.y);
+  Sp16::split2(v.b.x, v.b.y, p.fmt, h.z, l.z); Sp16::split2(v.b.z, v.b.w, p.fmt, h.w, l.w);
+  *reinterpret_cast<uint4 *>(p.p) = h;
+  *reinterpret_cast<uint4 *>(p.p + p.plane) = l;
+}
+template <int N> __device__ __forceinline__ Vf<N> ld_taps(const float *w) {     // fp32 filter taps
+  const float4 a = __ldg(reinterpret_cast<const float4 *>(w));
+  if constexpr (N == 4) return {a};
+  else return {a, __ldg(reinterpret_cast<const float4 *>(w + 4))};
+}
+__device__ __forceinline__ float4 fma4(float4 x, float4 w, float4 acc) {
+  return make_float4(fmaf(x.x, w.x, acc.x), fmaf(x.y, w.y, acc.y), fmaf(x.z, w.z, acc.z), fmaf(x.w, w.w, acc.w));
+}
+__device__ __forceinline__ Vf<4> vfma(Vf<4> x, Vf<4> w, Vf<4> acc) { return {fma4(x.a, w.a, acc.a)}; }
+__device__ __forceinline__ Vf<8> vfma(Vf<8> x, Vf<8> w, Vf<8> acc) { return {fma4(x.a, w.a, acc.a), fma4(x.b, w.b, acc.b)}; }
+// The epilogue activation follows the output format: act_fn for fp32, act_fast for bf16 and split planes (common.cuh).
+template <typename PO> __device__ __forceinline__ float act_io(float v, uint32_t act) {
+  if constexpr (std::is_same<PO, float *>::value) return cpb::act_fn(v, act);
+  else return cpb::act_fast(v, act);
+}
 
 struct ConvArgs {
   const void *src[4];
@@ -390,38 +447,13 @@ __global__ void __launch_bounds__(128) stem_kernel(const float *__restrict__ x, 
   }
 }
 
-// ---- IM2COL_W: NCHW fp32 (B,cin,H,W) -> NHWC (B,H,W,COUT): channel s*cin+c = x[c,h,w+s-pad], zero padded ----
-template <typename T, int COUT>
-__global__ void __launch_bounds__(256) im2col_w_kernel(const float *__restrict__ x, T *__restrict__ y, int B, int Cin,
-                                                       int H, int W, int kw, int pad) {
-  const long long M = (long long)B * H * W;
-  const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= M) return;
-  const int w = (int)(m % W);
-  const int h = (int)((m / W) % H);
-  const int b = (int)(m / ((long long)W * H));
-  float v[COUT];
-#pragma unroll
-  for (int i = 0; i < COUT; ++i) v[i] = 0.f;
-  for (int c = 0; c < Cin; ++c) {
-    const float *row = x + (((size_t)b * Cin + c) * H + h) * W;
-    for (int s_ = 0; s_ < kw; ++s_) {
-      const int wi = w + s_ - pad;
-      const float val = (wi >= 0 && wi < W) ? __ldg(row + wi) : 0.f;
-      const int ch = s_ * Cin + c;
-#pragma unroll
-      for (int i = 0; i < COUT; ++i) if (i == ch) v[i] = val;      // static indexing keeps v[] in registers
-    }
-  }
-  T *o = y + (size_t)m * COUT;
-#pragma unroll
-  for (int i = 0; i < COUT; i += 4) Act<T>::st4(o + i, make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]));
-}
+// ------------------------------------------------------------------------------------------------------------
+// Element-wise ops (run_eltwise below): one kernel per op for every activation format.  PI / PO are the input / output
+// handles: `const float *` / `float *`, `const bf16 *` / `bf16 *`, or SpC / SpM on split planes.  Arithmetic is fp32.
 
-// ---- MAXPOOL k x k / stride / pad, NHWC, 4 channels per thread ----
-template <typename T>
-__global__ void maxpool_kernel(const T *__restrict__ x, T *__restrict__ y, int B, int H, int W, int C,
-                               int Ho, int Wo, int k, int stride, int pad) {
+// ---- MAXPOOL k x k / stride / pad, NHWC, 4 channels per thread (exact on split planes: the maximum is one of the inputs) ----
+template <typename PI, typename PO>
+__global__ void maxpool_kernel(PI x, PO y, int B, int H, int W, int C, int Ho, int Wo, int k, int stride, int pad) {
   const int C4 = C >> 2;
   const long long total = (long long)B * Ho * Wo * C4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -438,41 +470,31 @@ __global__ void maxpool_kernel(const T *__restrict__ x, T *__restrict__ y, int B
       for (int q = 0; q < k; ++q) {
         const int wi = wo * stride - pad + q;
         if (wi < 0 || wi >= W) continue;
-        const float4 v = Act<T>::ld4(x + (((size_t)b * H + hi) * W + wi) * C + c4 * 4);
+        const float4 v = io_ld4(x + (((size_t)b * H + hi) * W + wi) * C + c4 * 4);
         m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
       }
     }
-    Act<T>::st4(y + (((size_t)b * Ho + ho) * Wo + wo) * C + c4 * 4, m);
+    io_st4(y + (((size_t)b * Ho + ho) * Wo + wo) * C + c4 * 4, m);
   }
 }
 
 // ---- depthwise ConvTranspose2d(k=2f, stride f, pad f/2) + skip add, NHWC ----
 // out[b,ho,wo,c] = skip[b,ho,wo,c] + sum_{kh,kw : (ho+p-kh)%f==0, (wo+p-kw)%f==0} x[b,(ho+p-kh)/f,(wo+p-kw)/f,c] * w[kh,kw,c]
-// One CTA = one output row (b, ho); thread = (wo, group of VEC channels), VEC*sizeof(T) = 16 bytes.  The
-// k*k*C filter taps sit in shared memory; no integer division in the inner loop.
-template <typename T, int VEC>
-__global__ void __launch_bounds__(256) dwdeconv_add_kernel(const T *__restrict__ x, const T *__restrict__ skip, T *__restrict__ y,
-                                                           const float *__restrict__ w, int H, int W, int C, int Ho, int Wo,
-                                                           int k, int f, int pad, int lf, int lcv) {
-  // f and C / VEC are powers of two (lf = log2 f, lcv = log2(C / VEC), or -1 -> generic division):
-  // the per-element index arithmetic is shifts and masks only.
-  extern __shared__ float sw[];                       // [k*k][C]
-  for (int i = threadIdx.x; i < k * k * C; i += blockDim.x) sw[i] = w[i];
-  __syncthreads();
+// One CTA = one output row (b, ho); thread = (wo, group of VEC channels).  The k*k*C filter taps are read through the
+// read-only cache, so any filter size is accepted.  No integer division in the inner loop when f and C / VEC are powers
+// of two (lf = log2 f, lcv = log2(C / VEC), or -1 -> generic division).
+template <int VEC, typename PI, typename PO>
+__global__ void __launch_bounds__(256) dwdeconv_add_kernel(PI x, PI skip, PO y, const float *__restrict__ w, int H, int W, int C,
+                                                           int Ho, int Wo, int k, int f, int pad, int lf, int lcv) {
   const int CV = C / VEC;
   const int b = blockIdx.x / Ho, ho = blockIdx.x % Ho;
   const int kh0 = (ho + pad) % f;
-  const T *xb = x + (size_t)b * H * W * C;
+  const PI xb = x + (size_t)b * H * W * C;
   const bool fast = lf >= 0 && lcv >= 0;
   for (int i = threadIdx.x; i < Wo * CV; i += blockDim.x) {
     const int wo = fast ? (i >> lcv) : (i / CV), cv = i - wo * CV;
     const size_t opix = (((size_t)b * Ho + ho) * Wo + wo) * C + cv * VEC;
-    float acc[VEC];
-#pragma unroll
-    for (int q = 0; q < VEC; q += 4) {
-      float4 s4 = skip ? Act<T>::ld4(skip + opix + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-      acc[q] = s4.x; acc[q + 1] = s4.y; acc[q + 2] = s4.z; acc[q + 3] = s4.w;
-    }
+    Vf<VEC> acc = skip ? io_ldv<VEC>(skip + opix) : Vf<VEC>{};
     const int kw0 = fast ? ((wo + pad) & (f - 1)) : ((wo + pad) % f);
     for (int khh = kh0; khh < k; khh += f) {
       const int hn = ho + pad - khh;
@@ -482,59 +504,37 @@ __global__ void __launch_bounds__(256) dwdeconv_add_kernel(const T *__restrict__
         const int wn = wo + pad - kww;
         const int wi = fast ? (wn >> lf) : (wn / f);
         if (wn < 0 || wi >= W) continue;
-        const T *xp = xb + ((size_t)hi * W + wi) * C + cv * VEC;
-        const float *wp = sw + (khh * k + kww) * C + cv * VEC;
-#pragma unroll
-        for (int q = 0; q < VEC; q += 4) {
-          const float4 v = Act<T>::ld4(xp + q);
-          const float4 ww = *reinterpret_cast<const float4 *>(wp + q);
-          acc[q] = fmaf(v.x, ww.x, acc[q]); acc[q + 1] = fmaf(v.y, ww.y, acc[q + 1]);
-          acc[q + 2] = fmaf(v.z, ww.z, acc[q + 2]); acc[q + 3] = fmaf(v.w, ww.w, acc[q + 3]);
-        }
+        acc = vfma(io_ldv<VEC>(xb + ((size_t)hi * W + wi) * C + cv * VEC), ld_taps<VEC>(w + (size_t)(khh * k + kww) * C + cv * VEC), acc);
       }
     }
-#pragma unroll
-    for (int q = 0; q < VEC; q += 4) Act<T>::st4(y + opix + q, make_float4(acc[q], acc[q + 1], acc[q + 2], acc[q + 3]));
+    io_stv(y + opix, acc);
   }
 }
 
-// Fast path for the shapes IDAUp uses (k == 2f, f and C/VEC powers of two, 256 % (f * C/VEC) == 0): every item a
-// thread visits in one output row has the same channel group and the same column parity class, so its four
-// (kh, kw) tap weight vectors are loaded into registers ONCE per CTA instead of 8 LDS.128 per item.
-template <typename T, int VEC>
-__global__ void __launch_bounds__(256) dwdeconv_add_fast_kernel(const T *__restrict__ x, const T *__restrict__ skip, T *__restrict__ y,
-                                                                const float *__restrict__ w, int H, int W, int C, int Ho, int Wo,
-                                                                int k, int f, int pad, int lf, int lcv) {
+// Fast path for the shapes IDAUp uses (see run_eltwise): every item a thread visits in one output row has the same
+// channel group and the same column parity class, so its four (kh, kw) tap weight vectors are loaded ONCE per CTA.
+// VEC channels = 16 bytes per plane.  6 CTAs per SM keep it at <= 40 registers, the occupancy it has always run at.
+template <int VEC, typename PI, typename PO>
+__global__ void __launch_bounds__(256, 6) dwdeconv_add_fast_kernel(PI x, PI skip, PO y, const float *__restrict__ w, int H, int W, int C,
+                                                                int Ho, int Wo, int k, int f, int pad, int lf, int lcv) {
   const int CV = C / VEC;
   const int b = blockIdx.x / Ho, ho = blockIdx.x % Ho;
   const int i0 = threadIdx.x;
   const int wo_first = i0 >> lcv, cv = i0 & (CV - 1);
   const int kh0 = (ho + pad) & (f - 1), kw0 = (wo_first + pad) & (f - 1);
-  float wt[2][2][VEC];
+  Vf<VEC> wt[2][2];
 #pragma unroll
   for (int a = 0; a < 2; ++a)
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      const float *wp = w + (size_t)((kh0 + a * f) * k + kw0 + c * f) * C + cv * VEC;
-#pragma unroll
-      for (int q = 0; q < VEC; q += 4) {
-        const float4 v = __ldg(reinterpret_cast<const float4 *>(wp + q));
-        wt[a][c][q] = v.x; wt[a][c][q + 1] = v.y; wt[a][c][q + 2] = v.z; wt[a][c][q + 3] = v.w;
-      }
-    }
-  const T *xb = x + (size_t)b * H * W * C + cv * VEC;
+    for (int c = 0; c < 2; ++c) wt[a][c] = ld_taps<VEC>(w + (size_t)((kh0 + a * f) * k + kw0 + c * f) * C + cv * VEC);
+  const PI xb = x + (size_t)b * H * W * C + cv * VEC;
   const int hn0 = ho + pad - kh0;                               // >= 0; tap a reads input row (hn0 >> lf) - a
   const int hi0 = hn0 >> lf;
   const size_t orow = ((size_t)b * Ho + ho) * Wo;
   for (int i = i0; i < Wo * CV; i += 256) {
     const int wo = i >> lcv;
     const size_t opix = (orow + wo) * C + cv * VEC;
-    float acc[VEC];
-#pragma unroll
-    for (int q = 0; q < VEC; q += 4) {
-      float4 s4 = skip ? Act<T>::ld4(skip + opix + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-      acc[q] = s4.x; acc[q + 1] = s4.y; acc[q + 2] = s4.z; acc[q + 3] = s4.w;
-    }
+    Vf<VEC> acc = skip ? io_ldv<VEC>(skip + opix) : Vf<VEC>{};
     const int wi0 = (wo + pad - kw0) >> lf;
 #pragma unroll
     for (int a = 0; a < 2; ++a) {
@@ -544,25 +544,19 @@ __global__ void __launch_bounds__(256) dwdeconv_add_fast_kernel(const T *__restr
       for (int c = 0; c < 2; ++c) {
         const int wi = wi0 - c;
         if (wi < 0 || wi >= W) continue;
-        const T *xp = xb + ((size_t)hi * W + wi) * C;
-#pragma unroll
-        for (int q = 0; q < VEC; q += 4) {
-          const float4 v = Act<T>::ld4(xp + q);
-          acc[q] = fmaf(v.x, wt[a][c][q], acc[q]); acc[q + 1] = fmaf(v.y, wt[a][c][q + 1], acc[q + 1]);
-          acc[q + 2] = fmaf(v.z, wt[a][c][q + 2], acc[q + 2]); acc[q + 3] = fmaf(v.w, wt[a][c][q + 3], acc[q + 3]);
-        }
+        acc = vfma(io_ldv<VEC>(xb + ((size_t)hi * W + wi) * C), wt[a][c], acc);
       }
     }
-#pragma unroll
-    for (int q = 0; q < VEC; q += 4) Act<T>::st4(y + opix + q, make_float4(acc[q], acc[q + 1], acc[q + 2], acc[q + 3]));
+    io_stv(y + opix, acc);
   }
 }
 
 // ---- nearest-neighbour upsample x f (+ skip add)(+ReLU), NHWC ----
 // out[b,ho,wo,c] = act(skip[b,ho,wo,c] + x[b,ho/f,wo/f,c])     (HRNet fuse_layers, pose_higher_hrnet.py:186-187,224-232)
-// Thread = 4 channels of one output pixel; f is a power of two (shift).
-template <typename T, typename PI = const T *, typename PO = T *>
-__global__ void __launch_bounds__(256) upsample_add_kernel(PI x, PI skip, PO y,
+// Thread = 4 channels of one output pixel; f is a power of two (shift).  On split planes the bound keeps it at <= 32
+// registers, the 8 CTAs per SM that the plain-pointer instantiations reach unbounded.
+template <typename PI, typename PO>
+__global__ void __launch_bounds__(256, std::is_same<PO, SpM>::value ? 8 : 1) upsample_add_kernel(PI x, PI skip, PO y,
                                                            long long total, int H, int W, int C4, int Ho, int Wo, int sh, uint32_t act) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int c4 = (int)(i % C4);
@@ -575,7 +569,7 @@ __global__ void __launch_bounds__(256) upsample_add_kernel(PI x, PI skip, PO y,
       const float4 s4 = io_ld4(skip + (size_t)i * 4);
       v.x += s4.x; v.y += s4.y; v.z += s4.z; v.w += s4.w;
     }
-    if (act) { v.x = cpb::act_out<T>(v.x, act); v.y = cpb::act_out<T>(v.y, act); v.z = cpb::act_out<T>(v.z, act); v.w = cpb::act_out<T>(v.w, act); }
+    if (act) { v.x = act_io<PO>(v.x, act); v.y = act_io<PO>(v.y, act); v.z = act_io<PO>(v.z, act); v.w = act_io<PO>(v.w, act); }
     io_st4(y + (size_t)i * 4, v);
   }
 }
@@ -583,7 +577,7 @@ __global__ void __launch_bounds__(256) upsample_add_kernel(PI x, PI skip, PO y,
 // ---- 2x2 / stride-2 average pool, floor mode, NHWC   (HarDNet nn.AvgPool2d(2, 2), hardnet.py:141) ----
 // Thread = 4 channels of one output pixel.  The taps are summed in row-major order and scaled by 1/4 (exact), the
 // order of PyTorch's CPU kernel.  Odd trailing rows / columns are never read.
-template <typename T, typename PI = const T *, typename PO = T *>
+template <typename PI, typename PO>
 __global__ void __launch_bounds__(256) avgpool2_kernel(PI x, PO y, long long total, int H, int W, int C4, int Ho, int Wo) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int c4 = (int)(i % C4);
@@ -603,7 +597,7 @@ __global__ void __launch_bounds__(256) avgpool2_kernel(PI x, PO y, long long tot
 // Thread = 4 channels of one output pixel.  Source coordinates and weights follow PyTorch's fp32 arithmetic
 // (scale = (in-1)/(out-1) from the host, src = scale*dst, i1 = i0 + (i0 < in-1), l0 = 1 - l1); the result is the
 // vertical blend of the two horizontal blends.
-template <typename T, typename PI = const T *, typename PO = T *>
+template <typename PI, typename PO>
 __global__ void __launch_bounds__(256) resize_bilinear_kernel(PI x, PO y, long long total, int H, int W, int C4, int Ho, int Wo,
                                                               float scale_h, float scale_w) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -626,38 +620,11 @@ __global__ void __launch_bounds__(256) resize_bilinear_kernel(PI x, PO y, long l
   }
 }
 
-// CPB200_OP_AVGPOOL2 / CPB200_OP_RESIZE_BILINEAR for every activation dtype: PI / PO are plain pointers (fp32, bf16) or
-// the split-plane handles (bf16x2, fp16x2), so the split formats never leave their planes.
-template <typename T, typename PI, typename PO>
-int launch_resample(const cpb200_op &op, PI x, PO y, cudaStream_t st) {
-  const bool pool = op.type == CPB200_OP_AVGPOOL2;
-  const char *name = pool ? "avgpool2" : "resize_bilinear";
-  const int C = op.cin[0];
-  if (op.nsrc != 1 || C % 4 || op.cout != C || (op.src_pitch[0] != 0 && op.src_pitch[0] != C))
-    return cpb::fail(CPB200_ERR_ARG, "%s: needs one dense input with C %% 4 == 0 and cout == C (nsrc %d, C %d, cout %d, src_pitch %d)",
-                     name, op.nsrc, C, op.cout, op.src_pitch[0]);
-  if (pool && (op.H < 2 || op.W < 2 || op.Ho != op.H / 2 || op.Wo != op.W / 2))
-    return cpb::fail(CPB200_ERR_ARG, "avgpool2: %dx%d -> %dx%d is not a 2x2 / stride-2 floor-mode pool (needs H, W >= 2)",
-                     op.H, op.W, op.Ho, op.Wo);
-  if (!pool && (op.Ho < 1 || op.Wo < 1))
-    return cpb::fail(CPB200_ERR_ARG, "resize_bilinear: output size %dx%d", op.Ho, op.Wo);
-  const long long total = (long long)op.B * op.Ho * op.Wo * (C / 4);
-  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
-  if (pool) {
-    avgpool2_kernel<T, PI, PO><<<grid, 256, 0, st>>>(x, y, total, op.H, op.W, C / 4, op.Ho, op.Wo);
-    return cpb::check_launch("avgpool2_kernel");
-  }
-  const float sh = op.Ho > 1 ? (float)(op.H - 1) / (float)(op.Ho - 1) : 0.f;
-  const float sw = op.Wo > 1 ? (float)(op.W - 1) / (float)(op.Wo - 1) : 0.f;
-  resize_bilinear_kernel<T, PI, PO><<<grid, 256, 0, st>>>(x, y, total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, sw);
-  return cpb::check_launch("resize_bilinear_kernel");
-}
-
 // ---- depthwise k x k conv (stride s, pad k/2) + bias + activation, NHWC   (mobilenetv3.py:124-127 conv2/bn2) ----
 // y[b,ho,wo,c] = act(bias[c] + sum_{r,q} x[b, ho*s-p+r, wo*s-p+q, c] * w[r,q,c]).  Thread = VEC channels of one
-// output pixel (VEC * sizeof(T) = 16 bytes); consecutive threads walk the channels of a pixel, so every tap is
-// a coalesced row read that the neighbouring output pixels re-read from L1.  HBM-bound: 2 bytes in + out per MAC x k^2.
-template <typename T, int VEC, typename PI = const T *, typename PO = T *>
+// output pixel; consecutive threads walk the channels of a pixel, so every tap is a coalesced row read that the
+// neighbouring output pixels re-read from L1.  HBM-bound: 2 bytes in + out per MAC x k^2.
+template <int VEC, typename PI, typename PO>
 __global__ void __launch_bounds__(256) dwconv_kernel(PI x, PO y, const float *__restrict__ w,
                                                      const float *__restrict__ bias, long long total, int H, int W, int C,
                                                      int Ho, int Wo, int k, int stride, int pad, uint32_t act) {
@@ -696,15 +663,15 @@ __global__ void __launch_bounds__(256) dwconv_kernel(PI x, PO y, const float *__
     const PO o = y + (size_t)i * VEC;
 #pragma unroll
     for (int q = 0; q < VEC; q += 4)
-      io_st4(o + q, make_float4(cpb::act_out<T>(acc[q], act), cpb::act_out<T>(acc[q + 1], act), cpb::act_out<T>(acc[q + 2], act),
-                                     cpb::act_out<T>(acc[q + 3], act)));
+      io_st4(o + q, make_float4(act_io<PO>(acc[q], act), act_io<PO>(acc[q + 1], act), act_io<PO>(acc[q + 2], act),
+                                act_io<PO>(acc[q + 3], act)));
   }
 }
 
 // Register-tiled variant for the shapes MobileNetV3 uses (k in {3,5}, stride in {1,2}): a thread produces PXW
 // adjacent output pixels of one row for VEC channels, so each input vector of the row segment is loaded once and
 // each tap's weight vector feeds PXW pixels (the generic kernel above issues 3 loads per tap per pixel).
-template <typename T, int VEC, int K, int S, int PXW, typename PI = const T *, typename PO = T *>
+template <int VEC, int K, int S, int PXW, typename PI, typename PO>
 __global__ void __launch_bounds__(256) dwconv_tiled_kernel(PI x, PO y, const float *__restrict__ w,
                                                            const float *__restrict__ bias, long long total, int H, int W, int C,
                                                            int Ho, int Wo, uint32_t act) {
@@ -763,15 +730,15 @@ __global__ void __launch_bounds__(256) dwconv_tiled_kernel(PI x, PO y, const flo
       const PO o = y + (((((size_t)b * Ho + ho) * Wo) + wo0 + px) * C + c0);
 #pragma unroll
       for (int q = 0; q < VEC; q += 4)
-        io_st4(o + q, make_float4(cpb::act_out<T>(acc[px][q], act), cpb::act_out<T>(acc[px][q + 1], act),
-                                       cpb::act_out<T>(acc[px][q + 2], act), cpb::act_out<T>(acc[px][q + 3], act)));
+        io_st4(o + q, make_float4(act_io<PO>(acc[px][q], act), act_io<PO>(acc[px][q + 1], act),
+                                  act_io<PO>(acc[px][q + 2], act), act_io<PO>(acc[px][q + 3], act)));
     }
   }
 }
 
 // ---- global average pool (B,H,W,C) -> (B,1,1,C)   (SeModule's AdaptiveAvgPool2d(1), mobilenetv3.py:100) ----
 // CTA = (image b, 64-channel chunk): 16 channel quads x 16 pixel lanes, fp32 partial sums, shared-memory tree.
-template <typename T, typename PI = const T *, typename PO = T *>
+template <typename PI, typename PO>
 __global__ void __launch_bounds__(256) avgpool_kernel(PI x, PO y, int HW, int C) {
   __shared__ float4 part[16][16];
   const int b = blockIdx.x, cq = blockIdx.y * 16 + (threadIdx.x & 15), lane = threadIdx.x >> 4;
@@ -793,7 +760,7 @@ __global__ void __launch_bounds__(256) avgpool_kernel(PI x, PO y, int HW, int C)
 }
 
 // ---- y[b,h,w,c] = x[b,h,w,c] * scale[b,c] (+ skip[b,h,w,c])   (SeModule gate + Block shortcut, mobilenetv3.py:111,146) ----
-template <typename T, typename PI = const T *, typename PS = const T *, typename PO = T *>
+template <typename PI, typename PS, typename PO>
 __global__ void __launch_bounds__(256) scale_add_kernel(PI x, PS scale, PI skip, PO y, long long total, long long per_image, int C4) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int b = (int)(i / per_image), c4 = (int)(i % C4);
@@ -817,139 +784,6 @@ __global__ void __launch_bounds__(256) convert_from_split_kernel(const uint16_t 
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x)
     reinterpret_cast<float4 *>(y)[i] = Sp16::ld4(x + i * 4, plane, fmt);
 }
-
-// max-pool on split planes (pose_dla_dcn.py:196, msra_resnet.py:126): exact (the maximum is one of the inputs)
-__global__ void maxpool_split_kernel(const uint16_t *__restrict__ x, uint16_t *__restrict__ y, int B, int H, int W, int C,
-                                     int Ho, int Wo, int k, int stride, int pad, uint32_t fmt) {
-  const int C4 = C >> 2;
-  const long long total = (long long)B * Ho * Wo * C4;
-  const size_t xplane = (size_t)B * H * W * C, yplane = (size_t)B * Ho * Wo * C;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int c4 = (int)(i % C4);
-    long long p = i / C4;
-    const int wo = (int)(p % Wo); p /= Wo;
-    const int ho = (int)(p % Ho);
-    const int b = (int)(p / Ho);
-    float4 m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
-    for (int r = 0; r < k; ++r) {
-      const int hi = ho * stride - pad + r;
-      if (hi < 0 || hi >= H) continue;
-      for (int q = 0; q < k; ++q) {
-        const int wi = wo * stride - pad + q;
-        if (wi < 0 || wi >= W) continue;
-        const float4 v = Sp16::ld4(x + (((size_t)b * H + hi) * W + wi) * C + c4 * 4, xplane, fmt);
-        m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
-      }
-    }
-    Sp16::st4(y + (((size_t)b * Ho + ho) * Wo + wo) * C + c4 * 4, yplane, fmt, m);
-  }
-}
-
-// depthwise ConvTranspose2d(k = 2f, stride f, pad f/2) + skip add on split planes (IDAUp up_*, pose_dla_dcn.py:361-364,374-377).
-// One CTA = one output row (b, ho); thread = (wo, 4 channels); every output pixel has exactly 2 x 2 contributing taps
-// (k == 2f).  fp32 arithmetic, tap weights fp32 [k*k][C].
-__global__ void __launch_bounds__(256) dwdeconv_add_split_kernel(const uint16_t *__restrict__ x, const uint16_t *__restrict__ skip,
-                                                                 uint16_t *__restrict__ y, const float *__restrict__ w, int B, int H, int W, int C,
-                                                                 int Ho, int Wo, int k, int f, int pad, uint32_t fmt) {
-  const int C4 = C >> 2;
-  const int b = blockIdx.x / Ho, ho = blockIdx.x % Ho;
-  const size_t xplane = (size_t)B * H * W * C, yplane = (size_t)B * Ho * Wo * C;
-  const int kh0 = (ho + pad) % f;
-  for (int i = threadIdx.x; i < Wo * C4; i += blockDim.x) {
-    const int wo = i / C4, c4 = i - wo * C4;
-    const size_t opix = (((size_t)b * Ho + ho) * Wo + wo) * C + c4 * 4;
-    float4 acc = skip ? Sp16::ld4(skip + opix, yplane, fmt) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const int kw0 = (wo + pad) % f;
-    for (int khh = kh0; khh < k; khh += f) {
-      const int hn = ho + pad - khh;
-      if (hn < 0) continue;
-      const int hi = hn / f;
-      if (hi >= H) continue;
-      for (int kww = kw0; kww < k; kww += f) {
-        const int wn = wo + pad - kww;
-        if (wn < 0) continue;
-        const int wi = wn / f;
-        if (wi >= W) continue;
-        const float4 v = Sp16::ld4(x + (((size_t)b * H + hi) * W + wi) * C + c4 * 4, xplane, fmt);
-        const float4 ww = __ldg(reinterpret_cast<const float4 *>(w + (size_t)(khh * k + kww) * C + c4 * 4));
-        acc.x = fmaf(v.x, ww.x, acc.x); acc.y = fmaf(v.y, ww.y, acc.y); acc.z = fmaf(v.z, ww.z, acc.z); acc.w = fmaf(v.w, ww.w, acc.w);
-      }
-    }
-    Sp16::st4(y + opix, yplane, fmt, acc);
-  }
-}
-
-// Fast path for the shapes IDAUp uses (k == 2f, f and C/8 powers of two, 256 % (f * C/8) == 0), mirroring
-// dwdeconv_add_fast_kernel: thread = (wo, 8 channels) with 16-byte loads per plane, its four (kh, kw) tap weight vectors
-// live in registers for the whole output row.  ~9 bytes of HBM traffic per output element (skip 4 + x 4/f^2 + out 4).
-__global__ void __launch_bounds__(256) dwdeconv_add_split_fast_kernel(const uint16_t *__restrict__ x, const uint16_t *__restrict__ skip,
-                                                                      uint16_t *__restrict__ y, const float *__restrict__ w, int B, int H, int W,
-                                                                      int C, int Ho, int Wo, int k, int f, int pad, int lf, int lcv, uint32_t fmt) {
-  constexpr int VEC = 8;
-  const int CV = C / VEC;
-  const int b = blockIdx.x / Ho, ho = blockIdx.x % Ho;
-  const int i0 = threadIdx.x;
-  const int wo_first = i0 >> lcv, cv = i0 & (CV - 1);
-  const int kh0 = (ho + pad) & (f - 1), kw0 = (wo_first + pad) & (f - 1);
-  const size_t xplane = (size_t)B * H * W * C, yplane = (size_t)B * Ho * Wo * C;
-  float wt[2][2][VEC];
-#pragma unroll
-  for (int a = 0; a < 2; ++a)
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      const float *wp = w + (size_t)((kh0 + a * f) * k + kw0 + c * f) * C + cv * VEC;
-#pragma unroll
-      for (int q = 0; q < VEC; q += 4) {
-        const float4 v = __ldg(reinterpret_cast<const float4 *>(wp + q));
-        wt[a][c][q] = v.x; wt[a][c][q + 1] = v.y; wt[a][c][q + 2] = v.z; wt[a][c][q + 3] = v.w;
-      }
-    }
-  const uint16_t *xb = x + (size_t)b * H * W * C + cv * VEC;
-  const int hn0 = ho + pad - kh0;                               // >= 0; tap a reads input row (hn0 >> lf) - a
-  const int hi0 = hn0 >> lf;
-  const size_t orow = ((size_t)b * Ho + ho) * Wo;
-  auto ld8 = [&](const uint16_t *p, size_t plane, float (&o)[VEC]) {
-    const uint4 h = __ldg(reinterpret_cast<const uint4 *>(p)), l = __ldg(reinterpret_cast<const uint4 *>(p + plane));
-    const uint32_t hw_[4] = {h.x, h.y, h.z, h.w}, lw_[4] = {l.x, l.y, l.z, l.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 a = Sp16::up(hw_[j], fmt), c = Sp16::up(lw_[j], fmt);
-      o[2 * j] = a.x + c.x; o[2 * j + 1] = a.y + c.y;
-    }
-  };
-#pragma unroll 2                                             // two pixels' loads in flight per thread (HBM-bound kernel)
-  for (int i = i0; i < Wo * CV; i += 256) {
-    const int wo = i >> lcv;
-    const size_t opix = (orow + wo) * C + cv * VEC;
-    float acc[VEC];
-    if (skip) ld8(skip + opix, yplane, acc);
-    else {
-#pragma unroll
-      for (int q = 0; q < VEC; ++q) acc[q] = 0.f;
-    }
-    const int wi0 = (wo + pad - kw0) >> lf;
-#pragma unroll
-    for (int a = 0; a < 2; ++a) {
-      const int hi = hi0 - a;
-      if (hi < 0 || hi >= H) continue;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const int wi = wi0 - c;
-        if (wi < 0 || wi >= W) continue;
-        float v[VEC];
-        ld8(xb + ((size_t)hi * W + wi) * C, xplane, v);
-#pragma unroll
-        for (int q = 0; q < VEC; ++q) acc[q] = fmaf(v[q], wt[a][c][q], acc[q]);
-      }
-    }
-    uint4 oh, ol;
-    Sp16::split2(acc[0], acc[1], fmt, oh.x, ol.x); Sp16::split2(acc[2], acc[3], fmt, oh.y, ol.y);
-    Sp16::split2(acc[4], acc[5], fmt, oh.z, ol.z); Sp16::split2(acc[6], acc[7], fmt, oh.w, ol.w);
-    *reinterpret_cast<uint4 *>(y + opix) = oh;
-    *reinterpret_cast<uint4 *>(y + opix + yplane) = ol;
-  }
-}
-
 
 // ---- space-to-depth of the network input (CPB200_OP_S2D): NCHW fp32 (B,3,H,W) -> split planes (B,H/2,W/2,16) ----
 // Thread = one output pixel: six coalesced float2 loads (channel c, row parity py: the two column parities), channel
@@ -1004,96 +838,6 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
       s2d_split_kernel<<<grid, 256, 0, st>>>(static_cast<const float *>(op.src[0]), static_cast<uint16_t *>(op.dst), op.B, op.H, op.W,
                                              (size_t)total * 16, fmt);
       return cpb::check_launch("s2d_split_kernel");
-    }
-    case CPB200_OP_MAXPOOL: {
-      if (op.cin[0] % 4) return cpb::fail(CPB200_ERR_ARG, "maxpool: C %% 4 != 0");
-      const long long total = (long long)op.B * op.Ho * op.Wo * (op.cin[0] / 4);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 32);
-      maxpool_split_kernel<<<grid, 256, 0, st>>>(static_cast<const uint16_t *>(op.src[0]), static_cast<uint16_t *>(op.dst),
-                                                 op.B, op.H, op.W, op.cin[0], op.Ho, op.Wo, op.kh, op.stride, op.pad_h, fmt);
-      return cpb::check_launch("maxpool_split_kernel");
-    }
-    case CPB200_OP_DWDECONV_ADD: {
-      if (op.cin[0] % 4 || op.kh != 2 * op.stride) return cpb::fail(CPB200_ERR_ARG, "dwdeconv (split): needs C %% 4 == 0 and k == 2 * stride");
-      {
-        auto ilog2 = [](int v) { int l = 0; while ((1 << l) < v) ++l; return (1 << l) == v ? l : -1; };
-        const int C = op.cin[0];
-        const int lf = ilog2(op.stride), lcv = (C % 8 == 0) ? ilog2(C / 8) : -1;
-        const int CVv = C / 8;
-        if (lf >= 0 && lcv >= 0 && CVv <= 256 && (256 / CVv) % op.stride == 0 && getenv("CPB200_DWDECONV_GENERIC") == nullptr) {
-          dwdeconv_add_split_fast_kernel<<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(static_cast<const uint16_t *>(op.src[0]),
-              static_cast<const uint16_t *>(op.aux), static_cast<uint16_t *>(op.dst), static_cast<const float *>(op.weight),
-              op.B, op.H, op.W, C, op.Ho, op.Wo, op.kh, op.stride, op.pad_h, lf, lcv, fmt);
-          return cpb::check_launch("dwdeconv_add_split_fast_kernel");
-        }
-      }
-      dwdeconv_add_split_kernel<<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(static_cast<const uint16_t *>(op.src[0]),
-          static_cast<const uint16_t *>(op.aux), static_cast<uint16_t *>(op.dst), static_cast<const float *>(op.weight),
-          op.B, op.H, op.W, op.cin[0], op.Ho, op.Wo, op.kh, op.stride, op.pad_h, fmt);
-      return cpb::check_launch("dwdeconv_add_split_kernel");
-    }
-    // The element-wise MobileNetV3 / HRNet ops run their fp32 kernels straight on the planes (SpC / SpM handles):
-    // no fp32 island, no CONVERT passes.  fp32 arithmetic on hi + lo, result re-split; the depthwise conv is instantiated
-    // with T = bf16 only to select act_out's multiply-by-1/6 h-swish (VEC stays 4: the handles load 8 bytes per plane).
-    case CPB200_OP_DWCONV: {
-      constexpr int VEC = 4;
-      const int C = op.cin[0];
-      if (C % VEC || op.kh != op.kw || op.cout != C || (op.src_pitch[0] != 0 && op.src_pitch[0] != C)) return cpb::fail(CPB200_ERR_ARG, "dwconv (split): C %% 4 != 0, non-square kernel or sliced input");
-      const SpC x{static_cast<const uint16_t *>(op.src[0]), (size_t)op.B * op.H * op.W * C, fmt};
-      const SpM y{static_cast<uint16_t *>(op.dst), (size_t)op.B * op.Ho * op.Wo * C, fmt};
-#define DW_TILED(KK, SS, PX)                                                                                   \
-  if (op.kh == KK && op.stride == SS && op.pad_h == KK / 2) {                                                    \
-    const long long tot = (long long)op.B * op.Ho * ((op.Wo + PX - 1) / PX) * (C / VEC);                         \
-    const unsigned g = (unsigned)std::min<long long>((tot + 255) / 256, 132LL * 32);                            \
-    dwconv_tiled_kernel<bf16, VEC, KK, SS, PX, SpC, SpM><<<g, 256, 0, st>>>(x, y, static_cast<const float *>(op.weight), \
-        op.bias, tot, op.H, op.W, C, op.Ho, op.Wo, op.flags & CPB_ACT_MASK);                                    \
-    return cpb::check_launch("dwconv_tiled_kernel");                                                            \
-  }
-      DW_TILED(3, 1, 4) DW_TILED(5, 1, 4) DW_TILED(3, 2, 2) DW_TILED(5, 2, 2)
-#undef DW_TILED
-      const long long total = (long long)op.B * op.Ho * op.Wo * (C / VEC);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 32);
-      dwconv_kernel<bf16, VEC, SpC, SpM><<<grid, 256, 0, st>>>(x, y, static_cast<const float *>(op.weight), op.bias, total,
-          op.H, op.W, C, op.Ho, op.Wo, op.kh, op.stride, op.pad_h, op.flags & CPB_ACT_MASK);
-      return cpb::check_launch("dwconv_kernel");
-    }
-    case CPB200_OP_AVGPOOL: {                           // split planes in, fp32 (B,1,1,C) out: the SE convs that follow run on fp32
-      const int C = op.cin[0];
-      if (C % 4 || op.Ho != 1 || op.Wo != 1 || (op.src_pitch[0] != 0 && op.src_pitch[0] != C)) return cpb::fail(CPB200_ERR_ARG, "avgpool (split): C %% 4 != 0, output not 1x1 or sliced input");
-      const SpC x{static_cast<const uint16_t *>(op.src[0]), (size_t)op.B * op.H * op.W * C, fmt};
-      avgpool_kernel<float, SpC, float *><<<dim3((unsigned)op.B, (unsigned)((C + 63) / 64)), 256, 0, st>>>(x, static_cast<float *>(op.dst), op.H * op.W, C);
-      return cpb::check_launch("avgpool_kernel");
-    }
-    case CPB200_OP_SCALE_ADD: {                         // x, skip, y: split planes; the gate vector (B,1,1,C) is fp32
-      const int C = op.cin[0];
-      if (C % 4 || !op.res || (op.src_pitch[0] != 0 && op.src_pitch[0] != C)) return cpb::fail(CPB200_ERR_ARG, "scale_add (split): C %% 4 != 0, missing scale vector or sliced input");
-      const size_t plane = (size_t)op.B * op.H * op.W * C;
-      const long long per_image = (long long)op.H * op.W * (C / 4), total = per_image * op.B;
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
-      scale_add_kernel<float, SpC, const float *, SpM><<<grid, 256, 0, st>>>(SpC{static_cast<const uint16_t *>(op.src[0]), plane, fmt},
-          static_cast<const float *>(op.res), SpC{static_cast<const uint16_t *>(op.aux), plane, fmt},
-          SpM{static_cast<uint16_t *>(op.dst), plane, fmt}, total, per_image, C / 4);
-      return cpb::check_launch("scale_add_kernel");
-    }
-    case CPB200_OP_UPSAMPLE_ADD: {
-      const int f = op.stride, C = op.cin[0];
-      int sh = 0;
-      while ((1 << sh) < f) ++sh;
-      if (f < 1 || (1 << sh) != f || op.Ho != op.H * f || op.Wo != op.W * f || C % 4 || (op.src_pitch[0] != 0 && op.src_pitch[0] != C))
-        return cpb::fail(CPB200_ERR_ARG, "upsample_add (split): factor %d must be a power of two, C %% 4 == 0, whole-tensor input", f);
-      const size_t plane_o = (size_t)op.B * op.Ho * op.Wo * C;
-      const long long total = (long long)op.B * op.Ho * op.Wo * (C / 4);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
-      upsample_add_kernel<float, SpC, SpM><<<grid, 256, 0, st>>>(SpC{static_cast<const uint16_t *>(op.src[0]), (size_t)op.B * op.H * op.W * C, fmt},
-          SpC{static_cast<const uint16_t *>(op.aux), plane_o, fmt}, SpM{static_cast<uint16_t *>(op.dst), plane_o, fmt},
-          total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, op.flags & CPB_ACT_MASK);
-      return cpb::check_launch("upsample_add_kernel");
-    }
-    case CPB200_OP_AVGPOOL2:
-    case CPB200_OP_RESIZE_BILINEAR: {
-      const int C = op.cin[0];
-      return launch_resample<float, SpC, SpM>(op, SpC{static_cast<const uint16_t *>(op.src[0]), (size_t)op.B * op.H * op.W * C, fmt},
-                                              SpM{static_cast<uint16_t *>(op.dst), (size_t)op.B * op.Ho * op.Wo * C, fmt}, st);
     }
     default:
       return cpb::fail(CPB200_ERR_ARG, "op type %d has no split-precision kernel (the host must route it through fp32)", op.type);
@@ -1169,111 +913,148 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
 #undef STEM_LAUNCH_K
       return cpb::check_launch("stem_kernel");
     }
-    case CPB200_OP_IM2COL_W: {
-      const int cin = op.cin[0];
-      if (op.cout != 32 || cin * op.kw > 32) return cpb::fail(CPB200_ERR_ARG, "im2col_w: needs kw*cin <= 32 output channels");
-      const long long M = (long long)op.B * op.H * op.W;
-      im2col_w_kernel<T, 32><<<(unsigned)((M + 255) / 256), 256, 0, st>>>(static_cast<const float *>(op.src[0]),
-          static_cast<T *>(op.dst), op.B, cin, op.H, op.W, op.kw, op.pad_w);
-      return cpb::check_launch("im2col_w_kernel");
-    }
+    default: return cpb::fail(CPB200_ERR_ARG, "unknown op type %d", op.type);
+  }
+}
+
+bool is_eltwise(int type) {
+  switch (type) {
+    case CPB200_OP_MAXPOOL: case CPB200_OP_DWDECONV_ADD: case CPB200_OP_DWCONV: case CPB200_OP_AVGPOOL:
+    case CPB200_OP_SCALE_ADD: case CPB200_OP_UPSAMPLE_ADD: case CPB200_OP_AVGPOOL2: case CPB200_OP_RESIZE_BILINEAR: return true;
+    default: return false;
+  }
+}
+
+int ilog2(int v) {                                      // log2 of a power of two, else -1
+  int l = 0;
+  while ((1 << l) < v) ++l;
+  return (1 << l) == v ? l : -1;
+}
+
+// Activation handle of type P over the op tensor at p, n elements per plane (plain pointers ignore n and fmt).
+template <typename P> P io_handle(const void *p, size_t n, uint32_t fmt) {
+  void *q = const_cast<void *>(p);
+  if constexpr (std::is_same<P, SpC>::value) return SpC{static_cast<const uint16_t *>(q), n, fmt};
+  else if constexpr (std::is_same<P, SpM>::value) return SpM{static_cast<uint16_t *>(q), n, fmt};
+  else return static_cast<P>(q);
+}
+
+// The element-wise ops (is_eltwise) on every activation format: PI / PO are `const float *` / `float *`,
+// `const bf16 *` / `bf16 *`, or SpC / SpM on split planes (fmt: 1 = fp16, 0 = bf16 planes).  T is the element type of
+// the plain vectors next to the activations, SCALE_ADD's gate and AVGPOOL's output: the activation type, or fp32 next
+// to split planes (the SE convs around them run on fp32).
+template <typename T, typename PI, typename PO>
+int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
+  constexpr int VEC = 16 / sizeof(T);                   // channels per thread: 16 bytes, or 8 bytes per split plane
+  constexpr int VEC_FAST = std::is_same<PO, SpM>::value ? 8 : VEC;   // the fast dwdeconv: 16 bytes per plane
+  const int C = op.cin[0];
+  if (op.src_pitch[0] != 0 && op.src_pitch[0] != C)
+    return cpb::fail(CPB200_ERR_ARG, "op type %d: needs a dense input (src_pitch %d, C %d)", op.type, op.src_pitch[0], C);
+  const size_t n_in = (size_t)op.B * op.H * op.W * C, n_out = (size_t)op.B * op.Ho * op.Wo * C;
+  const PI x = io_handle<PI>(op.src[0], n_in, fmt), skip = io_handle<PI>(op.aux, n_out, fmt);
+  const PO y = io_handle<PO>(op.dst, n_out, fmt);
+  const float *w = static_cast<const float *>(op.weight);
+  const uint32_t act = op.flags & CPB_ACT_MASK;
+  auto grid = [](long long total, int ctas_per_sm) { return (unsigned)std::min<long long>((total + 255) / 256, 132LL * ctas_per_sm); };
+  switch (op.type) {
     case CPB200_OP_MAXPOOL: {
-      if (op.cin[0] % 4) return cpb::fail(CPB200_ERR_ARG, "maxpool: C %% 4 != 0");
-      const long long total = (long long)op.B * op.Ho * op.Wo * (op.cin[0] / 4);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 32);
-      maxpool_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T *>(op.src[0]), static_cast<T *>(op.dst),
-                                              op.B, op.H, op.W, op.cin[0], op.Ho, op.Wo, op.kh, op.stride, op.pad_h);
+      if (C % 4) return cpb::fail(CPB200_ERR_ARG, "maxpool: C %% 4 != 0");
+      maxpool_kernel<PI, PO><<<grid((long long)op.B * op.Ho * op.Wo * (C / 4), 32), 256, 0, st>>>(x, y, op.B, op.H, op.W, C,
+          op.Ho, op.Wo, op.kh, op.stride, op.pad_h);
       return cpb::check_launch("maxpool_kernel");
     }
     case CPB200_OP_DWDECONV_ADD: {
-      constexpr int VEC = sizeof(T) == 2 ? 8 : 4;
-      if (op.cin[0] % VEC) return cpb::fail(CPB200_ERR_ARG, "dwdeconv: C %% %d != 0", VEC);
-      const size_t smem = (size_t)op.kh * op.kh * op.cin[0] * sizeof(float);
-      if (smem > 160 * 1024) return cpb::fail(CPB200_ERR_ARG, "dwdeconv: filter does not fit shared memory");
-      if (smem > 48 * 1024 &&
-          cudaFuncSetAttribute(dwdeconv_add_kernel<T, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return cpb::fail(CPB200_ERR_CUDA, "dwdeconv: cannot raise the shared-memory limit to %zu bytes", smem);
-      auto ilog2 = [](int v) { int l = 0; while ((1 << l) < v) ++l; return (1 << l) == v ? l : -1; };
-      {
-        const int lf = ilog2(op.stride), lcv = ilog2(op.cin[0] / VEC);
-        const int CVv = op.cin[0] / VEC;
-        if (lf >= 0 && lcv >= 0 && op.kh == 2 * op.stride && CVv <= 256 && (256 / CVv) % op.stride == 0 && getenv("CPB200_DWDECONV_GENERIC") == nullptr) {
-          dwdeconv_add_fast_kernel<T, VEC><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(static_cast<const T *>(op.src[0]),
-              static_cast<const T *>(op.aux), static_cast<T *>(op.dst), static_cast<const float *>(op.weight),
-              op.H, op.W, op.cin[0], op.Ho, op.Wo, op.kh, op.stride, op.pad_h, lf, lcv);
-          return cpb::check_launch("dwdeconv_add_fast_kernel");
-        }
+      if (C % VEC || op.stride < 1) return cpb::fail(CPB200_ERR_ARG, "dwdeconv: needs C %% %d == 0 and stride >= 1", VEC);
+      const int lf = ilog2(op.stride), CV = C / VEC_FAST, lcv = C % VEC_FAST ? -1 : ilog2(CV);
+      // the fast kernel's shapes: k == 2f, f and C / VEC_FAST powers of two, and each CTA's 256 threads cover whole
+      // output pixels of one column parity class
+      if (lf >= 0 && lcv >= 0 && op.kh == 2 * op.stride && CV <= 256 && (256 / CV) % op.stride == 0) {
+        dwdeconv_add_fast_kernel<VEC_FAST, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.H, op.W, C, op.Ho,
+            op.Wo, op.kh, op.stride, op.pad_h, lf, lcv);
+        return cpb::check_launch("dwdeconv_add_fast_kernel");
       }
-      dwdeconv_add_kernel<T, VEC><<<(unsigned)(op.B * op.Ho), 256, smem, st>>>(static_cast<const T *>(op.src[0]),
-          static_cast<const T *>(op.aux), static_cast<T *>(op.dst), static_cast<const float *>(op.weight),
-          op.H, op.W, op.cin[0], op.Ho, op.Wo, op.kh, op.stride, op.pad_h, ilog2(op.stride), ilog2(op.cin[0] / VEC));
+      dwdeconv_add_kernel<VEC, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.H, op.W, C, op.Ho, op.Wo,
+          op.kh, op.stride, op.pad_h, lf, ilog2(C / VEC));
       return cpb::check_launch("dwdeconv_add_kernel");
     }
     case CPB200_OP_DWCONV: {
-      constexpr int VEC = sizeof(T) == 2 ? 8 : 4;
-      const int C = op.cin[0];
       if (C % VEC || op.kh != op.kw || op.cout != C) return cpb::fail(CPB200_ERR_ARG, "dwconv: C %% %d != 0 or non-square kernel", VEC);
 #define DW_TILED(KK, SS, PX)                                                                                   \
   if (op.kh == KK && op.stride == SS && op.pad_h == KK / 2) {                                                    \
     const long long tot = (long long)op.B * op.Ho * ((op.Wo + PX - 1) / PX) * (C / VEC);                         \
-    const unsigned g = (unsigned)std::min<long long>((tot + 255) / 256, 132LL * 32);                            \
-    dwconv_tiled_kernel<T, VEC, KK, SS, PX><<<g, 256, 0, st>>>(static_cast<const T *>(op.src[0]),                \
-        static_cast<T *>(op.dst), static_cast<const float *>(op.weight), op.bias, tot, op.H, op.W, C, op.Ho,     \
-        op.Wo, op.flags & CPB_ACT_MASK);                                                                        \
+    dwconv_tiled_kernel<VEC, KK, SS, PX, PI, PO><<<grid(tot, 32), 256, 0, st>>>(x, y, w, op.bias, tot, op.H, op.W, C, \
+        op.Ho, op.Wo, act);                                                                                     \
     return cpb::check_launch("dwconv_tiled_kernel");                                                            \
   }
       DW_TILED(3, 1, 4) DW_TILED(5, 1, 4) DW_TILED(3, 2, 2) DW_TILED(5, 2, 2)
 #undef DW_TILED
       const long long total = (long long)op.B * op.Ho * op.Wo * (C / VEC);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 32);
-      dwconv_kernel<T, VEC><<<grid, 256, 0, st>>>(static_cast<const T *>(op.src[0]), static_cast<T *>(op.dst),
-          static_cast<const float *>(op.weight), op.bias, total, op.H, op.W, C, op.Ho, op.Wo, op.kh, op.stride, op.pad_h,
-          op.flags & CPB_ACT_MASK);
+      dwconv_kernel<VEC, PI, PO><<<grid(total, 32), 256, 0, st>>>(x, y, w, op.bias, total, op.H, op.W, C, op.Ho, op.Wo, op.kh,
+          op.stride, op.pad_h, act);
       return cpb::check_launch("dwconv_kernel");
     }
     case CPB200_OP_AVGPOOL: {
-      const int C = op.cin[0];
       if (C % 4 || op.Ho != 1 || op.Wo != 1) return cpb::fail(CPB200_ERR_ARG, "avgpool: C %% 4 != 0 or output not 1x1");
-      avgpool_kernel<T><<<dim3((unsigned)op.B, (unsigned)((C + 63) / 64)), 256, 0, st>>>(static_cast<const T *>(op.src[0]),
-          static_cast<T *>(op.dst), op.H * op.W, C);
+      avgpool_kernel<PI, T *><<<dim3((unsigned)op.B, (unsigned)((C + 63) / 64)), 256, 0, st>>>(x, static_cast<T *>(op.dst),
+          op.H * op.W, C);
       return cpb::check_launch("avgpool_kernel");
     }
-    case CPB200_OP_SCALE_ADD: {
-      const int C = op.cin[0];
+    case CPB200_OP_SCALE_ADD: {                         // the output and the skip have the input's shape
       if (C % 4 || !op.res) return cpb::fail(CPB200_ERR_ARG, "scale_add: C %% 4 != 0 or missing scale vector");
       const long long per_image = (long long)op.H * op.W * (C / 4), total = per_image * op.B;
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
-      scale_add_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T *>(op.src[0]), static_cast<const T *>(op.res),
-          static_cast<const T *>(op.aux), static_cast<T *>(op.dst), total, per_image, C / 4);
+      scale_add_kernel<PI, const T *, PO><<<grid(total, 16), 256, 0, st>>>(x, static_cast<const T *>(op.res),
+          io_handle<PI>(op.aux, n_in, fmt), io_handle<PO>(op.dst, n_in, fmt), total, per_image, C / 4);
       return cpb::check_launch("scale_add_kernel");
     }
     case CPB200_OP_UPSAMPLE_ADD: {
-      const int f = op.stride;
-      int sh = 0;
-      while ((1 << sh) < f) ++sh;
-      if (f < 1 || (1 << sh) != f || op.Ho != op.H * f || op.Wo != op.W * f || op.cin[0] % 4)
-        return cpb::fail(CPB200_ERR_ARG, "upsample_add: factor %d must be a power of two, C %% 4 == 0", f);
-      const long long total = (long long)op.B * op.Ho * op.Wo * (op.cin[0] / 4);
-      const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
-      upsample_add_kernel<T><<<grid, 256, 0, st>>>(static_cast<const T *>(op.src[0]), static_cast<const T *>(op.aux),
-          static_cast<T *>(op.dst), total, op.H, op.W, op.cin[0] / 4, op.Ho, op.Wo, sh, op.flags & CPB_ACT_MASK);
+      const int sh = ilog2(op.stride);
+      if (sh < 0 || op.Ho != op.H * op.stride || op.Wo != op.W * op.stride || C % 4)
+        return cpb::fail(CPB200_ERR_ARG, "upsample_add: factor %d must be a power of two, C %% 4 == 0", op.stride);
+      const long long total = (long long)op.B * op.Ho * op.Wo * (C / 4);
+      upsample_add_kernel<PI, PO><<<grid(total, 16), 256, 0, st>>>(x, skip, y, total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, act);
       return cpb::check_launch("upsample_add_kernel");
     }
-    case CPB200_OP_AVGPOOL2:
-    case CPB200_OP_RESIZE_BILINEAR:
-      return launch_resample<T, const T *, T *>(op, static_cast<const T *>(op.src[0]), static_cast<T *>(op.dst), st);
-    default: return cpb::fail(CPB200_ERR_ARG, "unknown op type %d", op.type);
+    default: {                                          // CPB200_OP_AVGPOOL2, CPB200_OP_RESIZE_BILINEAR
+      const bool pool = op.type == CPB200_OP_AVGPOOL2;
+      if (op.nsrc != 1 || C % 4 || op.cout != C)
+        return cpb::fail(CPB200_ERR_ARG, "%s: needs one input with C %% 4 == 0 and cout == C (nsrc %d, C %d, cout %d)",
+                         pool ? "avgpool2" : "resize_bilinear", op.nsrc, C, op.cout);
+      const long long total = (long long)op.B * op.Ho * op.Wo * (C / 4);
+      if (pool) {
+        if (op.H < 2 || op.W < 2 || op.Ho != op.H / 2 || op.Wo != op.W / 2)
+          return cpb::fail(CPB200_ERR_ARG, "avgpool2: %dx%d -> %dx%d is not a 2x2 / stride-2 floor-mode pool (needs H, W >= 2)",
+                           op.H, op.W, op.Ho, op.Wo);
+        avgpool2_kernel<PI, PO><<<grid(total, 16), 256, 0, st>>>(x, y, total, op.H, op.W, C / 4, op.Ho, op.Wo);
+        return cpb::check_launch("avgpool2_kernel");
+      }
+      if (op.Ho < 1 || op.Wo < 1) return cpb::fail(CPB200_ERR_ARG, "resize_bilinear: output size %dx%d", op.Ho, op.Wo);
+      const float sh = op.Ho > 1 ? (float)(op.H - 1) / (float)(op.Ho - 1) : 0.f;
+      const float sw = op.Wo > 1 ? (float)(op.W - 1) / (float)(op.Wo - 1) : 0.f;
+      resize_bilinear_kernel<PI, PO><<<grid(total, 16), 256, 0, st>>>(x, y, total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, sw);
+      return cpb::check_launch("resize_bilinear_kernel");
+    }
   }
 }
 
 }  // namespace
 
 namespace cpb {
+// Split-plane activations without CPB200_FLAG_TC: the element-wise ops and the two conversions run here; CONV, DCN and
+// STEM need the tensor-core path (the host runs their other shapes on fp32 between CONVERT ops).
+bool simt_runs_split(int type) { return is_eltwise(type) || type == CPB200_OP_CONVERT || type == CPB200_OP_S2D; }
+
 int run_op_simt_dispatch(const cpb200_op &op, cudaStream_t st) {
-  if (op.act_dtype == CPB200_BF16X2 || op.act_dtype == CPB200_F16X2) return run_op_split(op, st);
-  if (op.type == CPB200_OP_CONVERT) return fail(CPB200_ERR_ARG, "convert: act_dtype must name a split layout");
-  if (op.act_dtype == CPB200_F32) return run_op_simt<float>(op, st);
-  if (op.act_dtype == CPB200_BF16) return run_op_simt<__nv_bfloat16>(op, st);
+  const bool split = op.act_dtype == CPB200_BF16X2 || op.act_dtype == CPB200_F16X2;
+  if (is_eltwise(op.type)) {
+    if (split) return run_eltwise<float, SpC, SpM>(op, op.act_dtype == CPB200_F16X2 ? 1u : 0u, st);
+    if (op.act_dtype == CPB200_F32) return run_eltwise<float, const float *, float *>(op, 0, st);
+    if (op.act_dtype == CPB200_BF16) return run_eltwise<bf16, const bf16 *, bf16 *>(op, 0, st);
+  } else {
+    if (split) return run_op_split(op, st);
+    if (op.type == CPB200_OP_CONVERT) return fail(CPB200_ERR_ARG, "convert: act_dtype must name a split layout");
+    if (op.act_dtype == CPB200_F32) return run_op_simt<float>(op, st);
+    if (op.act_dtype == CPB200_BF16) return run_op_simt<bf16>(op, st);
+  }
   return fail(CPB200_ERR_ARG, "bad act_dtype %d", op.act_dtype);
 }
 }  // namespace cpb

@@ -24,7 +24,7 @@ import torch
 
 from . import _lib
 
-OP_CONV, OP_STEM, OP_MAXPOOL, OP_DWDECONV_ADD, OP_DCN, OP_IM2COL_W, OP_UPSAMPLE_ADD = 1, 2, 3, 4, 5, 6, 7
+OP_CONV, OP_STEM, OP_MAXPOOL, OP_DWDECONV_ADD, OP_DCN, OP_UPSAMPLE_ADD = 1, 2, 3, 4, 5, 7      # 6 is retired
 OP_DWCONV, OP_AVGPOOL, OP_SCALE_ADD, OP_CONVERT, OP_S2D = 8, 9, 10, 11, 12
 OP_AVGPOOL2, OP_RESIZE_BILINEAR = 13, 14
 FLAG_RELU, FLAG_OUT_NCHW_F32, FLAG_OUT_F32, FLAG_TC, FLAG_HSWISH, FLAG_HSIGMOID, FLAG_TO_F32 = 1, 2, 4, 8, 16, 32, 64
@@ -353,24 +353,12 @@ class PlanBuilder:
 
     # ---- ops -------------------------------------------------------------------------------
     # Split precisions (bf16x2 / fp16x2): convs, DCNs and the stride-1 stem run natively on the hi/lo planes (tensor-core
-    # kernels), max-pool and the IDAUp depthwise upsample have split kernels; everything else (and conv shapes the
-    # tensor-core kernels do not take, e.g. maps narrower than 8 pixels) runs on fp32 between two CONVERT ops — an
-    # "fp32 island": slower, never less precise.
+    # kernels), and so do the element-wise ops (_eltwise); everything else (conv shapes the tensor-core kernels do not
+    # take, e.g. maps narrower than 8 pixels, and element-wise ops on channel slices) runs on fp32 between two CONVERT
+    # ops — an "fp32 island": slower, never less precise.
     def stem(self, x: Sym, w, b, k, stride, pad, relu=True, act=None):
         co, ci = w.shape[0], w.shape[1]
         mode = os.environ.get("CPB200_TC_STEM", "1")
-        if (self.use_tc and not self.split and mode == "im2col" and stride == 1 and k * ci <= 32 and co % 16 == 0 and pad == k // 2):
-            # first tensor-core stem (kept for the record, CPB200_TC_STEM=im2col): gather the k horizontal taps of
-            # every pixel into 32 channels IN HBM, then a k x 1 conv with K = k * 32 on the halo-reuse kernel.
-            # Correct (tests/test_net_gpu.py::test_stem_im2col_path) but measured SLOWER than the CUDA-core stem at
-            # B=32 512x512 (1430 us vs 1045 us: 537 MB intermediate + 65 536 N=16 tiles).
-            t = self._sym(32, x.H, x.W)
-            self._emit(_PendingOp(type=OP_IM2COL_W, flags=0, k=(1, k), stride=1, pad=(0, pad), weight=None,
-                                  bias=None, cout=32), [x], t)
-            w2 = torch.zeros(co, 32, k, 1, dtype=torch.float32, device=w.device)
-            # w2[o, s*ci + c, r, 0] = w[o, c, r, s]
-            w2[:, :k * ci, :, 0] = w.float().permute(0, 3, 1, 2).reshape(co, k * ci, k)
-            return self.conv([t], w2, b.float(), stride=1, relu=relu, pad_hw=(pad, 0))
         if (self.use_tc and self.split and mode != "0" and stride == 2 and ci == 3 and k in (3, 7) and pad == k // 2
                 and co % 16 == 0 and x.H % 2 == 0 and x.W % 2 == 0 and x.kind == "nchw_in"
                 and os.environ.get("CPB200_S2D_STEM", "1") != "0"):
@@ -475,38 +463,35 @@ class PlanBuilder:
                           pad_hw=(1 - a, 1 - bb), out_map=(Ho, Wo, 2, 2, a, bb, x.H, x.W))
         return self._to_split(y) if island else y
 
+    def _eltwise(self, op: _PendingOp, x: Sym, C, H, W, extra=(), gate: Optional[Sym] = None, f32_out=False) -> Sym:
+        """Emit an element-wise op (csrc/net_simt.cu: run_eltwise).  fp32 / bf16 run it natively.  Split precisions run
+        it on the planes (SpC / SpM handles) when every activation operand is a whole split tensor; there the SCALE_ADD
+        ``gate`` is read as fp32 and ``f32_out`` (AVGPOOL) writes an fp32 result.  Otherwise it runs on fp32 between
+        CONVERT ops (an fp32 island).  ``extra`` and ``gate`` become the op's extra operands, gate first."""
+        if self.split and all(s is None or (s.kind == "act" and s.parent is None) for s in [x, *extra]) \
+                and (gate is None or gate.parent is None):
+            y = self._sym(C, H, W, "actf32" if f32_out else "act")
+            self._emit(op, [x], y, ([self._to_f32(gate)] if gate is not None else []) + list(extra))
+            return self._to_split(y)
+        if self.split:
+            op.dtype = F32
+        y = self._island_sym(C, H, W)
+        self._emit(op, [self._to_f32(x)], y, [self._to_f32(e) for e in ([gate] if gate is not None else []) + list(extra)])
+        return self._to_split(y)
+
     def maxpool(self, x: Sym, k=2, stride=2, pad=0):
         Ho = (x.H + 2 * pad - k) // stride + 1; Wo = (x.W + 2 * pad - k) // stride + 1
-        y = self._sym(x.C, Ho, Wo)
-        self._emit(_PendingOp(type=OP_MAXPOOL, flags=0, k=(k, k), stride=stride, pad=(pad, pad),
-                              weight=None, bias=None, cout=x.C), [x], y)
-        return y
+        return self._eltwise(_PendingOp(type=OP_MAXPOOL, flags=0, k=(k, k), stride=stride, pad=(pad, pad),
+                                        weight=None, bias=None, cout=x.C), x, x.C, Ho, Wo)
 
     def up_add(self, x: Sym, skip: Optional[Sym], w):
         """depthwise ConvTranspose2d weight (C,1,2f,2f), stride f, pad f//2, + skip."""
         C, _, k, _ = w.shape
         f = k // 2
         Ho = (x.H - 1) * f - 2 * (f // 2) + k; Wo = (x.W - 1) * f - 2 * (f // 2) + k
-        y = self._sym(C, Ho, Wo)
         wp = self._dev(w.float().reshape(C, k * k).t())          # [k*k][C]
-        self._emit(_PendingOp(type=OP_DWDECONV_ADD, flags=0, k=(k, k), stride=f, pad=(f // 2, f // 2),
-                              weight=wp, bias=None, cout=C), [x], y, [skip])
-        return y
-
-    def _f32_op(self, op: _PendingOp, srcs, C, H, W, extra=()):
-        """emit an op that has no split kernel: on fp32 between CONVERT ops in split mode, natively otherwise."""
-        if self.split:
-            op.dtype = F32
-            srcs = [self._to_f32(s_) for s_ in srcs]
-            extra = [self._to_f32(e) for e in extra]
-        y = self._island_sym(C, H, W)
-        self._emit(op, srcs, y, list(extra))
-        return self._to_split(y)
-
-    def _native_split(self, *syms) -> bool:
-        """split mode and every operand a whole split-plane tensor: the element-wise kernels then read / write the planes
-        directly (csrc/net_simt.cu: SpC / SpM handles) and no fp32 island is needed."""
-        return self.split and all(s is None or (s.kind == "act" and s.parent is None) for s in syms)
+        return self._eltwise(_PendingOp(type=OP_DWDECONV_ADD, flags=0, k=(k, k), stride=f, pad=(f // 2, f // 2),
+                                        weight=wp, bias=None, cout=C), x, C, Ho, Wo, [skip])
 
     def dwconv(self, x: Sym, w, b, stride=1, act=None):
         """depthwise conv, w (C,1,k,k) BN-folded, pad k//2   (mobilenetv3.py:124-127)."""
@@ -514,61 +499,35 @@ class PlanBuilder:
         assert C == x.C
         Ho = (x.H + 2 * (k // 2) - k) // stride + 1; Wo = (x.W + 2 * (k // 2) - k) // stride + 1
         wp = self._dev(w.float().reshape(C, k * k).t())          # [k*k][C]
-        op = _PendingOp(type=OP_DWCONV, flags=_ACT_FLAG[act], k=(k, k), stride=stride, pad=(k // 2, k // 2),
-                        weight=wp, bias=self._dev(b), cout=C)
-        if self._native_split(x):
-            y = self._sym(C, Ho, Wo, "act")
-            self._emit(op, [x], y)
-            return y
-        return self._f32_op(op, [x], C, Ho, Wo)
+        return self._eltwise(_PendingOp(type=OP_DWCONV, flags=_ACT_FLAG[act], k=(k, k), stride=stride, pad=(k // 2, k // 2),
+                                        weight=wp, bias=self._dev(b), cout=C), x, C, Ho, Wo)
 
     def avgpool(self, x: Sym):
         """global average pool -> (C, 1, 1)   (mobilenetv3.py:100).  Split mode: planes in, fp32 out (the 1x1-map SE convs
         that follow run on fp32 anyway)."""
-        op = _PendingOp(type=OP_AVGPOOL, flags=0, k=(x.H, x.W), stride=1, pad=(0, 0), weight=None, bias=None, cout=x.C)
-        if self._native_split(x):
-            y = self._island_sym(x.C, 1, 1)
-            self._emit(op, [x], y)
-            return self._to_split(y)                                # dead unless someone wants the planes; pruned
-        return self._f32_op(op, [x], x.C, 1, 1)
+        return self._eltwise(_PendingOp(type=OP_AVGPOOL, flags=0, k=(x.H, x.W), stride=1, pad=(0, 0), weight=None, bias=None,
+                                        cout=x.C), x, x.C, 1, 1, f32_out=True)
 
     def scale_add(self, x: Sym, gate: Sym, skip: Optional[Sym] = None):
         """x * gate[b, c] (+ skip)   (mobilenetv3.py:111,146).  Split mode: x / skip / result are planes, the gate is fp32."""
         assert gate.C == x.C and gate.H == 1 and gate.W == 1
-        op = _PendingOp(type=OP_SCALE_ADD, flags=0, k=(1, 1), stride=1, pad=(0, 0), weight=None, bias=None, cout=x.C)
-        if self._native_split(x, skip) and gate.parent is None:
-            y = self._sym(x.C, x.H, x.W, "act")
-            self._emit(op, [x], y, [self._to_f32(gate), skip])
-            return y
-        return self._f32_op(op, [x], x.C, x.H, x.W, [gate, skip])
+        return self._eltwise(_PendingOp(type=OP_SCALE_ADD, flags=0, k=(1, 1), stride=1, pad=(0, 0), weight=None, bias=None,
+                                        cout=x.C), x, x.C, x.H, x.W, [skip], gate=gate)
 
     def upsample_add(self, x: Sym, skip: Optional[Sym], f: int, relu=False):
         """nearest-neighbour upsample x f of ``x`` (+ skip)(+ReLU)   (pose_higher_hrnet.py:186-187,224-232)."""
-        op = _PendingOp(type=OP_UPSAMPLE_ADD, flags=FLAG_RELU if relu else 0, k=(1, 1), stride=f, pad=(0, 0),
-                        weight=None, bias=None, cout=x.C)
-        if self._native_split(x, skip):
-            y = self._sym(x.C, x.H * f, x.W * f, "act")
-            self._emit(op, [x], y, [skip])
-            return y
-        return self._f32_op(op, [x], x.C, x.H * f, x.W * f, [skip])
+        return self._eltwise(_PendingOp(type=OP_UPSAMPLE_ADD, flags=FLAG_RELU if relu else 0, k=(1, 1), stride=f, pad=(0, 0),
+                                        weight=None, bias=None, cout=x.C), x, x.C, x.H * f, x.W * f, [skip])
 
     def avgpool2(self, x: Sym):
         """2x2 / stride-2 average pool, floor mode   (hardnet.py:141 nn.AvgPool2d(2, 2))."""
-        op = _PendingOp(type=OP_AVGPOOL2, flags=0, k=(2, 2), stride=2, pad=(0, 0), weight=None, bias=None, cout=x.C)
-        if self._native_split(x):
-            y = self._sym(x.C, x.H // 2, x.W // 2, "act")
-            self._emit(op, [x], y)
-            return y
-        return self._f32_op(op, [x], x.C, x.H // 2, x.W // 2)
+        return self._eltwise(_PendingOp(type=OP_AVGPOOL2, flags=0, k=(2, 2), stride=2, pad=(0, 0), weight=None, bias=None,
+                                        cout=x.C), x, x.C, x.H // 2, x.W // 2)
 
     def resize_bilinear(self, x: Sym, Ho: int, Wo: int):
         """bilinear resize to (Ho, Wo) with align_corners=True   (hardnet.py:95-100, TransitionUp)."""
-        op = _PendingOp(type=OP_RESIZE_BILINEAR, flags=0, k=(1, 1), stride=1, pad=(0, 0), weight=None, bias=None, cout=x.C)
-        if self._native_split(x):
-            y = self._sym(x.C, Ho, Wo, "act")
-            self._emit(op, [x], y)
-            return y
-        return self._f32_op(op, [x], x.C, Ho, Wo)
+        return self._eltwise(_PendingOp(type=OP_RESIZE_BILINEAR, flags=0, k=(1, 1), stride=1, pad=(0, 0), weight=None,
+                                        bias=None, cout=x.C), x, x.C, Ho, Wo)
 
     def dcn(self, x: Sym, w, b, om_w, om_b, relu=True):
         """DCN module (dcn_v2.py:117-127) with BN already folded into (w, b)."""

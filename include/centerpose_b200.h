@@ -167,10 +167,10 @@ enum cpb200_op_type {
                                 (7x7, Cin 3, stride 1/2, cout 16/64, bf16) the im2col is built in shared memory and
                                 the arithmetic runs on wgmma (weight = pre-swizzled operand image, plan.py)     */
   CPB200_OP_MAXPOOL = 3,     /* k x k / stride s / pad p max-pool, NHWC                                     */
-  CPB200_OP_DWDECONV_ADD = 4,/* depthwise ConvTranspose2d(k=2f,s=f,p=f/2) (+ skip add), NHWC  (IDAUp up_*) */
+  CPB200_OP_DWDECONV_ADD = 4,/* depthwise ConvTranspose2d(k=2f,s=f,p=f/2) (+ skip add), NHWC  (IDAUp up_*);
+                                src[0], aux (the skip) and dst must be 16-byte aligned (16-byte vector accesses)  */
   CPB200_OP_DCN = 5,         /* modulated deformable 3x3 conv (DCNv2 forward) (+bias)(+ReLU)                */
-  CPB200_OP_IM2COL_W = 6,    /* NCHW fp32 image -> NHWC act: channel s*cin+c = x[c, h, w+s-pad_w], s < kw, zero-padded
-                                to `cout` channels.  Turns the 7x7 stem into a 7x1 tensor-core conv (K = 7 x 32).   */
+  /* 6 is retired (a horizontal-tap gather for the stem); the number is not reused */
   CPB200_OP_UPSAMPLE_ADD = 7,/* nearest-neighbour upsample x `stride` (power of two) of src[0] (+ aux skip add)(+ReLU),
                                 NHWC  (HRNet fuse_layers, pose_higher_hrnet.py:186-187,224-232)                     */
   CPB200_OP_DWCONV = 8,      /* depthwise k x k conv, stride s, pad k/2 (+bias)(+activation); weight fp32 [k*k][C]

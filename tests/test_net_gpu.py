@@ -193,13 +193,13 @@ def test_stem_maxpool_upadd_ops(precision):
         pb = _builder(B, precision)
         y = pb.maxpool(pb.external(_nhwc(t, dt)), k, s, p)
         assert torch.equal(_nchw(_run(pb, y)), F.max_pool2d(t, k, s, p))
-    # depthwise deconv (f = 2 and f = 4) + skip
-    for f in (2, 4):
-        C = 32
-        xx = torch.randn(B, C, 6, 7, generator=g).bfloat16().float()
-        ww = torch.rand(C, 1, 2 * f, 2 * f, generator=g)
+    # depthwise deconv (f = 2 and f = 4) + skip; C = 48 fails the fast kernel's shape condition (generic kernel) and
+    # draws from its own generator, so the cases after it see the same data as without it
+    for f, C, gen in ((2, 32, g), (4, 32, g), (2, 48, torch.Generator().manual_seed(48))):
+        xx = torch.randn(B, C, 6, 7, generator=gen).bfloat16().float()
+        ww = torch.rand(C, 1, 2 * f, 2 * f, generator=gen)
         ref_up = F.conv_transpose2d(xx, ww, None, stride=f, padding=f // 2, groups=C)
-        skip = torch.randn(ref_up.shape, generator=g).bfloat16().float()
+        skip = torch.randn(ref_up.shape, generator=gen).bfloat16().float()
         pb = _builder(B, precision)
         y = pb.up_add(pb.external(_nhwc(xx, dt)), pb.external(_nhwc(skip, dt)), ww.to(DEV))
         _check(_nchw(_run(pb, y)), ref_up + skip, precision)
@@ -290,27 +290,6 @@ def test_stem_tensor_core_kernel(co, stride, H, W):
     torch.cuda.synchronize()
     got = _nchw(plan.tensor(y))
     assert got.shape == ref.shape
-    err = (got - ref).abs().max().item()
-    assert err <= 1e-2 * ref.abs().max().item(), (err, ref.abs().max().item())
-
-
-def test_stem_im2col_path():
-    """7x7 stem lowered to im2col-W (32 ch) + 7x1 wgmma halo conv vs torch fp32 on bf16-rounded data."""
-    B, H, W = 2, 48, 40
-    g = torch.Generator().manual_seed(4)
-    x = torch.randn(B, 3, H, W, generator=g).bfloat16().float()
-    w = (torch.randn(16, 3, 7, 7, generator=g) * 0.1).bfloat16().float(); b = torch.randn(16, generator=g)
-    ref = F.relu(F.conv2d(x, w, b, padding=3))
-    os.environ["CPB200_TC_STEM"] = "im2col"
-    try:
-        pb = _builder(B, "bf16", tc=True); pb.H, pb.W = H, W
-        y = pb.stem(pb.input(3), w.to(DEV), b.to(DEV), 7, 1, 3, relu=True)
-    finally:
-        os.environ.pop("CPB200_TC_STEM", None)
-    assert [o.type for o in pb.ops] == [6, 1] and pb.ops[1].flags & 8
-    plan = pb.build(); plan.bind(x.to(DEV), {}); plan.run(torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    got = _nchw(plan.tensor(y))
     err = (got - ref).abs().max().item()
     assert err <= 1e-2 * ref.abs().max().item(), (err, ref.abs().max().item())
 

@@ -5,7 +5,7 @@ TAG=${1:-r02}; NPER=${2:-96}; shift; shift
 mkdir -p gpurun_out
 SKIP=$((NPER * 3))
 ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none \
-    -k regex:"avgpool_kernel|conv3x3_tc_kernel|conv_simt_kernel|conv_sp_kernel|conv_tc_kernel|convert_from_split_kernel|convert_to_split_kernel|decode_kernel|dwconv_kernel|dwconv_tiled_kernel|dwdeconv_add_fast_kernel|dwdeconv_add_kernel|dwdeconv_add_split_fast_kernel|dwdeconv_add_split_kernel|flip_merge_kernel|im2col_w_kernel|maxpool_kernel|maxpool_split_kernel|scale_add_kernel|sigmoid_kernel|soft_nms_kernel|stem_kernel|stem_tc_h_kernel|stem_tc_kernel|upsample_add_kernel" \
+    -k regex:"avgpool_kernel|conv3x3_tc_kernel|conv_simt_kernel|conv_sp_kernel|conv_tc_kernel|convert_from_split_kernel|convert_to_split_kernel|decode_kernel|dwconv_kernel|dwconv_tiled_kernel|dwdeconv_add_fast_kernel|dwdeconv_add_kernel|flip_merge_kernel|maxpool_kernel|scale_add_kernel|sigmoid_kernel|soft_nms_kernel|stem_kernel|stem_tc_h_kernel|stem_tc_kernel|upsample_add_kernel" \
     -s ${SKIP} -c ${NPER} --csv --log-file gpurun_out/traffic_${TAG}.csv \
     python bench.py --steps 1 --warmup 3 --no-cpu-baseline --no-extras "$@" > gpurun_out/traffic_${TAG}.log 2>&1
 python - gpurun_out/traffic_${TAG}.csv <<'PY' > gpurun_out/traffic_${TAG}_summary.txt
