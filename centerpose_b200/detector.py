@@ -80,10 +80,13 @@ class BaseDetector(object):
         height, width = image.shape[0:2]
         new_height, new_width, inp_height, inp_width, trans_input, meta = self._pre_process_geometry(height, width, scale)
         if self.device_preprocess and image.dtype == np.uint8 and image.ndim == 3 and image.shape[2] == 3:
-            # warp + normalise + HWC->CHW (+ mirrored copy) in one CUDA kernel, bit-exact with the cv2 / numpy lines
-            # below (csrc/post.cu); a scale != 1 keeps cv2.resize on the host, as in the reference
-            resized = image if (new_width, new_height) == (width, height) else cv2.resize(image, (new_width, new_height))
-            return self._pre_process_device(resized, trans_input, inp_height, inp_width), meta
+            # resize, then warp + normalise + HWC->CHW (+ mirrored copy), as CUDA kernels bit-exact with the cv2 / numpy
+            # lines below (csrc/post.cu)
+            if (new_width, new_height) == (width, height):
+                src = torch.from_numpy(np.ascontiguousarray(image)).to(torch.device("cuda"), non_blocking=True)
+            else:
+                src = self._resize_device(image, new_height, new_width)
+            return self._pre_process_device(src, trans_input, inp_height, inp_width), meta
         resized = cv2.resize(image, (new_width, new_height))
         inp = cv2.warpAffine(resized, trans_input, (inp_width, inp_height), flags=cv2.INTER_LINEAR)
         inp = ((inp / 255. - self.mean) / self.std).astype(np.float32)
@@ -93,18 +96,36 @@ class BaseDetector(object):
         images = torch.from_numpy(np.ascontiguousarray(images))
         return images, meta
 
-    def _pre_process_device(self, image_u8, trans_input, inp_height, inp_width):
+    def _resize_device(self, image_u8, new_height, new_width):
+        """``cv2.resize(image_u8, (new_width, new_height))`` on the device: one upload of the image behind its
+        one-entry table, one ``cpb200_resize_linear_u8_batch``.  Returns the (new_height, new_width, 3) uint8 CUDA
+        tensor."""
+        from . import _lib
+        dev = torch.device("cuda")
+        table = resize_table([image_u8.shape[0:2]], [(new_height, new_width)])
+        host = np.empty(table.nbytes + image_u8.nbytes, np.uint8)
+        host[:table.nbytes] = table.view(np.uint8)
+        host[table.nbytes:] = np.ascontiguousarray(image_u8).reshape(-1)
+        buf = torch.from_numpy(host).to(dev)
+        out = torch.empty((new_height, new_width, 3), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            st = _lib.lib().cpb200_resize_linear_u8_batch(buf.data_ptr() + table.nbytes, buf.data_ptr(), 1, out.data_ptr(),
+                                                          torch.cuda.current_stream(dev).cuda_stream)
+        _lib.check(st, "resize_linear_u8_batch")
+        return out
+
+    def _pre_process_device(self, src, trans_input, inp_height, inp_width):
+        """``src``: the (h, w, 3) uint8 image as a CUDA tensor."""
         import ctypes
         from . import _lib
         dev = torch.device("cuda")
-        src = torch.from_numpy(np.ascontiguousarray(image_u8)).to(dev, non_blocking=True)
         flip = bool(self.cfg.TEST.FLIP_TEST)
         out = torch.empty((2 if flip else 1, 3, inp_height, inp_width), dtype=torch.float32, device=dev)
         M = (ctypes.c_double * 6)(*np.asarray(trans_input, np.float64).reshape(-1))
         mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
         std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
         with torch.cuda.device(dev):
-            st = _lib.lib().cpb200_pre_process(src.data_ptr(), image_u8.shape[0], image_u8.shape[1], M, out.data_ptr(),
+            st = _lib.lib().cpb200_pre_process(src.data_ptr(), src.shape[0], src.shape[1], M, out.data_ptr(),
                                                inp_height, inp_width, mean, std, 1 if flip else 0,
                                                torch.cuda.current_stream(dev).cuda_stream)
         _lib.check(st, "pre_process")
@@ -192,6 +213,66 @@ def group_by_shape(keys, max_batch):
 # one entry of cpb200_pre_process_batch's device table (struct cpb200_pre_image, include/centerpose_b200.h)
 _PRE_IMAGE = np.dtype([("offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("trans_input", "<f8", (6,))])
 assert _PRE_IMAGE.itemsize == 64
+# one entry of cpb200_resize_linear_u8_batch's device table (struct cpb200_resize_image, include/centerpose_b200.h)
+_RESIZE_IMAGE = np.dtype([("src_offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("dst_offset", "<i8"), ("new_h", "<i4"),
+                          ("new_w", "<i4")])
+assert _RESIZE_IMAGE.itemsize == 32
+
+
+def resize_table(shapes, new_shapes):
+    """The ``cpb200_resize_linear_u8_batch`` table that resizes HWC uint8 BGR images of ``shapes`` (h, w), packed back
+    to back, to ``new_shapes`` (h, w), packed back to back in the destination.  The kernel trusts the table, so the
+    sizes are checked here: each must be at least 1 and each image below 2^31 pixels."""
+    table = np.zeros(len(shapes), _RESIZE_IMAGE)
+    src = dst = 0
+    for n, ((h, w), (new_h, new_w)) in enumerate(zip(shapes, new_shapes)):
+        if min(h, w, new_h, new_w) < 1 or max(h * w, new_h * new_w) >= 2 ** 31:
+            raise ValueError("resize: cannot resize a %dx%d image to %dx%d" % (h, w, new_h, new_w))
+        table[n] = (src, h, w, dst, new_h, new_w)
+        src += h * w * 3
+        dst += new_h * new_w * 3
+    return table
+
+
+def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda n: np.empty(n, np.uint8)):
+    """Lays out one upload of a ``run_images`` group of B images: ``[pre-process table (B x 64 B) | resize table
+    (B x 32 B) | back-projection affines (B x 6 fp32) | destination image index (B int64) | raw pixels]``.
+
+    ``images`` are the raw HWC uint8 images, ``new_shapes`` their (h, w) at the group's scale, ``trans_inputs`` their
+    forward 2x3 warp matrices, ``affine`` the (B, 6) float32 back-projections and ``dst_index`` where each image's rows
+    go.  When a size changes, the resize table sends every image into a scratch buffer of ``scratch`` bytes and the
+    pre-process table reads the resized images there; otherwise there is no resize table and the pre-process table
+    reads the raw pixels.  ``alloc(nbytes)`` returns the uint8 host buffer (a numpy array or a CPU tensor, e.g. pinned).
+    Returns ``(buffer, layout)``; ``layout`` holds the byte offsets ``o_rsz`` (None without a resize), ``o_aff``,
+    ``o_idx``, ``o_img`` and ``scratch``."""
+    B = len(images)
+    shapes = [im.shape[0:2] for im in images]
+    resize = any(tuple(s) != tuple(n) for s, n in zip(shapes, new_shapes))
+    pre = np.zeros(B, _PRE_IMAGE)
+    rsz = resize_table(shapes, new_shapes) if resize else None
+    pos = 0
+    for n, im in enumerate(images):
+        (h, w), off = (new_shapes[n], rsz[n]["dst_offset"]) if resize else (shapes[n], pos)
+        pre[n] = (off, h, w, np.asarray(trans_inputs[n], np.float64).reshape(6))
+        pos += im.nbytes
+    o_rsz = pre.nbytes if resize else None
+    o_aff = pre.nbytes + (rsz.nbytes if resize else 0)
+    o_idx = o_aff + B * 24                                       # B * 24 keeps the int64 index 8-byte aligned
+    o_img = o_idx + B * 8
+    o_img += (16 - o_img % 16) % 16
+    buf = alloc(o_img + sum(im.nbytes for im in images))
+    hv = buf.numpy() if isinstance(buf, torch.Tensor) else buf
+    hv[:pre.nbytes] = pre.view(np.uint8)
+    if resize:
+        hv[o_rsz:o_aff] = rsz.view(np.uint8)
+    hv[o_aff:o_idx] = np.ascontiguousarray(affine, np.float32).view(np.uint8).reshape(-1)
+    hv[o_idx:o_idx + B * 8] = np.asarray(dst_index, np.int64).view(np.uint8)
+    pos = o_img
+    for im in images:
+        hv[pos:pos + im.nbytes] = np.ascontiguousarray(im).reshape(-1)
+        pos += im.nbytes
+    scratch = sum(h * w * 3 for h, w in new_shapes) if resize else 0
+    return buf, {"o_rsz": o_rsz, "o_aff": o_aff, "o_idx": o_idx, "o_img": o_img, "scratch": scratch}
 
 
 def _swap_pairs(C, pairs, device):
@@ -359,10 +440,11 @@ class MultiPoseDetector(BaseDetector):
         arrays or image paths.  Returns one float32 ``(N_i, 56)`` array per image, in input order, equal to
         ``run(image)['results'][1]``: all rows, suppressed ones at the tail, as the reference's ``merge_outputs``.
 
-        Per test scale every image gets ``pre_process``'s geometry (a scale != 1 keeps ``cv2.resize`` on the host).
-        Images with the same (scale, input size) are batched, at most ``max_batch`` per forward (2x that many
-        network images with ``FLIP_TEST``): one pinned upload, one ``cpb200_pre_process_batch``, the forward, the
-        flip merge and the decode with the back-projection fused.  The per-scale rows are then concatenated per image
+        Per test scale every image gets ``pre_process``'s geometry.  Images with the same (scale, input size) are
+        batched, at most ``max_batch`` per forward (2x that many network images with ``FLIP_TEST``): one pinned upload
+        of the raw images, at a scale != 1 one ``cpb200_resize_linear_u8_batch`` (``cv2.resize`` on the device, bit for
+        bit), one ``cpb200_pre_process_batch``, the forward, the flip merge and the decode with the back-projection
+        fused.  The per-scale rows are then concatenated per image
         and, with ``TEST.NMS`` or several scales, go through one ``cpb200_soft_nms_39_batch`` for all images.  The
         only host wait is the final device-to-host copy."""
         import ctypes
@@ -393,36 +475,31 @@ class MultiPoseDetector(BaseDetector):
             height, width = image.shape[0:2]
             for si, scale in enumerate(self.scales):
                 new_h, new_w, inp_h, inp_w, trans_input, meta = self._pre_process_geometry(height, width, scale)
-                resized = image if (new_w, new_h) == (width, height) else cv2.resize(image, (new_w, new_h))
-                items.append((i, np.ascontiguousarray(resized), trans_input, meta))
+                items.append((i, (new_h, new_w), trans_input, meta))
                 keys.append((si, inp_h, inp_w))
         rows = torch.empty((len(loaded), S * K, 56), dtype=torch.float32, device=dev)
         for (si, inp_h, inp_w), idx in group_by_shape(keys, max_batch):
             B = len(idx)
-            # one pinned buffer, one upload: [table (B x 64 B) | affine (B x 6 fp32) | image index (B int64) | pixels]
-            o_aff = B * _PRE_IMAGE.itemsize
-            o_idx = o_aff + B * 24 + (8 - B * 24 % 8) % 8
-            o_img = o_idx + B * 8
-            o_img += (16 - o_img % 16) % 16
-            sizes = [items[j][1].nbytes for j in idx]
-            host = torch.empty(o_img + sum(sizes), dtype=torch.uint8, pin_memory=True)
-            hv = host.numpy()
-            table = np.zeros(B, _PRE_IMAGE)
-            pos = 0
-            for n, j in enumerate(idx):
-                img = items[j][1]
-                table[n] = (pos, img.shape[0], img.shape[1], np.asarray(items[j][2], np.float64).reshape(6))
-                hv[o_img + pos:o_img + pos + img.nbytes] = img.reshape(-1)
-                pos += img.nbytes
-            hv[:o_aff] = table.view(np.uint8)
-            hv[o_aff:o_aff + B * 24] = affine_for_meta([items[j][3] for j in idx], self.scales[si]).numpy().view(np.uint8).reshape(-1)
-            hv[o_idx:o_idx + B * 8] = np.array([items[j][0] for j in idx], np.int64).view(np.uint8)
+            # one pinned buffer, one upload of the raw images with their tables (pack_group)
+            host, at = pack_group([loaded[items[j][0]] for j in idx], [items[j][1] for j in idx], [items[j][2] for j in idx],
+                                  affine_for_meta([items[j][3] for j in idx], self.scales[si]).numpy(),
+                                  [items[j][0] for j in idx],
+                                  alloc=lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True))
             buf = host.to(dev, non_blocking=True)
-            aff = buf[o_aff:o_aff + B * 24].view(torch.float32).view(B, 6)
-            dst = buf[o_idx:o_idx + B * 8].view(torch.int64)
+            aff = buf[at["o_aff"]:at["o_aff"] + B * 24].view(torch.float32).view(B, 6)
+            dst = buf[at["o_idx"]:at["o_idx"] + B * 8].view(torch.int64)
+            pixels = buf.data_ptr() + at["o_img"]
+            if at["o_rsz"] is not None:
+                # the scaled images go into a device scratch buffer, where the pre-process table points
+                scratch = torch.empty(at["scratch"], dtype=torch.uint8, device=dev)
+                with torch.cuda.device(dev):
+                    st = _lib.lib().cpb200_resize_linear_u8_batch(pixels, buf.data_ptr() + at["o_rsz"], B,
+                                                                  scratch.data_ptr(), stream)
+                _lib.check(st, "resize_linear_u8_batch")
+                pixels = scratch.data_ptr()
             inp = torch.empty((2 * B if flip else B, 3, inp_h, inp_w), dtype=torch.float32, device=dev)
             with torch.cuda.device(dev):
-                st = _lib.lib().cpb200_pre_process_batch(buf.data_ptr() + o_img, buf.data_ptr(), B, inp.data_ptr(),
+                st = _lib.lib().cpb200_pre_process_batch(pixels, buf.data_ptr(), B, inp.data_ptr(),
                                                          inp_h, inp_w, mean, std, 1 if flip else 0, stream)
             _lib.check(st, "pre_process_batch")
             outputs = self.model(inp)

@@ -120,6 +120,22 @@ typedef struct cpb200_pre_image {
 int cpb200_pre_process_batch(const unsigned char *imgs, const cpb200_pre_image *table, int B, float *out, int out_h,
                              int out_w, const float *mean, const float *stdv, int flip, void *stream);
 
+/* One image of cpb200_resize_linear_u8_batch (32 bytes, lives in caller-owned DEVICE memory).  All sizes >= 1. */
+typedef struct cpb200_resize_image {
+  int64_t src_offset;        /* byte offset of the source image's first pixel in `src` */
+  int32_t h, w;              /* source size; HWC uint8 BGR, rows packed (pitch 3*w bytes) */
+  int64_t dst_offset;        /* byte offset of the resized image's first pixel in `dst` */
+  int32_t new_h, new_w;      /* resized size, rows packed (pitch 3*new_w bytes) */
+} cpb200_resize_image;
+
+/* cv2.resize(img, (new_w, new_h)) with the default INTER_LINEAR on 8-bit BGR images, the first step of
+ * BaseDetector.pre_process at a test scale != 1 (lib/detectors/base_detector.py:33-34).  Bit-exact with OpenCV's
+ * fixed-point path (11-bit coefficients; verified against cv2 4.13 for up- and downscales).  B images of any sizes in
+ * one launch: `src` and `dst` are device buffers, `table` a DEVICE array of B cpb200_resize_image whose sizes the
+ * caller has checked (the kernel trusts them).  The output regions must not overlap the inputs.  1 <= B <= 65535. */
+int cpb200_resize_linear_u8_batch(const unsigned char *src, const cpb200_resize_image *table, int B, unsigned char *dst,
+                                  void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)

@@ -1,10 +1,14 @@
 """Raw-image detection throughput on one GPU: ``MultiPoseDetector.run_images`` against a per-image ``run()`` loop.
 
-    python tools/bench_images.py [--images 64] [--rounds 3] [--max-batch 32] [--precision fp16x2]
+    python tools/bench_images.py [--arch dla_34] [--scales 1] [--images 64] [--rounds 3] [--max-batch 32]
+                                 [--precision fp16x2]
 
-DLA-34 with conditioned weights (``centerpose_b200.synth``) and the test section of the reference's
-``experiments/dla_34_512x512.yaml``: flip test, soft-NMS, ``FIX_RES: false`` (each image padded to (h|31)+1 x
-(w|31)+1), scales [1].  The images are seeded uint8 noise at COCO-like sizes, 640x480, 480x640 and 640x427 in turn.
+``--arch`` picks the network, with conditioned weights (``centerpose_b200.synth``), and the test section of its
+configuration in the reference: ``experiments/dla_34_512x512.yaml`` (flip test, soft-NMS, ``FIX_RES: false``, scales
+[1]) or ``experiments/hrnet_w32_512.yaml`` (flip test, ``FIX_RES: false``, scales [1, 2], so the rows of the two
+scales are merged by soft-NMS).  ``--scales`` replaces the section's test scales.  With ``FIX_RES: false`` each image
+is padded to (h|31)+1 x (w|31)+1 at every scale, so scale 2 on a 640x480 image runs a 1312x992 input.  The images are
+seeded uint8 noise at COCO-like sizes, 640x480, 480x640 and 640x427 in turn.
 Both paths take the same host arrays and return the same rows (original-image pixels, after soft-NMS), so each time
 covers upload, pre-process, forward, flip merge, decode, back-projection, NMS and the copy back.
 
@@ -35,15 +39,20 @@ from tools.bench_hardnet import gpu_info  # noqa: E402
 SIZES = [(480, 640), (640, 480), (427, 640)]     # (h, w)
 
 
-def detector(precision):
+# the TEST sections of experiments/dla_34_512x512.yaml and experiments/hrnet_w32_512.yaml
+TEST_SECTIONS = {"dla_34": {"FLIP_TEST": True, "NMS": True, "FIX_RES": False, "TEST_SCALES": [1]},
+                 "hrnet": {"FLIP_TEST": True, "NMS": False, "FIX_RES": False, "TEST_SCALES": [1, 2]}}
+
+
+def detector(arch, precision, scales=None):
     from centerpose_b200.config import default_cfg
     from centerpose_b200.detector import detector_factory
     from centerpose_b200.synth import conditioned_state_dict
-    cfg = default_cfg("dla_34")
-    cfg.TEST.FLIP_TEST = True                     # experiments/dla_34_512x512.yaml, TEST section
-    cfg.TEST.NMS = True
-    cfg.TEST.FIX_RES = False
-    cfg.TEST.TEST_SCALES = [1]
+    cfg = default_cfg(arch)
+    for k, v in TEST_SECTIONS[arch].items():
+        setattr(cfg.TEST, k, list(v) if isinstance(v, list) else v)
+    if scales:
+        cfg.TEST.TEST_SCALES = list(scales)
     cfg.B200.PRECISION = precision
     det = detector_factory[cfg.TEST.TASK](cfg)
     det.model.load_state_dict(conditioned_state_dict(det.model.state_dict(), 317))
@@ -53,6 +62,8 @@ def detector(precision):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--arch", default="dla_34", choices=sorted(TEST_SECTIONS))
+    ap.add_argument("--scales", type=float, nargs="+", default=None, help="test scales (default: the test section's)")
     ap.add_argument("--images", type=int, default=64)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--max-batch", type=int, default=32)
@@ -63,7 +74,7 @@ def main():
     torch.cuda.set_device(0)
     rng = np.random.RandomState(317)
     images = [rng.randint(0, 256, size=SIZES[i % len(SIZES)] + (3,)).astype(np.uint8) for i in range(args.images)]
-    det = detector(args.precision)
+    det = detector(args.arch, args.precision, args.scales)
     hw_before = gpu_info(0)
 
     def batched():
@@ -84,8 +95,8 @@ def main():
     kept_a = [int((g[:, 4] >= 0.001).sum()) for g in got]
     kept_b = [int((w[:, 4] >= 0.001).sum()) for w in want]
     result = {
-        "metric": "images/sec, raw uint8 images -> rows after flip test + soft-NMS, DLA-34, dla_34_512x512 test section",
-        "precision": args.precision, "images": args.images, "sizes_hw": SIZES, "max_batch": args.max_batch,
+        "metric": "images/sec, raw uint8 images -> rows after flip test + soft-NMS, %s, its test section" % args.arch,
+        "arch": args.arch, "scales": list(det.scales), "precision": args.precision, "images": args.images, "sizes_hw": SIZES, "max_batch": args.max_batch,
         "rounds": args.rounds,
         "run_images_images_per_s": [args.images / t for t in times["run_images"]],
         "run_loop_images_per_s": [args.images / t for t in times["run_loop"]],
