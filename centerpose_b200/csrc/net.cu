@@ -11,6 +11,9 @@ bool sp_eligible(const cpb200_op &op);
 int sp_run(const cpb200_op &op, cudaStream_t st);
 bool stem_tc_eligible(const cpb200_op &op);
 int stem_tc_run(const cpb200_op &op, cudaStream_t st);
+int heads_prepare(cpb200_op &op);
+void heads_release(cpb200_op &op);
+int heads_run(const cpb200_op &op, cudaStream_t st);
 }  // namespace cpb
 
 static int validate(const cpb200_op &op, int i) {
@@ -19,12 +22,12 @@ static int validate(const cpb200_op &op, int i) {
   if (op.nsrc < 1 || op.nsrc > 4) return cpb::fail(CPB200_ERR_ARG, "op %d: nsrc %d", i, op.nsrc);
   for (int s = 0; s < op.nsrc; ++s)
     if (!op.src[s] || op.cin[s] <= 0) return cpb::fail(CPB200_ERR_ARG, "op %d: null/empty input %d", i, s);
-  if (!op.dst) return cpb::fail(CPB200_ERR_ARG, "op %d: null dst", i);
+  if (!op.dst && op.type != CPB200_OP_HEADS) return cpb::fail(CPB200_ERR_ARG, "op %d: null dst", i);   // HEADS: per-head dst
   if (op.act_dtype < CPB200_F32 || op.act_dtype > CPB200_F16X2)
     return cpb::fail(CPB200_ERR_ARG, "op %d: bad act_dtype", i);
   if ((op.act_dtype == CPB200_BF16X2 || op.act_dtype == CPB200_F16X2) && !(op.flags & CPB200_FLAG_TC) && !cpb::simt_runs_split(op.type))
     return cpb::fail(CPB200_ERR_ARG, "op %d: split-precision activations need the tensor-core path (or an element-wise op / CONVERT)", i);
-  if ((op.type == CPB200_OP_CONV || op.type == CPB200_OP_DCN || op.type == CPB200_OP_STEM) && !op.weight)
+  if ((op.type == CPB200_OP_CONV || op.type == CPB200_OP_DCN || op.type == CPB200_OP_STEM || op.type == CPB200_OP_HEADS) && !op.weight)
     return cpb::fail(CPB200_ERR_ARG, "op %d: null weight", i);
   for (int s = 0; s < op.nsrc; ++s)
     if (op.src_pitch[s] != 0 && (op.src_pitch[s] < op.cin[s] || (op.type != CPB200_OP_CONV && op.src_pitch[s] != op.cin[s])))
@@ -41,7 +44,11 @@ extern "C" int cpb200_prepare_ops(cpb200_op *ops, int n) {
   for (int i = 0; i < n; ++i) {
     int rc = validate(ops[i], i);
     if (rc) return rc;
-    if (ops[i].type == CPB200_OP_STEM && (ops[i].flags & CPB200_FLAG_TC)) {
+    if (ops[i].type == CPB200_OP_HEADS) {
+      if (!(ops[i].flags & CPB200_FLAG_TC)) return cpb::fail(CPB200_ERR_ARG, "op %d: HEADS runs on the tensor-core path only", i);
+      rc = cpb::heads_prepare(ops[i]);
+      if (rc) return rc;
+    } else if (ops[i].type == CPB200_OP_STEM && (ops[i].flags & CPB200_FLAG_TC)) {
       if (!cpb::stem_tc_eligible(ops[i])) return cpb::fail(CPB200_ERR_ARG, "op %d: shape not supported by the tensor-core stem", i);
     } else if (cpb::sp_eligible(ops[i])) {
       // small-channel 3x3 conv: SIMT-fed wgmma kernel, nothing to prepare (csrc/net_tc_sp.cu)
@@ -56,7 +63,8 @@ extern "C" int cpb200_prepare_ops(cpb200_op *ops, int n) {
 extern "C" int cpb200_release_ops(cpb200_op *ops, int n) {
   if (!ops) return CPB200_OK;
   for (int i = 0; i < n; ++i)
-    if (ops[i].tc) cpb::tc_release_op(ops[i]);
+    if (ops[i].tc && ops[i].type == CPB200_OP_HEADS) cpb::heads_release(ops[i]);
+    else if (ops[i].tc) cpb::tc_release_op(ops[i]);
   return CPB200_OK;
 }
 
@@ -65,7 +73,8 @@ extern "C" int cpb200_run_ops(const cpb200_op *ops, int n, void *stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   for (int i = 0; i < n; ++i) {
     int rc;
-    if (!(ops[i].flags & CPB200_FLAG_TC)) rc = cpb::run_op_simt_dispatch(ops[i], st);
+    if (ops[i].type == CPB200_OP_HEADS) rc = cpb::heads_run(ops[i], st);
+    else if (!(ops[i].flags & CPB200_FLAG_TC)) rc = cpb::run_op_simt_dispatch(ops[i], st);
     else if (ops[i].type == CPB200_OP_STEM) rc = cpb::stem_tc_run(ops[i], st);
     else if (!ops[i].tc && cpb::sp_eligible(ops[i])) rc = cpb::sp_run(ops[i], st);
     else rc = cpb::tc_run_op(ops[i], st);

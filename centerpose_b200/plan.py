@@ -26,7 +26,7 @@ from . import _lib
 
 OP_CONV, OP_STEM, OP_MAXPOOL, OP_DWDECONV_ADD, OP_DCN, OP_UPSAMPLE_ADD = 1, 2, 3, 4, 5, 7      # 6 is retired
 OP_DWCONV, OP_AVGPOOL, OP_SCALE_ADD, OP_CONVERT, OP_S2D = 8, 9, 10, 11, 12
-OP_AVGPOOL2, OP_RESIZE_BILINEAR = 13, 14
+OP_AVGPOOL2, OP_RESIZE_BILINEAR, OP_HEADS = 13, 14, 15
 FLAG_RELU, FLAG_OUT_NCHW_F32, FLAG_OUT_F32, FLAG_TC, FLAG_HSWISH, FLAG_HSIGMOID, FLAG_TO_F32 = 1, 2, 4, 8, 16, 32, 64
 _ACT_FLAG = {None: 0, "relu": FLAG_RELU, "hswish": FLAG_HSWISH, "hsigmoid": FLAG_HSIGMOID}
 F32, BF16, BF16X2, F16X2 = 0, 1, 2, 3
@@ -88,6 +88,14 @@ class OpStruct(ctypes.Structure):
         ("dst", ctypes.c_void_p), ("weight", ctypes.c_void_p), ("bias", ctypes.c_void_p),
         ("tc", ctypes.c_void_p), ("src_pitch", ctypes.c_int32 * 4),
         ("acc_scale", ctypes.c_float), ("reserved_", ctypes.c_int32),
+    ]
+
+
+class HeadStruct(ctypes.Structure):
+    """``cpb200_head``: one entry of an OP_HEADS op's table."""
+    _fields_ = [
+        ("hidden", ctypes.c_int32), ("cout", ctypes.c_int32), ("weight", ctypes.c_void_p), ("bias", ctypes.c_void_p),
+        ("acc_scale3", ctypes.c_float), ("acc_scale1", ctypes.c_float), ("dst", ctypes.c_void_p),
     ]
 
 
@@ -577,11 +585,13 @@ class Plan:
         self.pb = pb
         self.device = pb.device
         self._prune(pb)
+        self._fuse_heads(pb)
         self._allocate(pb)
         n = len(pb.ops)
         self.ops = (OpStruct * n)()
         self.in_slots = []      # (op index, src slot) fed by the network input
-        self.out_slots = {}     # output name -> list of op indices writing it
+        self.out_slots = {}     # output name -> op indices writing it, or (op index, head) of an OP_HEADS table
+        self._head_tables = {}  # op index -> its cpb200_head table (host memory the op's aux points to)
         for i, po in enumerate(pb.ops):
             o = self.ops[i]
             o.type = po.type; o.flags = po.flags; o.act_dtype = po.dtype
@@ -596,6 +606,9 @@ class Plan:
                 else:
                     o.src[j] = s.buf.data_ptr() + s.ch_off * _ptr_esize(pb, s.kind)
                     o.src_pitch[j] = s.pitch if s.parent is not None else 0
+            if po.type == OP_HEADS:
+                self._set_heads(i, o, po)
+                continue
             o.cout = po.cout
             o.kh, o.kw = po.k; o.stride = po.stride; o.pad_h, o.pad_w = po.pad
             d = po.dst
@@ -652,6 +665,10 @@ class Plan:
             d = self._root(ops[i].dst)
             live[i] = i == len(ops) - 1 or d.fixed or d.keep or any(live[c] for c in consumers.get(id(d), ()) if c > i)
         pb.ops = [po for i, po in enumerate(ops) if live[i]]
+        self._reindex(pb)
+
+    def _reindex(self, pb: PlanBuilder):
+        """recompute the producer / last-use indices the allocator works from after ops were removed or merged"""
         for s in pb.syms:
             s.producer = -1
             if s.parent is None:
@@ -663,6 +680,78 @@ class Plan:
             if d.producer < 0:
                 d.producer = i
             d.last_use = max(d.last_use, i)
+
+    def _fuse_heads(self, pb: PlanBuilder):
+        """Replace (tensor-core 3x3 conv + ReLU -> 1x1 conv with NCHW fp32 output) pairs over one shared input by ONE
+        OP_HEADS op (csrc/net_heads.cu): the hidden maps, otherwise written by each 3x3 conv and read back once by its 1x1
+        conv, stay on the chip and are never allocated.  The kernel sums the same products in the same order, so the
+        outputs are bit-identical.  A pair qualifies when the 3x3 conv is stride 1 / pad 1 over one dense input of at
+        most 64 channels (C % 16 == 0) and maps of at least 8 x 8, writes a multiple of 128 channels, and its result is
+        read by the 1x1 conv alone; nothing involved may be marked keep."""
+        if not pb.use_tc:
+            return
+        ops = pb.ops
+        readers = {}                                    # id(root sym) -> op indices reading it
+        for i, po in enumerate(ops):
+            for s in list(po.srcs) + [e for e in po.extra if e is not None]:
+                readers.setdefault(id(self._root(s)), []).append(i)
+        pairs = []
+        for i, a in enumerate(ops):
+            if not (a.type == OP_CONV and a.flags == FLAG_TC | FLAG_RELU and a.k == (3, 3) and a.stride == 1
+                    and a.pad == (1, 1) and len(a.srcs) == 1 and not any(e is not None for e in a.extra)
+                    and getattr(a, "ch_off", 0) == 0):
+                continue
+            x, h = a.srcs[0], a.dst
+            if not (x.kind == "act" and x.parent is None and x.C % 16 == 0 and x.C <= 64 and x.H >= 8 and x.W >= 8
+                    and a.out_map == (x.H, x.W, 1, 1, 0, 0) and a.HoWo == (x.H, x.W)
+                    and h.kind == "act" and h.parent is None and not h.keep and not h.fixed and h.C % 128 == 0):
+                continue
+            r = readers.get(id(h), [])
+            if len(r) != 1:
+                continue
+            b = ops[r[0]]
+            d = b.dst
+            if not (b.type == OP_CONV and b.flags == FLAG_TC | FLAG_OUT_NCHW_F32 and b.k == (1, 1) and len(b.srcs) == 1
+                    and b.srcs[0] is h and not any(e is not None for e in b.extra) and b.cout <= 48
+                    and d.kind == "nchw_out" and d.C == b.cout and getattr(b, "ch_off", 0) == 0
+                    and b.out_map == (x.H, x.W, 1, 1, 0, 0) and not readers.get(id(d))):
+                continue
+            pairs.append((i, r[0]))
+        if not pairs:
+            return
+        x0, hid = ops[pairs[0][0]].srcs[0], ops[pairs[0][0]].cout
+        pairs = [p for p in pairs if ops[p[0]].srcs[0] is x0 and ops[p[0]].cout == hid][:8]
+        first = min(i for i, _ in pairs)
+        if any(self._root(po.dst) is x0 for po in ops[first:]):
+            return
+        heads = [(ops[i], ops[j]) for i, j in pairs]
+        w = torch.stack([a.weight for a, _ in heads]).contiguous()       # [head][(plane)][tap][K-slab][hid][bk]
+        bias = torch.cat([a.bias for a, _ in heads]).contiguous()
+        pb.keep += [w, bias]
+        fused = _PendingOp(type=OP_HEADS, flags=FLAG_TC | FLAG_OUT_NCHW_F32, k=(3, 3), stride=1, pad=(1, 1), weight=w,
+                           bias=bias, cout=sum(b.cout for _, b in heads), dtype=pb.act_dtype, acc_scale=1.0, heads=heads,
+                           srcs=[x0], dst=heads[0][1].dst, extra=[])
+        drop = {k for p in pairs for k in p}
+        pb.ops = [fused if k == first else po for k, po in enumerate(ops) if k == first or k not in drop]
+        self._reindex(pb)
+
+    def _set_heads(self, i: int, o: OpStruct, po: _PendingOp):
+        s0 = po.srcs[0]
+        o.cout = po.cout
+        o.kh = o.kw = 3; o.stride = 1; o.pad_h = o.pad_w = 1
+        o.Ho, o.Wo, o.Hd, o.Wd = s0.H, s0.W, s0.H, s0.W
+        o.out_sy = o.out_sx = 1
+        o.out_ch_total = po.cout
+        tab = (HeadStruct * len(po.heads))()
+        for k, (a, b) in enumerate(po.heads):
+            e = tab[k]
+            e.hidden, e.cout = a.cout, b.cout
+            e.weight, e.bias = b.weight.data_ptr(), b.bias.data_ptr()
+            e.acc_scale3, e.acc_scale1 = float(a.acc_scale), float(b.acc_scale)
+            self.out_slots.setdefault(b.dst.name, []).append((i, k))
+        self._head_tables[i] = tab
+        o.aux = ctypes.addressof(tab); o.aux_pitch = len(tab)
+        o.weight = po.weight.data_ptr(); o.bias = po.bias.data_ptr()
 
     def _allocate(self, pb: PlanBuilder):
         """Liveness-based buffer reuse: a buffer returns to the pool after its last consumer."""
@@ -710,7 +799,10 @@ class Plan:
         for name, idxs in self.out_slots.items():
             p = outs[name].data_ptr()
             for i in idxs:
-                self.ops[i].dst = p
+                if isinstance(i, tuple):
+                    self._head_tables[i[0]][i[1]].dst = p
+                else:
+                    self.ops[i].dst = p
 
     def run(self, stream: int):
         L = _lib.lib()

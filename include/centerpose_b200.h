@@ -205,11 +205,20 @@ enum cpb200_op_type {
   CPB200_OP_AVGPOOL2 = 13,   /* 2x2 / stride-2 average pool, NHWC, floor mode, no padding: (B,H,W,C) -> (B,H/2,W/2,C)
                                 with Ho == H/2, Wo == W/2, H, W >= 2, C % 4 == 0, one dense input
                                 (HarDNet nn.AvgPool2d(2, 2), hardnet.py:141).  All four activation dtypes.          */
-  CPB200_OP_RESIZE_BILINEAR = 14 /* bilinear resize with align_corners=True, NHWC: (B,H,W,C) -> (B,Ho,Wo,C), Ho, Wo >= 1,
+  CPB200_OP_RESIZE_BILINEAR = 14,/* bilinear resize with align_corners=True, NHWC: (B,H,W,C) -> (B,Ho,Wo,C), Ho, Wo >= 1,
                                 C % 4 == 0, one dense input (HarDNet TransitionUp, hardnet.py:95-100).  PyTorch's
                                 arithmetic in fp32: scale = (in-1)/(out-1) (0 when out == 1), src = scale*dst,
                                 i0 = (int)src, i1 = i0 + (i0 < in-1), l1 = src - i0, l0 = 1 - l1; the vertical blend
                                 of the two horizontal blends.  All four activation dtypes.                          */
+  CPB200_OP_HEADS = 15       /* the keypoint heads (keypoint.py:40-42) in one op: for each entry h of the cpb200_head
+                                table `aux` (aux_pitch entries, 1..8)  dst_h = conv1x1_h(relu(conv3x3_h(src[0]))),
+                                written NCHW fp32 (B, cout_h, Ho, Wo); the hidden maps never leave the chip.  One dense
+                                input, C % 16 == 0, C <= 64, 3x3 / stride 1 / pad 1, maps >= 8 x 8; act_dtype BF16 /
+                                BF16X2 / F16X2 with CPB200_FLAG_TC.  `weight` = the heads' 3x3 weights packed as for a
+                                tensor-core 3x3 conv, one head after the other; `bias` = their biases, [head][hidden];
+                                `cout` = the sum of the heads' channels; `dst` is unused (the table holds the outputs).
+                                The results are bit-identical to each head's 3x3 conv (+ReLU) followed by its 1x1 conv
+                                with NCHW output.                                                                    */
 };
 /* A dense ConvTranspose2d(k4,s2,p1) (msra_resnet.py:168-193) is lowered by the host into four
  * 2x2 CONV ops, one per output parity, using pad_h/pad_w and the strided-output fields below. */
@@ -251,6 +260,18 @@ typedef struct cpb200_op {
                                 added — the inverse of the scale the host applied to the weights; 0 is read as 1     */
   int32_t reserved_;
 } cpb200_op;
+
+/* One head of a CPB200_OP_HEADS op (a HOST array the op's `aux` points to; it is read at every cpb200_run_ops call, so
+ * `dst` may be re-pointed between runs like cpb200_op.dst). */
+typedef struct cpb200_head {
+  int32_t hidden;            /* 3x3 output channels (the same for every head, a multiple of 128)               */
+  int32_t cout;              /* 1x1 output channels, 1..48                                                      */
+  const void *weight;        /* the 1x1 weights packed as for a tensor-core 1x1 conv over `hidden` channels    */
+  const float *bias;         /* fp32 [cout]                                                                     */
+  float acc_scale3;          /* acc_scale of the head's 3x3 conv (split precisions; 0 is read as 1)             */
+  float acc_scale1;          /* acc_scale of the head's 1x1 conv                                                */
+  float *dst;                /* NCHW fp32 (B, cout, Ho, Wo)                                                     */
+} cpb200_head;
 
 /* Validate the program and build device-side descriptors (TMA tensor maps) for ops flagged
  * CPB200_FLAG_TC.  Must be called once after the INPUT activation / weight pointers in `ops` are final (they are

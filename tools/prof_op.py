@@ -1,8 +1,11 @@
 """Run ONE fused op of the DLA-34 program at benchmark size (B=32, 512x512 input) a few times, for
 `ncu --set full -k regex:<kernel> -s 2 -c 1 python tools/prof_op.py <op>` captures and quick timing.
 ops: dcn64 (64->64 @128^2), dcn128 (128->128 @64^2), head3x3 (64->256 @128^2), conv64 (64->64 @128^2),
-     conv256 (256->256 @32^2), om64 (64->27 @128^2), level0 (16->16 @512^2), level1 (16->32 s2), stem, head1x1"""
+     conv256 (256->256 @32^2), om64 (64->27 @128^2), level0 (16->16 @512^2), level1 (16->32 s2), stem, head1x1
+     heads: the keypoint-head ops of the whole DLA-34 program (PROF_ARCH overrides the backbone), each timed on its own
+            with Plan.profile_ops, with the card's name and power limit"""
 import os
+import subprocess
 import sys
 
 import torch
@@ -19,9 +22,43 @@ OPS = {
 }
 
 
+def heads(B, prec, reps):
+    from centerpose_b200.config import default_cfg
+    from centerpose_b200.model import create_model
+    from centerpose_b200.synth import conditioned_state_dict, synth_images
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       stdout=subprocess.PIPE, text=True).stdout.strip()
+    print("card:", q)
+    dev = torch.device("cuda:0")
+    arch = os.environ.get("PROF_ARCH", "dla_34")
+    cfg = default_cfg(arch)
+    model = create_model(cfg.MODEL.NAME, cfg.MODEL.HEAD_CONV, cfg)
+    model.load_state_dict(conditioned_state_dict(model.state_dict(), 317))
+    model = model.to(dev).set_precision(prec)
+    x = synth_images(B, 512, 512, 317).to(dev)
+    model(x)
+    plan = model._plan(B, 512, 512, dev)
+    prof = plan.profile_ops(torch.cuda.current_stream().cuda_stream, reps=reps)
+    # the heads are the program's tail from its first NCHW-output op: the fused HEADS op, or a 1x1 conv whose 3x3 conv
+    # comes right before it
+    first = min(i for i in range(plan.n) if plan.ops[i].flags & 2)
+    first -= plan.ops[first].type == 1
+    sums = {}
+    for i in range(first, plan.n):
+        typ, fl, b_, ho, wo, co, ci, kh, kw, ms = prof[i]
+        kind = "1x1 nchw" if fl & 2 else ("type%d %dx%d" % (typ, kh, kw))
+        sums[kind] = sums.get(kind, 0.0) + ms
+        print(f"op {i:3d} type {typ} {kind:8s} {ci:4d}->{co:4d} @ {ho}x{wo}: {ms * 1e3:8.1f} us")
+    for k, v in sums.items():
+        print(f"HEADS {arch} [{prec}] B={B}: {k} total {v * 1e3:.1f} us")
+    print(f"whole program (sum of per-op times): {sum(p[-1] for p in prof) * 1e3:.1f} us over {plan.n} ops")
+
+
 def main():
     name = sys.argv[1]
     B = int(os.environ.get("PROF_B", "32"))
+    if name == "heads":
+        return heads(B, os.environ.get("PROF_PREC", "fp16x2"), int(os.environ.get("PROF_REPS", "5")))
     reps = int(os.environ.get("PROF_REPS", "5"))
     dev = torch.device("cuda:0")
     spec = OPS[name]
