@@ -50,6 +50,9 @@ def lib() -> ctypes.CDLL:
                                            ctypes.c_int, ctypes.c_void_p]
     L.cpb200_resize_linear_u8_batch.restype = ctypes.c_int
     L.cpb200_resize_linear_u8_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+    L.cpb200_jpeg_decode_batch.restype = ctypes.c_int
+    L.cpb200_jpeg_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
+                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     L.cpb200_soft_nms_39.restype = ctypes.c_int
     L.cpb200_soft_nms_39.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                      ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]

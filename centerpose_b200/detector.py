@@ -234,7 +234,8 @@ def resize_table(shapes, new_shapes):
     return table
 
 
-def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda n: np.empty(n, np.uint8)):
+def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda n: np.empty(n, np.uint8),
+               src_offsets=None):
     """Lays out one upload of a ``run_images`` group of B images: ``[pre-process table (B x 64 B) | resize table
     (B x 32 B) | back-projection affines (B x 6 fp32) | destination image index (B int64) | raw pixels]``.
 
@@ -244,23 +245,29 @@ def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda
     pre-process table reads the resized images there; otherwise there is no resize table and the pre-process table
     reads the raw pixels.  ``alloc(nbytes)`` returns the uint8 host buffer (a numpy array or a CPU tensor, e.g. pinned).
     Returns ``(buffer, layout)``; ``layout`` holds the byte offsets ``o_rsz`` (None without a resize), ``o_aff``,
-    ``o_idx``, ``o_img`` and ``scratch``."""
+    ``o_idx``, ``o_img`` and ``scratch``.
+
+    With ``src_offsets``, the images already lie in one device buffer at those byte offsets: the tables read them
+    there, ``images`` only need a ``shape``, and the buffer ends at ``o_img`` with no pixel section."""
     B = len(images)
     shapes = [im.shape[0:2] for im in images]
     resize = any(tuple(s) != tuple(n) for s, n in zip(shapes, new_shapes))
     pre = np.zeros(B, _PRE_IMAGE)
     rsz = resize_table(shapes, new_shapes) if resize else None
+    if resize and src_offsets is not None:
+        rsz["src_offset"] = src_offsets
     pos = 0
     for n, im in enumerate(images):
-        (h, w), off = (new_shapes[n], rsz[n]["dst_offset"]) if resize else (shapes[n], pos)
+        (h, w), off = (new_shapes[n], rsz[n]["dst_offset"]) if resize else \
+            (shapes[n], pos if src_offsets is None else src_offsets[n])
         pre[n] = (off, h, w, np.asarray(trans_inputs[n], np.float64).reshape(6))
-        pos += im.nbytes
+        pos += im.nbytes if src_offsets is None else 0
     o_rsz = pre.nbytes if resize else None
     o_aff = pre.nbytes + (rsz.nbytes if resize else 0)
     o_idx = o_aff + B * 24                                       # B * 24 keeps the int64 index 8-byte aligned
     o_img = o_idx + B * 8
     o_img += (16 - o_img % 16) % 16
-    buf = alloc(o_img + sum(im.nbytes for im in images))
+    buf = alloc(o_img + (0 if src_offsets is not None else sum(im.nbytes for im in images)))
     hv = buf.numpy() if isinstance(buf, torch.Tensor) else buf
     hv[:pre.nbytes] = pre.view(np.uint8)
     if resize:
@@ -268,11 +275,17 @@ def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda
     hv[o_aff:o_idx] = np.ascontiguousarray(affine, np.float32).view(np.uint8).reshape(-1)
     hv[o_idx:o_idx + B * 8] = np.asarray(dst_index, np.int64).view(np.uint8)
     pos = o_img
-    for im in images:
+    for im in images if src_offsets is None else ():
         hv[pos:pos + im.nbytes] = np.ascontiguousarray(im).reshape(-1)
         pos += im.nbytes
     scratch = sum(h * w * 3 for h, w in new_shapes) if resize else 0
     return buf, {"o_rsz": o_rsz, "o_aff": o_aff, "o_idx": o_idx, "o_img": o_img, "scratch": scratch}
+
+
+# run_images decodes JPEG files on the device in launches of at most this many images, whose coefficient and plane
+# workspace (reused from launch to launch) stays below JPEG_CHUNK_WORKSPACE bytes unless one image needs more
+JPEG_CHUNK_IMAGES = 256
+JPEG_CHUNK_WORKSPACE = 512 << 20
 
 
 def _swap_pairs(C, pairs, device):
@@ -433,6 +446,96 @@ class MultiPoseDetector(BaseDetector):
         Returns the merged ``(N, 56)`` rows (numpy) in original-image pixels, like ``run()['results'][1]``."""
         return self.run_images([image])[0]
 
+    def _load_checked(self, n, src):
+        """Input ``n`` of ``run_images`` as a BGR uint8 HWC array (a path through ``cv2.imread``)."""
+        if not isinstance(src, (np.ndarray, str)):
+            raise ValueError("run_images: image %d is a %s, expected a BGR uint8 HWC array or a path"
+                             % (n, type(src).__name__))
+        image = self._load(src)[0]
+        if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+            raise ValueError("run_images: image %d must be uint8 (H, W, 3), got %s %s" % (n, image.dtype, image.shape))
+        return image
+
+    def _load_images_device(self, images):
+        """Every input of ``run_images`` in one device buffer of packed HWC uint8 BGR images.  Returns
+        ``(views, offsets, buffer)``: per input a (h, w, 3) view of its slot and the slot's byte offset.
+
+        The files' headers are parsed first (``jpeg.parse``), so every size is known before any pixel exists.  The
+        files the device can decode, with their tables, go up in one pinned buffer and are decoded by
+        ``cpb200_jpeg_decode_batch`` in chunks of at most ``JPEG_CHUNK_IMAGES`` images that reuse one workspace.  The
+        other files (``cv2.imread``) and the arrays take the host path, and their pixels go up in one copy into
+        slots after the decoded ones.  One read of the decode status follows; a file whose entropy data the device
+        found bad is read by ``cv2.imread`` and copied into its slot."""
+        from . import _lib, jpeg
+        dev = torch.device("cuda")
+        datas, infos, host = {}, {}, {}
+        for n, src in enumerate(images):
+            if not isinstance(src, str):
+                host[n] = self._load_checked(n, src)
+                continue
+            try:
+                with open(src, "rb") as f:
+                    data = f.read()
+            except OSError:
+                raise FileNotFoundError(src)
+            try:
+                info = jpeg.parse(data, src)
+            except ValueError:
+                info = None
+            if info is not None and info.eligible:
+                datas[n], infos[n] = data, info
+            else:
+                host[n] = self._load_checked(n, src)
+        shape = {n: (infos[n].oh, infos[n].ow, 3) for n in infos}
+        shape.update({n: im.shape for n, im in host.items()})
+        offsets, pos = {}, 0
+        for n in list(infos) + list(host):                   # decoded slots first, then the host ones in one run
+            offsets[n] = pos
+            pos += int(np.prod(shape[n]))
+        host_start = pos - sum(im.nbytes for im in host.values())
+        pixels = torch.empty(max(pos, 1), dtype=torch.uint8, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        dec = list(infos)
+        if dec:
+            chunks, start, ws = [], 0, 0
+            for k, n in enumerate(dec):
+                if k > start and (k - start == JPEG_CHUNK_IMAGES or ws + infos[n].workspace_bytes() > JPEG_CHUNK_WORKSPACE):
+                    chunks.append((start, k)); start, ws = k, 0
+                ws += infos[n].workspace_bytes()
+            chunks.append((start, len(dec)))
+            packed = [jpeg.pack([infos[n] for n in dec[a:b]], [datas[n] for n in dec[a:b]], [offsets[n] for n in dec[a:b]])
+                      for a, b in chunks]
+            at = np.cumsum([0] + [p[0].nbytes + (-p[0].nbytes) % 16 for p in packed])
+            up = torch.empty(int(at[-1]), dtype=torch.uint8, pin_memory=True)
+            uv = up.numpy()
+            for (b, _), o in zip(packed, at):
+                uv[o:o + b.nbytes] = b
+            src = up.to(dev, non_blocking=True)
+            work = torch.empty(max(p[1] for p in packed), dtype=torch.uint8, device=dev)
+            status = torch.empty(len(dec), dtype=torch.int32, device=dev)
+            with torch.cuda.device(dev):
+                for (a, b), o in zip(chunks, at):
+                    st = _lib.lib().cpb200_jpeg_decode_batch(src.data_ptr() + int(o), src.data_ptr() + int(o), b - a,
+                                                             work.data_ptr(), work.numel(), pixels.data_ptr(),
+                                                             status.data_ptr() + 4 * a, stream)
+                    _lib.check(st, "jpeg_decode_batch")
+        if host:
+            staged = torch.empty(pos - host_start, dtype=torch.uint8, pin_memory=True)
+            sv = staged.numpy()
+            for n, im in host.items():
+                sv[offsets[n] - host_start:offsets[n] - host_start + im.nbytes] = np.ascontiguousarray(im).reshape(-1)
+            pixels[host_start:pos].copy_(staged, non_blocking=True)
+        if dec:
+            for k in np.flatnonzero(status.cpu().numpy()):
+                n = dec[k]
+                image = self._load_checked(n, images[n])
+                if image.shape != shape[n]:
+                    raise RuntimeError("run_images: %s decodes to %s on the host, its header says %s"
+                                       % (images[n], image.shape, shape[n]))
+                pixels[offsets[n]:offsets[n] + image.nbytes].copy_(torch.from_numpy(image.reshape(-1)))
+        views = [pixels[offsets[n]:offsets[n] + int(np.prod(shape[n]))].view(shape[n]) for n in range(len(images))]
+        return views, [offsets[n] for n in range(len(images))], pixels
+
     @torch.no_grad()
     def run_images(self, images, max_batch=32):
         """Additive: ``run()`` for many images at once, with the reference's test-time settings (``FLIP_TEST``,
@@ -446,21 +549,25 @@ class MultiPoseDetector(BaseDetector):
         bit), one ``cpb200_pre_process_batch``, the forward, the flip merge and the decode with the back-projection
         fused.  The per-scale rows are then concatenated per image
         and, with ``TEST.NMS`` or several scales, go through one ``cpb200_soft_nms_39_batch`` for all images.  The
-        only host wait is the final device-to-host copy."""
+        only host wait is the final device-to-host copy.
+
+        With ``B200.DEVICE_PREPROCESS`` on (the default) and any path among the inputs, the images are decoded into
+        one device buffer first (``_load_images_device``): sequential-Huffman JPEG files by
+        ``cpb200_jpeg_decode_batch``, byte for byte as ``cv2.imread``; every other file, and every array, on the
+        host and uploaded into its slot.  The groups then read that buffer in place.  That adds one small
+        device-to-host read of the decode status.  The call then needs device memory for the decoded images (3 bytes
+        per pixel) and one decode chunk's workspace (int16 coefficients and 8-bit planes: 4.5 bytes per pixel at
+        4:2:0, 9 at 4:4:4, at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image needs more)."""
         import ctypes
         from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch
         if int(max_batch) < 1:
             raise ValueError("run_images: max_batch must be >= 1, got %r" % (max_batch,))
-        loaded = []
-        for n, src in enumerate(images):
-            if not isinstance(src, (np.ndarray, str)):
-                raise ValueError("run_images: image %d is a %s, expected a BGR uint8 HWC array or a path"
-                                 % (n, type(src).__name__))
-            image = self._load(src)[0]
-            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
-                raise ValueError("run_images: image %d must be uint8 (H, W, 3), got %s %s" % (n, image.dtype, image.shape))
-            loaded.append(image)
+        offsets = None
+        if self.device_preprocess and any(isinstance(src, str) for src in images):
+            loaded, offsets, pixels_dev = self._load_images_device(images)
+        else:
+            loaded = [self._load_checked(n, src) for n, src in enumerate(images)]
         if not loaded:
             return []
         cfg = self.cfg
@@ -484,11 +591,12 @@ class MultiPoseDetector(BaseDetector):
             host, at = pack_group([loaded[items[j][0]] for j in idx], [items[j][1] for j in idx], [items[j][2] for j in idx],
                                   affine_for_meta([items[j][3] for j in idx], self.scales[si]).numpy(),
                                   [items[j][0] for j in idx],
-                                  alloc=lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True))
+                                  alloc=lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True),
+                                  src_offsets=None if offsets is None else [offsets[items[j][0]] for j in idx])
             buf = host.to(dev, non_blocking=True)
             aff = buf[at["o_aff"]:at["o_aff"] + B * 24].view(torch.float32).view(B, 6)
             dst = buf[at["o_idx"]:at["o_idx"] + B * 8].view(torch.int64)
-            pixels = buf.data_ptr() + at["o_img"]
+            pixels = buf.data_ptr() + at["o_img"] if offsets is None else pixels_dev.data_ptr()
             if at["o_rsz"] is not None:
                 # the scaled images go into a device scratch buffer, where the pre-process table points
                 scratch = torch.empty(at["scratch"], dtype=torch.uint8, device=dev)

@@ -1,0 +1,327 @@
+"""Host side of the device JPEG decoder (``cpb200_jpeg_decode_batch``, ``csrc/jpeg.cu``).
+
+``parse(data, name)`` reads a file's headers and decides whether the device can decode it byte for byte as
+``cv2.imread(path, IMREAD_COLOR)`` does (libjpeg-turbo's sequential Huffman decoder, ISLOW IDCT, fancy upsampling,
+integer YCbCr->BGR, then OpenCV's EXIF orientation).  ``pack(...)`` lays out the device table of a launch.
+
+The device decodes a file only when it is 8-bit, sequential Huffman (SOF0 / SOF1), grayscale or YCbCr, one interleaved
+scan over every component, chroma sampled (1, 1) and luma (1, 1), (2, 1), (1, 2) or (2, 2).  Everything else is
+``eligible == False`` and stays with ``cv2.imread``.  The kernels trust the table, so everything read from the file
+that sizes or indexes it is checked here; a file the parser cannot read raises ``ValueError`` naming the image.
+"""
+from __future__ import annotations
+
+import numpy as np
+
+# zigzag index -> natural (row-major) index, T.81 figure A.6
+ZIGZAG = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13,
+                   6, 7, 14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38,
+                   31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63], np.int64)
+LUT_BITS = 9
+# libjpeg refuses dimensions above JPEG_MAX_DIMENSION, so cv2.imread returns nothing for them: they stay on the host
+MAX_DIMENSION = 65500
+
+# struct cpb200_jpeg_huff (include/centerpose_b200.h): a 9-bit lookup (code length << 8 | symbol, 0 = longer code),
+# then T.81 F.2.2.3's maxcode / (valptr - mincode) per code length 0..17 and the symbols
+HUFF = np.dtype([("lut", "<u2", (1 << LUT_BITS,)), ("maxcode", "<i4", (18,)), ("valoff", "<i4", (18,)),
+                 ("val", "u1", (256,))])
+assert HUFF.itemsize == 1424
+# struct cpb200_jpeg_image (include/centerpose_b200.h)
+JPEG_IMAGE = np.dtype([("seg_offset", "<i8"), ("huff_offset", "<i8"), ("coef_offset", "<i8"), ("plane_offset", "<i8"),
+                       ("dst_offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("ncomp", "<i4"), ("hs", "<i4"), ("vs", "<i4"),
+                       ("orientation", "<i4"), ("restart_interval", "<i4"), ("nseg", "<i4"), ("dc_tbl", "u1", (4,)),
+                       ("ac_tbl", "u1", (4,)), ("qt", "<u2", (3, 64))])
+assert JPEG_IMAGE.itemsize == 464
+
+
+class JpegInfo:
+    """What ``parse`` found.  ``eligible`` says whether the device decodes the file (``reason`` says why not).  For
+    eligible files: ``h, w`` the coded size, ``oh, ow`` the size after the EXIF ``orientation`` (what ``cv2.imread``
+    returns), ``ncomp``, luma sampling ``hs, vs``, per component quantisation tables (natural order, ``qt``) and
+    Huffman table numbers (``dc``, ``ac``), the tables themselves (``huff[(class, id)]`` = (bits, values, ``HUFF``)),
+    ``restart_interval`` and ``segments``, the (start, end) byte range of each entropy-coded segment."""
+
+    def __init__(self):
+        self.eligible = False
+        self.reason = ""
+        self.orientation = 1
+        self.restart_interval = 0
+
+    def size_after_orientation(self):
+        return (self.w, self.h) if self.orientation >= 5 else (self.h, self.w)
+
+    @property
+    def mcu(self):
+        """MCUs per row and per column."""
+        return -(-self.w // (8 * self.hs)), -(-self.h // (8 * self.vs))
+
+    def blocks(self):
+        """(blocks per row, block rows) of each component in the coefficient workspace: whole MCUs."""
+        mx, my = self.mcu
+        return [(mx * self.hs, my * self.vs)] + [(mx, my)] * (self.ncomp - 1)
+
+    def workspace_bytes(self):
+        """int16 coefficients (128 bytes per block) and 8-bit planes (64 bytes per block)."""
+        return sum(bw * bh for bw, bh in self.blocks()) * 192
+
+
+def _exif_orientation(seg):
+    """The orientation tag (0x0112) of IFD0 in an APP1 Exif payload, 1 when absent or unreadable."""
+    if len(seg) < 14 or seg[:6] != b"Exif\x00\x00":
+        return 1
+    t = seg[6:]
+    if t[:2] == b"II":
+        order = "<"
+    elif t[:2] == b"MM":
+        order = ">"
+    else:
+        return 1
+    u16 = lambda o: int(np.frombuffer(t, order + "u2", 1, o)[0])
+    u32 = lambda o: int(np.frombuffer(t, order + "u4", 1, o)[0])
+    ifd = u32(4)
+    if ifd + 2 > len(t):
+        return 1
+    for n in range(u16(ifd)):
+        e = ifd + 2 + 12 * n
+        if e + 12 > len(t):
+            return 1
+        if u16(e) == 0x0112:
+            v = u16(e + 8)
+            return v if 1 <= v <= 8 else 1
+    return 1
+
+
+def build_huff(bits, vals, name, dc):
+    """One ``HUFF`` table from the DHT code-length counts ``bits[1..16]`` and symbols; rejects counts that do not form
+    a prefix code (T.81 C.2) and, for DC tables, symbols above 15 (libjpeg refuses both)."""
+    if sum(bits) > 256 or sum(bits) > len(vals):
+        raise ValueError("%s: bad Huffman table (%d codes)" % (name, sum(bits)))
+    if dc and any(v > 15 for v in vals):
+        raise ValueError("%s: DC Huffman symbol above 15" % name)
+    t = np.zeros((), HUFF)
+    t["maxcode"][:] = -1
+    t["maxcode"][17] = 0x7FFFFFFF
+    t["val"][:len(vals)] = vals
+    code, k = 0, 0
+    for ln in range(1, 17):
+        n = bits[ln - 1]
+        if n:
+            t["valoff"][ln] = k - code
+            for _ in range(n):
+                if ln <= LUT_BITS:
+                    lo = code << (LUT_BITS - ln)
+                    t["lut"][lo:lo + (1 << (LUT_BITS - ln))] = (ln << 8) | vals[k]
+                code += 1
+                k += 1
+            t["maxcode"][ln] = code - 1
+        if code > (1 << ln):
+            raise ValueError("%s: Huffman code lengths do not form a prefix code" % name)
+        code <<= 1
+    return t
+
+
+def parse(data, name="image"):
+    """Headers of one file (bytes or a uint8 array).  Returns a ``JpegInfo``; raises ``ValueError`` naming ``name``
+    when the file is not a JPEG the parser can read (truncated or garbled headers)."""
+    d = np.frombuffer(data, np.uint8) if not isinstance(data, np.ndarray) else data
+    n = len(d)
+    info = JpegInfo()
+    if n < 4 or d[0] != 0xFF or d[1] != 0xD8:
+        raise ValueError("%s: not a JPEG file (no SOI marker)" % name)
+    qt, huff = {}, {}
+    jfif = False
+    adobe = None
+    sof = None
+    pos = 2
+    while True:
+        while pos < n and d[pos] == 0xFF and pos + 1 < n and d[pos + 1] == 0xFF:
+            pos += 1                                               # fill bytes
+        if pos + 4 > n or d[pos] != 0xFF:
+            raise ValueError("%s: truncated or garbled header at byte %d" % (name, pos))
+        m = int(d[pos + 1])
+        if m == 0xD8 or m == 0xD9 or 0xD0 <= m <= 0xD7 or m == 0x01:
+            raise ValueError("%s: unexpected marker 0x%02X before the scan" % (name, m))
+        ln = (int(d[pos + 2]) << 8) | int(d[pos + 3])
+        if ln < 2 or pos + 2 + ln > n:
+            raise ValueError("%s: segment 0x%02X of length %d runs past the end of the file" % (name, m, ln))
+        seg = d[pos + 4:pos + 2 + ln].tobytes()
+        pos += 2 + ln
+        if m == 0xE0 and seg[:5] == b"JFIF\x00":
+            jfif = True
+        elif m == 0xE1 and seg[:6] == b"Exif\x00\x00" and info.orientation == 1:
+            info.orientation = _exif_orientation(seg)
+        elif m == 0xEE and seg[:5] == b"Adobe" and len(seg) >= 12:
+            adobe = seg[11]
+        elif m == 0xDB:
+            o = 0
+            while o < len(seg):
+                pq, tq = seg[o] >> 4, seg[o] & 15
+                size = 128 if pq else 64
+                if pq > 1 or tq > 3 or o + 1 + size > len(seg):
+                    raise ValueError("%s: bad quantisation table" % name)
+                q = np.frombuffer(seg, ">u2" if pq else "u1", 64, o + 1).astype(np.int64)
+                nat = np.zeros(64, np.int64)
+                nat[ZIGZAG] = q
+                qt[tq] = nat
+                o += 1 + size
+        elif m == 0xC4:
+            o = 0
+            while o < len(seg):
+                if o + 17 > len(seg):
+                    raise ValueError("%s: bad Huffman table" % name)
+                tc, th = seg[o] >> 4, seg[o] & 15
+                bits = list(seg[o + 1:o + 17])
+                cnt = sum(bits)
+                if tc > 1 or th > 3 or o + 17 + cnt > len(seg):
+                    raise ValueError("%s: bad Huffman table" % name)
+                vals = list(seg[o + 17:o + 17 + cnt])
+                huff[(tc, th)] = (bits, vals, build_huff(bits, vals, name, tc == 0))
+                o += 17 + cnt
+        elif m == 0xDD:
+            if len(seg) < 2:
+                raise ValueError("%s: bad DRI segment" % name)
+            info.restart_interval = (seg[0] << 8) | seg[1]
+        elif 0xC0 <= m <= 0xCF and m not in (0xC4, 0xC8, 0xCC):
+            if len(seg) < 6 or len(seg) < 6 + 3 * seg[5]:
+                raise ValueError("%s: bad SOF segment" % name)
+            sof = (m, seg[0], (seg[1] << 8) | seg[2], (seg[3] << 8) | seg[4],
+                   [(seg[6 + 3 * i], seg[7 + 3 * i] >> 4, seg[7 + 3 * i] & 15, seg[8 + 3 * i]) for i in range(seg[5])])
+        elif m == 0xCC:
+            info.reason = "arithmetic coding"
+            return info
+        elif m == 0xDA:
+            break
+    if sof is None:
+        raise ValueError("%s: no SOF segment before the scan" % name)
+    kind, prec, h, w, comps = sof
+    info.h, info.w = h, w
+    if not (1 <= h <= MAX_DIMENSION and 1 <= w <= MAX_DIMENSION):
+        raise ValueError("%s: image size %dx%d outside 1..%d" % (name, w, h, MAX_DIMENSION))
+    info.oh, info.ow = info.size_after_orientation()
+    if kind not in (0xC0, 0xC1):
+        info.reason = "SOF%d (not sequential Huffman)" % (kind - 0xC0)
+        return info
+    if prec != 8:
+        info.reason = "%d-bit precision" % prec
+        return info
+    nc = len(comps)
+    if nc == 3:
+        cid = [c[0] for c in comps]
+        if jfif:
+            ycc = True
+        elif adobe is not None:
+            ycc = adobe == 1
+        else:
+            ycc = cid != [82, 71, 66]
+        if not ycc:
+            info.reason = "RGB or Adobe transform %s" % adobe
+            return info
+        samp = [(c[1], c[2]) for c in comps]
+        if samp[1] != (1, 1) or samp[2] != (1, 1) or samp[0] not in ((1, 1), (2, 1), (1, 2), (2, 2)):
+            info.reason = "sampling %s" % samp
+            return info
+        info.hs, info.vs = samp[0]
+    elif nc == 1:
+        info.hs = info.vs = 1                    # a lone component is one non-interleaved scan of plain blocks
+    else:
+        info.reason = "%d components" % nc
+        return info
+    info.ncomp = nc
+    # the SOS header (seg still holds its payload)
+    ns = seg[0] if seg else 0
+    if len(seg) < 4 + 2 * ns or ns < 1:
+        raise ValueError("%s: bad SOS segment" % name)
+    scomp = [(seg[1 + 2 * i], seg[2 + 2 * i] >> 4, seg[2 + 2 * i] & 15) for i in range(ns)]
+    ss, se, ahal = seg[1 + 2 * ns], seg[2 + 2 * ns], seg[3 + 2 * ns]
+    if ns != nc or [s[0] for s in scomp] != [c[0] for c in comps]:
+        info.reason = "multi-scan sequential file"
+        return info
+    if ss != 0 or se != 63 or ahal != 0:
+        raise ValueError("%s: bad spectral selection in a sequential scan" % name)
+    info.qt, info.dc, info.ac = [], [], []
+    for (cid, td, ta), c in zip(scomp, comps):
+        if c[3] not in qt or (0, td) not in huff or (1, ta) not in huff:
+            raise ValueError("%s: the scan uses an undefined table" % name)
+        info.qt.append(qt[c[3]])
+        info.dc.append(td)
+        info.ac.append(ta)
+    info.huff = huff
+    # entropy-coded segments: RST markers up to the first other marker (or the end of a truncated file)
+    body = d[pos:]
+    ff = np.flatnonzero(body[:-1] == 0xFF)
+    nxt = body[ff + 1]
+    mk = (nxt != 0) & (nxt != 0xFF)
+    ff, nxt = ff[mk], nxt[mk]
+    rst = (nxt & 0xF8) == 0xD0
+    stop = np.flatnonzero(~rst)
+    end = int(ff[stop[0]]) if len(stop) else len(body)
+    ff, nxt = ff[rst], nxt[rst]
+    keep = ff < end
+    ff, nxt = ff[keep], nxt[keep]
+    mx, my = info.mcu
+    total = mx * my
+    ri = info.restart_interval
+    nseg = -(-total // ri) if ri else 1
+    if len(ff) > nseg - 1 or (len(ff) and not ri):
+        info.reason = "restart markers do not match the restart interval"
+        return info
+    if not np.array_equal(nxt & 7, np.arange(len(ff)) % 8):
+        info.reason = "restart markers out of sequence"
+        return info
+    starts = np.concatenate([[0], ff + 2]) + pos
+    ends = np.concatenate([ff, [end]]) + pos
+    segs = np.full((nseg, 2), pos + end, np.int64)         # segments past a cut have no data (the device flags them)
+    segs[:len(starts), 0] = starts
+    segs[:len(starts), 1] = ends
+    info.segments = segs
+    if w * h * 3 >= 2 ** 62 or info.workspace_bytes() >= 2 ** 62:
+        raise ValueError("%s: image too large" % name)
+    info.eligible = True
+    return info
+
+
+def pack(infos, datas, dst_offsets, alloc=lambda n: np.empty(n, np.uint8)):
+    """One ``cpb200_jpeg_decode_batch`` launch over the eligible ``infos`` with file bytes ``datas``: a buffer
+    ``[table (B x 464 B) | per image: Huffman tables | segments | file bytes]`` whose offsets are relative to its own
+    start, so the same device copy is both ``src`` and ``table``.  ``dst_offsets`` are the byte offsets of the decoded
+    images in ``dst``.  ``alloc(nbytes)`` returns the uint8 host buffer.  Returns ``(buffer, workspace_bytes)``."""
+    B = len(infos)
+    table = np.zeros(B, JPEG_IMAGE)
+    up = lambda x, a: x + (-x) % a
+    pos = up(table.nbytes, 16)
+    ws = 0
+    place = []
+    for n, (info, data) in enumerate(zip(infos, datas)):
+        keys = sorted({(0, t) for t in info.dc} | {(1, t) for t in info.ac})
+        e = table[n]
+        e["huff_offset"] = pos
+        pos += len(keys) * HUFF.itemsize
+        e["seg_offset"] = pos
+        pos = up(pos + len(info.segments) * 16, 16)
+        place.append((keys, pos))
+        pos = up(pos + len(data), 16)
+        e["coef_offset"] = ws
+        nblk = sum(bw * bh for bw, bh in info.blocks())
+        e["plane_offset"] = ws + nblk * 128
+        ws += nblk * 192
+        e["dst_offset"] = dst_offsets[n]
+        e["h"], e["w"], e["ncomp"], e["hs"], e["vs"] = info.h, info.w, info.ncomp, info.hs, info.vs
+        e["orientation"], e["restart_interval"], e["nseg"] = info.orientation, info.restart_interval, len(info.segments)
+        for c in range(info.ncomp):
+            e["dc_tbl"][c] = keys.index((0, info.dc[c]))
+            e["ac_tbl"][c] = keys.index((1, info.ac[c]))
+            e["qt"][c] = info.qt[c]
+    if pos >= 2 ** 62:
+        raise ValueError("jpeg: launch buffer too large")
+    buf = alloc(pos)
+    hv = buf.numpy() if hasattr(buf, "numpy") else buf
+    hv[:table.nbytes] = table.view(np.uint8)
+    for info, data, e, (keys, base) in zip(infos, datas, table, place):
+        h0 = int(e["huff_offset"])
+        for k, key in enumerate(keys):
+            hv[h0 + k * HUFF.itemsize:h0 + (k + 1) * HUFF.itemsize] = info.huff[key][2].reshape(1).view(np.uint8)
+        s0 = int(e["seg_offset"])
+        # the parser's segment bounds are file offsets; the kernel reads them as offsets into the buffer
+        hv[s0:s0 + len(info.segments) * 16] = (info.segments + base).astype("<i8").view(np.uint8).reshape(-1)
+        hv[base:base + len(data)] = np.frombuffer(data, np.uint8) if not isinstance(data, np.ndarray) else data
+    return buf, ws

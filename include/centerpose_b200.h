@@ -136,6 +136,48 @@ typedef struct cpb200_resize_image {
 int cpb200_resize_linear_u8_batch(const unsigned char *src, const cpb200_resize_image *table, int B, unsigned char *dst,
                                   void *stream);
 
+/* One Huffman table of cpb200_jpeg_decode_batch (1424 bytes, 4-byte aligned in `src`).  lut[b] for the next 9 bits b
+ * is (code length << 8 | symbol), or 0 when the code is longer than 9 bits; then maxcode[l] (largest code of length
+ * l, -1 if none, maxcode[17] = INT32_MAX) and valoff[l] (index in val of the first code of length l, minus that code),
+ * T.81 F.2.2.3.  The code lengths form a prefix code; DC symbols are <= 15. */
+typedef struct cpb200_jpeg_huff {
+  uint16_t lut[512];
+  int32_t maxcode[18];
+  int32_t valoff[18];
+  uint8_t val[256];
+} cpb200_jpeg_huff;
+
+/* One image of cpb200_jpeg_decode_batch (464 bytes, lives in caller-owned DEVICE memory).  Offsets are bytes. */
+typedef struct cpb200_jpeg_image {
+  int64_t seg_offset;        /* in `src`: nseg x {int64 start, end}, the byte ranges in `src` of the entropy-coded
+                                segments (restart intervals; the whole scan without DRI), 8-byte aligned */
+  int64_t huff_offset;       /* in `src`: the image's cpb200_jpeg_huff tables, 4-byte aligned */
+  int64_t coef_offset;       /* in `workspace`: int16 coefficient blocks, 128 bytes per block, 16-byte aligned */
+  int64_t plane_offset;      /* in `workspace`: uint8 component planes, 64 bytes per block */
+  int64_t dst_offset;        /* in `dst`: the decoded HWC uint8 BGR image, rows packed, size after orientation */
+  int32_t h, w;              /* coded size, 1..65500 */
+  int32_t ncomp;             /* 1 (grayscale) or 3 (YCbCr) */
+  int32_t hs, vs;            /* luma sampling factors, each 1 or 2 (1, 1 for grayscale); chroma is sampled (1, 1) */
+  int32_t orientation;       /* EXIF orientation 1..8, applied as cv2.imread does */
+  int32_t restart_interval;  /* MCUs per segment; 0: one segment */
+  int32_t nseg;              /* ceil(MCUs / restart_interval), or 1 */
+  uint8_t dc_tbl[4], ac_tbl[4];  /* per component: index of its DC / AC table at huff_offset */
+  uint16_t qt[3][64];        /* per component: quantisation table in natural (row-major) order */
+} cpb200_jpeg_image;
+
+/* cv2.imread(path, IMREAD_COLOR) of sequential-Huffman JPEG files, byte for byte (libjpeg-turbo's ISLOW IDCT, fancy
+ * upsampling and integer YCbCr->BGR, then OpenCV's EXIF orientation; verified against cv2 4.13 with libjpeg-turbo
+ * 3.1).  B files in one launch: `src` holds the file bytes and the Huffman tables and segment lists the table points
+ * to, `table` is a DEVICE array of B cpb200_jpeg_image that the caller has checked (the kernels trust it; see
+ * centerpose_b200/jpeg.py), `workspace` holds every image's coefficients and planes (an image whose workspace would
+ * end past `workspace_bytes` is not decoded and gets status 2).  Each image's segments are decoded by one thread
+ * each, then IDCT, upsampling and colour conversion run over the whole launch.  status[b] (DEVICE int array) is 0 when
+ * image b decoded, non-zero when its entropy data was bad (a code longer than 16 bits, a run past coefficient 63 or
+ * data ending before a segment's last MCU); the image's pixels are then undefined, other images are unaffected.
+ * 1 <= B <= 65535. */
+int cpb200_jpeg_decode_batch(const unsigned char *src, const cpb200_jpeg_image *table, int B, void *workspace,
+                             size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)
