@@ -1,7 +1,9 @@
-// cpb200_jpeg_decode_batch: cv2.imread(path, IMREAD_COLOR) of sequential-Huffman JPEG files on the device, byte for
-// byte, for many files per launch.  Three kernels:
-//   jpeg_entropy_kernel  one CTA per image, one thread per entropy-coded segment (restart interval; the whole scan
-//                        without DRI): Huffman decode into de-zigzagged int16 coefficient blocks,
+// cpb200_jpeg_decode_batch: cv2.imread(path, IMREAD_COLOR) of sequential- and progressive-Huffman JPEG files on the
+// device, byte for byte, for many files per launch.  Four kernels:
+//   jpeg_entropy_kernel  sequential images: one CTA per image, one thread per entropy-coded segment (restart interval;
+//                        the whole scan without DRI): Huffman decode into de-zigzagged int16 coefficient blocks,
+//   jpeg_progressive_kernel  progressive images: one CTA per image runs the scans in file order into the same blocks,
+//                        one thread per segment of a scan,
 //   jpeg_idct_kernel     dequantise + libjpeg's ISLOW integer IDCT (jidctint.c), 8 threads per block, into 8-bit
 //                        component planes padded to whole MCUs,
 //   jpeg_color_kernel    one thread per output pixel: libjpeg-turbo's fancy upsampling (jdsample.c), integer
@@ -11,7 +13,8 @@
 
 namespace {
 
-static_assert(sizeof(cpb200_jpeg_image) == 464, "cpb200_jpeg_image layout is part of the C ABI");
+static_assert(sizeof(cpb200_jpeg_image) == 480, "cpb200_jpeg_image layout is part of the C ABI");
+static_assert(sizeof(cpb200_jpeg_scan) == 40, "cpb200_jpeg_scan layout is part of the C ABI");
 static_assert(sizeof(cpb200_jpeg_huff) == 1424, "cpb200_jpeg_huff layout is part of the C ABI");
 
 __constant__ unsigned char kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,
@@ -98,6 +101,13 @@ struct Bits {
     skip(s);
     return v < (1 << (s - 1)) ? v - (1 << s) + 1 : v;
   }
+  // the next k (1..16) bits, unsigned
+  __device__ __forceinline__ int get(int k) {
+    fill();
+    const int v = (int)(acc >> (64 - k));
+    skip(k);
+    return v;
+  }
 };
 
 // grid B CTAs x 32 threads: CTA b decodes image b, its threads stride over the image's segments
@@ -106,6 +116,7 @@ __global__ void __launch_bounds__(32) jpeg_entropy_kernel(const unsigned char *_
                                                           unsigned char *__restrict__ ws, size_t ws_bytes,
                                                           int *__restrict__ status) {
   const cpb200_jpeg_image &e = table[blockIdx.x];
+  if (e.nscan) return;                                      // progressive: jpeg_progressive_kernel
   const Geo g = geometry(e);
   if (!fits(e, g, ws_bytes)) {
     if (threadIdx.x == 0) status[blockIdx.x] = 2;
@@ -161,6 +172,149 @@ __global__ void __launch_bounds__(32) jpeg_entropy_kernel(const unsigned char *_
   bad:
     status[blockIdx.x] = 1;
     return;
+  }
+}
+
+// AC refinement of one coefficient with nonzero history: a correction bit adds p1 (or m1 below zero) unless that bit is
+// already set; the sum is stored to 16 bits as libjpeg's JCOEF
+__device__ __forceinline__ void refine(short *cf, Bits &r, int p1, int m1) {
+  if (r.get(1) && !(*cf & p1)) *cf = (short)(*cf >= 0 ? *cf + p1 : *cf + m1);
+}
+
+// One restart segment of a progressive scan, units [u0, u1), as libjpeg-turbo's jdphuff.c decodes T.81 G.1.2: DC first
+// (difference << Al), DC refinement (one bit), AC first (EOBRUN runs of empty blocks), AC refinement (correction bits
+// on coefficients with nonzero history; zero runs and EOBRUN count only zero-history coefficients).  A unit is an MCU
+// when the scan has several components, else one block of the component's own grid, `cbw` blocks per row.  Returns
+// false on a code longer than 16 bits, a run past Se, a refinement size other than 0 or 1, or data ending before the
+// segment's last unit.
+__device__ __forceinline__ bool progressive_segment(const cpb200_jpeg_scan &s, const cpb200_jpeg_image &e, const Geo &g,
+                                                    short *coef,
+                                                    const cpb200_jpeg_huff *__restrict__ huff, Bits &r, int64_t u0,
+                                                    int64_t u1, int cbw) {
+  const int ss = s.ss, se = s.se, al = s.al, nc = s.ncomp;
+  const int p1 = 1 << al, m1 = -p1;
+  const int kind = ss == 0 ? (s.ah == 0 ? 0 : 1) : (s.ah == 0 ? 2 : 3);
+  const cpb200_jpeg_huff *ac = huff + s.ac_tbl[0];
+  int pred0 = 0, pred1 = 0, pred2 = 0, eobrun = 0;
+  for (int64_t u = u0; u < u1; ++u) {
+    const int uw = nc > 1 ? g.mcux : cbw;
+    const int uy = (int)(u / uw), ux = (int)(u - (int64_t)uy * uw);
+    for (int i = 0; i < nc; ++i) {
+      const int c = s.comp[i];
+      const int hs = nc > 1 && c == 0 ? e.hs : 1, vs = nc > 1 && c == 0 ? e.vs : 1;
+      for (int b = 0; b < hs * vs; ++b) {
+        short *blk = coef + (pick(g.base, c) + (int64_t)(uy * vs + b / hs) * pick(g.bw, c) + ux * hs + b % hs) * 64;
+        if (kind == 0) {                                      // DC first
+          const int sym = r.symbol(huff + s.dc_tbl[i]);
+          if (sym < 0) return false;
+          const int dc = r.receive(sym) + (i == 0 ? pred0 : i == 1 ? pred1 : pred2);
+          if (i == 0) pred0 = dc; else if (i == 1) pred1 = dc; else pred2 = dc;
+          blk[0] = (short)((unsigned)dc << al);
+        } else if (kind == 1) {                               // DC refinement
+          if (r.get(1)) blk[0] = (short)(blk[0] | p1);
+        } else if (kind == 2) {                               // AC first
+          if (eobrun) { --eobrun; continue; }
+          for (int k = ss; k <= se; ++k) {
+            const int sym = r.symbol(ac);
+            if (sym < 0) return false;
+            const int run = sym >> 4, sz = sym & 15;
+            if (sz) {
+              k += run;
+              if (k > se) return false;
+              blk[kZigzag[k]] = (short)((unsigned)r.receive(sz) << al);
+            } else if (run == 15) {
+              k += 15;
+            } else {
+              eobrun = (1 << run) - 1;
+              if (run) eobrun += r.get(run);
+              break;
+            }
+          }
+        } else {                                              // AC refinement
+          int k = ss;
+          if (!eobrun) {
+            for (; k <= se; ++k) {
+              const int sym = r.symbol(ac);
+              if (sym < 0) return false;
+              int run = sym >> 4, v = 0;
+              const int sz = sym & 15;
+              if (sz) {
+                if (sz != 1) return false;
+                v = r.get(1) ? p1 : m1;
+              } else if (run != 15) {
+                eobrun = 1 << run;
+                if (run) eobrun += r.get(run);
+                break;
+              }
+              for (; k <= se; ++k) {
+                short *cf = blk + kZigzag[k];
+                if (*cf) refine(cf, r, p1, m1);
+                else if (--run < 0) break;
+              }
+              if (v) {
+                if (k > se) return false;
+                blk[kZigzag[k]] = (short)v;
+              }
+            }
+          }
+          if (eobrun) {
+            for (; k <= se; ++k) {
+              short *cf = blk + kZigzag[k];
+              if (*cf) refine(cf, r, p1, m1);
+            }
+            --eobrun;
+          }
+        }
+      }
+    }
+    if (r.used > r.real) return false;                      // the segment's data ended before this unit did
+  }
+  return true;
+}
+
+// grid B CTAs x 32 threads: CTA b zeroes image b's coefficients, then runs its scans in file order, its threads
+// striding over each scan's segments; sequential images return at once.  The minimum of one block per SM lets ptxas
+// use the 90 registers the four decoders need (it caps the plain bound at 64 and spills)
+__global__ void __launch_bounds__(32, 1) jpeg_progressive_kernel(const unsigned char *__restrict__ src,
+                                                                 const cpb200_jpeg_image *__restrict__ table,
+                                                                 unsigned char *__restrict__ ws, size_t ws_bytes,
+                                                                 int *__restrict__ status) {
+  __shared__ int failed;
+  const cpb200_jpeg_image &e = table[blockIdx.x];
+  if (!e.nscan) return;
+  const Geo g = geometry(e);
+  if (!fits(e, g, ws_bytes)) {
+    if (threadIdx.x == 0) status[blockIdx.x] = 2;
+    return;
+  }
+  if (threadIdx.x == 0) {
+    status[blockIdx.x] = 0;
+    failed = 0;
+  }
+  int4 *z = reinterpret_cast<int4 *>(ws + e.coef_offset);
+  for (int64_t i = threadIdx.x; i < g.nblk * 8; i += blockDim.x) z[i] = make_int4(0, 0, 0, 0);
+  __syncthreads();
+  const cpb200_jpeg_scan *scans = reinterpret_cast<const cpb200_jpeg_scan *>(src + e.scan_offset);
+  const cpb200_jpeg_huff *huff = reinterpret_cast<const cpb200_jpeg_huff *>(src + e.huff_offset);
+  short *coef = reinterpret_cast<short *>(ws + e.coef_offset);
+  for (int n = 0; n < e.nscan; ++n) {
+    const cpb200_jpeg_scan &s = scans[n];
+    // one component: its own block grid, which for luma sampled (2, x) can be a column / row short of whole MCUs
+    const int c = s.comp[0], hs = c == 0 ? e.hs : 1, vs = c == 0 ? e.vs : 1;
+    const int cbw = ((e.w * hs + e.hs - 1) / e.hs + 7) / 8, cbh = ((e.h * vs + e.vs - 1) / e.vs + 7) / 8;
+    const int64_t total = s.ncomp > 1 ? (int64_t)g.mcux * g.mcuy : (int64_t)cbw * cbh;
+    const int64_t ri = s.restart_interval ? s.restart_interval : total;
+    const int64_t *seg = reinterpret_cast<const int64_t *>(src + s.seg_offset);
+    for (int q = threadIdx.x; q < s.nseg; q += blockDim.x) {
+      Bits r{src, seg[2 * q], seg[2 * q + 1], 0ull, 0, 0, 0};
+      if (!progressive_segment(s, e, g, coef, huff, r, (int64_t)q * ri, min((int64_t)(q + 1) * ri, total), cbw)) {
+        status[blockIdx.x] = 1;
+        failed = 1;
+        break;
+      }
+    }
+    __syncthreads();                                        // the next scan refines what this one wrote
+    if (failed) return;
   }
 }
 
@@ -308,6 +462,9 @@ extern "C" int cpb200_jpeg_decode_batch(const unsigned char *src, const cpb200_j
   unsigned char *ws = static_cast<unsigned char *>(workspace);
   jpeg_entropy_kernel<<<B, 32, 0, st>>>(src, table, ws, workspace_bytes, status);
   int rc = cpb::check_launch("jpeg_entropy_kernel");
+  if (rc) return rc;
+  jpeg_progressive_kernel<<<B, 32, 0, st>>>(src, table, ws, workspace_bytes, status);
+  rc = cpb::check_launch("jpeg_progressive_kernel");
   if (rc) return rc;
   // the sizes live on the device: enough blocks per image to fill the GPU for one large image, fewer as B grows
   const dim3 grid((unsigned)std::max(1, 132 * 8 / B), (unsigned)B);

@@ -482,7 +482,7 @@ class MultiPoseDetector(BaseDetector):
                 info = jpeg.parse(data, src)
             except ValueError:
                 info = None
-            if info is not None and info.eligible:
+            if info is not None and (info.eligible or info.progressive):
                 datas[n], infos[n] = data, info
             else:
                 host[n] = self._load_checked(n, src)
@@ -552,7 +552,7 @@ class MultiPoseDetector(BaseDetector):
         only host wait is the final device-to-host copy.
 
         With ``B200.DEVICE_PREPROCESS`` on (the default) and any path among the inputs, the images are decoded into
-        one device buffer first (``_load_images_device``): sequential-Huffman JPEG files by
+        one device buffer first (``_load_images_device``): sequential- and progressive-Huffman JPEG files by
         ``cpb200_jpeg_decode_batch``, byte for byte as ``cv2.imread``; every other file, and every array, on the
         host and uploaded into its slot.  The groups then read that buffer in place.  That adds one small
         device-to-host read of the decode status.  The call then needs device memory for the decoded images (3 bytes

@@ -1,13 +1,24 @@
 """Host side of the device JPEG decoder (``cpb200_jpeg_decode_batch``, ``csrc/jpeg.cu``).
 
 ``parse(data, name)`` reads a file's headers and decides whether the device can decode it byte for byte as
-``cv2.imread(path, IMREAD_COLOR)`` does (libjpeg-turbo's sequential Huffman decoder, ISLOW IDCT, fancy upsampling,
-integer YCbCr->BGR, then OpenCV's EXIF orientation).  ``pack(...)`` lays out the device table of a launch.
+``cv2.imread(path, IMREAD_COLOR)`` does (libjpeg-turbo's Huffman decoders, ISLOW IDCT, fancy upsampling, integer
+YCbCr->BGR, then OpenCV's EXIF orientation).  ``pack(...)`` lays out the device table of a launch.
 
-The device decodes a file only when it is 8-bit, sequential Huffman (SOF0 / SOF1), grayscale or YCbCr, one interleaved
-scan over every component, chroma sampled (1, 1) and luma (1, 1), (2, 1), (1, 2) or (2, 2).  Everything else is
-``eligible == False`` and stays with ``cv2.imread``.  The kernels trust the table, so everything read from the file
-that sizes or indexes it is checked here; a file the parser cannot read raises ``ValueError`` naming the image.
+The device decodes 8-bit grayscale or YCbCr files with chroma sampled (1, 1) and luma (1, 1), (2, 1), (1, 2) or
+(2, 2), in one of two forms, which ``parse`` reports as a pair:
+
+- ``info.eligible``: sequential Huffman (SOF0 / SOF1), one interleaved scan over every component.  The sequential
+  entropy kernel decodes it.
+- ``info.progressive``: progressive Huffman (SOF2), the list of its scans (``JpegScan``).  The progressive entropy
+  kernel decodes it.  The scans must be legal (T.81 G.1.1.1) and consistent (each scan sends coefficient bits not sent
+  before, or refines the bit the previous scan stopped at; no AC scan before its component's first DC scan), at most
+  ``MAX_SCANS``, with no DQT or other frame marker between them, and must code every coefficient down to bit 0 by the
+  end of the file.  With an incomplete progression libjpeg smooths the low-frequency coefficients of each block
+  (``jdcoefct.c``), which the device does not do.
+
+Everything else has ``eligible == False`` and ``progressive is None``, ``reason`` says why, and the file stays with
+``cv2.imread``.  The kernels trust the table, so everything read from the file that sizes or indexes it is checked
+here; a file the parser cannot read raises ``ValueError`` naming the image.
 """
 from __future__ import annotations
 
@@ -30,8 +41,16 @@ assert HUFF.itemsize == 1424
 JPEG_IMAGE = np.dtype([("seg_offset", "<i8"), ("huff_offset", "<i8"), ("coef_offset", "<i8"), ("plane_offset", "<i8"),
                        ("dst_offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("ncomp", "<i4"), ("hs", "<i4"), ("vs", "<i4"),
                        ("orientation", "<i4"), ("restart_interval", "<i4"), ("nseg", "<i4"), ("dc_tbl", "u1", (4,)),
-                       ("ac_tbl", "u1", (4,)), ("qt", "<u2", (3, 64))])
-assert JPEG_IMAGE.itemsize == 464
+                       ("ac_tbl", "u1", (4,)), ("qt", "<u2", (3, 64)), ("scan_offset", "<i8"), ("nscan", "<i4"),
+                       ("pad", "<i4")])
+assert JPEG_IMAGE.itemsize == 480
+# struct cpb200_jpeg_scan (include/centerpose_b200.h): one scan of a progressive image
+SCAN = np.dtype([("seg_offset", "<i8"), ("nseg", "<i4"), ("restart_interval", "<i4"), ("ncomp", "<i4"),
+                 ("comp", "u1", (4,)), ("dc_tbl", "u1", (4,)), ("ac_tbl", "u1", (4,)), ("ss", "u1"), ("se", "u1"),
+                 ("ah", "u1"), ("al", "u1"), ("pad", "<i4")])
+assert SCAN.itemsize == 40
+# scans per progressive file the device takes (libjpeg's simple progression writes 10 for colour, 6 for grayscale)
+MAX_SCANS = 64
 
 
 class JpegInfo:
@@ -39,10 +58,14 @@ class JpegInfo:
     eligible files: ``h, w`` the coded size, ``oh, ow`` the size after the EXIF ``orientation`` (what ``cv2.imread``
     returns), ``ncomp``, luma sampling ``hs, vs``, per component quantisation tables (natural order, ``qt``) and
     Huffman table numbers (``dc``, ``ac``), the tables themselves (``huff[(class, id)]`` = (bits, values, ``HUFF``)),
-    ``restart_interval`` and ``segments``, the (start, end) byte range of each entropy-coded segment."""
+    ``restart_interval`` and ``segments``, the (start, end) byte range of each entropy-coded segment.  For progressive
+    files the device takes, ``progressive`` is the list of scans (``JpegScan``) and ``tables`` the ``HUFF`` tables
+    they bind, in the order of their first use; ``qt`` is set, and ``dc``, ``ac``, ``restart_interval`` and
+    ``segments`` are per scan."""
 
     def __init__(self):
         self.eligible = False
+        self.progressive = None
         self.reason = ""
         self.orientation = 1
         self.restart_interval = 0
@@ -63,6 +86,32 @@ class JpegInfo:
     def workspace_bytes(self):
         """int16 coefficients (128 bytes per block) and 8-bit planes (64 bytes per block)."""
         return sum(bw * bh for bw, bh in self.blocks()) * 192
+
+    def coded_blocks(self, c):
+        """(blocks per row, block rows) that a scan of component ``c`` alone covers: its own samples, not whole MCUs
+        (T.81 A.2.2)."""
+        hs, vs = (self.hs, self.vs) if c == 0 else (1, 1)
+        cw, ch = -(-self.w * hs // self.hs), -(-self.h * vs // self.vs)
+        return -(-cw // 8), -(-ch // 8)
+
+
+class JpegScan:
+    """One scan of a progressive file: component indices ``comps`` (frame order), spectral selection ``ss..se``,
+    successive approximation ``ah, al``, per component the index in ``JpegInfo.tables`` of its DC table (``dc``, for a
+    first DC scan) and AC table (``ac``, for an AC scan), 0 where the scan uses none, ``restart_interval`` (units: MCUs
+    for several components, blocks of ``coded_blocks`` for one) and ``segments`` as for sequential files."""
+
+    def __init__(self, comps, ss, se, ah, al, dc, ac, restart_interval, segments):
+        self.comps, self.ss, self.se, self.ah, self.al = comps, ss, se, ah, al
+        self.dc, self.ac, self.restart_interval, self.segments = dc, ac, restart_interval, segments
+
+    def units(self, info):
+        """Units the scan codes: MCUs when it interleaves components, else the component's blocks."""
+        if len(self.comps) > 1:
+            mx, my = info.mcu
+            return mx * my
+        bw, bh = info.coded_blocks(self.comps[0])
+        return bw * bh
 
 
 def _exif_orientation(seg):
@@ -120,6 +169,59 @@ def build_huff(bits, vals, name, dc):
     return t
 
 
+def _read_dht(seg, huff, name):
+    """The tables of one DHT payload into ``huff[(class, id)]``."""
+    o = 0
+    while o < len(seg):
+        if o + 17 > len(seg):
+            raise ValueError("%s: bad Huffman table" % name)
+        tc, th = seg[o] >> 4, seg[o] & 15
+        bits = list(seg[o + 1:o + 17])
+        cnt = sum(bits)
+        if tc > 1 or th > 3 or o + 17 + cnt > len(seg):
+            raise ValueError("%s: bad Huffman table" % name)
+        vals = list(seg[o + 17:o + 17 + cnt])
+        huff[(tc, th)] = (bits, vals, build_huff(bits, vals, name, tc == 0))
+        o += 17 + cnt
+
+
+def _read_dri(seg, name):
+    if len(seg) < 2:
+        raise ValueError("%s: bad DRI segment" % name)
+    return (seg[0] << 8) | seg[1]
+
+
+def _markers(d, pos):
+    """File offsets and codes of the markers from byte ``pos`` on: 0xFF followed by neither a stuffed zero nor a fill
+    byte."""
+    ff = np.flatnonzero(d[pos:-1] == 0xFF) + pos
+    code = d[ff + 1]
+    mk = (code != 0) & (code != 0xFF)
+    return ff[mk], code[mk]
+
+
+def _segments(markers, pos, n, units, ri):
+    """The entropy-coded segments of a scan whose data starts at byte ``pos`` of an ``n``-byte file: RST markers up to
+    the first other marker (or the end of a truncated file), ``units`` MCUs at ``ri`` per segment (0: one segment).
+    Returns ``(segments, end, reason)``: the (start, end) file offsets as an (nseg, 2) int64 array, the offset of the
+    marker that ends the scan (``n`` when none does), and why the markers do not fit the interval (else "")."""
+    mpos, mcode = markers
+    i = int(np.searchsorted(mpos, pos))
+    stop = np.flatnonzero((mcode[i:] & 0xF8) != 0xD0)
+    j = i + int(stop[0]) if len(stop) else len(mpos)
+    end = int(mpos[j]) if j < len(mpos) else n
+    ff, nxt = mpos[i:j], mcode[i:j]
+    nseg = -(-units // ri) if ri else 1
+    if len(ff) > nseg - 1 or (len(ff) and not ri):
+        return None, end, "restart markers do not match the restart interval"
+    if not np.array_equal(nxt & 7, np.arange(len(ff)) % 8):
+        return None, end, "restart markers out of sequence"
+    segs = np.full((nseg, 2), end, np.int64)               # segments past a cut have no data (the device flags them)
+    segs[:len(ff) + 1, 0] = np.concatenate([[pos], ff + 2])
+    segs[:len(ff) + 1, 1] = np.concatenate([ff, [end]])
+    return segs, end, ""
+
+
 def parse(data, name="image"):
     """Headers of one file (bytes or a uint8 array).  Returns a ``JpegInfo``; raises ``ValueError`` naming ``name``
     when the file is not a JPEG the parser can read (truncated or garbled headers)."""
@@ -165,22 +267,9 @@ def parse(data, name="image"):
                 qt[tq] = nat
                 o += 1 + size
         elif m == 0xC4:
-            o = 0
-            while o < len(seg):
-                if o + 17 > len(seg):
-                    raise ValueError("%s: bad Huffman table" % name)
-                tc, th = seg[o] >> 4, seg[o] & 15
-                bits = list(seg[o + 1:o + 17])
-                cnt = sum(bits)
-                if tc > 1 or th > 3 or o + 17 + cnt > len(seg):
-                    raise ValueError("%s: bad Huffman table" % name)
-                vals = list(seg[o + 17:o + 17 + cnt])
-                huff[(tc, th)] = (bits, vals, build_huff(bits, vals, name, tc == 0))
-                o += 17 + cnt
+            _read_dht(seg, huff, name)
         elif m == 0xDD:
-            if len(seg) < 2:
-                raise ValueError("%s: bad DRI segment" % name)
-            info.restart_interval = (seg[0] << 8) | seg[1]
+            info.restart_interval = _read_dri(seg, name)
         elif 0xC0 <= m <= 0xCF and m not in (0xC4, 0xC8, 0xCC):
             if len(seg) < 6 or len(seg) < 6 + 3 * seg[5]:
                 raise ValueError("%s: bad SOF segment" % name)
@@ -198,8 +287,8 @@ def parse(data, name="image"):
     if not (1 <= h <= MAX_DIMENSION and 1 <= w <= MAX_DIMENSION):
         raise ValueError("%s: image size %dx%d outside 1..%d" % (name, w, h, MAX_DIMENSION))
     info.oh, info.ow = info.size_after_orientation()
-    if kind not in (0xC0, 0xC1):
-        info.reason = "SOF%d (not sequential Huffman)" % (kind - 0xC0)
+    if kind not in (0xC0, 0xC1, 0xC2):
+        info.reason = "SOF%d (not sequential or progressive Huffman)" % (kind - 0xC0)
         return info
     if prec != 8:
         info.reason = "%d-bit precision" % prec
@@ -227,16 +316,25 @@ def parse(data, name="image"):
         info.reason = "%d components" % nc
         return info
     info.ncomp = nc
+    if w * h * 3 >= 2 ** 62 or info.workspace_bytes() >= 2 ** 62:
+        raise ValueError("%s: image too large" % name)
+    if kind == 0xC2:
+        if any(c[3] not in qt for c in comps):
+            raise ValueError("%s: the scan uses an undefined table" % name)
+        scans, tables, why = _progressive_scans(d, pos, seg, info, comps, huff, name)
+        if why:
+            info.reason = "progressive: " + why
+            return info
+        info.qt = [qt[c[3]] for c in comps]
+        info.progressive, info.tables = scans, tables
+        info.reason = "SOF2 (not sequential Huffman)"
+        return info
     # the SOS header (seg still holds its payload)
-    ns = seg[0] if seg else 0
-    if len(seg) < 4 + 2 * ns or ns < 1:
-        raise ValueError("%s: bad SOS segment" % name)
-    scomp = [(seg[1 + 2 * i], seg[2 + 2 * i] >> 4, seg[2 + 2 * i] & 15) for i in range(ns)]
-    ss, se, ahal = seg[1 + 2 * ns], seg[2 + 2 * ns], seg[3 + 2 * ns]
-    if ns != nc or [s[0] for s in scomp] != [c[0] for c in comps]:
+    scomp, ss, se, ah, al = _read_sos(seg, name)
+    if len(scomp) != nc or [s[0] for s in scomp] != [c[0] for c in comps]:
         info.reason = "multi-scan sequential file"
         return info
-    if ss != 0 or se != 63 or ahal != 0:
+    if ss != 0 or se != 63 or ah or al:
         raise ValueError("%s: bad spectral selection in a sequential scan" % name)
     info.qt, info.dc, info.ac = [], [], []
     for (cid, td, ta), c in zip(scomp, comps):
@@ -246,45 +344,105 @@ def parse(data, name="image"):
         info.dc.append(td)
         info.ac.append(ta)
     info.huff = huff
-    # entropy-coded segments: RST markers up to the first other marker (or the end of a truncated file)
-    body = d[pos:]
-    ff = np.flatnonzero(body[:-1] == 0xFF)
-    nxt = body[ff + 1]
-    mk = (nxt != 0) & (nxt != 0xFF)
-    ff, nxt = ff[mk], nxt[mk]
-    rst = (nxt & 0xF8) == 0xD0
-    stop = np.flatnonzero(~rst)
-    end = int(ff[stop[0]]) if len(stop) else len(body)
-    ff, nxt = ff[rst], nxt[rst]
-    keep = ff < end
-    ff, nxt = ff[keep], nxt[keep]
     mx, my = info.mcu
-    total = mx * my
-    ri = info.restart_interval
-    nseg = -(-total // ri) if ri else 1
-    if len(ff) > nseg - 1 or (len(ff) and not ri):
-        info.reason = "restart markers do not match the restart interval"
+    info.segments, _, why = _segments(_markers(d, pos), pos, n, mx * my, info.restart_interval)
+    if why:
+        info.reason = why
         return info
-    if not np.array_equal(nxt & 7, np.arange(len(ff)) % 8):
-        info.reason = "restart markers out of sequence"
-        return info
-    starts = np.concatenate([[0], ff + 2]) + pos
-    ends = np.concatenate([ff, [end]]) + pos
-    segs = np.full((nseg, 2), pos + end, np.int64)         # segments past a cut have no data (the device flags them)
-    segs[:len(starts), 0] = starts
-    segs[:len(starts), 1] = ends
-    info.segments = segs
-    if w * h * 3 >= 2 ** 62 or info.workspace_bytes() >= 2 ** 62:
-        raise ValueError("%s: image too large" % name)
     info.eligible = True
     return info
 
 
+def _read_sos(seg, name):
+    """(components as (id, DC table, AC table), Ss, Se, Ah, Al) of an SOS payload."""
+    ns = seg[0] if seg else 0
+    if len(seg) < 4 + 2 * ns or ns < 1:
+        raise ValueError("%s: bad SOS segment" % name)
+    scomp = [(seg[1 + 2 * i], seg[2 + 2 * i] >> 4, seg[2 + 2 * i] & 15) for i in range(ns)]
+    return scomp, seg[1 + 2 * ns], seg[2 + 2 * ns], seg[3 + 2 * ns] >> 4, seg[3 + 2 * ns] & 15
+
+
+def _progressive_scans(d, pos, seg, info, comps, huff, name):
+    """The scans of a progressive file whose first SOS payload is ``seg``, with its entropy data at byte ``pos``, up to
+    EOI.  Returns ``(scans, tables, reason)``: the ``JpegScan`` list, the ``HUFF`` tables the scans index, and why the
+    device does not take the file ("" when it does)."""
+    n = len(d)
+    cids = [c[0] for c in comps]
+    # per component and zigzag coefficient: Al of the last scan that coded it, -1 before any (libjpeg's coef_bits)
+    coded = np.full((len(comps), 64), -1, np.int64)
+    markers = _markers(d, pos)
+    ri = info.restart_interval
+    scans, used, index = [], [], {}
+
+    def table(key):
+        if key not in huff:
+            raise ValueError("%s: the scan uses an undefined table" % name)
+        t = huff[key]                            # the table current at this SOS; a later DHT replaces the entry
+        if id(t) not in index:
+            index[id(t)] = len(used)
+            used.append(t)
+        return index[id(t)]
+
+    while True:
+        if len(scans) == MAX_SCANS:
+            return None, None, "more than %d scans" % MAX_SCANS
+        k = len(scans)
+        scomp, ss, se, ah, al = _read_sos(seg, name)
+        idx = [cids.index(s[0]) if s[0] in cids else -1 for s in scomp]
+        if -1 in idx or idx != sorted(set(idx)):
+            return None, None, "scan %d: components %s not a subset of the frame's in frame order" % (k, idx)
+        dc = ss == 0
+        # T.81 G.1.1.1, as libjpeg-turbo's jdphuff.c checks it (it refuses the file otherwise)
+        if (se != 0 if dc else (se > 63 or ss > se or len(idx) != 1)) or (ah and ah != al + 1) or al > 13:
+            return None, None, "scan %d: illegal progression Ss %d Se %d Ah %d Al %d" % (k, ss, se, ah, al)
+        # what libjpeg only warns about (a bogus progression) changes its output, so those files stay on the host
+        if (coded[idx, ss:se + 1] != (ah if ah else -1)).any() or (not dc and coded[idx[0], 0] < 0):
+            return None, None, "scan %d: inconsistent progression Ss %d Se %d Ah %d Al %d" % (k, ss, se, ah, al)
+        coded[idx, ss:se + 1] = al
+        scan = JpegScan(idx, ss, se, ah, al, [table((0, s[1])) if dc and not ah else 0 for s in scomp],
+                        [0 if dc else table((1, s[2])) for s in scomp], ri, None)
+        scan.segments, end, why = _segments(markers, pos, n, scan.units(info), ri)
+        if why:
+            return None, None, "scan %d: %s" % (k, why)
+        scans.append(scan)
+        if end >= n:
+            break                                # cut inside this scan's data: the device flags what is missing
+        # the markers up to the next scan: tables and restart intervals may change, nothing else may
+        pos, m = end, 0
+        while m != 0xDA:
+            while pos + 1 < n and d[pos] == 0xFF and d[pos + 1] == 0xFF:
+                pos += 1                                           # fill bytes
+            if pos + 2 > n:
+                return None, None, "the file ends between scans"
+            if d[pos] != 0xFF:
+                return None, None, "extraneous bytes between scans"
+            m = int(d[pos + 1])
+            if m == 0xD9:
+                break
+            ln = (int(d[pos + 2]) << 8) | int(d[pos + 3]) if pos + 4 <= n else 0
+            if ln < 2 or pos + 2 + ln > n:
+                return None, None, "the file ends between scans"
+            seg = d[pos + 4:pos + 2 + ln].tobytes()
+            pos += 2 + ln
+            if m == 0xC4:
+                _read_dht(seg, huff, name)
+            elif m == 0xDD:
+                ri = _read_dri(seg, name)
+            elif m != 0xDA and not (0xE0 <= m <= 0xEF or m == 0xFE):
+                return None, None, "marker 0x%02X between scans" % m
+        if m == 0xD9:
+            break
+    if (coded != 0).any():
+        return None, None, "incomplete progression (libjpeg would smooth the blocks)"
+    return scans, [t[2] for t in used], ""
+
+
 def pack(infos, datas, dst_offsets, alloc=lambda n: np.empty(n, np.uint8)):
-    """One ``cpb200_jpeg_decode_batch`` launch over the eligible ``infos`` with file bytes ``datas``: a buffer
-    ``[table (B x 464 B) | per image: Huffman tables | segments | file bytes]`` whose offsets are relative to its own
-    start, so the same device copy is both ``src`` and ``table``.  ``dst_offsets`` are the byte offsets of the decoded
-    images in ``dst``.  ``alloc(nbytes)`` returns the uint8 host buffer.  Returns ``(buffer, workspace_bytes)``."""
+    """One ``cpb200_jpeg_decode_batch`` launch over ``infos`` (each ``eligible`` or ``progressive``) with file bytes
+    ``datas``: a buffer ``[table (B x 480 B) | per image: Huffman tables | scans (progressive) | segments | file bytes]``
+    whose offsets are relative to its own start, so the same device copy is both ``src`` and ``table``.
+    ``dst_offsets`` are the byte offsets of the decoded images in ``dst``.  ``alloc(nbytes)`` returns the uint8 host
+    buffer.  Returns ``(buffer, workspace_bytes)``."""
     B = len(infos)
     table = np.zeros(B, JPEG_IMAGE)
     up = lambda x, a: x + (-x) % a
@@ -292,13 +450,30 @@ def pack(infos, datas, dst_offsets, alloc=lambda n: np.empty(n, np.uint8)):
     ws = 0
     place = []
     for n, (info, data) in enumerate(zip(infos, datas)):
-        keys = sorted({(0, t) for t in info.dc} | {(1, t) for t in info.ac})
         e = table[n]
         e["huff_offset"] = pos
-        pos += len(keys) * HUFF.itemsize
+        if info.progressive is None:
+            keys = sorted({(0, t) for t in info.dc} | {(1, t) for t in info.ac})
+            tables, segs = [info.huff[k][2] for k in keys], [info.segments]
+            for c in range(info.ncomp):
+                e["dc_tbl"][c] = keys.index((0, info.dc[c]))
+                e["ac_tbl"][c] = keys.index((1, info.ac[c]))
+            e["restart_interval"], e["nseg"] = info.restart_interval, len(info.segments)
+        else:
+            tables, segs = info.tables, [sc.segments for sc in info.progressive]
+        pos += len(tables) * HUFF.itemsize
+        scans = np.zeros(len(info.progressive or ()), SCAN)
+        e["scan_offset"], e["nscan"] = pos, len(scans)
+        pos += scans.nbytes
         e["seg_offset"] = pos
-        pos = up(pos + len(info.segments) * 16, 16)
-        place.append((keys, pos))
+        for sc, rec, sg in zip(info.progressive or (), scans, segs):
+            rec["seg_offset"], rec["nseg"], rec["restart_interval"] = pos, len(sg), sc.restart_interval
+            rec["ncomp"], rec["ss"], rec["se"], rec["ah"], rec["al"] = len(sc.comps), sc.ss, sc.se, sc.ah, sc.al
+            rec["comp"][:len(sc.comps)], rec["dc_tbl"][:len(sc.comps)], rec["ac_tbl"][:len(sc.comps)] = \
+                sc.comps, sc.dc, sc.ac
+            pos += len(sg) * 16
+        pos = up(e["seg_offset"] + sum(len(sg) for sg in segs) * 16, 16)
+        place.append((tables, scans, segs, pos))
         pos = up(pos + len(data), 16)
         e["coef_offset"] = ws
         nblk = sum(bw * bh for bw, bh in info.blocks())
@@ -306,22 +481,23 @@ def pack(infos, datas, dst_offsets, alloc=lambda n: np.empty(n, np.uint8)):
         ws += nblk * 192
         e["dst_offset"] = dst_offsets[n]
         e["h"], e["w"], e["ncomp"], e["hs"], e["vs"] = info.h, info.w, info.ncomp, info.hs, info.vs
-        e["orientation"], e["restart_interval"], e["nseg"] = info.orientation, info.restart_interval, len(info.segments)
+        e["orientation"] = info.orientation
         for c in range(info.ncomp):
-            e["dc_tbl"][c] = keys.index((0, info.dc[c]))
-            e["ac_tbl"][c] = keys.index((1, info.ac[c]))
             e["qt"][c] = info.qt[c]
     if pos >= 2 ** 62:
         raise ValueError("jpeg: launch buffer too large")
     buf = alloc(pos)
     hv = buf.numpy() if hasattr(buf, "numpy") else buf
     hv[:table.nbytes] = table.view(np.uint8)
-    for info, data, e, (keys, base) in zip(infos, datas, table, place):
+    for data, e, (tables, scans, segs, base) in zip(datas, table, place):
         h0 = int(e["huff_offset"])
-        for k, key in enumerate(keys):
-            hv[h0 + k * HUFF.itemsize:h0 + (k + 1) * HUFF.itemsize] = info.huff[key][2].reshape(1).view(np.uint8)
+        for k, t in enumerate(tables):
+            hv[h0 + k * HUFF.itemsize:h0 + (k + 1) * HUFF.itemsize] = t.reshape(1).view(np.uint8)
+        s0 = int(e["scan_offset"])
+        hv[s0:s0 + scans.nbytes] = scans.view(np.uint8)
+        # the parser's segment bounds are file offsets; the kernels read them as offsets into the buffer
         s0 = int(e["seg_offset"])
-        # the parser's segment bounds are file offsets; the kernel reads them as offsets into the buffer
-        hv[s0:s0 + len(info.segments) * 16] = (info.segments + base).astype("<i8").view(np.uint8).reshape(-1)
+        sg = np.concatenate(segs) + base
+        hv[s0:s0 + sg.nbytes] = sg.astype("<i8").view(np.uint8).reshape(-1)
         hv[base:base + len(data)] = np.frombuffer(data, np.uint8) if not isinstance(data, np.ndarray) else data
     return buf, ws

@@ -147,7 +147,23 @@ typedef struct cpb200_jpeg_huff {
   uint8_t val[256];
 } cpb200_jpeg_huff;
 
-/* One image of cpb200_jpeg_decode_batch (464 bytes, lives in caller-owned DEVICE memory).  Offsets are bytes. */
+/* One scan of a progressive image of cpb200_jpeg_decode_batch (40 bytes, 8-byte aligned in `src`). */
+typedef struct cpb200_jpeg_scan {
+  int64_t seg_offset;        /* in `src`: nseg x {int64 start, end}, the byte ranges of the scan's entropy-coded
+                                segments, 8-byte aligned */
+  int32_t nseg;              /* ceil(units / restart_interval), or 1 */
+  int32_t restart_interval;  /* units per segment, 0: one segment.  A unit is an MCU when the scan has several
+                                components, else one block of that component's own grid, ceil(ceil(w * h_c / hs) / 8)
+                                x ceil(ceil(h * v_c / vs) / 8) (T.81 A.2.2) */
+  int32_t ncomp;             /* components in the scan, 1..3 (1 for an AC scan) */
+  uint8_t comp[4];           /* their indices 0..2, increasing */
+  uint8_t dc_tbl[4], ac_tbl[4];  /* per scan component: index of its DC table (first DC scan) or AC table (AC scan)
+                                    at the image's huff_offset */
+  uint8_t ss, se, ah, al;    /* spectral selection and successive approximation, legal under T.81 G.1.1.1 */
+  int32_t pad;
+} cpb200_jpeg_scan;
+
+/* One image of cpb200_jpeg_decode_batch (480 bytes, lives in caller-owned DEVICE memory).  Offsets are bytes. */
 typedef struct cpb200_jpeg_image {
   int64_t seg_offset;        /* in `src`: nseg x {int64 start, end}, the byte ranges in `src` of the entropy-coded
                                 segments (restart intervals; the whole scan without DRI), 8-byte aligned */
@@ -163,18 +179,26 @@ typedef struct cpb200_jpeg_image {
   int32_t nseg;              /* ceil(MCUs / restart_interval), or 1 */
   uint8_t dc_tbl[4], ac_tbl[4];  /* per component: index of its DC / AC table at huff_offset */
   uint16_t qt[3][64];        /* per component: quantisation table in natural (row-major) order */
+  int64_t scan_offset;       /* progressive images: in `src`, nscan cpb200_jpeg_scan, 8-byte aligned */
+  int32_t nscan;             /* 0: sequential, every field above as described.  > 0: progressive, decoded scan by
+                                scan; seg_offset, restart_interval, nseg, dc_tbl and ac_tbl are unused, the scans
+                                carry them */
+  int32_t pad;
 } cpb200_jpeg_image;
 
-/* cv2.imread(path, IMREAD_COLOR) of sequential-Huffman JPEG files, byte for byte (libjpeg-turbo's ISLOW IDCT, fancy
- * upsampling and integer YCbCr->BGR, then OpenCV's EXIF orientation; verified against cv2 4.13 with libjpeg-turbo
- * 3.1).  B files in one launch: `src` holds the file bytes and the Huffman tables and segment lists the table points
- * to, `table` is a DEVICE array of B cpb200_jpeg_image that the caller has checked (the kernels trust it; see
- * centerpose_b200/jpeg.py), `workspace` holds every image's coefficients and planes (an image whose workspace would
- * end past `workspace_bytes` is not decoded and gets status 2).  Each image's segments are decoded by one thread
- * each, then IDCT, upsampling and colour conversion run over the whole launch.  status[b] (DEVICE int array) is 0 when
- * image b decoded, non-zero when its entropy data was bad (a code longer than 16 bits, a run past coefficient 63 or
- * data ending before a segment's last MCU); the image's pixels are then undefined, other images are unaffected.
- * 1 <= B <= 65535. */
+/* cv2.imread(path, IMREAD_COLOR) of sequential- and progressive-Huffman JPEG files, byte for byte (libjpeg-turbo's
+ * ISLOW IDCT, fancy upsampling and integer YCbCr->BGR, then OpenCV's EXIF orientation; verified against cv2 4.13 with
+ * libjpeg-turbo 3.1).  B files in one launch, either kind mixed: `src` holds the file bytes and the Huffman tables,
+ * scans and segment lists the table points to, `table` is a DEVICE array of B cpb200_jpeg_image that the caller has
+ * checked (the kernels trust it; see centerpose_b200/jpeg.py), `workspace` holds every image's coefficients and
+ * planes (an image whose workspace would end past `workspace_bytes` is not decoded and gets status 2).  A sequential
+ * image's segments are decoded by one thread each.  A progressive image is decoded by one CTA that zeroes its
+ * coefficients and runs its scans in file order, one thread per segment of a scan; its progression must be complete
+ * (every coefficient coded down to bit 0), since libjpeg smooths blocks otherwise.  IDCT, upsampling and colour
+ * conversion then run over the whole launch.  status[b] (DEVICE int array) is 0 when image b decoded, non-zero when
+ * its entropy data was bad (a code longer than 16 bits, a run past the scan's last coefficient, a refinement symbol
+ * of size other than 0 or 1, or data ending before a segment's last unit); the image's pixels are then undefined,
+ * other images are unaffected.  1 <= B <= 65535. */
 int cpb200_jpeg_decode_batch(const unsigned char *src, const cpb200_jpeg_image *table, int B, void *workspace,
                              size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
 

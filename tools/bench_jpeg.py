@@ -1,11 +1,11 @@
 """Device JPEG decode throughput on one GPU: ``cpb200_jpeg_decode_batch`` against ``cv2.imdecode``, and
 ``run_images`` from JPEG files with the device decode against the host ``cv2.imread`` (``DEVICE_PREPROCESS: false``).
 
-    python tools/bench_jpeg.py [--images 256] [--rounds 3] [--out DIR] [--precision fp16x2]
+    python tools/bench_jpeg.py [--images 256] [--rounds 3] [--out DIR] [--precision fp16x2] [--progressive]
 
 The files are seeded gradients with noise (``tests/test_jpeg_cpu.make_image``) at COCO-like sizes, 640x480, 480x640
-and 640x427 in turn, encoded 4:2:0 at qualities 75 and 95 in turn by ``cv2.imencode``, and written to ``--out``
-(a temporary directory by default).
+and 640x427 in turn, encoded 4:2:0 at qualities 75 and 95 in turn by ``cv2.imencode`` (with ``--progressive``, as
+progressive files, ``IMWRITE_JPEG_PROGRESSIVE``), and written to ``--out`` (a temporary directory by default).
 
 1. Decode alone.  Device: the kernels of one ``cpb200_jpeg_decode_batch`` over all images (CUDA events, median of
    ``--rounds`` launches, after a warm-up launch), and separately the host's parse + pack of the launch buffer.  Host:
@@ -48,6 +48,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", default=None, help="directory for the JPEG files (default: a temporary one)")
     ap.add_argument("--precision", default="fp16x2")
+    ap.add_argument("--progressive", action="store_true", help="write progressive files")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise RuntimeError("tools/bench_jpeg.py needs a CUDA device (there is no CPU path to time)")
@@ -58,7 +59,8 @@ def main():
     datas, paths = [], []
     for i in range(args.images):
         h, w = SIZES[i % len(SIZES)]
-        data = encode(make_image(h, w, "smooth_noise", 1000 + i), 75 if i % 2 == 0 else 95, "420")
+        data = encode(make_image(h, w, "smooth_noise", 1000 + i), 75 if i % 2 == 0 else 95, "420",
+                      progressive=args.progressive)
         p = os.path.join(out, "img%04d.jpg" % i)
         with open(p, "wb") as f:
             f.write(data)
@@ -70,6 +72,8 @@ def main():
     # 1. decode alone
     t0 = time.perf_counter()
     infos = [jpeg.parse(d, p) for d, p in zip(datas, paths)]
+    if not all(i.eligible or i.progressive for i in infos):
+        raise RuntimeError("tools/bench_jpeg.py: the device decoder does not take every file")
     sizes = [i.oh * i.ow * 3 for i in infos]
     offs = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
     buf, ws_bytes = jpeg.pack(infos, datas, offs[:-1])
@@ -131,6 +135,7 @@ def main():
     result = {
         "metric": "JPEG decode images/s (device kernels vs cv2.imdecode) and run_images images/s from files",
         "images": n, "sizes_hw": SIZES, "sampling": "4:2:0", "qualities": [75, 95], "compressed_mb": round(mb, 3),
+        "progressive": args.progressive,
         "device_status_ok": int((status.cpu().numpy() == 0).sum()), "device_exact_images": int(exact),
         "device_decode_images_per_s": [n / t for t in t_dev],
         "device_decode_mb_per_s": [mb / t for t in t_dev],
