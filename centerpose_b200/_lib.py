@@ -28,6 +28,10 @@ def lib() -> ctypes.CDLL:
     L.cpb200_version.restype = ctypes.c_int
     L.cpb200_last_error.restype = ctypes.c_char_p
     L.cpb200_launch_count.restype = ctypes.c_ulonglong
+    L.cpb200_route_log_start.restype = None
+    L.cpb200_route_log_start.argtypes = []
+    L.cpb200_route_log_read.restype = ctypes.c_int
+    L.cpb200_route_log_read.argtypes = [ctypes.c_char_p, ctypes.c_size_t]
     L.cpb200_decode_workspace_bytes.restype = ctypes.c_size_t
     L.cpb200_decode_workspace_bytes.argtypes = [ctypes.c_int] * 3
     L.cpb200_multi_pose_decode.restype = ctypes.c_int

@@ -29,6 +29,16 @@ inline int check_launch(const char *what) {
   return CPB200_OK;
 }
 
+// Route log (cpb200_route_log_start / _read): network-op launch sites pass their kernel, which is recorded while the
+// log is on.  Off, the cost is one relaxed atomic load per launch.
+void note_launch(const void *kernel);
+
+template <typename K>
+inline int check_launch(const char *what, K *kernel) {
+  note_launch(reinterpret_cast<const void *>(kernel));
+  return check_launch(what);
+}
+
 #define CPB_CUDA(call)                                                                 \
   do {                                                                                 \
     cudaError_t e_ = (call);                                                           \

@@ -289,7 +289,7 @@ int launch_hd(const HdOp &t, const HdArgs &args, cudaStream_t st) {
   static SmemAttrCache cache;
   if (int rc = ensure_smem(heads_tc_kernel<P>, t.smem, cache)) return rc;
   heads_tc_kernel<P><<<t.grid, HD_THREADS, t.smem, st>>>(args);
-  return cpb::check_launch("heads_tc_kernel");
+  return cpb::check_launch("heads_tc_kernel", heads_tc_kernel<P>);
 }
 
 }  // namespace

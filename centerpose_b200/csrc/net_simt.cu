@@ -824,11 +824,12 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
       const long long n = (long long)op.B * op.H * op.W * op.cin[0];
       if (n % 4) return cpb::fail(CPB200_ERR_ARG, "convert: element count must be a multiple of 4");
       const unsigned grid = (unsigned)std::min<long long>((n / 4 + 255) / 256, 132LL * 16);
-      if (op.flags & CPB200_FLAG_TO_F32)
+      if (op.flags & CPB200_FLAG_TO_F32) {
         convert_from_split_kernel<<<grid, 256, 0, st>>>(static_cast<const uint16_t *>(op.src[0]), static_cast<float *>(op.dst), n / 4, (size_t)n, fmt);
-      else
-        convert_to_split_kernel<<<grid, 256, 0, st>>>(static_cast<const float *>(op.src[0]), static_cast<uint16_t *>(op.dst), n / 4, (size_t)n, fmt);
-      return cpb::check_launch("convert_split_kernel");
+        return cpb::check_launch("convert_split_kernel", convert_from_split_kernel);
+      }
+      convert_to_split_kernel<<<grid, 256, 0, st>>>(static_cast<const float *>(op.src[0]), static_cast<uint16_t *>(op.dst), n / 4, (size_t)n, fmt);
+      return cpb::check_launch("convert_split_kernel", convert_to_split_kernel);
     }
     case CPB200_OP_S2D: {
       if (op.cin[0] != 3 || op.cout != 16 || (op.H & 1) || (op.W & 1) || op.Ho != op.H / 2 || op.Wo != op.W / 2)
@@ -837,7 +838,7 @@ int run_op_split(const cpb200_op &op, cudaStream_t st) {
       const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 132LL * 16);
       s2d_split_kernel<<<grid, 256, 0, st>>>(static_cast<const float *>(op.src[0]), static_cast<uint16_t *>(op.dst), op.B, op.H, op.W,
                                              (size_t)total * 16, fmt);
-      return cpb::check_launch("s2d_split_kernel");
+      return cpb::check_launch("s2d_split_kernel", s2d_split_kernel);
     }
     default:
       return cpb::fail(CPB200_ERR_ARG, "op type %d has no split-precision kernel (the host must route it through fp32)", op.type);
@@ -867,14 +868,16 @@ int launch_conv(const cpb200_op &op, cudaStream_t st) {
   if (op.cout <= 16) {
     dim3 grid((unsigned)((M + 255) / 256), (op.cout + 15) / 16);
     conv_simt_kernel<T, 256, 16, DCN><<<grid, 256, 0, st>>>(a);
+    return cpb::check_launch("conv_simt_kernel", conv_simt_kernel<T, 256, 16, DCN>);
   } else if (op.cout <= 32) {
     dim3 grid((unsigned)((M + 127) / 128), (op.cout + 31) / 32);
     conv_simt_kernel<T, 128, 32, DCN><<<grid, 256, 0, st>>>(a);
+    return cpb::check_launch("conv_simt_kernel", conv_simt_kernel<T, 128, 32, DCN>);
   } else {
     dim3 grid((unsigned)((M + 63) / 64), (op.cout + 63) / 64);
     conv_simt_kernel<T, 64, 64, DCN><<<grid, 256, 0, st>>>(a);
+    return cpb::check_launch("conv_simt_kernel", conv_simt_kernel<T, 64, 64, DCN>);
   }
-  return cpb::check_launch("conv_simt_kernel");
 }
 
 template <typename T>
@@ -898,6 +901,7 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
     stem_kernel<T, CO, PX, ST, KW><<<(unsigned)((M + 127) / 128), 128, smem, st>>>(                           \
         static_cast<const float *>(op.src[0]), static_cast<T *>(op.dst), static_cast<const float *>(op.weight), \
         op.bias, op.B, cin, op.H, op.W, op.Ho, op.Wo, op.kh, op.pad_h, op.pad_w, act);                      \
+    return cpb::check_launch("stem_kernel", stem_kernel<T, CO, PX, ST, KW>);                                  \
   }
       if (op.kw == 3) {                               // HRNet conv1 (pose_higher_hrnet.py:243-244)
         if (op.cout == 64 && op.stride == 2) STEM_LAUNCH_K(64, 1, 2, 3)
@@ -911,7 +915,6 @@ int run_op_simt(const cpb200_op &op, cudaStream_t st) {
       else return cpb::fail(CPB200_ERR_ARG, "stem: cout %d / stride %d unsupported", op.cout, op.stride);
 #undef STEM_LAUNCH
 #undef STEM_LAUNCH_K
-      return cpb::check_launch("stem_kernel");
     }
     default: return cpb::fail(CPB200_ERR_ARG, "unknown op type %d", op.type);
   }
@@ -961,7 +964,7 @@ int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
       if (C % 4) return cpb::fail(CPB200_ERR_ARG, "maxpool: C %% 4 != 0");
       maxpool_kernel<PI, PO><<<grid((long long)op.B * op.Ho * op.Wo * (C / 4), 32), 256, 0, st>>>(x, y, op.B, op.H, op.W, C,
           op.Ho, op.Wo, op.kh, op.stride, op.pad_h);
-      return cpb::check_launch("maxpool_kernel");
+      return cpb::check_launch("maxpool_kernel", maxpool_kernel<PI, PO>);
     }
     case CPB200_OP_DWDECONV_ADD: {
       if (C % VEC || op.stride < 1) return cpb::fail(CPB200_ERR_ARG, "dwdeconv: needs C %% %d == 0 and stride >= 1", VEC);
@@ -971,11 +974,11 @@ int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
       if (lf >= 0 && lcv >= 0 && op.kh == 2 * op.stride && CV <= 256 && (256 / CV) % op.stride == 0) {
         dwdeconv_add_fast_kernel<VEC_FAST, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.H, op.W, C, op.Ho,
             op.Wo, op.kh, op.stride, op.pad_h, lf, lcv);
-        return cpb::check_launch("dwdeconv_add_fast_kernel");
+        return cpb::check_launch("dwdeconv_add_fast_kernel", dwdeconv_add_fast_kernel<VEC_FAST, PI, PO>);
       }
       dwdeconv_add_kernel<VEC, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.H, op.W, C, op.Ho, op.Wo,
           op.kh, op.stride, op.pad_h, lf, ilog2(C / VEC));
-      return cpb::check_launch("dwdeconv_add_kernel");
+      return cpb::check_launch("dwdeconv_add_kernel", dwdeconv_add_kernel<VEC, PI, PO>);
     }
     case CPB200_OP_DWCONV: {
       if (C % VEC || op.kh != op.kw || op.cout != C) return cpb::fail(CPB200_ERR_ARG, "dwconv: C %% %d != 0 or non-square kernel", VEC);
@@ -984,27 +987,27 @@ int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
     const long long tot = (long long)op.B * op.Ho * ((op.Wo + PX - 1) / PX) * (C / VEC);                         \
     dwconv_tiled_kernel<VEC, KK, SS, PX, PI, PO><<<grid(tot, 32), 256, 0, st>>>(x, y, w, op.bias, tot, op.H, op.W, C, \
         op.Ho, op.Wo, act);                                                                                     \
-    return cpb::check_launch("dwconv_tiled_kernel");                                                            \
+    return cpb::check_launch("dwconv_tiled_kernel", dwconv_tiled_kernel<VEC, KK, SS, PX, PI, PO>);              \
   }
       DW_TILED(3, 1, 4) DW_TILED(5, 1, 4) DW_TILED(3, 2, 2) DW_TILED(5, 2, 2)
 #undef DW_TILED
       const long long total = (long long)op.B * op.Ho * op.Wo * (C / VEC);
       dwconv_kernel<VEC, PI, PO><<<grid(total, 32), 256, 0, st>>>(x, y, w, op.bias, total, op.H, op.W, C, op.Ho, op.Wo, op.kh,
           op.stride, op.pad_h, act);
-      return cpb::check_launch("dwconv_kernel");
+      return cpb::check_launch("dwconv_kernel", dwconv_kernel<VEC, PI, PO>);
     }
     case CPB200_OP_AVGPOOL: {
       if (C % 4 || op.Ho != 1 || op.Wo != 1) return cpb::fail(CPB200_ERR_ARG, "avgpool: C %% 4 != 0 or output not 1x1");
       avgpool_kernel<PI, T *><<<dim3((unsigned)op.B, (unsigned)((C + 63) / 64)), 256, 0, st>>>(x, static_cast<T *>(op.dst),
           op.H * op.W, C);
-      return cpb::check_launch("avgpool_kernel");
+      return cpb::check_launch("avgpool_kernel", avgpool_kernel<PI, T *>);
     }
     case CPB200_OP_SCALE_ADD: {                         // the output and the skip have the input's shape
       if (C % 4 || !op.res) return cpb::fail(CPB200_ERR_ARG, "scale_add: C %% 4 != 0 or missing scale vector");
       const long long per_image = (long long)op.H * op.W * (C / 4), total = per_image * op.B;
       scale_add_kernel<PI, const T *, PO><<<grid(total, 16), 256, 0, st>>>(x, static_cast<const T *>(op.res),
           io_handle<PI>(op.aux, n_in, fmt), io_handle<PO>(op.dst, n_in, fmt), total, per_image, C / 4);
-      return cpb::check_launch("scale_add_kernel");
+      return cpb::check_launch("scale_add_kernel", scale_add_kernel<PI, const T *, PO>);
     }
     case CPB200_OP_UPSAMPLE_ADD: {
       const int sh = ilog2(op.stride);
@@ -1012,7 +1015,7 @@ int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
         return cpb::fail(CPB200_ERR_ARG, "upsample_add: factor %d must be a power of two, C %% 4 == 0", op.stride);
       const long long total = (long long)op.B * op.Ho * op.Wo * (C / 4);
       upsample_add_kernel<PI, PO><<<grid(total, 16), 256, 0, st>>>(x, skip, y, total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, act);
-      return cpb::check_launch("upsample_add_kernel");
+      return cpb::check_launch("upsample_add_kernel", upsample_add_kernel<PI, PO>);
     }
     default: {                                          // CPB200_OP_AVGPOOL2, CPB200_OP_RESIZE_BILINEAR
       const bool pool = op.type == CPB200_OP_AVGPOOL2;
@@ -1025,13 +1028,13 @@ int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
           return cpb::fail(CPB200_ERR_ARG, "avgpool2: %dx%d -> %dx%d is not a 2x2 / stride-2 floor-mode pool (needs H, W >= 2)",
                            op.H, op.W, op.Ho, op.Wo);
         avgpool2_kernel<PI, PO><<<grid(total, 16), 256, 0, st>>>(x, y, total, op.H, op.W, C / 4, op.Ho, op.Wo);
-        return cpb::check_launch("avgpool2_kernel");
+        return cpb::check_launch("avgpool2_kernel", avgpool2_kernel<PI, PO>);
       }
       if (op.Ho < 1 || op.Wo < 1) return cpb::fail(CPB200_ERR_ARG, "resize_bilinear: output size %dx%d", op.Ho, op.Wo);
       const float sh = op.Ho > 1 ? (float)(op.H - 1) / (float)(op.Ho - 1) : 0.f;
       const float sw = op.Wo > 1 ? (float)(op.W - 1) / (float)(op.Wo - 1) : 0.f;
       resize_bilinear_kernel<PI, PO><<<grid(total, 16), 256, 0, st>>>(x, y, total, op.H, op.W, C / 4, op.Ho, op.Wo, sh, sw);
-      return cpb::check_launch("resize_bilinear_kernel");
+      return cpb::check_launch("resize_bilinear_kernel", resize_bilinear_kernel<PI, PO>);
     }
   }
 }

@@ -382,7 +382,7 @@ int launch_stem_h(const cpb200_op &op, cudaStream_t st) {
   const int sms = tc::num_sms();
   const int grid = a.total_tiles < sms ? a.total_tiles : sms;
   stem_tc_h_kernel<N, P><<<grid, H_THREADS, smem, st>>>(a);
-  return cpb::check_launch("stem_tc_h_kernel");
+  return cpb::check_launch("stem_tc_h_kernel", stem_tc_h_kernel<N, P>);
 }
 
 template <int N, int S>
@@ -402,7 +402,7 @@ int launch_stem(const cpb200_op &op, cudaStream_t st) {
   const int sms = tc::num_sms();
   const int grid = a.total_tiles < sms ? a.total_tiles : sms;
   stem_tc_kernel<N, S><<<grid, ST_THREADS, smem, st>>>(a);
-  return cpb::check_launch("stem_tc_kernel");
+  return cpb::check_launch("stem_tc_kernel", stem_tc_kernel<N, S>);
 }
 
 }  // namespace

@@ -446,7 +446,7 @@ int launch_tc(const TcOp &t, const TcArgs &args, cudaStream_t st) {
   static SmemAttrCache cache;
   if (int rc = ensure_smem(conv_tc_kernel<BN, DCN, P>, t.smem, cache)) return rc;
   conv_tc_kernel<BN, DCN, P><<<t.grid, DCN ? DCN_THREADS : TC_THREADS, t.smem, st>>>(args);
-  return cpb::check_launch(DCN ? "dcn_tc_kernel" : "conv_tc_kernel");
+  return cpb::check_launch(DCN ? "dcn_tc_kernel" : "conv_tc_kernel", conv_tc_kernel<BN, DCN, P>);
 }
 
 }  // namespace

@@ -248,7 +248,7 @@ int launch_c3(const C3Op &t, const C3Args &args, cudaStream_t st) {
   static SmemAttrCache cache;
   if (int rc = ensure_smem(conv3x3_tc_kernel<BN, P>, t.smem, cache)) return rc;
   conv3x3_tc_kernel<BN, P><<<t.grid, C3_THREADS, t.smem, st>>>(args);
-  return cpb::check_launch("conv3x3_tc_kernel");
+  return cpb::check_launch("conv3x3_tc_kernel", conv3x3_tc_kernel<BN, P>);
 }
 
 }  // namespace

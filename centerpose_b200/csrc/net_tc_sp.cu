@@ -253,7 +253,7 @@ int launch_sp(const cpb200_op &op, cudaStream_t st) {
   const int sms = tc::num_sms();
   const int grid = a.total_tiles < sms ? a.total_tiles : sms;
   conv_sp_kernel<C, N, S, P><<<grid, SP_THREADS, smem, st>>>(a);
-  return cpb::check_launch("conv_sp_kernel");
+  return cpb::check_launch("conv_sp_kernel", conv_sp_kernel<C, N, S, P>);
 }
 
 template <int C, int S>

@@ -38,6 +38,12 @@ int cpb200_version(void);
 const char *cpb200_last_error(void);
 /* Number of kernels this library has launched since load (used by bench.py "gpu_launches"). */
 unsigned long long cpb200_launch_count(void);
+/* Route log (diagnostics and tests): cpb200_route_log_start() clears the log and records every kernel the network-op
+ * entry points (cpb200_run_ops) launch from then on; cpb200_route_log_read() stops recording and writes the demangled
+ * kernel names into buf, one per line in launch order.  Returns the number of launches, or -1 (cpb200_last_error())
+ * when buf is too small or a name cannot be read.  Recording is process-wide. */
+void cpb200_route_log_start(void);
+int cpb200_route_log_read(char *buf, size_t n);
 
 /* ------------------------------------------------------------------------------------
  * Fused decode.  Replaces lib/models/decode.py:235-308 `multi_pose_decode` together with

@@ -177,8 +177,10 @@ def _act(y, act=None, relu=False):
 
 
 def _ref_conv(a):
-    assert a["pad_hw"] is None and a["out_map"] is None, "strided-output convs are replayed through deconv_k4s2"
-    y = F.conv2d(torch.cat(a["srcs"], 1), a["w"], a["b"], stride=a["stride"], padding=a["pad"])
+    assert a["out_map"] is None, "strided-output convs are replayed through deconv_k4s2"
+    # pad_hw = (top, left) of a conv without out_map pads bottom / right alike (PlanBuilder.conv's Ho / Wo)
+    y = F.conv2d(torch.cat(a["srcs"], 1), a["w"], a["b"], stride=a["stride"],
+                 padding=tuple(a["pad_hw"]) if a["pad_hw"] is not None else a["pad"])
     if a["res"] is not None:
         y = y + a["res"]
     return _act(y, a["act"], a["relu"])
