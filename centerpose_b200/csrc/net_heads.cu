@@ -19,6 +19,7 @@
 // accumulators, 48 head accumulators and the 64 fragment registers of the chunk, so the producers give their registers
 // away (setmaxnreg).
 #include "tc_common.cuh"
+#include <memory>
 
 using namespace tc;
 
@@ -66,12 +67,10 @@ __device__ __forceinline__ void heads_1x1(float (&out)[HD_MAXN / 2], float (&out
     const uint32_t first = (first_chunk && kk == 0) ? 0u : 1u;
     const uint32_t fh[4] = {ahi[4 * kk], ahi[4 * kk + 1], ahi[4 * kk + 2], ahi[4 * kk + 3]};
     if constexpr (P == 1) {
-      wgmma_rs_k16<N>(out, fh, bh, first, 1u);
+      mma_step_rs<N, 1>(out, out2, fh, fh, bh, bl, first, bf);
     } else {
       const uint32_t fl[4] = {alo[4 * kk], alo[4 * kk + 1], alo[4 * kk + 2], alo[4 * kk + 3]};
-      wgmma_rs_k16<N>(out, fh, bh, first, bf);
-      wgmma_rs_k16<N>(out2, fh, bl, first, bf);
-      wgmma_rs_k16<N>(out2, fl, bh, 1u, bf);
+      mma_step_rs<N, 2>(out, out2, fh, fl, bh, bl, first, bf);
     }
   }
 }
@@ -178,15 +177,9 @@ __global__ void __launch_bounds__(HD_THREADS, 1) heads_tc_kernel(const __grid_co
       const uint32_t hbuf = a_lo14 + (uint32_t)hs * hbufstep;
       for (int h = 0; h < a.nheads; ++h) {
         const int npad = a.npad[h];
-#pragma unroll
-        for (int i = 0; i < HD_MAXN / 2; ++i) out[i] = 0.f;
-#pragma unroll
-        for (int i = 0; i < (P == 2 ? HD_MAXN / 2 : 1); ++i) out2[i] = 0.f;
+        acc_zero(out, out2);
         for (int c = 0; c < a.chunks; ++c) {
-#pragma unroll
-          for (int i = 0; i < HD_CHUNK / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-          for (int i = 0; i < (P == 2 ? HD_CHUNK / 2 : 1); ++i) acc2[i] = 0.f;
+          acc_zero(acc, acc2);
           // ---- 3x3 GEMM of hidden channels [c * 128, c * 128 + 128) ----
           uint32_t accf = 0u;
           int prev = -1;
@@ -199,16 +192,8 @@ __global__ void __launch_bounds__(HD_THREADS, 1) heads_tc_kernel(const __grid_co
               const uint64_t bd = dB + (w_lo14 + (uint32_t)sb * wstep);
               const uint64_t adh = ah0 + toff, adl = al0 + toff;
               wg_fence();
-              for (int k = 0; k < ksteps; ++k) {
-                const uint32_t first = k == 0 ? accf : 1u;
-                if constexpr (P == 1) {
-                  wgmma_k16<HD_CHUNK>(acc, adh + 2 * k, bd + 2 * k, first, 1u);
-                } else {
-                  wgmma_k16<HD_CHUNK>(acc, adh + 2 * k, bd + 2 * k, first, bf);
-                  wgmma_k16<HD_CHUNK>(acc2, adh + 2 * k, bd + wtile + 2 * k, first, bf);
-                  wgmma_k16<HD_CHUNK>(acc2, adl + 2 * k, bd + 2 * k, 1u, bf);
-                }
-              }
+              for (int k = 0; k < ksteps; ++k)
+                mma_step<HD_CHUNK, P>(acc, acc2, adh, adl, bd, bd + wtile, k, k == 0 ? accf : 1u, bf);
               accf = 1u;
               wg_commit();
               wg_wait<1>();
@@ -220,7 +205,7 @@ __global__ void __launch_bounds__(HD_THREADS, 1) heads_tc_kernel(const __grid_co
           wg_wait<0>();
           if (lane == 0) mbar_arrive(wempty0 + 8 * prev);
           acc_fence(acc); acc_fence(acc2);
-          // ---- chunk epilogue: what conv3x3_tc_kernel's store_pair16 stores, kept as 1x1 A fragments ----
+          // ---- chunk epilogue: what conv3x3_tc_kernel's epilogue_pair stores, kept as 1x1 A fragments ----
           uint32_t ahi[32], alo[P == 2 ? 32 : 1];
           const float *b3 = a.bias3 + h * a.hid + c * HD_CHUNK;
           const float s3 = a.scale3[h];
@@ -251,25 +236,21 @@ __global__ void __launch_bounds__(HD_THREADS, 1) heads_tc_kernel(const __grid_co
           if (++sb == a.nb) { sb = 0; phb ^= 1; }
         }
         acc_fence(out); acc_fence(out2);
-        // ---- head epilogue: NCHW fp32 (conv_tc_kernel's out_nchw branch) ----
+        // ---- head epilogue: NCHW fp32, as conv_tc_kernel stores it ----
         const int cout = a.cout[h];
         const float *b1p = a.bias1[h];
         const float s1 = a.scale1[h];
         float *dst = a.dst[h];
-        const size_t plane = (size_t)a.Ho * a.Wo;
+        const long long plane = (long long)a.Ho * a.Wo;
 #pragma unroll
         for (int j = 0; j < HD_MAXN / 4; ++j) {
           const int row = wg * 64 + frag_row(t, j), nb = frag_col(t, j);
           const int ho = h0 + (row >> 3), wo = w0 + (row & 7);
           if (4 * j >= npad || ho >= a.Ho || wo >= a.Wo || nb >= cout) continue;
-          float v0 = out[2 * j], v1 = out[2 * j + 1];
-          if constexpr (P == 2) { v0 += out2[2 * j]; v1 += out2[2 * j + 1]; }
           const bool has1 = nb + 1 < cout;
           const float b0 = __ldg(b1p + nb), b1 = has1 ? __ldg(b1p + nb + 1) : 0.f;
-          const float f0 = P == 2 ? fmaf(v0, s1, b0) : v0 + b0, f1 = P == 2 ? fmaf(v1, s1, b1) : v1 + b1;
-          float *o = dst + (((size_t)n * cout + nb) * a.Ho + ho) * a.Wo + wo;
-          o[0] = P == 2 ? cpb::act_fn(f0, 0u) : cpb::act_out<__nv_bfloat16>(f0, 0u);
-          if (has1) o[plane] = P == 2 ? cpb::act_fn(f1, 0u) : cpb::act_out<__nv_bfloat16>(f1, 0u);
+          epilogue_pair<P>(out, out2, j, b0, b1, s1, 0u, OUT_NCHW, dst, nullptr, (((size_t)n * cout + nb) * a.Ho + ho) * a.Wo + wo,
+                           plane, has1, a.fmt);
         }
       }
       if (lane == 0) mbar_arrive(hempty0 + 8 * hs);
@@ -278,30 +259,22 @@ __global__ void __launch_bounds__(HD_THREADS, 1) heads_tc_kernel(const __grid_co
   }
 }
 
-struct HdOp {
+struct HdOp : cpb::Prepared {
+  HdOp() : Prepared(cpb::Route::HEADS) {}
   HdArgs args;
-  int P, grid;
+  int P;
   size_t smem;
 };
-
-template <int P>
-int launch_hd(const HdOp &t, const HdArgs &args, cudaStream_t st) {
-  static SmemAttrCache cache;
-  if (int rc = ensure_smem(heads_tc_kernel<P>, t.smem, cache)) return rc;
-  heads_tc_kernel<P><<<t.grid, HD_THREADS, t.smem, st>>>(args);
-  return cpb::check_launch("heads_tc_kernel", heads_tc_kernel<P>);
-}
 
 }  // namespace
 
 namespace cpb {
 
-int heads_prepare(cpb200_op &op) {
+int heads_prepare(const cpb200_op &op, Prepared **out) {
   const cpb200_head *hd = static_cast<const cpb200_head *>(op.aux);
   const int nheads = op.aux_pitch;
   if (!hd || nheads < 1 || nheads > HD_MAX) return fail(CPB200_ERR_ARG, "heads: 1..%d head entries required", HD_MAX);
-  if (op.act_dtype != CPB200_BF16 && op.act_dtype != CPB200_BF16X2 && op.act_dtype != CPB200_F16X2)
-    return fail(CPB200_ERR_ARG, "heads: bf16 or split (bf16x2 / fp16x2) activations required");
+  if (!tc_dtype(op.act_dtype)) return fail(CPB200_ERR_ARG, "heads: bf16 or split (bf16x2 / fp16x2) activations required");
   if (op.nsrc != 1 || op.cin[0] % 16 || op.cin[0] > 64 || (op.src_pitch[0] != 0 && op.src_pitch[0] != op.cin[0]))
     return fail(CPB200_ERR_ARG, "heads: one dense input with C %% 16 == 0 and C <= 64 required");
   if (op.kh != 3 || op.kw != 3 || op.stride != 1 || op.pad_h != 1 || op.pad_w != 1 || op.H != op.Ho || op.W != op.Wo ||
@@ -309,44 +282,34 @@ int heads_prepare(cpb200_op &op) {
     return fail(CPB200_ERR_ARG, "heads: 3x3 / stride 1 / pad 1 over maps of at least 8 x 8 required");
   const int hid = hd[0].hidden;
   if (hid <= 0 || hid % HD_CHUNK) return fail(CPB200_ERR_ARG, "heads: hidden width %d is not a multiple of %d", hid, HD_CHUNK);
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(CPB200_ERR_STATE, "heads: cuTensorMapEncodeTiled unavailable");
-  HdOp *t = new HdOp();
+  std::unique_ptr<HdOp> t(new HdOp());
   HdArgs &a = t->args;
   memset(&a, 0, sizeof(a));
-  const int P = op.act_dtype == CPB200_BF16 ? 1 : 2;
+  const Prec pr = prec_of(op);
+  const int P = pr.P;
   t->P = P;
-  a.fmt = op.act_dtype == CPB200_F16X2 ? 1u : 0u;
-  const CUtensorMapDataType dt = a.fmt ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  const cuuint32_t es[4] = {1, 1, 1, 1};
+  a.fmt = pr.fmt;
   a.nheads = nheads; a.hid = hid; a.chunks = hid / HD_CHUNK;
   int npad_max = 16;
   for (int h = 0; h < nheads; ++h) {
-    if (hd[h].hidden != hid || hd[h].cout < 1 || hd[h].cout > HD_MAXN || !hd[h].weight || !hd[h].bias) {
-      delete t; return fail(CPB200_ERR_ARG, "heads: entry %d: same hidden width, 1..%d channels, weight and bias required", h, HD_MAXN);
-    }
+    if (hd[h].hidden != hid || hd[h].cout < 1 || hd[h].cout > HD_MAXN || !hd[h].weight || !hd[h].bias)
+      return fail(CPB200_ERR_ARG, "heads: entry %d: same hidden width, 1..%d channels, weight and bias required", h, HD_MAXN);
     a.cout[h] = hd[h].cout; a.npad[h] = (hd[h].cout + 15) / 16 * 16;
     if (a.npad[h] > npad_max) npad_max = a.npad[h];
-    a.bias1[h] = hd[h].bias;
     a.scale3[h] = hd[h].acc_scale3 != 0.f ? hd[h].acc_scale3 : 1.f;
     a.scale1[h] = hd[h].acc_scale1 != 0.f ? hd[h].acc_scale1 : 1.f;
-    // 1x1 weights as packed for a 1x1 conv (plan.py::_pack_conv_tc, K slab 64): [plane][hid / 64][npad][64]
-    const cuuint64_t dims[3] = {64, (cuuint64_t)a.npad[h], (cuuint64_t)(hid / 64) * P};
-    const cuuint64_t strides[2] = {128, (cuuint64_t)a.npad[h] * 128};
-    const cuuint32_t box[3] = {64, (cuuint32_t)a.npad[h], 1};
-    CUresult r = enc(&a.wmap1[h], dt, 3, const_cast<void *>(hd[h].weight), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { delete t; return fail(CPB200_ERR_CUDA, "heads: cuTensorMapEncodeTiled(1x1 %d) failed: %d", h, (int)r); }
+    // 1x1 weights as packed for a 1x1 conv over the hidden channels (K slab 64): [plane][hid / 64][npad][64]
+    if (int rc = encode_weight_map(&a.wmap1[h], hd[h].weight, pr.fmt, 64, a.npad[h], a.npad[h], (long long)(hid / 64) * P,
+                                   CU_TENSOR_MAP_SWIZZLE_128B, "heads (1x1)"))
+      return rc;
   }
-  const int cin = op.cin[0];
-  const int bk = (cin % 64 == 0) ? 64 : (cin % 32 == 0) ? 32 : 16;
-  const CUtensorMapSwizzle sw = bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-  a.BK = bk; a.slabs = cin / bk;
-  a.swizzle_bits = bk == 64 ? 1u : bk == 32 ? 2u : 3u;
+  const Slab sl = slab_for(op.cin, 1);
+  const int bk = sl.bk;
+  a.BK = bk; a.slabs = op.cin[0] / bk;
+  a.swizzle_bits = sl.layout;
   a.B = op.B; a.Ho = op.Ho; a.Wo = op.Wo;
   a.tiles_h = (op.Ho + TH - 1) / TH; a.tiles_w = (op.Wo + TW - 1) / TW;
   a.total_tiles = op.B * a.tiles_h * a.tiles_w;
-  a.bias3 = op.bias;
   a.halo_tx_bytes = HW * HH * bk * 2;
   a.halo_stage_bytes = (a.halo_tx_bytes + 1023u) & ~1023u;
   a.halo_buf_bytes = a.slabs * P * a.halo_stage_bytes;
@@ -358,50 +321,32 @@ int heads_prepare(cpb200_op &op) {
   a.nh = 2 * (size_t)a.halo_buf_bytes + 3 * (size_t)a.w_stage_bytes <= budget ? 2 : 1;
   int nb = (int)((budget - a.nh * (size_t)a.halo_buf_bytes) / a.w_stage_bytes);
   if (nb > HD_MAX_NB) nb = HD_MAX_NB;
-  if (nb < 2) { delete t; return fail(CPB200_ERR_ARG, "heads: tile does not fit shared memory"); }
+  if (nb < 2) return fail(CPB200_ERR_ARG, "heads: tile does not fit shared memory");
   a.nb = nb;
   t->smem = a.nh * (size_t)a.halo_buf_bytes + nb * (size_t)a.w_stage_bytes + 1024;
-  const int nsm = num_sms();
-  t->grid = a.total_tiles < nsm ? a.total_tiles : nsm;
-  {
-    // split activations: the lo plane follows the hi plane, i.e. a batch of 2B images
-    const cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.B * P};
-    const cuuint64_t strides[3] = {(cuuint64_t)cin * 2, (cuuint64_t)op.W * cin * 2, (cuuint64_t)op.H * op.W * cin * 2};
-    const cuuint32_t box[4] = {(cuuint32_t)bk, HW, HH, 1};
-    CUresult r = enc(&a.amap, dt, 4, const_cast<void *>(op.src[0]), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { delete t; return fail(CPB200_ERR_CUDA, "heads: cuTensorMapEncodeTiled(A) failed: %d", (int)r); }
-  }
-  {
-    // 3x3 weights: the heads' packed 3x3 convs back to back, [head][plane][tap][K-slab][hid][bk]
-    const cuuint64_t dims[3] = {(cuuint64_t)bk, (cuuint64_t)hid, (cuuint64_t)nheads * P * 9 * a.slabs};
-    const cuuint64_t strides[2] = {(cuuint64_t)bk * 2, (cuuint64_t)hid * bk * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)bk, HD_CHUNK, 1};
-    CUresult r = enc(&a.wmap3, dt, 3, const_cast<void *>(op.weight), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { delete t; return fail(CPB200_ERR_CUDA, "heads: cuTensorMapEncodeTiled(3x3) failed: %d", (int)r); }
-  }
-  op.tc = t;
+  const cuuint32_t box[4] = {(cuuint32_t)bk, HW, HH, 1}, estr[4] = {1, 1, 1, 1};
+  if (int rc = encode_act_map(&a.amap, op.src[0], op.cin[0], op.cin[0], op.W, op.H, op.B, P, pr.fmt, sl.swizzle, box, estr, "heads"))
+    return rc;
+  // 3x3 weights: the heads' packed 3x3 convs back to back, [head][plane][tap][K-slab][hid][bk]
+  if (int rc = encode_weight_map(&a.wmap3, op.weight, pr.fmt, bk, hid, HD_CHUNK, (long long)nheads * P * 9 * a.slabs, sl.swizzle,
+                                 "heads (3x3)"))
+    return rc;
+  *out = t.release();
   return CPB200_OK;
 }
 
-void heads_release(cpb200_op &op) {
-  delete static_cast<HdOp *>(op.tc);
-  op.tc = nullptr;
-}
-
 // the output pointers and biases are read from the live table: outputs may be re-bound between runs
-int heads_run(const cpb200_op &op, cudaStream_t st) {
-  const HdOp *t = static_cast<const HdOp *>(op.tc);
-  if (!t) return fail(CPB200_ERR_STATE, "heads: op not prepared");
+int heads_run(const Prepared &p, const cpb200_op &op, cudaStream_t st) {
+  const HdOp &t = static_cast<const HdOp &>(p);
   const cpb200_head *hd = static_cast<const cpb200_head *>(op.aux);
-  HdArgs args = t->args;
+  HdArgs args = t.args;
   args.bias3 = op.bias;
   for (int h = 0; h < args.nheads; ++h) {
     if (!hd[h].dst) return fail(CPB200_ERR_ARG, "heads: entry %d: null dst", h);
     args.dst[h] = hd[h].dst; args.bias1[h] = hd[h].bias;
   }
-  return t->P == 2 ? launch_hd<2>(*t, args, st) : launch_hd<1>(*t, args, st);
+  return t.P == 2 ? launch<heads_tc_kernel<2>>("heads_tc_kernel", args.total_tiles, HD_THREADS, t.smem, st, args)
+                  : launch<heads_tc_kernel<1>>("heads_tc_kernel", args.total_tiles, HD_THREADS, t.smem, st, args);
 }
 
 }  // namespace cpb

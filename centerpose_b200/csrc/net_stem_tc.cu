@@ -174,8 +174,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1) stem_tc_kernel(const StemArgs a
         const int m = wg * 64 + frag_row(tq, j), c = frag_col(tq, j);
         const int ho = h0 + (m >> 4), wo = w0 + (m & 15);
         if (ho >= a.Ho || wo >= a.Wo) continue;
-        store_pair16<1>(a.y, nullptr, (((size_t)n * a.Ho + ho) * a.Wo + wo) * N + c, 0, acc[2 * j] + s_bias[c], acc[2 * j + 1] + s_bias[c + 1],
-                        a.act, 0u);
+        epilogue_pair<1>(acc, acc, j, s_bias[c], s_bias[c + 1], 1.f, a.act, OUT_16, a.y, nullptr, (((size_t)n * a.Ho + ho) * a.Wo + wo) * N + c,
+                         0, true, 0u);
       }
     }
   }
@@ -200,8 +200,7 @@ template <int N_, int P_> struct HStages { static constexpr int value = (P_ == 2
 
 // P = 2 (split operands, CPB200_BF16X2 / CPB200_F16X2): every producer thread splits its 21 fp32 input values into a hi and a
 // lo 64-byte vector; a stage is [hi vectors | lo vectors], the weight image per horizontal tap [hi tile | lo tile]
-// (plan.py::_pack_stem_tc_h); A_hi x W_hi goes to one accumulator array, A_hi x W_lo and
-// A_lo x W_hi to a second one; the epilogue adds them and stores the hi / lo planes of the output.
+// (plan.py::_pack_stem_tc_h).
 template <int N, int P>
 __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs a) {
   constexpr int H_NSTAGE = HStages<N, P>::value;
@@ -316,11 +315,8 @@ __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs 
     // =============================== consumers: wgmma + epilogue ===============================
     const int wg = warp >> 2, tq = threadIdx.x & 127;
     const uint32_t bf = (P == 1 || a.fmt == 0) ? 1u : 0u;
-    float acc[N / 2], acc2[P == 2 ? N / 2 : 1];                 // hi x W_hi | hi x W_lo + lo x W_hi (split operands)
-#pragma unroll
-    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (P == 2 ? N / 2 : 1); ++i) acc2[i] = 0.f;
+    float acc[N / 2], acc2[P == 2 ? N / 2 : 1];
+    acc_zero(acc, acc2);
     int stage = 0; uint32_t phase = 0;
     for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
       mbar_wait(full0 + 8 * stage, phase);
@@ -332,15 +328,9 @@ __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs 
       for (int s = 0; s < 7; ++s) {
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
-          const uint32_t first = (s > 0 || k > 0) ? 1u : 0u;
-          const uint64_t ad = ad0 + (uint32_t)(s * 4 + 2 * k), bd = bd0 + (uint32_t)(s * (B_TAP_BYTES >> 4) + 2 * k);
-          if constexpr (P == 2) {
-            wgmma_k16<N>(acc, ad, bd, first, bf);                                            // A_hi x W_hi
-            wgmma_k16<N>(acc2, ad, bd + (uint32_t)(B_TILE_BYTES >> 4), first, bf);           // A_hi x W_lo
-            wgmma_k16<N>(acc2, ad + (uint32_t)(HA_PLANE_BYTES >> 4), bd, 1u, bf);            // A_lo x W_hi
-          } else {
-            wgmma_k16<N>(acc, ad, bd, first, 1u);
-          }
+          const uint64_t ad = ad0 + (uint32_t)(s * 4), bd = bd0 + (uint32_t)(s * (B_TAP_BYTES >> 4));
+          mma_step<N, P>(acc, acc2, ad, ad + (uint32_t)(HA_PLANE_BYTES >> 4), bd, bd + (uint32_t)(B_TILE_BYTES >> 4), k,
+                         (s > 0 || k > 0) ? 1u : 0u, bf);
         }
       }
       wg_commit();
@@ -354,11 +344,8 @@ __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs 
         const int m = wg * 64 + frag_row(tq, j), c = frag_col(tq, j);
         const int ho = h0 + (m >> 3), wo = w0 + (m & 7);
         if (ho >= a.Ho || wo >= a.Wo) continue;
-        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
-        if constexpr (P == 2) { v0 += acc2[2 * j]; v1 += acc2[2 * j + 1]; }
-        const float f0 = P == 2 ? fmaf(v0, a.acc_scale, s_bias[c]) : v0 + s_bias[c];
-        const float f1 = P == 2 ? fmaf(v1, a.acc_scale, s_bias[c + 1]) : v1 + s_bias[c + 1];
-        store_pair16<P>(a.y, nullptr, (((size_t)n * a.Ho + ho) * a.Wo + wo) * N + c, a.y_plane, f0, f1, a.act, a.fmt);
+        epilogue_pair<P>(acc, acc2, j, s_bias[c], s_bias[c + 1], a.acc_scale, a.act, OUT_16, a.y, nullptr,
+                         (((size_t)n * a.Ho + ho) * a.Wo + wo) * N + c, a.y_plane, true, a.fmt);
       }
     }
   }
@@ -367,8 +354,8 @@ __global__ void __launch_bounds__(H_THREADS, 1) stem_tc_h_kernel(const StemArgs 
 template <int N, int P>
 int launch_stem_h(const cpb200_op &op, cudaStream_t st) {
   StemArgs a;
-  a.fmt = op.act_dtype == CPB200_F16X2 ? 1u : 0u;
-  a.acc_scale = op.acc_scale != 0.f ? op.acc_scale : 1.f;
+  const Prec pr = prec_of(op);
+  a.fmt = pr.fmt; a.acc_scale = pr.acc_scale;
   a.y_plane = (long long)op.B * op.Ho * op.Wo * N;
   a.x = static_cast<const float *>(op.src[0]); a.y = static_cast<__nv_bfloat16 *>(op.dst);
   a.wimg = static_cast<const uint4 *>(op.weight); a.bias = op.bias;
@@ -377,12 +364,7 @@ int launch_stem_h(const cpb200_op &op, cudaStream_t st) {
   a.total_tiles = op.B * a.tiles_h * a.tiles_w;
   a.act = op.flags & CPB_ACT_MASK;
   const size_t smem = 1024 + (size_t)HStages<N, P>::value * P * HA_STAGE_BYTES + 7 * (size_t)P * N * 64;
-  static SmemAttrCache cache;
-  if (int rc = ensure_smem(stem_tc_h_kernel<N, P>, smem, cache)) return rc;
-  const int sms = tc::num_sms();
-  const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  stem_tc_h_kernel<N, P><<<grid, H_THREADS, smem, st>>>(a);
-  return cpb::check_launch("stem_tc_h_kernel", stem_tc_h_kernel<N, P>);
+  return launch<stem_tc_h_kernel<N, P>>("stem_tc_h_kernel", a.total_tiles, H_THREADS, smem, st, a);
 }
 
 template <int N, int S>
@@ -397,12 +379,7 @@ int launch_stem(const cpb200_op &op, cudaStream_t st) {
   a.act = op.flags & CPB_ACT_MASK;
   a.fmt = 0; a.acc_scale = 1.f; a.y_plane = 0;
   const size_t smem = 1024 + (size_t)NSTAGE * A_STAGE_BYTES + (size_t)SLABS * N * 128 + (size_t)PGROUPS * 2 * CIN * PH * PP * sizeof(float);
-  static SmemAttrCache cache;
-  if (int rc = ensure_smem(stem_tc_kernel<N, S>, smem, cache)) return rc;
-  const int sms = tc::num_sms();
-  const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  stem_tc_kernel<N, S><<<grid, ST_THREADS, smem, st>>>(a);
-  return cpb::check_launch("stem_tc_kernel", stem_tc_kernel<N, S>);
+  return launch<stem_tc_kernel<N, S>>("stem_tc_kernel", a.total_tiles, ST_THREADS, smem, st, a);
 }
 
 }  // namespace
@@ -418,7 +395,6 @@ bool stem_tc_eligible(const cpb200_op &op) {
 }
 
 int stem_tc_run(const cpb200_op &op, cudaStream_t st) {
-  if (!stem_tc_eligible(op)) return fail(CPB200_ERR_ARG, "stem_tc: unsupported shape (needs 7x7, Cin 3, stride 1/2, cout 16/64; split precisions stride 1 only)");
   const bool split = op.act_dtype != CPB200_BF16;
   // stride 1: vertical-fold kernel (weight image = 7 taps x N rows x 64 B); stride 2: full im2col rows (3 slabs x N x 128 B)
   if (op.cout == 16 && op.stride == 1) return split ? launch_stem_h<16, 2>(op, st) : launch_stem_h<16, 1>(op, st);

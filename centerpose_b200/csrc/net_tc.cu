@@ -20,14 +20,11 @@
 // with full/empty mbarriers feeds the tensor cores, and a stage is released as soon as the MMAs of the NEXT stage are queued.
 //
 // Split-operand precisions (P = 2, CPB200_BF16X2 / CPB200_F16X2, see tc_common.cuh): a stage is
-// [A_hi | A_lo | W_hi | W_lo]; per K step the consumers issue three N = BN products: A_hi x W_hi into one accumulator array,
-// A_hi x W_lo and A_lo x W_hi into a second one (added in the epilogue).  Separate arrays keep the wgmma of one K step
-// independent of each other, so ptxas does not serialise them.
-// The DCN gather blends the four corners of BOTH planes in fp32 and re-splits the sample.
+// [A_hi | A_lo | W_hi | W_lo]; per K step the consumers issue the three products of tc::mma_step.  The DCN gather blends the four corners of BOTH planes in fp32 and re-splits the sample.
 #include <type_traits>
 #include "tc_common.cuh"
 #include <mutex>
-#include <cstdlib>
+#include <memory>
 
 namespace {
 
@@ -362,13 +359,9 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
     const uint32_t aplane = a_bytes >> 4, bplane = b_bytes >> 4, boff = (uint32_t)(P * a_bytes) >> 4;
     const int ksteps = a.BK / 16;
     const uint32_t act = a.flags & CPB_ACT_MASK;
-    const bool out_f32 = a.flags & CPB200_FLAG_OUT_F32;
-    const bool out_nchw = a.flags & CPB200_FLAG_OUT_NCHW_F32;
-    float acc[BN / 2], acc2[P == 2 ? BN / 2 : 1];                 // hi x W_hi | hi x W_lo + lo x W_hi (split operands)
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (P == 2 ? BN / 2 : 1); ++i) acc2[i] = 0.f;
+    const int form = out_form(a.flags);
+    float acc[BN / 2], acc2[P == 2 ? BN / 2 : 1];
+    acc_zero(acc, acc2);
     int stage = 0; uint32_t phase = 0;
     for (int tt = blockIdx.x; tt < a.total_tiles; tt += gridDim.x) {
       int prev = -1;                                       // stage whose MMAs may still be running
@@ -377,18 +370,8 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
         const uint64_t sd = dT + (base14 + (uint32_t)stage * sstep);
         const uint64_t ad = sd + aoff, bd = sd + boff;
         wg_fence();
-        for (int k = 0; k < ksteps; ++k) {
-          const uint32_t first = (kb > 0 || k > 0) ? 1u : 0u;
-          if constexpr (P == 1) {
-            wgmma_k16<BN>(acc, ad + 2 * k, bd + 2 * k, first, 1u);
-          } else {
-            wgmma_k16<BN>(acc, ad + 2 * k, bd + 2 * k, first, bf);                     // A_hi x W_hi
-            wgmma_k16<BN>(acc2, ad + 2 * k, bd + bplane + 2 * k, first, bf);           // A_hi x W_lo
-            // A_lo x W_hi joins the other small term (see net_tc3.cu: the fp32 accumulator truncates per instruction in
-            // proportion to its magnitude)
-            wgmma_k16<BN>(acc2, ad + aplane + 2 * k, bd + 2 * k, 1u, bf);
-          }
-        }
+        for (int k = 0; k < ksteps; ++k)
+          mma_step<BN, P>(acc, acc2, ad, ad + aplane, bd, bd + bplane, k, (kb > 0 || k > 0) ? 1u : 0u, bf);
         wg_commit();
         wg_wait<1>();                                      // the previous stage's MMAs have retired: release it
         if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
@@ -405,48 +388,32 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
         const int row = wg * 64 + frag_row(t, j), nb = n0 + frag_col(t, j);
         const int ho = h0 + row / a.TW, wo = w0 + row % a.TW;
         if (ho >= a.Ho || wo >= a.Wo || nb >= a.cout) continue;
-        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
-        if constexpr (P == 2) { v0 += acc2[2 * j]; v1 += acc2[2 * j + 1]; }
         const bool has1 = nb + 1 < a.cout;
         const float b0 = a.bias ? __ldg(a.bias + nb) : 0.f, b1 = (a.bias && has1) ? __ldg(a.bias + nb + 1) : 0.f;
-        const float f0 = P == 2 ? fmaf(v0, a.acc_scale, b0) : v0 + b0, f1 = P == 2 ? fmaf(v1, a.acc_scale, b1) : v1 + b1;
-        const size_t pix = ((size_t)n * a.Hd + (ho * a.sy + a.oy)) * a.Wd + (wo * a.sx + a.ox);
-        if (out_nchw) {
-          // head outputs: NCHW fp32 channel slice of dst
-          float *o = static_cast<float *>(a.dst) +
-                     (((size_t)n * a.out_ch_total + a.out_ch_off + nb) * a.Hd + (ho * a.sy + a.oy)) * a.Wd + (wo * a.sx + a.ox);
-          const size_t plane = (size_t)a.Hd * a.Wd;
-          o[0] = P == 2 ? cpb::act_fn(f0, act) : cpb::act_out<__nv_bfloat16>(f0, act);
-          if (has1) o[plane] = P == 2 ? cpb::act_fn(f1, act) : cpb::act_out<__nv_bfloat16>(f1, act);
-        } else if (out_f32) {
-          float *o = static_cast<float *>(a.dst) + pix * a.cout_store + nb;
-          o[0] = cpb::act_out<__nv_bfloat16>(f0, act);
-          if (has1) o[1] = cpb::act_out<__nv_bfloat16>(f1, act);
-        } else {
-          store_pair16<P>(a.dst, a.res, pix * a.cout_store + nb, a.dst_plane, f0, f1, act, a.fmt);
-        }
+        const int y = ho * a.sy + a.oy, x = wo * a.sx + a.ox;     // strided output lattice of the deconv parity convs
+        // NCHW: the head outputs, a channel slice of dst
+        const size_t e = form == OUT_NCHW ? (((size_t)n * a.out_ch_total + a.out_ch_off + nb) * a.Hd + y) * a.Wd + x
+                                          : (((size_t)n * a.Hd + y) * a.Wd + x) * a.cout_store + nb;
+        const long long plane = form == OUT_NCHW ? (long long)a.Hd * a.Wd : a.dst_plane;
+        epilogue_pair<P>(acc, acc2, j, b0, b1, a.acc_scale, act, form, a.dst, a.res, e, plane, has1, a.fmt);
       }
     }
   }
 }
 
 // ------------------------------------------------------------------------------- host side
-struct TcOp {
+struct TcOp : cpb::Prepared {
+  TcOp() : Prepared(cpb::Route::TAP) {}
   TcArgs args;
   int BN, P;
   bool dcn;
-  void *c3 = nullptr;      // halo-reuse 3x3 kernel handle (net_tc3.cu) when that path was chosen
-  int grid;
   size_t smem;
 };
 
-
 template <int BN, bool DCN, int P>
 int launch_tc(const TcOp &t, const TcArgs &args, cudaStream_t st) {
-  static SmemAttrCache cache;
-  if (int rc = ensure_smem(conv_tc_kernel<BN, DCN, P>, t.smem, cache)) return rc;
-  conv_tc_kernel<BN, DCN, P><<<t.grid, DCN ? DCN_THREADS : TC_THREADS, t.smem, st>>>(args);
-  return cpb::check_launch(DCN ? "dcn_tc_kernel" : "conv_tc_kernel", conv_tc_kernel<BN, DCN, P>);
+  return launch<conv_tc_kernel<BN, DCN, P>>(DCN ? "dcn_tc_kernel" : "conv_tc_kernel", args.total_tiles,
+                                            DCN ? DCN_THREADS : TC_THREADS, t.smem, st, args);
 }
 
 }  // namespace
@@ -480,150 +447,145 @@ int num_sms() {
   }
   return v;
 }
+
+bool tc_dtype(int d) { return d == CPB200_BF16 || d == CPB200_BF16X2 || d == CPB200_F16X2; }
+
+Prec prec_of(const cpb200_op &op) {
+  return {op.act_dtype == CPB200_BF16 ? 1 : 2, op.act_dtype == CPB200_F16X2 ? 1u : 0u, op.acc_scale != 0.f ? op.acc_scale : 1.f};
+}
+
+Slab slab_for(const int *cin, int nsrc) {
+  int bk = 64;
+  for (int s = 0; s < nsrc; ++s)
+    if (cin[s] % 64) bk = (cin[s] % 32 == 0) ? (bk < 32 ? bk : 32) : 16;
+  if (bk == 64) return {64, CU_TENSOR_MAP_SWIZZLE_128B, 1u};
+  if (bk == 32) return {32, CU_TENSOR_MAP_SWIZZLE_64B, 2u};
+  return {16, CU_TENSOR_MAP_SWIZZLE_32B, 3u};
+}
+
+int bn_for(int cout, int P) {
+  int BN = 16;
+  while (BN < cout && BN < 256) BN <<= 1;
+  return P == 2 && BN > 128 ? 128 : BN;
+}
+
+int encode_act_map(CUtensorMap *map, const void *src, int C, int pitch, int W, int H, int B, int P, uint32_t fmt,
+                   CUtensorMapSwizzle sw, const cuuint32_t (&box)[4], const cuuint32_t (&estr)[4], const char *what) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return cpb::fail(CPB200_ERR_STATE, "%s: cuTensorMapEncodeTiled unavailable", what);
+  const cuuint64_t p = (cuuint64_t)pitch;
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B * P};
+  const cuuint64_t strides[3] = {p * 2, (cuuint64_t)W * p * 2, (cuuint64_t)H * W * p * 2};
+  CUresult r = enc(map, fmt ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(src), dims,
+                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return cpb::fail(CPB200_ERR_CUDA, "%s: cuTensorMapEncodeTiled(activations) failed: %d", what, (int)r);
+  return CPB200_OK;
+}
+
+int encode_weight_map(CUtensorMap *map, const void *w, uint32_t fmt, int bk, int rows, int box_rows, long long blocks,
+                      CUtensorMapSwizzle sw, const char *what) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return cpb::fail(CPB200_ERR_STATE, "%s: cuTensorMapEncodeTiled unavailable", what);
+  const cuuint64_t dims[3] = {(cuuint64_t)bk, (cuuint64_t)rows, (cuuint64_t)blocks};
+  const cuuint64_t strides[2] = {(cuuint64_t)bk * 2, (cuuint64_t)rows * bk * 2};
+  const cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)box_rows, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(map, fmt ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(w), dims,
+                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return cpb::fail(CPB200_ERR_CUDA, "%s: cuTensorMapEncodeTiled(weights) failed: %d", what, (int)r);
+  return CPB200_OK;
+}
 }  // namespace tc
 
 namespace cpb {
 
-bool c3_eligible(const cpb200_op &op);
-void *c3_prepare(const cpb200_op &op, int *rc);
-void c3_release(void *h);
-int c3_run(const void *h, const cpb200_op &op, cudaStream_t st);
-
-static bool halo_enabled() {
-  const char *e = getenv("CPB200_TC_HALO");
-  return !(e && e[0] == '0');
-}
-
-int tc_prepare_op(cpb200_op &op) {
-  if (halo_enabled() && c3_eligible(op)) {
-    int rc = CPB200_OK;
-    void *h = c3_prepare(op, &rc);
-    if (!h) return rc;
-    TcOp *t = new TcOp();
-    t->c3 = h;
-    op.tc = t;
-    return CPB200_OK;
-  }
+int tap_prepare(const cpb200_op &op, Prepared **out) {
   const bool dcn = op.type == CPB200_OP_DCN;
   if (op.type != CPB200_OP_CONV && !dcn) return fail(CPB200_ERR_ARG, "tc: only CONV / DCN ops run on the tensor-core path");
   if (dcn && (op.kh != 3 || op.kw != 3 || op.stride != 1 || op.pad_h != 1 || op.pad_w != 1 || op.nsrc != 1 ||
               op.cin[0] % 64 || !op.aux || op.H != op.Ho || op.W != op.Wo))
     return fail(CPB200_ERR_ARG, "tc: DCN needs 3x3/s1/p1, one input with C %% 64 == 0 and the offset/mask tensor");
-  if (op.act_dtype != CPB200_BF16 && op.act_dtype != CPB200_BF16X2 && op.act_dtype != CPB200_F16X2)
-    return fail(CPB200_ERR_ARG, "tc: bf16 or split (bf16x2 / fp16x2) activations required");
+  if (!tc_dtype(op.act_dtype)) return fail(CPB200_ERR_ARG, "tc: bf16 or split (bf16x2 / fp16x2) activations required");
   if (op.stride < 1 || op.stride > 2) return fail(CPB200_ERR_ARG, "tc: stride %d", op.stride);
   if (op.Wo < 8 || op.Ho < 1) return fail(CPB200_ERR_ARG, "tc: output too small");
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(CPB200_ERR_STATE, "tc: cuTensorMapEncodeTiled unavailable");
-  const int g_num_sms = tc::num_sms();
-  TcOp *t = new TcOp();
-  TcArgs &a = t->args;
-  memset(&a, 0, sizeof(a));
-  const int P = op.act_dtype == CPB200_BF16 ? 1 : 2;
-  t->P = P;
-  a.fmt = op.act_dtype == CPB200_F16X2 ? 1u : 0u;
-  a.acc_scale = op.acc_scale != 0.f ? op.acc_scale : 1.f;
-  int cin_total = 0, bk = 64;
+  int cin_total = 0;
   for (int s = 0; s < op.nsrc; ++s) {
-    const int c = op.cin[s];
-    if (c % 16) { delete t; return fail(CPB200_ERR_ARG, "tc: cin %d not a multiple of 16", c); }
-    if (c % 64) bk = (c % 32 == 0) ? (bk < 32 ? bk : 32) : 16;
-    a.cin[s] = c; cin_total += c;
+    if (op.cin[s] % 16) return fail(CPB200_ERR_ARG, "tc: cin %d not a multiple of 16", op.cin[s]);
+    cin_total += op.cin[s];
   }
-  a.nsrc = op.nsrc; a.BK = bk;
-  const CUtensorMapSwizzle sw = bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-  a.swizzle_bits = bk == 64 ? 1u : bk == 32 ? 2u : 3u;
-  a.kh = op.kh; a.kw = op.kw; a.stride = op.stride; a.pad_h = op.pad_h; a.pad_w = op.pad_w;
-  a.B = op.B; a.Ho = op.Ho; a.Wo = op.Wo;
-  a.TW = op.Wo >= 16 ? 16 : 8; a.TH = TILE_M / a.TW;
-  a.tiles_h = (op.Ho + a.TH - 1) / a.TH; a.tiles_w = (op.Wo + a.TW - 1) / a.TW;
-  int BN = 16;
-  while (BN < op.cout && BN < 256) BN <<= 1;
-  if (P == 2 && BN > 128) BN = 128;            // split operands: two accumulator halves of BN columns each (2 * BN <= 256)
+  if (!(op.flags & (CPB200_FLAG_OUT_F32 | CPB200_FLAG_OUT_NCHW_F32)) && (op.cout % 16))
+    return fail(CPB200_ERR_ARG, "tc: 16-bit output needs cout %% 16 == 0");
+  const Prec pr = prec_of(op);
+  const Slab sl = slab_for(op.cin, op.nsrc);
+  const int P = pr.P, bk = sl.bk;
+  const long long src_plane = (long long)op.B * op.H * op.W * op.cin[0];
+  if (dcn && P == 2 && src_plane * 4 >= (1LL << 32))
+    return fail(CPB200_ERR_ARG, "tc: split-precision DCN input must stay below 4 GiB (32-bit gather offsets)");
+  int BN = bn_for(op.cout, P);
   // DCN: the gather warps leave 120 registers per thread, so a consumer holds at most 64 accumulator registers
   if (dcn && BN > 128 / P) BN = 128 / P;
-  t->BN = BN; t->dcn = dcn;
-  a.dcn_src = static_cast<const __nv_bfloat16 *>(op.src[0]); a.dcn_om = static_cast<const float *>(op.aux);
-  a.H = op.H; a.W = op.W; a.om_pitch = op.aux_pitch > 0 ? op.aux_pitch : 27;
-  a.Hd = op.Hd; a.Wd = op.Wd; a.sy = op.out_sy; a.sx = op.out_sx; a.oy = op.out_oy; a.ox = op.out_ox;
-  a.n_tiles = (op.cout + BN - 1) / BN;
-  a.cout = op.cout; a.cout_store = op.cout;
-  if (!(op.flags & (CPB200_FLAG_OUT_F32 | CPB200_FLAG_OUT_NCHW_F32)) && (op.cout % 16)) { delete t; return fail(CPB200_ERR_ARG, "tc: 16-bit output needs cout %% 16 == 0"); }
-  a.out_ch_off = op.out_ch_off; a.out_ch_total = op.out_ch_total;
-  a.total_tiles = op.B * a.tiles_h * a.tiles_w * a.n_tiles;
-  a.dst = op.dst; a.res = op.res; a.bias = op.bias; a.flags = op.flags;
-  a.dst_plane = (long long)op.B * op.Hd * op.Wd * op.cout;
-  a.src_plane = (long long)op.B * op.H * op.W * op.cin[0];
-  if (dcn && P == 2 && a.src_plane * 4 >= (1LL << 32)) { delete t;
-    return fail(CPB200_ERR_ARG, "tc: split-precision DCN input must stay below 4 GiB (32-bit gather offsets)"); }
-  a.wplane = op.kh * op.kw * (cin_total / bk);
   const size_t a_bytes = (size_t)P * TILE_M * bk * 2, b_bytes = ((size_t)P * BN * bk * 2 + 1023) / 1024 * 1024;
   const size_t budget = dcn ? 176 * 1024 : 200 * 1024;     // the DCN variant keeps 37 KB of sampling parameters in static smem
   int stages = (int)(budget / (a_bytes + b_bytes));
   if (stages > 8) stages = 8;
   if (dcn && stages > 4) stages = 4;      // leave the rest of the 256 KB to L1: the 9 taps x 4 corners re-read one ~30 KB footprint
-  if (stages < 2) { delete t; return fail(CPB200_ERR_ARG, "tc: tile does not fit shared memory"); }
-  a.stages = stages;
-  t->smem = stages * (a_bytes + b_bytes) + 1024;
-  t->grid = a.total_tiles < g_num_sms ? a.total_tiles : g_num_sms;
-  const CUtensorMapDataType dt = a.fmt ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  if (stages < 2) return fail(CPB200_ERR_ARG, "tc: tile does not fit shared memory");
 
+  std::unique_ptr<TcOp> t(new TcOp());
+  TcArgs &a = t->args;
+  memset(&a, 0, sizeof(a));
+  t->P = P; t->BN = BN; t->dcn = dcn;
+  t->smem = stages * (a_bytes + b_bytes) + 1024;
+  a.fmt = pr.fmt; a.acc_scale = pr.acc_scale;
+  for (int s = 0; s < op.nsrc; ++s) a.cin[s] = op.cin[s];
+  a.nsrc = op.nsrc; a.BK = bk; a.swizzle_bits = sl.layout; a.stages = stages;
+  a.kh = op.kh; a.kw = op.kw; a.stride = op.stride; a.pad_h = op.pad_h; a.pad_w = op.pad_w;
+  a.B = op.B; a.Ho = op.Ho; a.Wo = op.Wo;
+  a.TW = op.Wo >= 16 ? 16 : 8; a.TH = TILE_M / a.TW;
+  a.tiles_h = (op.Ho + a.TH - 1) / a.TH; a.tiles_w = (op.Wo + a.TW - 1) / a.TW;
+  a.dcn_src = static_cast<const __nv_bfloat16 *>(op.src[0]);
+  a.H = op.H; a.W = op.W; a.om_pitch = op.aux_pitch > 0 ? op.aux_pitch : 27;
+  a.Hd = op.Hd; a.Wd = op.Wd; a.sy = op.out_sy; a.sx = op.out_sx; a.oy = op.out_oy; a.ox = op.out_ox;
+  a.n_tiles = (op.cout + BN - 1) / BN;
+  a.cout = op.cout; a.cout_store = op.cout;
+  a.out_ch_off = op.out_ch_off; a.out_ch_total = op.out_ch_total;
+  a.total_tiles = op.B * a.tiles_h * a.tiles_w * a.n_tiles;
+  a.flags = op.flags;
+  a.dst_plane = (long long)op.B * op.Hd * op.Wd * op.cout;
+  a.src_plane = src_plane;
+  a.wplane = op.kh * op.kw * (cin_total / bk);
   for (int s = 0; s < op.nsrc && !dcn; ++s) {
-    // a channel slice of a wider tensor: `pitch` elements between pixels, op.src[s] already points at the slice.
-    // Split activations: the lo plane follows the hi plane of the (parent) tensor, i.e. a batch of 2B images.
-    const cuuint64_t pitch = op.src_pitch[s] > 0 ? (cuuint64_t)op.src_pitch[s] : (cuuint64_t)op.cin[s];
-    const cuuint64_t dims[4] = {(cuuint64_t)op.cin[s], (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.B * P};
-    const cuuint64_t strides[3] = {pitch * 2, (cuuint64_t)op.W * pitch * 2, (cuuint64_t)op.H * op.W * pitch * 2};
+    // a channel slice of a wider tensor: op.src[s] already points at the slice
     const cuuint32_t box[4] = {(cuuint32_t)bk, (cuuint32_t)(a.TW * op.stride), (cuuint32_t)(a.TH * op.stride), 1};
     const cuuint32_t estr[4] = {1, (cuuint32_t)op.stride, (cuuint32_t)op.stride, 1};
-    CUresult r = enc(&a.amap[s], dt, 4, const_cast<void *>(op.src[s]), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { delete t; return fail(CPB200_ERR_CUDA, "tc: cuTensorMapEncodeTiled(A[%d]) failed: %d", s, (int)r); }
+    if (int rc = encode_act_map(&a.amap[s], op.src[s], op.cin[s], op.src_pitch[s] > 0 ? op.src_pitch[s] : op.cin[s], op.W, op.H,
+                                op.B, P, pr.fmt, sl.swizzle, box, estr, "tc"))
+      return rc;
   }
-  {
-    // weights are packed slab-major [plane][tap][K-slab][cout_pad][bk] (plan.py::_pack_conv_tc): a box is one dense run
-    const int cout_pad = (op.cout + 15) / 16 * 16;
-    const cuuint64_t dims[3] = {(cuuint64_t)bk, (cuuint64_t)cout_pad, (cuuint64_t)(op.kh * op.kw) * (cuuint64_t)(cin_total / bk) * P};
-    const cuuint64_t strides[2] = {(cuuint64_t)bk * 2, (cuuint64_t)cout_pad * bk * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)BN, 1};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&a.bmap, dt, 3, const_cast<void *>(op.weight), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { delete t; return fail(CPB200_ERR_CUDA, "tc: cuTensorMapEncodeTiled(B) failed: %d", (int)r); }
-  }
-  op.tc = t;
+  if (int rc = encode_weight_map(&a.bmap, op.weight, pr.fmt, bk, (op.cout + 15) / 16 * 16, BN, (long long)P * a.wplane, sl.swizzle, "tc"))
+    return rc;
+  *out = t.release();
   return CPB200_OK;
 }
 
-int tc_release_op(cpb200_op &op) {
-  TcOp *t = static_cast<TcOp *>(op.tc);
-  if (t && t->c3) c3_release(t->c3);
-  delete t;
-  op.tc = nullptr;
-  return CPB200_OK;
-}
-
-int tc_run_op(const cpb200_op &op, cudaStream_t st) {
-  const TcOp *t = static_cast<const TcOp *>(op.tc);
-  if (!t) return fail(CPB200_ERR_STATE, "tc: op not prepared");
-  if (t->c3) return c3_run(t->c3, op, st);
-  // dst / res / bias / the DCN offset tensor are taken from the live op: the model binds new output tensors every
-  // forward (include/centerpose_b200.h); input activations and weights were baked into the tensor maps at prepare.
-  TcArgs args = t->args;
+int tap_run(const Prepared &p, const cpb200_op &op, cudaStream_t st) {
+  const TcOp &t = static_cast<const TcOp &>(p);
+  // input activations and weights are baked into the tensor maps; the rest comes from the live op (tc_common.cuh: Route)
+  TcArgs args = t.args;
   args.dst = op.dst; args.res = op.res; args.bias = op.bias;
   args.dcn_om = static_cast<const float *>(op.aux);
 #define TC_CASE(N, D)                                                                                  \
-  case N: return t->P == 2 ? launch_tc<N, D, 2>(*t, args, st) : launch_tc<N, D, 1>(*t, args, st);
-  if (t->dcn) {
-    switch (t->BN) {
+  case N: return t.P == 2 ? launch_tc<N, D, 2>(t, args, st) : launch_tc<N, D, 1>(t, args, st);
+  if (t.dcn) {
+    switch (t.BN) {
       TC_CASE(16, true) TC_CASE(32, true) TC_CASE(64, true)
-      case 128: if (t->P == 1) return launch_tc<128, true, 1>(*t, args, st); break;
+      case 128: if (t.P == 1) return launch_tc<128, true, 1>(t, args, st); break;
     }
-    return fail(CPB200_ERR_STATE, "tc: DCN supports cout tiles of 16..128 (bf16) / 16..64 (split) only");
-  }
-  switch (t->BN) {
-    TC_CASE(16, false) TC_CASE(32, false) TC_CASE(64, false) TC_CASE(128, false)
-    case 256: if (t->P == 1) return launch_tc<256, false, 1>(*t, args, st); break;
+  } else {
+    switch (t.BN) {
+      TC_CASE(16, false) TC_CASE(32, false) TC_CASE(64, false) TC_CASE(128, false)
+      case 256: if (t.P == 1) return launch_tc<256, false, 1>(t, args, st); break;
+    }
   }
 #undef TC_CASE
   return fail(CPB200_ERR_STATE, "tc: bad BN");

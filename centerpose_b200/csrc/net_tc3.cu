@@ -19,12 +19,11 @@
 //
 // Split-operand precisions (P = 2, act_dtype CPB200_BF16X2 / CPB200_F16X2; tc_common.cuh): activations and weights arrive
 // as hi / lo 16-bit planes.  The halo ring is plane-granular (the planes of a slab are two consecutive stages, TMA batch
-// coordinate n and n + B); a weight stage holds the hi tile immediately followed by the lo tile.  A_hi*W_hi goes to one
-// accumulator array, A_hi*W_lo and A_lo*W_hi to a second one; the epilogue adds them, scales by acc_scale, and writes
-// hi / lo planes.
+// coordinate n and n + B); a weight stage holds the hi tile immediately followed by the lo tile (tc::mma_step,
+// tc::epilogue_pair).
 #include <type_traits>
 #include "tc_common.cuh"
-#include <cstdlib>
+#include <memory>
 
 using namespace tc;
 
@@ -136,9 +135,7 @@ __global__ void __launch_bounds__(C3_THREADS, 1) conv3x3_tc_kernel(const __grid_
     // =============================== consumers: wgmma + epilogue ===============================
     // Per slab the halo plane(s) are waited for once, then every tap issues its products.  Streamed weights: one weight stage
     // per (slab, tap), released once the MMAs of the next one are queued; resident weights: nothing to wait for but the halo.
-    // The halo stages of a slab are released after its last tap.  The small cross term A_lo x W_hi joins A_hi x W_lo in the
-    // SECOND accumulator: the tensor core's fp32 accumulator truncates (round toward zero) at every instruction, an error
-    // proportional to the accumulator's magnitude — the large hi x hi sum must see as few additions as possible.
+    // The halo stages of a slab are released after its last tap.
     const int wg = warp >> 2, t = threadIdx.x & 127;
     const uint32_t bf = (P == 1 || a.fmt == 0) ? 1u : 0u;
     const int ksteps = a.BK / 16;
@@ -149,12 +146,9 @@ __global__ void __launch_bounds__(C3_THREADS, 1) conv3x3_tc_kernel(const __grid_
     const uint32_t astep = a.a_stage_bytes >> 4, bstep = a.b_stage_bytes >> 4, rowstep = (uint32_t)a.hw * pstep;
     const uint32_t btile = a.b_tile_bytes >> 4;                                  // W_lo follows W_hi in a weight stage
     const uint32_t act = a.flags & CPB_ACT_MASK;
-    const bool out_f32 = a.flags & CPB200_FLAG_OUT_F32;
-    float acc[BN / 2], acc2[P == 2 ? BN / 2 : 1];                 // hi x W_hi | hi x W_lo + lo x W_hi (split operands)
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (P == 2 ? BN / 2 : 1); ++i) acc2[i] = 0.f;
+    const int form = (a.flags & CPB200_FLAG_OUT_F32) ? OUT_F32 : OUT_16;      // c3_eligible: no NCHW output
+    float acc[BN / 2], acc2[P == 2 ? BN / 2 : 1];
+    acc_zero(acc, acc2);
     int sa = 0; uint32_t pha = 0; int sb = 0; uint32_t phb = 0;
     if (a.b_resident) mbar_wait(ball, 0);
     int n, h0, w0, nt;
@@ -184,16 +178,8 @@ __global__ void __launch_bounds__(C3_THREADS, 1) conv3x3_tc_kernel(const __grid_
           }
           const uint64_t adh = ah0 + toff, adl = al0 + toff;
           wg_fence();
-          for (int k = 0; k < ksteps; ++k) {
-            const uint32_t first = k == 0 ? accf : 1u;
-            if constexpr (P == 1) {
-              wgmma_k16<BN>(acc, adh + 2 * k, bd + 2 * k, first, 1u);
-            } else {
-              wgmma_k16<BN>(acc, adh + 2 * k, bd + 2 * k, first, bf);
-              wgmma_k16<BN>(acc2, adh + 2 * k, bd + btile + 2 * k, first, bf);
-              wgmma_k16<BN>(acc2, adl + 2 * k, bd + 2 * k, 1u, bf);           // small terms share one accumulator
-            }
-          }
+          for (int k = 0; k < ksteps; ++k)
+            mma_step<BN, P>(acc, acc2, adh, adl, bd, bd + btile, k, k == 0 ? accf : 1u, bf);
           accf = 1u;
           wg_commit();
           wg_wait<1>();
@@ -219,43 +205,30 @@ __global__ void __launch_bounds__(C3_THREADS, 1) conv3x3_tc_kernel(const __grid_
         const int row = wg * 64 + frag_row(t, j), nb = n0 + frag_col(t, j);
         const int ho = h0 + (row >> 3), wo = w0 + (row & 7);
         if (ho >= a.Ho || wo >= a.Wo || nb >= a.cout) continue;
-        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
-        if constexpr (P == 2) { v0 += acc2[2 * j]; v1 += acc2[2 * j + 1]; }
         const bool has1 = nb + 1 < a.cout;
         const float b0 = a.bias ? __ldg(a.bias + nb) : 0.f, b1 = (a.bias && has1) ? __ldg(a.bias + nb + 1) : 0.f;
-        const float f0 = P == 2 ? fmaf(v0, a.acc_scale, b0) : v0 + b0, f1 = P == 2 ? fmaf(v1, a.acc_scale, b1) : v1 + b1;
         const size_t pix = ((size_t)n * a.Ho + ho) * a.Wo + wo;
-        if (out_f32) {
-          float *o = static_cast<float *>(a.dst) + pix * a.cout_store + nb;
-          o[0] = cpb::act_out<__nv_bfloat16>(f0, act);
-          if (has1) o[1] = cpb::act_out<__nv_bfloat16>(f1, act);
-        } else {
-          store_pair16<P>(a.dst, a.res, pix * a.cout_store + nb, a.dst_plane, f0, f1, act, a.fmt);
-        }
+        epilogue_pair<P>(acc, acc2, j, b0, b1, a.acc_scale, act, form, a.dst, a.res, pix * a.cout_store + nb, a.dst_plane, has1, a.fmt);
       }
     }
   }
 }
 
-struct C3Op {
+struct C3Op : cpb::Prepared {
+  C3Op() : Prepared(cpb::Route::HALO) {}
   C3Args args;
-  int BN, P, grid;
+  int BN, P;
   size_t smem;
 };
 
 template <int BN, int P>
 int launch_c3(const C3Op &t, const C3Args &args, cudaStream_t st) {
-  static SmemAttrCache cache;
-  if (int rc = ensure_smem(conv3x3_tc_kernel<BN, P>, t.smem, cache)) return rc;
-  conv3x3_tc_kernel<BN, P><<<t.grid, C3_THREADS, t.smem, st>>>(args);
-  return cpb::check_launch("conv3x3_tc_kernel", conv3x3_tc_kernel<BN, P>);
+  return launch<conv3x3_tc_kernel<BN, P>>("conv3x3_tc_kernel", args.total_tiles, C3_THREADS, t.smem, st, args);
 }
 
 }  // namespace
 
 namespace cpb {
-
-static bool tc_act_dtype(int d) { return d == CPB200_BF16 || d == CPB200_BF16X2 || d == CPB200_F16X2; }
 
 bool c3_eligible(const cpb200_op &op) {
   const bool geom = (op.kh == 3 && op.kw == 3) || (op.kh == 7 && op.kw == 1) || (op.kh == 1 && op.kw == 7) || (op.kh == 5 && op.kw == 5);
@@ -263,38 +236,30 @@ bool c3_eligible(const cpb200_op &op) {
          op.nsrc == 1 && op.cin[0] % 16 == 0 && (op.src_pitch[0] == 0 || op.src_pitch[0] == op.cin[0]) && op.Wo >= 8 && op.Ho >= 8 &&
          op.H == op.Ho && op.W == op.Wo &&
          op.out_sy == 1 && op.out_sx == 1 && !op.out_oy && !op.out_ox && op.Hd == op.Ho && op.Wd == op.Wo &&
-         !(op.flags & CPB200_FLAG_OUT_NCHW_F32) && tc_act_dtype(op.act_dtype) &&
+         !(op.flags & CPB200_FLAG_OUT_NCHW_F32) && tc_dtype(op.act_dtype) &&
          ((op.flags & CPB200_FLAG_OUT_F32) || op.cout % 16 == 0);
 }
 
-// returns an opaque handle (C3Op*) or nullptr + error
-void *c3_prepare(const cpb200_op &op, int *rc) {
-  *rc = CPB200_OK;
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { *rc = fail(CPB200_ERR_STATE, "tc3: cuTensorMapEncodeTiled unavailable"); return nullptr; }
-  C3Op *t = new C3Op();
+int c3_prepare(const cpb200_op &op, Prepared **out) {
+  std::unique_ptr<C3Op> t(new C3Op());
   C3Args &a = t->args;
   memset(&a, 0, sizeof(a));
-  const int P = op.act_dtype == CPB200_BF16 ? 1 : 2;
+  const Prec pr = prec_of(op);
+  const Slab sl = slab_for(op.cin, 1);
+  const int P = pr.P, cin = op.cin[0], bk = sl.bk;
   t->P = P;
-  a.fmt = op.act_dtype == CPB200_F16X2 ? 1u : 0u;
-  a.acc_scale = (op.acc_scale != 0.f ? op.acc_scale : 1.f);
+  a.fmt = pr.fmt; a.acc_scale = pr.acc_scale;
   a.dst_plane = (long long)op.B * op.Ho * op.Wo * op.cout;
-  const int cin = op.cin[0];
-  const int bk = (cin % 64 == 0) ? 64 : (cin % 32 == 0) ? 32 : 16;
   a.cin = cin; a.BK = bk; a.slabs = cin / bk;
-  const CUtensorMapSwizzle sw = bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-  a.swizzle_bits = bk == 64 ? 1u : bk == 32 ? 2u : 3u;
+  a.swizzle_bits = sl.layout;
   a.B = op.B; a.Ho = op.Ho; a.Wo = op.Wo;
   a.tiles_h = (op.Ho + TH - 1) / TH; a.tiles_w = (op.Wo + TW - 1) / TW;
-  int BN = 16;
-  while (BN < op.cout && BN < 256) BN <<= 1;
-  if (P == 2 && BN > 128) BN = 128;       // split operands: [hi x hi | hi x lo + lo x hi] accumulator halves need 2 * BN <= 256 columns
+  const int BN = bn_for(op.cout, P);
   t->BN = BN;
   a.n_tiles = (op.cout + BN - 1) / BN;
   a.cout = op.cout; a.cout_store = op.cout;
   a.total_tiles = op.B * a.tiles_h * a.tiles_w * a.n_tiles;
-  a.dst = op.dst; a.res = op.res; a.bias = op.bias; a.flags = op.flags;
+  a.flags = op.flags;
   a.kh = op.kh; a.kw = op.kw; a.taps = op.kh * op.kw; a.hw = TW + op.kw - 1;
   const int hh = TH + op.kh - 1;
   a.a_tx_bytes = (unsigned)(a.hw * hh * bk * 2);
@@ -322,49 +287,28 @@ void *c3_prepare(const cpb200_op &op, int *rc) {
     if (P == 2 && (a.na & 1)) --a.na;                       // streamed weights consume the planes in pairs
     int nb = (int)((budget - a.na * (size_t)a.a_stage_bytes) / a.b_stage_bytes);
     if (nb > MAX_NB) nb = MAX_NB;
-    if (nb < 2 || a.na < 2) { delete t; *rc = fail(CPB200_ERR_ARG, "tc3: tile does not fit shared memory"); return nullptr; }
+    if (nb < 2 || a.na < 2) return fail(CPB200_ERR_ARG, "tc3: tile does not fit shared memory");
     a.nb = nb;
     t->smem = a.na * (size_t)a.a_stage_bytes + nb * (size_t)a.b_stage_bytes + 1024;
   }
-  const int nsm = num_sms();
-  t->grid = a.total_tiles < nsm ? a.total_tiles : nsm;
-  const CUtensorMapDataType dt = a.fmt ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  {
-    // split activations: the lo plane follows the hi plane, i.e. a batch of 2B images
-    const cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)op.W, (cuuint64_t)op.H, (cuuint64_t)op.B * P};
-    const cuuint64_t strides[3] = {(cuuint64_t)cin * 2, (cuuint64_t)op.W * cin * 2, (cuuint64_t)op.H * op.W * cin * 2};
-    const cuuint32_t box[4] = {(cuuint32_t)bk, (cuuint32_t)a.hw, (cuuint32_t)hh, 1};
-    const cuuint32_t es[4] = {1, 1, 1, 1};
-    CUresult r = enc(&a.amap, dt, 4, const_cast<void *>(op.src[0]), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { delete t; *rc = fail(CPB200_ERR_CUDA, "tc3: cuTensorMapEncodeTiled(A) failed: %d", (int)r); return nullptr; }
-  }
-  {
-    // weights are packed slab-major [plane][tap][K-slab][cout_pad][bk] (plan.py::_pack_conv_tc): a box is one dense run
-    const int cout_pad = (op.cout + 15) / 16 * 16;
-    const cuuint64_t dims[3] = {(cuuint64_t)bk, (cuuint64_t)cout_pad, (cuuint64_t)a.taps * (cuuint64_t)a.slabs * P};
-    const cuuint64_t strides[2] = {(cuuint64_t)bk * 2, (cuuint64_t)cout_pad * bk * 2};
-    const cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)BN, 1};
-    const cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(&a.bmap, dt, 3, const_cast<void *>(op.weight), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { delete t; *rc = fail(CPB200_ERR_CUDA, "tc3: cuTensorMapEncodeTiled(B) failed: %d", (int)r); return nullptr; }
-  }
-  return t;
+  const cuuint32_t box[4] = {(cuuint32_t)bk, (cuuint32_t)a.hw, (cuuint32_t)hh, 1}, estr[4] = {1, 1, 1, 1};
+  if (int rc = encode_act_map(&a.amap, op.src[0], cin, cin, op.W, op.H, op.B, P, pr.fmt, sl.swizzle, box, estr, "tc3")) return rc;
+  if (int rc = encode_weight_map(&a.bmap, op.weight, pr.fmt, bk, (op.cout + 15) / 16 * 16, BN, (long long)a.taps * a.slabs * P,
+                                 sl.swizzle, "tc3"))
+    return rc;
+  *out = t.release();
+  return CPB200_OK;
 }
 
-void c3_release(void *h) { delete static_cast<C3Op *>(h); }
-
-// `op` supplies the pointers that may be re-bound between runs (dst / res / bias); everything else was fixed at prepare.
-int c3_run(const void *h, const cpb200_op &op, cudaStream_t st) {
-  const C3Op *t = static_cast<const C3Op *>(h);
-  C3Args args = t->args;
+int c3_run(const Prepared &p, const cpb200_op &op, cudaStream_t st) {
+  const C3Op &t = static_cast<const C3Op &>(p);
+  C3Args args = t.args;
   args.dst = op.dst; args.res = op.res; args.bias = op.bias;
 #define C3_CASE(N)                                                                                   \
-  case N: return t->P == 2 ? launch_c3<N, 2>(*t, args, st) : launch_c3<N, 1>(*t, args, st);
-  switch (t->BN) {
+  case N: return t.P == 2 ? launch_c3<N, 2>(t, args, st) : launch_c3<N, 1>(t, args, st);
+  switch (t.BN) {
     C3_CASE(16) C3_CASE(32) C3_CASE(64) C3_CASE(128)
-    case 256: if (t->P == 1) return launch_c3<256, 1>(*t, args, st); break;
+    case 256: if (t.P == 1) return launch_c3<256, 1>(t, args, st); break;
   }
 #undef C3_CASE
   return fail(CPB200_ERR_STATE, "tc3: bad BN");

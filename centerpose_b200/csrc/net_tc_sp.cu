@@ -19,12 +19,9 @@
 //   warps    0-7 two consumer warpgroups (rows 0-63 / 64-127 of the tile: wgmma + epilogue), 8-15 producers.
 //   split    P = 2 (CPB200_BF16X2 / CPB200_F16X2, tc_common.cuh): the stage ring is plane-granular — a tile occupies two
 //            consecutive stages (hi halo, lo halo), fetched as two units of the producers' load pipeline; weights sit in
-//            shared memory as [tap][hi tile | lo tile]; A_hi x W_hi goes to one accumulator array, A_hi x W_lo and
-//            A_lo x W_hi to a second one; the epilogue adds them, applies
-//            acc_scale / bias / residual / activation in fp32 and stores the hi and lo planes.
+//            shared memory as [tap][hi tile | lo tile].  A K step spans the two plane stages, so the consumers issue the
+//            split products themselves: A_hi x W_hi and A_hi x W_lo with the hi stage, A_lo x W_hi with the lo stage.
 #include "tc_common.cuh"
-
-#include <cstdlib>
 
 namespace {
 
@@ -177,11 +174,8 @@ __global__ void __launch_bounds__(SP_THREADS, 1) conv_sp_kernel(const SpArgs a) 
     // =============================== consumers: wgmma + epilogue ===============================
     const int wg = warp >> 2, tq = threadIdx.x & 127;
     const uint32_t bf = (P == 1 || a.fmt == 0) ? 1u : 0u;
-    float acc[N / 2], acc2[P == 2 ? N / 2 : 1];                 // hi x W_hi | hi x W_lo + lo x W_hi (split operands)
-#pragma unroll
-    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < (P == 2 ? N / 2 : 1); ++i) acc2[i] = 0.f;
+    float acc[N / 2], acc2[P == 2 ? N / 2 : 1];
+    acc_zero(acc, acc2);
     int stage = 0; uint32_t phase = 0;
     for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
 #pragma unroll
@@ -221,12 +215,8 @@ __global__ void __launch_bounds__(SP_THREADS, 1) conv_sp_kernel(const SpArgs a) 
         const int m = wg * 64 + frag_row(tq, j), c = frag_col(tq, j);
         const int ho = h0 + (m >> 3), wo = w0 + (m & 7);
         if (ho >= a.Ho || wo >= a.Wo) continue;
-        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
-        if constexpr (P == 2) { v0 += acc2[2 * j]; v1 += acc2[2 * j + 1]; }
-        const float f0 = P == 2 ? fmaf(v0, a.acc_scale, s_bias[c]) : v0 + s_bias[c];
-        const float f1 = P == 2 ? fmaf(v1, a.acc_scale, s_bias[c + 1]) : v1 + s_bias[c + 1];
         const size_t pix = ((size_t)n * a.Ho + ho) * a.Wo + wo;
-        store_pair16<P>(a.y, a.res, pix * N + c, a.y_plane, f0, f1, a.act, a.fmt);
+        epilogue_pair<P>(acc, acc2, j, s_bias[c], s_bias[c + 1], a.acc_scale, a.act, OUT_16, a.y, a.res, pix * N + c, a.y_plane, true, a.fmt);
       }
     }
   }
@@ -243,17 +233,12 @@ int launch_sp(const cpb200_op &op, cudaStream_t st) {
   a.tiles_h = (op.Ho + SP_TH - 1) / SP_TH; a.tiles_w = (op.Wo + SP_TW - 1) / SP_TW;
   a.total_tiles = op.B * a.tiles_h * a.tiles_w;
   a.act = op.flags & CPB_ACT_MASK;
-  a.fmt = op.act_dtype == CPB200_F16X2 ? 1u : 0u;
-  a.acc_scale = op.acc_scale != 0.f ? op.acc_scale : 1.f;
+  const Prec pr = prec_of(op);
+  a.fmt = pr.fmt; a.acc_scale = pr.acc_scale;
   a.x_plane = (long long)op.B * op.H * op.W * C;
   a.y_plane = (long long)op.B * op.Ho * op.Wo * N;
   const size_t smem = 1024 + (size_t)NSTAGE * G::STAGE_BYTES + (size_t)P * 9 * N * G::PIX_B;
-  static SmemAttrCache cache;
-  if (int rc = ensure_smem(conv_sp_kernel<C, N, S, P>, smem, cache)) return rc;
-  const int sms = tc::num_sms();
-  const int grid = a.total_tiles < sms ? a.total_tiles : sms;
-  conv_sp_kernel<C, N, S, P><<<grid, SP_THREADS, smem, st>>>(a);
-  return cpb::check_launch("conv_sp_kernel", conv_sp_kernel<C, N, S, P>);
+  return launch<conv_sp_kernel<C, N, S, P>>("conv_sp_kernel", a.total_tiles, SP_THREADS, smem, st, a);
 }
 
 template <int C, int S>
@@ -272,9 +257,7 @@ int dispatch_n(const cpb200_op &op, cudaStream_t st) {
 namespace cpb {
 
 bool sp_eligible(const cpb200_op &op) {
-  static const bool enabled = []() { const char *e = getenv("CPB200_SP"); return !(e && e[0] == '0'); }();
-  return enabled && op.type == CPB200_OP_CONV && (op.flags & CPB200_FLAG_TC) &&
-         (op.act_dtype == CPB200_BF16 || op.act_dtype == CPB200_BF16X2 || op.act_dtype == CPB200_F16X2) && op.nsrc == 1 &&
+  return op.type == CPB200_OP_CONV && tc_dtype(op.act_dtype) && op.nsrc == 1 &&
          (op.src_pitch[0] == 0 || op.src_pitch[0] == op.cin[0]) &&
          (op.cin[0] == 16 || op.cin[0] == 32) && (op.cout == 16 || op.cout == 32 || op.cout == 64) && op.kh == 3 && op.kw == 3 &&
          op.pad_h == 1 && op.pad_w == 1 && (op.stride == 1 || op.stride == 2) &&
@@ -284,7 +267,6 @@ bool sp_eligible(const cpb200_op &op) {
 }
 
 int sp_run(const cpb200_op &op, cudaStream_t st) {
-  if (!sp_eligible(op)) return fail(CPB200_ERR_ARG, "conv_sp: unsupported shape");
   if (op.cin[0] == 16) return op.stride == 1 ? dispatch_n<16, 1>(op, st) : dispatch_n<16, 2>(op, st);
   return op.stride == 1 ? dispatch_n<32, 1>(op, st) : dispatch_n<32, 2>(op, st);
 }

@@ -125,12 +125,81 @@ __device__ __forceinline__ float2 join2(uint32_t hi, uint32_t lo, uint32_t fmt) 
   return make_float2(h.x + l.x, h.y + l.y);
 }
 
-// 16-bit NHWC output of one pixel, channels (nb, nb + 1): f0 / f1 already carry bias and accumulator scale; adds the
-// residual (same layout as the output), applies the activation, stores (P = 2: hi plane at e, lo plane `plane` later).
+// ------------------------------------------------------------------------------------------------------------
+// What every wgmma kernel's consumers share: the accumulators, the K step and the epilogue.  Each kernel keeps its own
+// producers and its own pixel mapping.
+//
+// acc holds A_hi x W_hi (P = 1: A x W); acc2 holds the split operands' small cross terms (one unused register when P = 1).
+template <int R, int R2>
+__device__ __forceinline__ void acc_zero(float (&acc)[R], float (&acc2)[R2]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < R2; ++i) acc2[i] = 0.f;
+}
+
+// K step k (16 channels: +32 bytes in each descriptor) of an N-column product from shared-memory descriptors.  P = 2
+// issues A_hi x W_hi into acc, then A_hi x W_lo and A_lo x W_hi into acc2.  The cross terms share the second array because the tensor core's fp32
+// accumulator truncates (round toward zero) at every instruction, an error proportional to the accumulator's magnitude:
+// the large hi x hi sum must see as few additions as possible.  Separate arrays also keep the three products of a step
+// independent, so ptxas does not serialise them.  `first` = 0 overwrites the accumulators instead of adding to them.
+template <int N, int P>
+__device__ __forceinline__ void mma_step(float *acc, float *acc2, uint64_t a_hi, uint64_t a_lo, uint64_t w_hi, uint64_t w_lo,
+                                         int k, uint32_t first, uint32_t bf) {
+  if constexpr (P == 1) {
+    wgmma_k16<N>(acc, a_hi + 2 * k, w_hi + 2 * k, first, 1u);
+  } else {
+    wgmma_k16<N>(acc, a_hi + 2 * k, w_hi + 2 * k, first, bf);
+    wgmma_k16<N>(acc2, a_hi + 2 * k, w_lo + 2 * k, first, bf);
+    wgmma_k16<N>(acc2, a_lo + 2 * k, w_hi + 2 * k, 1u, bf);
+  }
+}
+// the same with the A fragments in registers (wgmma_rs_k16)
+template <int N, int P>
+__device__ __forceinline__ void mma_step_rs(float *acc, float *acc2, const uint32_t (&a_hi)[4], const uint32_t (&a_lo)[4],
+                                            uint64_t w_hi, uint64_t w_lo, uint32_t first, uint32_t bf) {
+  if constexpr (P == 1) {
+    wgmma_rs_k16<N>(acc, a_hi, w_hi, first, 1u);
+  } else {
+    wgmma_rs_k16<N>(acc, a_hi, w_hi, first, bf);
+    wgmma_rs_k16<N>(acc2, a_hi, w_lo, first, bf);
+    wgmma_rs_k16<N>(acc2, a_lo, w_hi, 1u, bf);
+  }
+}
+
+// Output forms of an epilogue: 16-bit NHWC (P = 2: hi and lo planes), NHWC fp32, NCHW fp32.
+enum : int { OUT_16, OUT_F32, OUT_NCHW };
+__device__ __forceinline__ int out_form(uint32_t flags) {
+  return (flags & CPB200_FLAG_OUT_NCHW_F32) ? OUT_NCHW : (flags & CPB200_FLAG_OUT_F32) ? OUT_F32 : OUT_16;
+}
+
+// Finishes channels (c, c + 1) of one output pixel from accumulator registers 2j, 2j + 1: adds acc2 (P = 2), scales by
+// acc_scale and adds the bias (P = 2: fmaf(v, acc_scale, bias), the inverse of the host's power-of-two weight scale;
+// P = 1: v + bias), adds the residual (16-bit form only; same layout as dst), applies the activation and stores element
+// e of dst.  `plane`: elements between the hi and lo planes (16-bit form) or between two channels (NCHW).  `has1`:
+// channel c + 1 exists; the fp32 forms check it, 16-bit outputs always hold whole pairs (cout % 16 == 0).
+// The activation is the multiply-by-1/6 form everywhere except NCHW fp32 in the split precisions: those are the
+// network's result maps at fp32 accuracy and take act_fn, the IEEE division of the fp32 CUDA-core kernels.  NHWC fp32
+// keeps the fast form: plan.py uses it for the DCN offset / mask maps, which have no activation.
 template <int P>
-__device__ __forceinline__ void store_pair16(void *dst, const void *res, size_t e, long long plane, float f0, float f1, uint32_t act,
-                                             uint32_t fmt) {
+__device__ __forceinline__ void epilogue_pair(const float *acc, const float *acc2, int j, float b0, float b1, float acc_scale,
+                                              uint32_t act, int form, void *dst, const void *res, size_t e, long long plane,
+                                              bool has1, uint32_t fmt) {
+  float f0 = acc[2 * j], f1 = acc[2 * j + 1];
   if constexpr (P == 2) {
+    f0 = fmaf(f0 + acc2[2 * j], acc_scale, b0); f1 = fmaf(f1 + acc2[2 * j + 1], acc_scale, b1);
+  } else {
+    f0 += b0; f1 += b1;
+  }
+  if (form == OUT_NCHW) {
+    float *o = static_cast<float *>(dst) + e;
+    o[0] = P == 2 ? cpb::act_fn(f0, act) : cpb::act_fast(f0, act);
+    if (has1) o[plane] = P == 2 ? cpb::act_fn(f1, act) : cpb::act_fast(f1, act);
+  } else if (form == OUT_F32) {
+    float *o = static_cast<float *>(dst) + e;
+    o[0] = cpb::act_fast(f0, act);
+    if (has1) o[1] = cpb::act_fast(f1, act);
+  } else if constexpr (P == 2) {
     uint16_t *o = static_cast<uint16_t *>(dst) + e;
     if (res) {
       const uint16_t *r = static_cast<const uint16_t *>(res) + e;
@@ -147,16 +216,40 @@ __device__ __forceinline__ void store_pair16(void *dst, const void *res, size_t 
       const float2 x = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162 *>(static_cast<const __nv_bfloat16 *>(res) + e)));
       f0 += x.x; f1 += x.y;
     }
-    *reinterpret_cast<__nv_bfloat162 *>(o) = __floats2bfloat162_rn(cpb::act_out<__nv_bfloat16>(f0, act), cpb::act_out<__nv_bfloat16>(f1, act));
+    *reinterpret_cast<__nv_bfloat162 *>(o) = __floats2bfloat162_rn(cpb::act_fast(f0, act), cpb::act_fast(f1, act));
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn get_encode();
 int num_sms();          // SM count of the CURRENT device (cached per device)
 int cur_device();
+
+// Activation formats the wgmma kernels take: bf16, or the split planes (bf16x2 / fp16x2).
+bool tc_dtype(int act_dtype);
+// P = 2 planes for the split precisions, fmt 1 for fp16 planes; an acc_scale of 0 is read as 1
+struct Prec { int P; uint32_t fmt; float acc_scale; };
+Prec prec_of(const cpb200_op &op);
+
+// K slab: bk = 64 / 32 / 16 channels, one 128B / 64B / 32B swizzle atom, the widest that divides every input's channel
+// count.  `layout` is the matching wgmma descriptor layout type.  PlanBuilder._tc_bk (plan.py) mirrors this choice when
+// it packs the weights.
+struct Slab { int bk; CUtensorMapSwizzle swizzle; uint32_t layout; };
+Slab slab_for(const int *cin, int nsrc);
+// N tile: the next power of two >= cout, 16..256; split operands hold two BN-column accumulator arrays, so BN <= 128.
+int bn_for(int cout, int P);
+
+// 4-D map {C, W, H, B * P} of an NHWC activation with `pitch` elements per pixel (a channel slice of a wider tensor
+// when pitch > C); split planes: the lo plane follows the hi plane of the parent tensor, i.e. a batch of 2B images.
+int encode_act_map(CUtensorMap *map, const void *src, int C, int pitch, int W, int H, int B, int P, uint32_t fmt,
+                   CUtensorMapSwizzle sw, const cuuint32_t (&box)[4], const cuuint32_t (&estr)[4], const char *what);
+// 3-D map {bk, rows, blocks} of weights packed slab-major (plan.py::_pack_conv_tc): block = [plane][tap][K slab],
+// `rows` output channels of bk each, one box = box_rows rows of one block, a dense run.
+int encode_weight_map(CUtensorMap *map, const void *w, uint32_t fmt, int bk, int rows, int box_rows, long long blocks,
+                      CUtensorMapSwizzle sw, const char *what);
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per (function, device): remember the largest value set on each device.
 constexpr int MAX_DEVICES = 64;
@@ -172,4 +265,29 @@ inline int ensure_smem(F *func, size_t smem, SmemAttrCache &cache) {
   return CPB200_OK;
 }
 
+// Launches a persistent kernel: one CTA per SM of the current device, or one per tile when there are fewer tiles.
+// The shared-memory attribute cache is per instantiation, i.e. per kernel.
+template <auto Kernel, typename Args>
+int launch(const char *name, int tiles, int threads, size_t smem, cudaStream_t st, const Args &args) {
+  static SmemAttrCache cache;
+  if (int rc = ensure_smem(Kernel, smem, cache)) return rc;
+  const int sms = num_sms();
+  Kernel<<<tiles < sms ? tiles : sms, threads, smem, st>>>(args);
+  return cpb::check_launch(name, Kernel);
+}
+
 }  // namespace tc
+
+namespace cpb {
+// Kernel families of the tensor-core ops.  cpb200_prepare_ops picks one per op and stores it behind op.tc with the
+// route's prepared state (op.tc == NULL: the CUDA-core kernels); cpb200_run_ops switches on it and
+// cpb200_release_ops deletes it.  Whatever Plan.bind can re-bind between runs is read from the live op at every run,
+// never from prepared state: dst, res and bias for every route, the DCN offset / mask tensor (aux), and src[0] for the
+// stem, which reads the network input.
+enum class Route { HEADS, STEM, SP, HALO, TAP };
+struct Prepared {
+  const Route route;
+  explicit Prepared(Route r) : route(r) {}
+  virtual ~Prepared() = default;
+};
+}  // namespace cpb

@@ -9,8 +9,6 @@ product has no CPU path and raises if the CUDA library is missing.
 """
 from __future__ import annotations
 
-import os
-
 import torch
 from torch import nn
 
@@ -152,7 +150,7 @@ class BackBoneWithHead(nn.Module):
                 return w0
 
             hc = self.head_conv
-            fuse = pb.use_tc and hc % 16 == 0 and hc <= 128 and os.environ.get("CPB200_FUSE_HEADS", "1") != "0"
+            fuse = pb.use_tc and hc % 16 == 0 and hc <= 128
             if fuse:
                 # Narrow heads (ResNet-50 / HRNet: head_conv 64): ONE 3x3 conv produces all six hidden maps: wide N tiles
                 # issue fewer MMA instructions per output than six N=64 convs, and the feature map is read once instead of

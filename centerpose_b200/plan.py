@@ -171,9 +171,9 @@ class PlanBuilder:
         self.ops: List[_PendingOp] = []
         self.keep: List[torch.Tensor] = []      # weights / biases kept alive
         self.syms: List[Sym] = []
-        # tensor-core (wgmma) path: 16-bit operands only; CPB200_TC=0 forces the SIMT kernels (bf16: debugging)
+        # tensor-core (wgmma) path: 16-bit operands only; tc=False forces the SIMT kernels (bf16: debugging)
         if tc is None:
-            tc = os.environ.get("CPB200_TC", "1") != "0"
+            tc = True
         if self.split and not tc:
             raise ValueError("split precisions run on the tensor-core path only")
         self.use_tc = bool(tc) and precision != "fp32"
@@ -296,7 +296,7 @@ class PlanBuilder:
 
     @staticmethod
     def _tc_bk(srcs) -> int:
-        """K-slab width the tensor-core kernels use for these inputs (csrc/net_tc.cu, net_tc3.cu: 64 / 32 / 16)."""
+        """K-slab width the tensor-core kernels use for these inputs (64 / 32 / 16): mirrors tc::slab_for (csrc/net_tc.cu)."""
         bk = 64
         for s in srcs:
             if s.C % 64:
@@ -366,8 +366,7 @@ class PlanBuilder:
     # ops — an "fp32 island": slower, never less precise.
     def stem(self, x: Sym, w, b, k, stride, pad, relu=True, act=None):
         co, ci = w.shape[0], w.shape[1]
-        mode = os.environ.get("CPB200_TC_STEM", "1")
-        if (self.use_tc and self.split and mode != "0" and stride == 2 and ci == 3 and k in (3, 7) and pad == k // 2
+        if (self.use_tc and self.split and stride == 2 and ci == 3 and k in (3, 7) and pad == k // 2
                 and co % 16 == 0 and x.H % 2 == 0 and x.W % 2 == 0 and x.kind == "nchw_in"
                 and os.environ.get("CPB200_S2D_STEM", "1") != "0"):
             # Stride-2 stems in split precisions (ResNet 7x7, HRNet 3x3): space-to-depth of the image (OP_S2D: 2x2 pixel
@@ -391,7 +390,7 @@ class PlanBuilder:
             return self.conv([z], w2, b.float(), stride=1, pad=p2, relu=relu, act=act)
         flags = _ACT_FLAG[act] if act else (FLAG_RELU if relu else 0)
         Ho = (x.H + 2 * pad - k) // stride + 1; Wo = (x.W + 2 * pad - k) // stride + 1
-        if (self.use_tc and mode != "0" and k == 7 and ci == 3 and pad == 3 and stride in (1, 2) and co in (16, 64)
+        if (self.use_tc and k == 7 and ci == 3 and pad == 3 and stride in (1, 2) and co in (16, 64)
                 and not (self.split and stride != 1)):
             # tensor-core stem with the im2col done in shared memory (csrc/net_stem_tc.cu); split precisions: stride 1 only
             y = self._sym(co, Ho, Wo)
@@ -544,8 +543,7 @@ class PlanBuilder:
         om_b32 = torch.zeros(32, dtype=torch.float32, device=om_b.device); om_b32[:27] = om_b.float()
         om = self.conv([x], om_w32, om_b32, stride=1, pad=1, relu=False, out="f32")
         co = w.shape[0]
-        tc = (self.use_tc and x.kind == "act" and x.C % 64 == 0 and co % 16 == 0 and 32 <= co and x.W >= 8
-              and os.environ.get("CPB200_TC_DCN", "1") != "0")
+        tc = self.use_tc and x.kind == "act" and x.C % 64 == 0 and co % 16 == 0 and 32 <= co and x.W >= 8
         island = self.split and not tc
         xin = self._to_f32(x) if island else x
         y = self._sym(co, x.H, x.W, "actf32" if island else "act")

@@ -345,8 +345,8 @@ typedef struct cpb200_head {
   float *dst;                /* NCHW fp32 (B, cout, Ho, Wo)                                                     */
 } cpb200_head;
 
-/* Validate the program and build device-side descriptors (TMA tensor maps) for ops flagged
- * CPB200_FLAG_TC.  Must be called once after the INPUT activation / weight pointers in `ops` are final (they are
+/* Validate the program, choose the kernel of every op flagged CPB200_FLAG_TC and build its device-side descriptors
+ * (TMA tensor maps).  Must be called once after the INPUT activation / weight pointers in `ops` are final (they are
  * baked into the tensor maps).  `dst`, `res`, `bias`, `aux` and the STEM op's `src[0]` are read from the op at every
  * cpb200_run_ops call and may be re-pointed between runs (the model binds fresh output tensors per forward). */
 int cpb200_prepare_ops(cpb200_op *ops, int n);

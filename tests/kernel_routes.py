@@ -77,17 +77,17 @@ def k_elt(name, fmt, vec=None):
 # ------------------------------------------------------------------------------------------------------ route table
 def _routes():
     r = {}
-    tc = "net_tc.cu tc_prepare_op (not c3_eligible / sp_eligible; PlanBuilder._tc_ok: Wo >= 8); BN = next pow2 >= cout, " \
-         "<= 256, split <= 128; tc_run_op switch"
+    tc = "net.cu route TAP: net_tc.cu tap_prepare (not c3_eligible / sp_eligible; PlanBuilder._tc_ok: Wo >= 8); BN = tc::bn_for: " \
+         "next pow2 >= cout, <= 256, split <= 128; tap_run switch"
     for bn in (16, 32, 64, 128):
         for p in (1, 2):
             r[k_tc(bn, p)] = tc
     r[k_tc(256, 1)] = tc
-    dcn = "net_tc.cu tc_prepare_op DCN branch (PlanBuilder.dcn: C % 64 == 0, cout % 16 == 0, cout >= 32, W >= 8); " \
+    dcn = "net.cu route TAP: net_tc.cu tap_prepare DCN branch (PlanBuilder.dcn: C % 64 == 0, cout % 16 == 0, cout >= 32, W >= 8); " \
           "BN <= 128 / P"
     for bn, p in ((32, 1), (64, 1), (128, 1), (32, 2), (64, 2)):
         r[k_tc(bn, p, True)] = dcn
-    c3 = "net_tc3.cu c3_eligible (3x3 / 5x5 / 7x1 / 1x7, stride 1, same padding, one dense input, Ho, Wo >= 8) + c3_run switch"
+    c3 = "net.cu route HALO: net_tc3.cu c3_eligible (3x3 / 5x5 / 7x1 / 1x7, stride 1, same padding, one dense input, Ho, Wo >= 8) + c3_run switch"
     for bn in (16, 32, 64, 128):
         for p in (1, 2):
             r[k_c3(bn, p)] = c3
@@ -96,13 +96,13 @@ def _routes():
         for n in (16, 32, 64):
             for s in (1, 2):
                 for p in (1, 2):
-                    r[k_sp(c, n, s, p)] = "net_tc_sp.cu sp_eligible (3x3 pad 1, cin 16 / 32, cout 16 / 32 / 64, Wo >= 8) + dispatch_n"
+                    r[k_sp(c, n, s, p)] = "net.cu route SP: net_tc_sp.cu sp_eligible (3x3 pad 1, cin 16 / 32, cout 16 / 32 / 64, Wo >= 8) + dispatch_n"
     for n in (16, 64):
-        r[f"stem_tc_kernel<{n},2>"] = "net_stem_tc.cu stem_tc_eligible + stem_tc_run (bf16, stride 2)"
+        r[f"stem_tc_kernel<{n},2>"] = "net.cu route STEM: net_stem_tc.cu stem_tc_eligible + stem_tc_run (bf16, stride 2)"
         for p in (1, 2):
-            r[f"stem_tc_h_kernel<{n},{p}>"] = "net_stem_tc.cu stem_tc_eligible + stem_tc_run (stride 1)"
+            r[f"stem_tc_h_kernel<{n},{p}>"] = "net.cu route STEM: net_stem_tc.cu stem_tc_eligible + stem_tc_run (stride 1)"
     for p in (1, 2):
-        r[f"heads_tc_kernel<{p}>"] = "net_heads.cu heads_prepare / heads_run (plan.py Plan._fuse_heads)"
+        r[f"heads_tc_kernel<{p}>"] = "net.cu route HEADS: net_heads.cu heads_prepare / heads_run (plan.py Plan._fuse_heads)"
     for t in ("float", "bf16"):
         for co in (16, 32, 64):
             for d in (False, True):
