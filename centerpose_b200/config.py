@@ -43,6 +43,8 @@ _ARCH = {
     "mobilenetv3": (256, 24),  # experiments/mobilenetv3_512x512.yaml:28-29
     "hrnet": (64, 32),        # experiments/hrnet_w32_512.yaml:62,73 (MODEL.EXTRA defaults to W32, archs/hrnet.py)
     "hardnet": (256, 48),     # experiments/hardnet_512x512.yaml:24,29
+    "mobilenetv2": (256, 24),  # experiments/mobilenetv2_512x512.yaml:28-29
+    "ghostnet": (256, 160),   # experiments/ghost_net.yaml:28-29
 }
 
 _DEFAULT = {

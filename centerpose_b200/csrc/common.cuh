@@ -48,14 +48,20 @@ inline int check_launch(const char *what, K *kernel) {
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
-#define CPB_ACT_MASK (CPB200_FLAG_RELU | CPB200_FLAG_HSWISH | CPB200_FLAG_HSIGMOID)
-// Epilogue non-linearity selected by the op flags (at most one of RELU / HSWISH / HSIGMOID).  hswish and
-// hsigmoid keep the reference's operation order x * relu6(x + 3) / 6 (mobilenetv3.py:84-93).
+#define CPB_ACT_MASK (CPB200_FLAG_RELU | CPB200_FLAG_HSWISH | CPB200_FLAG_HSIGMOID | CPB200_FLAG_RELU6 | CPB200_FLAG_CLIP01)
+// Epilogue non-linearity selected by the op flags (at most one of RELU / HSWISH / HSIGMOID / RELU6 / CLIP01).  hswish
+// and hsigmoid keep the reference's operation order x * relu6(x + 3) / 6 (mobilenetv3.py:84-93).  ReLU6 and the hard
+// [0, 1] clamp take the same clamp without the + 3 and the / 6: min(max(x, 0), 6 or 1).  Their result is exact in every
+// format, so the split epilogues clamp before the hi / lo re-split and a clamped 6 or 1 has lo == 0.  After the ReLU and
+// identity tests the code is straight-line (selects on the flag, no further branch), as it was for hswish / hsigmoid
+// alone: the tensor-core epilogues inline it for every accumulator pair.
 __device__ __forceinline__ float act_fn(float v, uint32_t act) {
   if (act == CPB200_FLAG_RELU) return fmaxf(v, 0.f);
   if (act == 0u) return v;
-  const float r = fminf(fmaxf(v + 3.f, 0.f), 6.f);
-  return act == CPB200_FLAG_HSWISH ? v * r / 6.f : r / 6.f;
+  const bool hs = act < CPB200_FLAG_RELU6;                     // HSWISH / HSIGMOID
+  const float c = fminf(fmaxf(hs ? v + 3.f : v, 0.f), act == CPB200_FLAG_CLIP01 ? 1.f : 6.f);
+  const float n = act == CPB200_FLAG_HSWISH ? v * c : c;
+  return hs ? n / 6.f : c;
 }
 // bf16-output variant: multiply by 1/6 instead of the IEEE division (differs from act_fn by <= 1 ulp of fp32,
 // far below the bf16 rounding that follows).  The division costs 20+ instructions per element, enough to make the
@@ -66,19 +72,15 @@ __device__ __forceinline__ float act_fn(float v, uint32_t act) {
 __device__ __forceinline__ float act_fast(float v, uint32_t act) {
   if (act == CPB200_FLAG_RELU) return fmaxf(v, 0.f);
   if (act == 0u) return v;
-  const float r = fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f);
+  const bool hs = act < CPB200_FLAG_RELU6;
+  const float c = fminf(fmaxf(hs ? v + 3.f : v, 0.f), act == CPB200_FLAG_CLIP01 ? 1.f : 6.f);
+  const float r = hs ? c * (1.f / 6.f) : c;
   return act == CPB200_FLAG_HSWISH ? v * r : r;
 }
 template <typename T>
 __device__ __forceinline__ float act_out(float v, uint32_t act) {
-  if constexpr (sizeof(T) == 4) {
-    return act_fn(v, act);
-  } else {
-    if (act == CPB200_FLAG_RELU) return fmaxf(v, 0.f);
-    if (act == 0u) return v;
-    const float r = fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f);
-    return act == CPB200_FLAG_HSWISH ? v * r : r;
-  }
+  if constexpr (sizeof(T) == 4) return act_fn(v, act);
+  else return act_fast(v, act);
 }
 
 }  // namespace cpb

@@ -8,7 +8,8 @@
 //   STEM          pose_dla_dcn.py:226-231 base_layer (7x7, 3->16) on the NCHW fp32 image
 //   MAXPOOL       pose_dla_dcn.py:196 nn.MaxPool2d(stride), msra_resnet.py:126
 //   DWDECONV_ADD  pose_dla_dcn.py:361-364,374-377: depthwise ConvTranspose2d(2f, stride f,
-//                 pad f/2) followed by `+ layers[i-1]`
+//                 pad f/2) followed by `+ layers[i-1]`; with a bias, mobilenetv2.py:174-179:
+//                 relu(bn(ConvTranspose2d(2, stride 2))) + the lateral conv
 //   DCN           DCNv2/dcn_v2.py:117-127 + DCNv2/src/cuda/dcn_v2_im2col_cuda.cu:25-54,125-195
 //                 + dcn_v2_cuda.cu:123-163: sigmoid(mask) * bilinear sample, then the GEMM —
 //                 fused here: the sampled im2col tile lives in shared memory only (the
@@ -158,6 +159,14 @@ template <typename PO> __device__ __forceinline__ float act_io(float v, uint32_t
   if constexpr (std::is_same<PO, float *>::value) return cpb::act_fn(v, act);
   else return cpb::act_fast(v, act);
 }
+template <typename PO> __device__ __forceinline__ float4 act4(float4 v, uint32_t act) {
+  return make_float4(act_io<PO>(v.x, act), act_io<PO>(v.y, act), act_io<PO>(v.z, act), act_io<PO>(v.w, act));
+}
+template <typename PO> __device__ __forceinline__ Vf<4> vact(Vf<4> v, uint32_t act) { return {act4<PO>(v.a, act)}; }
+template <typename PO> __device__ __forceinline__ Vf<8> vact(Vf<8> v, uint32_t act) { return {act4<PO>(v.a, act), act4<PO>(v.b, act)}; }
+__device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
+__device__ __forceinline__ Vf<4> vadd(Vf<4> a, Vf<4> b) { return {add4(a.a, b.a)}; }
+__device__ __forceinline__ Vf<8> vadd(Vf<8> a, Vf<8> b) { return {add4(a.a, b.a), add4(a.b, b.b)}; }
 
 struct ConvArgs {
   const void *src[4];
@@ -480,12 +489,15 @@ __global__ void maxpool_kernel(PI x, PO y, int B, int H, int W, int C, int Ho, i
 
 // ---- depthwise ConvTranspose2d(k=2f, stride f, pad f/2) + skip add, NHWC ----
 // out[b,ho,wo,c] = skip[b,ho,wo,c] + sum_{kh,kw : (ho+p-kh)%f==0, (wo+p-kw)%f==0} x[b,(ho+p-kh)/f,(wo+p-kw)/f,c] * w[kh,kw,c]
+// With a bias (MobileNetV2 IDAUp: k 2, stride 2, pad 0, folded BN + ReLU, mobilenetv2.py:162-183) the sum starts from
+// the bias, takes the activation, and the skip is added last: out = skip + act(bias + sum ...).
 // One CTA = one output row (b, ho); thread = (wo, group of VEC channels).  The k*k*C filter taps are read through the
 // read-only cache, so any filter size is accepted.  No integer division in the inner loop when f and C / VEC are powers
 // of two (lf = log2 f, lcv = log2(C / VEC), or -1 -> generic division).
 template <int VEC, typename PI, typename PO>
-__global__ void __launch_bounds__(256) dwdeconv_add_kernel(PI x, PI skip, PO y, const float *__restrict__ w, int H, int W, int C,
-                                                           int Ho, int Wo, int k, int f, int pad, int lf, int lcv) {
+__global__ void __launch_bounds__(256) dwdeconv_add_kernel(PI x, PI skip, PO y, const float *__restrict__ w,
+                                                           const float *__restrict__ bias, int H, int W, int C, int Ho, int Wo,
+                                                           int k, int f, int pad, int lf, int lcv, uint32_t act) {
   const int CV = C / VEC;
   const int b = blockIdx.x / Ho, ho = blockIdx.x % Ho;
   const int kh0 = (ho + pad) % f;
@@ -494,7 +506,7 @@ __global__ void __launch_bounds__(256) dwdeconv_add_kernel(PI x, PI skip, PO y, 
   for (int i = threadIdx.x; i < Wo * CV; i += blockDim.x) {
     const int wo = fast ? (i >> lcv) : (i / CV), cv = i - wo * CV;
     const size_t opix = (((size_t)b * Ho + ho) * Wo + wo) * C + cv * VEC;
-    Vf<VEC> acc = skip ? io_ldv<VEC>(skip + opix) : Vf<VEC>{};
+    Vf<VEC> acc = bias ? ld_taps<VEC>(bias + cv * VEC) : skip ? io_ldv<VEC>(skip + opix) : Vf<VEC>{};
     const int kw0 = fast ? ((wo + pad) & (f - 1)) : ((wo + pad) % f);
     for (int khh = kh0; khh < k; khh += f) {
       const int hn = ho + pad - khh;
@@ -506,6 +518,10 @@ __global__ void __launch_bounds__(256) dwdeconv_add_kernel(PI x, PI skip, PO y, 
         if (wn < 0 || wi >= W) continue;
         acc = vfma(io_ldv<VEC>(xb + ((size_t)hi * W + wi) * C + cv * VEC), ld_taps<VEC>(w + (size_t)(khh * k + kww) * C + cv * VEC), acc);
       }
+    }
+    if (bias) {
+      acc = vact<PO>(acc, act);
+      if (skip) acc = vadd(acc, io_ldv<VEC>(skip + opix));
     }
     io_stv(y + opix, acc);
   }
@@ -968,16 +984,17 @@ int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
     }
     case CPB200_OP_DWDECONV_ADD: {
       if (C % VEC || op.stride < 1) return cpb::fail(CPB200_ERR_ARG, "dwdeconv: needs C %% %d == 0 and stride >= 1", VEC);
+      if (act && !op.bias) return cpb::fail(CPB200_ERR_ARG, "dwdeconv: an activation needs the bias form");
       const int lf = ilog2(op.stride), CV = C / VEC_FAST, lcv = C % VEC_FAST ? -1 : ilog2(CV);
-      // the fast kernel's shapes: k == 2f, f and C / VEC_FAST powers of two, and each CTA's 256 threads cover whole
-      // output pixels of one column parity class
-      if (lf >= 0 && lcv >= 0 && op.kh == 2 * op.stride && CV <= 256 && (256 / CV) % op.stride == 0) {
+      // the fast kernel's shapes: no bias, k == 2f, f and C / VEC_FAST powers of two, and each CTA's 256 threads cover
+      // whole output pixels of one column parity class
+      if (!op.bias && lf >= 0 && lcv >= 0 && op.kh == 2 * op.stride && CV <= 256 && (256 / CV) % op.stride == 0) {
         dwdeconv_add_fast_kernel<VEC_FAST, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.H, op.W, C, op.Ho,
             op.Wo, op.kh, op.stride, op.pad_h, lf, lcv);
         return cpb::check_launch("dwdeconv_add_fast_kernel", dwdeconv_add_fast_kernel<VEC_FAST, PI, PO>);
       }
-      dwdeconv_add_kernel<VEC, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.H, op.W, C, op.Ho, op.Wo,
-          op.kh, op.stride, op.pad_h, lf, ilog2(C / VEC));
+      dwdeconv_add_kernel<VEC, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.bias, op.H, op.W, C, op.Ho,
+          op.Wo, op.kh, op.stride, op.pad_h, lf, ilog2(C / VEC), act);
       return cpb::check_launch("dwdeconv_add_kernel", dwdeconv_add_kernel<VEC, PI, PO>);
     }
     case CPB200_OP_DWCONV: {

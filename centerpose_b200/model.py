@@ -39,6 +39,16 @@ def _hardnet_arch():
     return _hd
 
 
+def _mobilenetv2_arch():
+    from .archs import mobilenetv2 as _mb2
+    return _mb2
+
+
+def _ghostnet_arch():
+    from .archs import ghostnet as _gh
+    return _gh
+
+
 _backbone_factory = {
     # arch name -> (module with build_params(cfg)/lower(), feature channels or None = ask the module)   model.py:24-38
     "dla": lambda n: (_dla, 64) if n == 34 else None,
@@ -46,6 +56,9 @@ _backbone_factory = {
     "hrnet": lambda n: (_hrnet_arch(), None),
     "mobilenetv3": lambda n: (_mobilenet_arch(), 24),
     "hardnet": lambda n: (_hardnet_arch(), 48) if n == 0 else None,
+    # both ignore the _N suffix, as the reference does (mobilenetv2.py:256 always builds width 0.5, ghost_net.py:198-200)
+    "mobilenetv2": lambda n: (_mobilenetv2_arch(), 24),
+    "ghostnet": lambda n: (_ghostnet_arch(), 160),
 }
 
 
@@ -74,7 +87,7 @@ class BackBoneWithHead(nn.Module):
         arch_name = arch[:arch.find("_")] if "_" in arch else arch
         if arch_name not in _backbone_factory or _backbone_factory[arch_name](num_layers) is None:
             raise KeyError(f"centerpose_b200: backbone {arch!r} is not implemented "
-                           f"(available: dla_34, res_50, hrnet, mobilenetv3, hardnet)")
+                           f"(available: dla_34, res_50, hrnet, mobilenetv3, hardnet, mobilenetv2, ghostnet)")
         self._arch_mod, feat_c = _backbone_factory[arch_name](num_layers)
         if feat_c is None:
             feat_c = self._arch_mod.feature_channels(cfg)

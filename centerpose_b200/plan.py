@@ -28,7 +28,9 @@ OP_CONV, OP_STEM, OP_MAXPOOL, OP_DWDECONV_ADD, OP_DCN, OP_UPSAMPLE_ADD = 1, 2, 3
 OP_DWCONV, OP_AVGPOOL, OP_SCALE_ADD, OP_CONVERT, OP_S2D = 8, 9, 10, 11, 12
 OP_AVGPOOL2, OP_RESIZE_BILINEAR, OP_HEADS = 13, 14, 15
 FLAG_RELU, FLAG_OUT_NCHW_F32, FLAG_OUT_F32, FLAG_TC, FLAG_HSWISH, FLAG_HSIGMOID, FLAG_TO_F32 = 1, 2, 4, 8, 16, 32, 64
-_ACT_FLAG = {None: 0, "relu": FLAG_RELU, "hswish": FLAG_HSWISH, "hsigmoid": FLAG_HSIGMOID}
+FLAG_RELU6, FLAG_CLIP01 = 128, 256
+_ACT_FLAG = {None: 0, "relu": FLAG_RELU, "hswish": FLAG_HSWISH, "hsigmoid": FLAG_HSIGMOID, "relu6": FLAG_RELU6,
+             "clip01": FLAG_CLIP01}
 F32, BF16, BF16X2, F16X2 = 0, 1, 2, 3
 PRECISIONS = {"fp32": F32, "bf16": BF16, "bf16x2": BF16X2, "fp16x2": F16X2}
 BN_EPS = 1e-5
@@ -145,14 +147,14 @@ class _PendingOp:
         self.__dict__.update(kw)
 
 
-def fold_bn(w: torch.Tensor, b: Optional[torch.Tensor], bn: Optional[dict]):
-    """conv weight (Co,Ci,kh,kw) [+bias] followed by eval BatchNorm -> equivalent weight/bias."""
+def fold_bn(w: torch.Tensor, b: Optional[torch.Tensor], bn: Optional[dict], eps: float = BN_EPS):
+    """conv weight (Co,Ci,kh,kw) [+bias] followed by eval BatchNorm (epsilon ``eps``) -> equivalent weight/bias."""
     w = w.float()
     co = w.shape[0]
     b = torch.zeros(co, device=w.device) if b is None else b.float()
     if bn is None:
         return w, b
-    scale = bn["weight"].float() / torch.sqrt(bn["running_var"].float() + BN_EPS)
+    scale = bn["weight"].float() / torch.sqrt(bn["running_var"].float() + eps)
     return w * scale.view(-1, 1, 1, 1), (b - bn["running_mean"].float()) * scale + bn["bias"].float()
 
 
@@ -422,7 +424,7 @@ class PlanBuilder:
             Hd, Wd, sy, sx, oy, ox = Ho, Wo, 1, 1, 0, 0
         else:
             Hd, Wd, sy, sx, oy, ox, Ho, Wo = out_map
-        flags = _ACT_FLAG[act] if act else (FLAG_RELU if relu else 0)     # act: 'relu' | 'hswish' | 'hsigmoid'
+        flags = _ACT_FLAG[act] if act else (FLAG_RELU if relu else 0)     # act: a key of _ACT_FLAG
         tc = self._tc_ok(srcs, co, kh, kw, stride, out, out_map, Wo)
         island = self.split and not tc                                     # fp32 island (see above)
         if island:
@@ -491,14 +493,18 @@ class PlanBuilder:
         return self._eltwise(_PendingOp(type=OP_MAXPOOL, flags=0, k=(k, k), stride=stride, pad=(pad, pad),
                                         weight=None, bias=None, cout=x.C), x, x.C, Ho, Wo)
 
-    def up_add(self, x: Sym, skip: Optional[Sym], w):
-        """depthwise ConvTranspose2d weight (C,1,2f,2f), stride f, pad f//2, + skip."""
+    def up_add(self, x: Sym, skip: Optional[Sym], w, *, b=None, act=None, stride=None, pad=None):
+        """depthwise ConvTranspose2d weight (C,1,2f,2f), stride f, pad f//2, + skip.
+        With a BN-folded bias ``b`` (C): act(deconv + b) + skip, and ``stride`` / ``pad`` may be given (MobileNetV2's
+        IDAUp: k 2, stride 2, pad 0, ReLU, mobilenetv2.py:162-183).  Without one, ``act`` must be None."""
         C, _, k, _ = w.shape
-        f = k // 2
-        Ho = (x.H - 1) * f - 2 * (f // 2) + k; Wo = (x.W - 1) * f - 2 * (f // 2) + k
+        f = k // 2 if stride is None else stride
+        p = f // 2 if pad is None else pad
+        assert b is not None or act is None, "an activation needs the bias form"
+        Ho = (x.H - 1) * f - 2 * p + k; Wo = (x.W - 1) * f - 2 * p + k
         wp = self._dev(w.float().reshape(C, k * k).t())          # [k*k][C]
-        return self._eltwise(_PendingOp(type=OP_DWDECONV_ADD, flags=0, k=(k, k), stride=f, pad=(f // 2, f // 2),
-                                        weight=wp, bias=None, cout=C), x, C, Ho, Wo, [skip])
+        return self._eltwise(_PendingOp(type=OP_DWDECONV_ADD, flags=_ACT_FLAG[act], k=(k, k), stride=f, pad=(p, p),
+                                        weight=wp, bias=None if b is None else self._dev(b), cout=C), x, C, Ho, Wo, [skip])
 
     def dwconv(self, x: Sym, w, b, stride=1, act=None):
         """depthwise conv, w (C,1,k,k) BN-folded, pad k//2   (mobilenetv3.py:124-127)."""

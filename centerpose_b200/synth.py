@@ -12,7 +12,9 @@ heat-map is constant to ~1e-6 (every cell ties) and the deformable sampling path
 exercised.  This recipe keeps the architecture and shapes and only changes the VALUES:
 
   * every 4-D conv weight        ~ N(0, gain/sqrt(fan_in)), gain sqrt(2) (ReLU-preserving)
-  * depthwise deconv ``up_*``    bilinear kernel (``pose_dla_dcn.py:324-333`` formula) x U(0.8,1.2)
+  * depthwise deconv ``up_*``    bilinear kernel (``pose_dla_dcn.py:324-333`` formula) x U(0.8,1.2); a 2x2 kernel
+                                 (stride 2: no overlap) is all ones x U(0.8,1.2)
+  * ``nn.Linear`` weight         ~ N(0, 2/fan_in)
   * ``conv_offset_mask``         weight ~ N(0, 0.05/sqrt(fan_in)), bias ~ N(0, 0.5): every tap samples at a
                                  fractional position (|offset| ~ 0.5 px from the bias, mask != 0.5) with a small
                                  data-dependent part.  Measured (float64 oracle): with weight gain 0.7 the
@@ -22,8 +24,8 @@ exercised.  This recipe keeps the architecture and shapes and only changes the V
                                  amplification is 1.7 and fp32-vs-fp64 noise is 2e-6.  Large data-dependent
                                  offsets (gain 1.5, many samples out of bounds) are covered at op level
                                  (tests/test_net_gpu.py::test_dcn_op_matches_oracle).
-  * BatchNorm                    weight ~ U(0.5,1.5) (U(0.1,0.3) for a bottleneck's last ``bn3`` and an HRNet branch
-                                 block's last ``bn2``; U(0.2,0.6) inside HRNet ``fuse_layers``; U(0.4,0.8) for a
+  * BatchNorm                    weight ~ U(0.5,1.5) (U(0.1,0.3) for a bottleneck's last ``bn3``, an HRNet branch
+                                 block's last ``bn2`` and a Ghost bottleneck's second ghost module; U(0.2,0.6) inside HRNet ``fuse_layers``; U(0.4,0.8) for a
                                  MobileNetV3 block's projection ``bn3``), bias ~ N(0,0.1),
                                  mean ~ N(0,0.1), var ~ U(0.5,1.5)
   * conv / DCN biases            ~ N(0, 0.1)
@@ -80,7 +82,10 @@ def conditioned_state_dict(template: "OrderedDict[str, torch.Tensor]", seed: int
                     # MobileNetV3 blocks: bn3 is the linear-bottleneck projection, not a damped residual branch;
                     # U(0.4,0.8) keeps the 15 blocks' activations O(1..25) (0.3-0.6 decays to 1e-1, 0.5-1.0 explodes)
                     new[k] = rand(shape, 0.4, 0.8) if k.endswith(".bn3.weight") else rand(shape, 0.5, 1.5)
-                elif k.endswith(".bn3.weight") or (".branches." in k and k.endswith(".bn2.weight")):
+                elif k.endswith(".bn3.weight") or (".branches." in k and k.endswith(".bn2.weight")) \
+                        or ".conv.3.primary_conv.1." in k or ".conv.3.cheap_operation.1." in k:
+                    # (GhostNet: the residual branch ends in a ghost module's two BNs; undamped, the 16 bottlenecks
+                    # grow the features to ~1e7)
                     new[k] = rand(shape, 0.1, 0.3)
                 elif ".fuse_layers." in k:                         # HRNet cross-resolution terms: y_i = sum_j f_ij(x_j)
                     new[k] = rand(shape, 0.2, 0.6)
@@ -93,7 +98,9 @@ def conditioned_state_dict(template: "OrderedDict[str, torch.Tensor]", seed: int
             continue
         if v.dim() == 4:
             if ".up_" in k and shape[1] == 1:                     # depthwise ConvTranspose2d
-                base = _bilinear_kernel(shape[2]).view(1, 1, shape[2], shape[3])
+                # k = 2 (stride 2, MobileNetV2's IDAUp): every output reads one tap, so every tap carries weight (the
+                # bilinear formula would give the (0, 0) tap only)
+                base = (torch.ones(shape[2], shape[3]) if shape[2] == 2 else _bilinear_kernel(shape[2])).view(1, 1, shape[2], shape[3])
                 new[k] = base * rand(shape, 0.8, 1.2)
                 continue
             if "deconv_layers" in k:                              # dense ConvTranspose2d (Cin,Cout,k,k)
@@ -108,7 +115,10 @@ def conditioned_state_dict(template: "OrderedDict[str, torch.Tensor]", seed: int
             else:
                 new[k] = randn(shape) * math.sqrt(2.0 / fan_in)
             continue
-        if v.dim() == 1:                                          # conv / DCN bias
+        if v.dim() == 2:                                          # nn.Linear (GhostNet's SE): ReLU-preserving gain
+            new[k] = randn(shape) * math.sqrt(2.0 / shape[1])
+            continue
+        if v.dim() == 1:                                          # conv / DCN / Linear bias
             if "conv_offset_mask" in k:
                 new[k] = 0.5 * randn(shape)
             elif k.startswith("head_model.") and k.endswith(".2.bias"):

@@ -256,7 +256,11 @@ enum cpb200_op_type {
                                 the arithmetic runs on wgmma (weight = pre-swizzled operand image, plan.py)     */
   CPB200_OP_MAXPOOL = 3,     /* k x k / stride s / pad p max-pool, NHWC                                     */
   CPB200_OP_DWDECONV_ADD = 4,/* depthwise ConvTranspose2d(k=2f,s=f,p=f/2) (+ skip add), NHWC  (IDAUp up_*);
-                                src[0], aux (the skip) and dst must be 16-byte aligned (16-byte vector accesses)  */
+                                src[0], aux (the skip) and dst must be 16-byte aligned (16-byte vector accesses).
+                                With a non-NULL `bias` (fp32 [C]): dst = act(deconv(src[0]) + bias) (+ skip), the
+                                activation from the flags, for any kernel size k = kh, stride and pad_h (MobileNetV2
+                                IDAUp: k 2, stride 2, pad 0, folded BN + ReLU, then + the lateral conv,
+                                mobilenetv2.py:162-183).  Without a bias the activation flags must be 0.          */
   CPB200_OP_DCN = 5,         /* modulated deformable 3x3 conv (DCNv2 forward) (+bias)(+ReLU)                */
   /* 6 is retired (a horizontal-tap gather for the stem); the number is not reused */
   CPB200_OP_UPSAMPLE_ADD = 7,/* nearest-neighbour upsample x `stride` (power of two) of src[0] (+ aux skip add)(+ReLU),
@@ -302,6 +306,8 @@ enum cpb200_op_type {
 #define CPB200_FLAG_HSWISH 16u       /* x * relu6(x + 3) / 6 in the epilogue (mobilenetv3.py:84-87)   */
 #define CPB200_FLAG_HSIGMOID 32u     /* relu6(x + 3) / 6 in the epilogue     (mobilenetv3.py:90-93)   */
 #define CPB200_FLAG_TO_F32 64u       /* CPB200_OP_CONVERT direction: split planes -> fp32                    */
+#define CPB200_FLAG_RELU6 128u       /* min(max(x, 0), 6) in the epilogue (MobileNetV2 ConvBNReLU, mobilenetv2.py:34-41) */
+#define CPB200_FLAG_CLIP01 256u      /* min(max(x, 0), 1) in the epilogue (GhostNet SELayer's clamp, ghost_net.py:43)    */
 
 typedef struct cpb200_op {
   int32_t type;              /* enum cpb200_op_type */
