@@ -16,157 +16,10 @@
 //                 reference round-trips a (B, 9C, HW) fp32 `columns` buffer through HBM).
 //   AVGPOOL2      hardnet.py:141 nn.AvgPool2d(2, 2)
 //   RESIZE_BILINEAR  hardnet.py:95-100 F.interpolate(bilinear, align_corners=True)
-#include "common.cuh"
-#include <cuda_fp16.h>
+#include "simt_io.cuh"
 #include <algorithm>
-#include <type_traits>
 
 namespace {
-
-using bf16 = __nv_bfloat16;
-
-template <typename T> struct Act;
-template <> struct Act<float> {
-  __device__ static float4 ld4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
-  __device__ static float ld(const float *p) { return __ldg(p); }
-  __device__ static void st4(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
-  __device__ static void st(float *p, float v) { *p = v; }
-};
-template <> struct Act<bf16> {
-  __device__ static float4 ld4(const bf16 *p) {
-    uint2 r = __ldg(reinterpret_cast<const uint2 *>(p));
-    float2 a = __bfloat1622float2(*reinterpret_cast<__nv_bfloat162 *>(&r.x));
-    float2 b = __bfloat1622float2(*reinterpret_cast<__nv_bfloat162 *>(&r.y));
-    return make_float4(a.x, a.y, b.x, b.y);
-  }
-  __device__ static float ld(const bf16 *p) { return __bfloat162float(*p); }
-  __device__ static void st4(bf16 *p, float4 v) {
-    __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-    uint2 r; r.x = *reinterpret_cast<unsigned *>(&a); r.y = *reinterpret_cast<unsigned *>(&b);
-    *reinterpret_cast<uint2 *>(p) = r;
-  }
-  __device__ static void st(bf16 *p, float v) { *p = __float2bfloat16_rn(v); }
-};
-
-// ------------------------------------------------------------------------------------------------------------
-// Split-operand activations (CPB200_BF16X2 / CPB200_F16X2): a value is hi + lo, two 16-bit planes `plane` elements apart
-// (include/centerpose_b200.h).  hi + lo is exact in fp32 and split(hi + lo) reproduces the value exactly, so max-pooling
-// and copies are lossless; arithmetic happens in fp32 and the result is re-split.
-struct Sp16 {
-  __device__ static float2 up(uint32_t v, uint32_t fmt) {
-    if (fmt) return __half22float2(*reinterpret_cast<const __half2 *>(&v));
-    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&v));
-  }
-  __device__ static float4 ld4(const uint16_t *p, size_t plane, uint32_t fmt) {
-    const uint2 h = __ldg(reinterpret_cast<const uint2 *>(p)), l = __ldg(reinterpret_cast<const uint2 *>(p + plane));
-    const float2 h0 = up(h.x, fmt), h1 = up(h.y, fmt), l0 = up(l.x, fmt), l1 = up(l.y, fmt);
-    return make_float4(h0.x + l0.x, h0.y + l0.y, h1.x + l1.x, h1.y + l1.y);
-  }
-  __device__ static void split2(float a, float b, uint32_t fmt, uint32_t &hi, uint32_t &lo) {
-    if (fmt) {
-      a = fminf(fmaxf(a, -65504.f), 65504.f); b = fminf(fmaxf(b, -65504.f), 65504.f);
-      const __half2 h = __floats2half2_rn(a, b);
-      const float2 hf = __half22float2(h);
-      const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-      hi = *reinterpret_cast<const uint32_t *>(&h); lo = *reinterpret_cast<const uint32_t *>(&l);
-    } else {
-      const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-      const float2 hf = __bfloat1622float2(h);
-      const __nv_bfloat162 l = __floats2bfloat162_rn(a - hf.x, b - hf.y);
-      hi = *reinterpret_cast<const uint32_t *>(&h); lo = *reinterpret_cast<const uint32_t *>(&l);
-    }
-  }
-  __device__ static void st4(uint16_t *p, size_t plane, uint32_t fmt, float4 v) {
-    uint2 h, l;
-    split2(v.x, v.y, fmt, h.x, l.x); split2(v.z, v.w, fmt, h.y, l.y);
-    *reinterpret_cast<uint2 *>(p) = h;
-    *reinterpret_cast<uint2 *>(p + plane) = l;
-  }
-};
-
-
-// Pointer-like handles of split activations, so the element-wise kernels below take fp32, bf16 or split tensors on
-// either side through the same source: `p + n` advances both planes, io_ld4 joins hi + lo, io_st4 re-splits.
-// `p + n` is force-inlined: outlined (NVVM -O1), it returns the handle through the stack and stores through it become
-// generic instead of global.
-struct SpC {
-  const uint16_t *p; size_t plane; uint32_t fmt;
-  __host__ __device__ __forceinline__ SpC operator+(size_t n) const { return SpC{p + n, plane, fmt}; }
-  __host__ __device__ explicit operator bool() const { return p != nullptr; }
-};
-struct SpM {
-  uint16_t *p; size_t plane; uint32_t fmt;
-  __host__ __device__ __forceinline__ SpM operator+(size_t n) const { return SpM{p + n, plane, fmt}; }
-};
-__device__ __forceinline__ float4 io_ld4(const float *p) { return Act<float>::ld4(p); }
-__device__ __forceinline__ float4 io_ld4(const bf16 *p) { return Act<bf16>::ld4(p); }
-__device__ __forceinline__ float4 io_ld4(SpC p) { return Sp16::ld4(p.p, p.plane, p.fmt); }
-__device__ __forceinline__ void io_st4(float *p, float4 v) { Act<float>::st4(p, v); }
-__device__ __forceinline__ void io_st4(bf16 *p, float4 v) { Act<bf16>::st4(p, v); }
-__device__ __forceinline__ void io_st4(SpM p, float4 v) { Sp16::st4(p.p, p.plane, p.fmt, v); }
-// N = 4 or 8 consecutive values as float4 members, not an array: NVVM's -O1 pipeline does not unroll loops, so an
-// array indexed in a loop would live in local memory.  The 8-element accesses are one 16-byte access per plane.
-template <int N> struct Vf;
-template <> struct Vf<4> { float4 a; };
-template <> struct Vf<8> { float4 a, b; };
-__device__ __forceinline__ float4 bf16x4(uint32_t lo, uint32_t hi) {
-  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&lo));
-  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&hi));
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-__device__ __forceinline__ float4 sp16x4(uint32_t h0, uint32_t h1, uint32_t l0, uint32_t l1, uint32_t fmt) {
-  const float2 a = Sp16::up(h0, fmt), b = Sp16::up(h1, fmt), c = Sp16::up(l0, fmt), d = Sp16::up(l1, fmt);
-  return make_float4(a.x + c.x, a.y + c.y, b.x + d.x, b.y + d.y);
-}
-__device__ __forceinline__ Vf<8> io_ld8(const bf16 *p) {
-  const uint4 r = __ldg(reinterpret_cast<const uint4 *>(p));
-  return {bf16x4(r.x, r.y), bf16x4(r.z, r.w)};
-}
-__device__ __forceinline__ Vf<8> io_ld8(SpC p) {
-  const uint4 h = __ldg(reinterpret_cast<const uint4 *>(p.p)), l = __ldg(reinterpret_cast<const uint4 *>(p.p + p.plane));
-  return {sp16x4(h.x, h.y, l.x, l.y, p.fmt), sp16x4(h.z, h.w, l.z, l.w, p.fmt)};
-}
-template <int N, typename P> __device__ __forceinline__ Vf<N> io_ldv(P p) {
-  if constexpr (N == 4) return {io_ld4(p)};
-  else return io_ld8(p);
-}
-template <typename P> __device__ __forceinline__ void io_stv(P p, Vf<4> v) { io_st4(p, v.a); }
-__device__ __forceinline__ void io_stv(bf16 *p, Vf<8> v) {
-  const __nv_bfloat162 a = __floats2bfloat162_rn(v.a.x, v.a.y), b = __floats2bfloat162_rn(v.a.z, v.a.w);
-  const __nv_bfloat162 c = __floats2bfloat162_rn(v.b.x, v.b.y), d = __floats2bfloat162_rn(v.b.z, v.b.w);
-  *reinterpret_cast<uint4 *>(p) = make_uint4(*reinterpret_cast<const uint32_t *>(&a), *reinterpret_cast<const uint32_t *>(&b),
-                                             *reinterpret_cast<const uint32_t *>(&c), *reinterpret_cast<const uint32_t *>(&d));
-}
-__device__ __forceinline__ void io_stv(SpM p, Vf<8> v) {
-  uint4 h, l;
-  Sp16::split2(v.a.x, v.a.y, p.fmt, h.x, l.x); Sp16::split2(v.a.z, v.a.w, p.fmt, h.y, l.y);
-  Sp16::split2(v.b.x, v.b.y, p.fmt, h.z, l.z); Sp16::split2(v.b.z, v.b.w, p.fmt, h.w, l.w);
-  *reinterpret_cast<uint4 *>(p.p) = h;
-  *reinterpret_cast<uint4 *>(p.p + p.plane) = l;
-}
-template <int N> __device__ __forceinline__ Vf<N> ld_taps(const float *w) {     // fp32 filter taps
-  const float4 a = __ldg(reinterpret_cast<const float4 *>(w));
-  if constexpr (N == 4) return {a};
-  else return {a, __ldg(reinterpret_cast<const float4 *>(w + 4))};
-}
-__device__ __forceinline__ float4 fma4(float4 x, float4 w, float4 acc) {
-  return make_float4(fmaf(x.x, w.x, acc.x), fmaf(x.y, w.y, acc.y), fmaf(x.z, w.z, acc.z), fmaf(x.w, w.w, acc.w));
-}
-__device__ __forceinline__ Vf<4> vfma(Vf<4> x, Vf<4> w, Vf<4> acc) { return {fma4(x.a, w.a, acc.a)}; }
-__device__ __forceinline__ Vf<8> vfma(Vf<8> x, Vf<8> w, Vf<8> acc) { return {fma4(x.a, w.a, acc.a), fma4(x.b, w.b, acc.b)}; }
-// The epilogue activation follows the output format: act_fn for fp32, act_fast for bf16 and split planes (common.cuh).
-template <typename PO> __device__ __forceinline__ float act_io(float v, uint32_t act) {
-  if constexpr (std::is_same<PO, float *>::value) return cpb::act_fn(v, act);
-  else return cpb::act_fast(v, act);
-}
-template <typename PO> __device__ __forceinline__ float4 act4(float4 v, uint32_t act) {
-  return make_float4(act_io<PO>(v.x, act), act_io<PO>(v.y, act), act_io<PO>(v.z, act), act_io<PO>(v.w, act));
-}
-template <typename PO> __device__ __forceinline__ Vf<4> vact(Vf<4> v, uint32_t act) { return {act4<PO>(v.a, act)}; }
-template <typename PO> __device__ __forceinline__ Vf<8> vact(Vf<8> v, uint32_t act) { return {act4<PO>(v.a, act), act4<PO>(v.b, act)}; }
-__device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
-__device__ __forceinline__ Vf<4> vadd(Vf<4> a, Vf<4> b) { return {add4(a.a, b.a)}; }
-__device__ __forceinline__ Vf<8> vadd(Vf<8> a, Vf<8> b) { return {add4(a.a, b.a), add4(a.b, b.b)}; }
 
 struct ConvArgs {
   const void *src[4];
@@ -460,112 +313,6 @@ __global__ void __launch_bounds__(128) stem_kernel(const float *__restrict__ x, 
 // Element-wise ops (run_eltwise below): one kernel per op for every activation format.  PI / PO are the input / output
 // handles: `const float *` / `float *`, `const bf16 *` / `bf16 *`, or SpC / SpM on split planes.  Arithmetic is fp32.
 
-// ---- MAXPOOL k x k / stride / pad, NHWC, 4 channels per thread (exact on split planes: the maximum is one of the inputs) ----
-template <typename PI, typename PO>
-__global__ void maxpool_kernel(PI x, PO y, int B, int H, int W, int C, int Ho, int Wo, int k, int stride, int pad) {
-  const int C4 = C >> 2;
-  const long long total = (long long)B * Ho * Wo * C4;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int c4 = (int)(i % C4);
-    long long p = i / C4;
-    const int wo = (int)(p % Wo); p /= Wo;
-    const int ho = (int)(p % Ho);
-    const int b = (int)(p / Ho);
-    float4 m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
-    for (int r = 0; r < k; ++r) {
-      const int hi = ho * stride - pad + r;
-      if (hi < 0 || hi >= H) continue;
-      for (int q = 0; q < k; ++q) {
-        const int wi = wo * stride - pad + q;
-        if (wi < 0 || wi >= W) continue;
-        const float4 v = io_ld4(x + (((size_t)b * H + hi) * W + wi) * C + c4 * 4);
-        m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
-      }
-    }
-    io_st4(y + (((size_t)b * Ho + ho) * Wo + wo) * C + c4 * 4, m);
-  }
-}
-
-// ---- depthwise ConvTranspose2d(k=2f, stride f, pad f/2) + skip add, NHWC ----
-// out[b,ho,wo,c] = skip[b,ho,wo,c] + sum_{kh,kw : (ho+p-kh)%f==0, (wo+p-kw)%f==0} x[b,(ho+p-kh)/f,(wo+p-kw)/f,c] * w[kh,kw,c]
-// With a bias (MobileNetV2 IDAUp: k 2, stride 2, pad 0, folded BN + ReLU, mobilenetv2.py:162-183) the sum starts from
-// the bias, takes the activation, and the skip is added last: out = skip + act(bias + sum ...).
-// One CTA = one output row (b, ho); thread = (wo, group of VEC channels).  The k*k*C filter taps are read through the
-// read-only cache, so any filter size is accepted.  No integer division in the inner loop when f and C / VEC are powers
-// of two (lf = log2 f, lcv = log2(C / VEC), or -1 -> generic division).
-template <int VEC, typename PI, typename PO>
-__global__ void __launch_bounds__(256) dwdeconv_add_kernel(PI x, PI skip, PO y, const float *__restrict__ w,
-                                                           const float *__restrict__ bias, int H, int W, int C, int Ho, int Wo,
-                                                           int k, int f, int pad, int lf, int lcv, uint32_t act) {
-  const int CV = C / VEC;
-  const int b = blockIdx.x / Ho, ho = blockIdx.x % Ho;
-  const int kh0 = (ho + pad) % f;
-  const PI xb = x + (size_t)b * H * W * C;
-  const bool fast = lf >= 0 && lcv >= 0;
-  for (int i = threadIdx.x; i < Wo * CV; i += blockDim.x) {
-    const int wo = fast ? (i >> lcv) : (i / CV), cv = i - wo * CV;
-    const size_t opix = (((size_t)b * Ho + ho) * Wo + wo) * C + cv * VEC;
-    Vf<VEC> acc = bias ? ld_taps<VEC>(bias + cv * VEC) : skip ? io_ldv<VEC>(skip + opix) : Vf<VEC>{};
-    const int kw0 = fast ? ((wo + pad) & (f - 1)) : ((wo + pad) % f);
-    for (int khh = kh0; khh < k; khh += f) {
-      const int hn = ho + pad - khh;
-      const int hi = fast ? (hn >> lf) : (hn / f);
-      if (hn < 0 || hi >= H) continue;
-      for (int kww = kw0; kww < k; kww += f) {
-        const int wn = wo + pad - kww;
-        const int wi = fast ? (wn >> lf) : (wn / f);
-        if (wn < 0 || wi >= W) continue;
-        acc = vfma(io_ldv<VEC>(xb + ((size_t)hi * W + wi) * C + cv * VEC), ld_taps<VEC>(w + (size_t)(khh * k + kww) * C + cv * VEC), acc);
-      }
-    }
-    if (bias) {
-      acc = vact<PO>(acc, act);
-      if (skip) acc = vadd(acc, io_ldv<VEC>(skip + opix));
-    }
-    io_stv(y + opix, acc);
-  }
-}
-
-// Fast path for the shapes IDAUp uses (see run_eltwise): every item a thread visits in one output row has the same
-// channel group and the same column parity class, so its four (kh, kw) tap weight vectors are loaded ONCE per CTA.
-// VEC channels = 16 bytes per plane.  6 CTAs per SM keep it at <= 40 registers, the occupancy it has always run at.
-template <int VEC, typename PI, typename PO>
-__global__ void __launch_bounds__(256, 6) dwdeconv_add_fast_kernel(PI x, PI skip, PO y, const float *__restrict__ w, int H, int W, int C,
-                                                                int Ho, int Wo, int k, int f, int pad, int lf, int lcv) {
-  const int CV = C / VEC;
-  const int b = blockIdx.x / Ho, ho = blockIdx.x % Ho;
-  const int i0 = threadIdx.x;
-  const int wo_first = i0 >> lcv, cv = i0 & (CV - 1);
-  const int kh0 = (ho + pad) & (f - 1), kw0 = (wo_first + pad) & (f - 1);
-  Vf<VEC> wt[2][2];
-#pragma unroll
-  for (int a = 0; a < 2; ++a)
-#pragma unroll
-    for (int c = 0; c < 2; ++c) wt[a][c] = ld_taps<VEC>(w + (size_t)((kh0 + a * f) * k + kw0 + c * f) * C + cv * VEC);
-  const PI xb = x + (size_t)b * H * W * C + cv * VEC;
-  const int hn0 = ho + pad - kh0;                               // >= 0; tap a reads input row (hn0 >> lf) - a
-  const int hi0 = hn0 >> lf;
-  const size_t orow = ((size_t)b * Ho + ho) * Wo;
-  for (int i = i0; i < Wo * CV; i += 256) {
-    const int wo = i >> lcv;
-    const size_t opix = (orow + wo) * C + cv * VEC;
-    Vf<VEC> acc = skip ? io_ldv<VEC>(skip + opix) : Vf<VEC>{};
-    const int wi0 = (wo + pad - kw0) >> lf;
-#pragma unroll
-    for (int a = 0; a < 2; ++a) {
-      const int hi = hi0 - a;
-      if (hi < 0 || hi >= H) continue;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const int wi = wi0 - c;
-        if (wi < 0 || wi >= W) continue;
-        acc = vfma(io_ldv<VEC>(xb + ((size_t)hi * W + wi) * C), wt[a][c], acc);
-      }
-    }
-    io_stv(y + opix, acc);
-  }
-}
 
 // ---- nearest-neighbour upsample x f (+ skip add)(+ReLU), NHWC ----
 // out[b,ho,wo,c] = act(skip[b,ho,wo,c] + x[b,ho/f,wo/f,c])     (HRNet fuse_layers, pose_higher_hrnet.py:186-187,224-232)
@@ -944,28 +691,14 @@ bool is_eltwise(int type) {
   }
 }
 
-int ilog2(int v) {                                      // log2 of a power of two, else -1
-  int l = 0;
-  while ((1 << l) < v) ++l;
-  return (1 << l) == v ? l : -1;
-}
 
-// Activation handle of type P over the op tensor at p, n elements per plane (plain pointers ignore n and fmt).
-template <typename P> P io_handle(const void *p, size_t n, uint32_t fmt) {
-  void *q = const_cast<void *>(p);
-  if constexpr (std::is_same<P, SpC>::value) return SpC{static_cast<const uint16_t *>(q), n, fmt};
-  else if constexpr (std::is_same<P, SpM>::value) return SpM{static_cast<uint16_t *>(q), n, fmt};
-  else return static_cast<P>(q);
-}
-
-// The element-wise ops (is_eltwise) on every activation format: PI / PO are `const float *` / `float *`,
+// The element-wise ops (is_eltwise) other than MAXPOOL and DWDECONV_ADD (net_eltwise.cu) on every activation format: PI / PO are `const float *` / `float *`,
 // `const bf16 *` / `bf16 *`, or SpC / SpM on split planes (fmt: 1 = fp16, 0 = bf16 planes).  T is the element type of
 // the plain vectors next to the activations, SCALE_ADD's gate and AVGPOOL's output: the activation type, or fp32 next
 // to split planes (the SE convs around them run on fp32).
 template <typename T, typename PI, typename PO>
 int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
   constexpr int VEC = 16 / sizeof(T);                   // channels per thread: 16 bytes, or 8 bytes per split plane
-  constexpr int VEC_FAST = std::is_same<PO, SpM>::value ? 8 : VEC;   // the fast dwdeconv: 16 bytes per plane
   const int C = op.cin[0];
   if (op.src_pitch[0] != 0 && op.src_pitch[0] != C)
     return cpb::fail(CPB200_ERR_ARG, "op type %d: needs a dense input (src_pitch %d, C %d)", op.type, op.src_pitch[0], C);
@@ -976,27 +709,6 @@ int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
   const uint32_t act = op.flags & CPB_ACT_MASK;
   auto grid = [](long long total, int ctas_per_sm) { return (unsigned)std::min<long long>((total + 255) / 256, 132LL * ctas_per_sm); };
   switch (op.type) {
-    case CPB200_OP_MAXPOOL: {
-      if (C % 4) return cpb::fail(CPB200_ERR_ARG, "maxpool: C %% 4 != 0");
-      maxpool_kernel<PI, PO><<<grid((long long)op.B * op.Ho * op.Wo * (C / 4), 32), 256, 0, st>>>(x, y, op.B, op.H, op.W, C,
-          op.Ho, op.Wo, op.kh, op.stride, op.pad_h);
-      return cpb::check_launch("maxpool_kernel", maxpool_kernel<PI, PO>);
-    }
-    case CPB200_OP_DWDECONV_ADD: {
-      if (C % VEC || op.stride < 1) return cpb::fail(CPB200_ERR_ARG, "dwdeconv: needs C %% %d == 0 and stride >= 1", VEC);
-      if (act && !op.bias) return cpb::fail(CPB200_ERR_ARG, "dwdeconv: an activation needs the bias form");
-      const int lf = ilog2(op.stride), CV = C / VEC_FAST, lcv = C % VEC_FAST ? -1 : ilog2(CV);
-      // the fast kernel's shapes: no bias, k == 2f, f and C / VEC_FAST powers of two, and each CTA's 256 threads cover
-      // whole output pixels of one column parity class
-      if (!op.bias && lf >= 0 && lcv >= 0 && op.kh == 2 * op.stride && CV <= 256 && (256 / CV) % op.stride == 0) {
-        dwdeconv_add_fast_kernel<VEC_FAST, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.H, op.W, C, op.Ho,
-            op.Wo, op.kh, op.stride, op.pad_h, lf, lcv);
-        return cpb::check_launch("dwdeconv_add_fast_kernel", dwdeconv_add_fast_kernel<VEC_FAST, PI, PO>);
-      }
-      dwdeconv_add_kernel<VEC, PI, PO><<<(unsigned)(op.B * op.Ho), 256, 0, st>>>(x, skip, y, w, op.bias, op.H, op.W, C, op.Ho,
-          op.Wo, op.kh, op.stride, op.pad_h, lf, ilog2(C / VEC), act);
-      return cpb::check_launch("dwdeconv_add_kernel", dwdeconv_add_kernel<VEC, PI, PO>);
-    }
     case CPB200_OP_DWCONV: {
       if (C % VEC || op.kh != op.kw || op.cout != C) return cpb::fail(CPB200_ERR_ARG, "dwconv: C %% %d != 0 or non-square kernel", VEC);
 #define DW_TILED(KK, SS, PX)                                                                                   \
@@ -1059,12 +771,15 @@ int run_eltwise(const cpb200_op &op, uint32_t fmt, cudaStream_t st) {
 }  // namespace
 
 namespace cpb {
+int run_op_pool_deconv(const cpb200_op &op, cudaStream_t st);   // net_eltwise.cu
+
 // Split-plane activations without CPB200_FLAG_TC: the element-wise ops and the two conversions run here; CONV, DCN and
 // STEM need the tensor-core path (the host runs their other shapes on fp32 between CONVERT ops).
 bool simt_runs_split(int type) { return is_eltwise(type) || type == CPB200_OP_CONVERT || type == CPB200_OP_S2D; }
 
 int run_op_simt_dispatch(const cpb200_op &op, cudaStream_t st) {
   const bool split = op.act_dtype == CPB200_BF16X2 || op.act_dtype == CPB200_F16X2;
+  if (op.type == CPB200_OP_MAXPOOL || op.type == CPB200_OP_DWDECONV_ADD) return run_op_pool_deconv(op, st);
   if (is_eltwise(op.type)) {
     if (split) return run_eltwise<float, SpC, SpM>(op, op.act_dtype == CPB200_F16X2 ? 1u : 0u, st);
     if (op.act_dtype == CPB200_F32) return run_eltwise<float, const float *, float *>(op, 0, st);
