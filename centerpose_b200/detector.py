@@ -282,10 +282,16 @@ def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda
     return buf, {"o_rsz": o_rsz, "o_aff": o_aff, "o_idx": o_idx, "o_img": o_img, "scratch": scratch}
 
 
-# run_images decodes JPEG files on the device in launches of at most this many images, whose coefficient and plane
-# workspace (reused from launch to launch) stays below JPEG_CHUNK_WORKSPACE bytes unless one image needs more
+# run_images decodes JPEG and PNG files on the device in launches of at most this many images, whose workspace (JPEG
+# coefficients and planes, PNG scanlines; reused from launch to launch) stays below JPEG_CHUNK_WORKSPACE bytes unless
+# one image needs more
 JPEG_CHUNK_IMAGES = 256
 JPEG_CHUNK_WORKSPACE = 512 << 20
+# PNG files go to the device only when a call holds at least this many of them.  The inflate is serial within a file,
+# so a launch takes about as long for one file as for 256 (141-165 ms for 640x480 files on one H100), while
+# cv2.imread takes 9-17 ms per file on one host thread; below this count the host decode is faster
+# (tools/bench_png.py)
+PNG_DEVICE_MIN_IMAGES = 16
 
 
 def _swap_pairs(C, pairs, device):
@@ -460,13 +466,15 @@ class MultiPoseDetector(BaseDetector):
         """Every input of ``run_images`` in one device buffer of packed HWC uint8 BGR images.  Returns
         ``(views, offsets, buffer)``: per input a (h, w, 3) view of its slot and the slot's byte offset.
 
-        The files' headers are parsed first (``jpeg.parse``), so every size is known before any pixel exists.  The
-        files the device can decode, with their tables, go up in one pinned buffer and are decoded by
-        ``cpb200_jpeg_decode_batch`` in chunks of at most ``JPEG_CHUNK_IMAGES`` images that reuse one workspace.  The
-        other files (``cv2.imread``) and the arrays take the host path, and their pixels go up in one copy into
-        slots after the decoded ones.  One read of the decode status follows; a file whose entropy data the device
-        found bad is read by ``cv2.imread`` and copied into its slot."""
-        from . import _lib, jpeg
+        The files' headers are parsed first (``jpeg.parse``, ``png.parse``), so every size is known before any pixel
+        exists.  The files the device can decode, with their tables, go up in one pinned buffer and are decoded by
+        ``cpb200_jpeg_decode_batch`` and ``cpb200_png_decode_batch`` in chunks of at most ``JPEG_CHUNK_IMAGES``
+        images that reuse one workspace; PNG files only when the call holds at least ``PNG_DEVICE_MIN_IMAGES`` of them,
+        since one PNG launch costs about as much as a dozen host decodes.  The other files (``cv2.imread``) and the
+        arrays take the host path, and
+        their pixels go up in one copy into slots after the decoded ones.  One read of the decode status follows; a
+        file whose compressed data the device found bad is read by ``cv2.imread`` and copied into its slot."""
+        from . import _lib, jpeg, png
         dev = torch.device("cuda")
         datas, infos, host = {}, {}, {}
         for n, src in enumerate(images):
@@ -478,15 +486,21 @@ class MultiPoseDetector(BaseDetector):
                     data = f.read()
             except OSError:
                 raise FileNotFoundError(src)
+            fmt = png if data[:8] == png.SIGNATURE else jpeg
             try:
-                info = jpeg.parse(data, src)
+                info = fmt.parse(data, src)
             except ValueError:
                 info = None
-            if info is not None and (info.eligible or info.progressive):
-                datas[n], infos[n] = data, info
+            if info is not None and (info.eligible or getattr(info, "progressive", None)):
+                datas[n], infos[n] = data, (fmt, info)
             else:
                 host[n] = self._load_checked(n, src)
-        shape = {n: (infos[n].oh, infos[n].ow, 3) for n in infos}
+        pngs = [n for n in infos if infos[n][0] is png]
+        if len(pngs) < PNG_DEVICE_MIN_IMAGES:
+            for n in pngs:                                    # cv2.imread is faster for a handful of PNG files
+                del infos[n], datas[n]
+                host[n] = self._load_checked(n, images[n])
+        shape = {n: (info.oh, info.ow, 3) for n, (_, info) in infos.items()}
         shape.update({n: im.shape for n, im in host.items()})
         offsets, pos = {}, 0
         for n in list(infos) + list(host):                   # decoded slots first, then the host ones in one run
@@ -495,15 +509,19 @@ class MultiPoseDetector(BaseDetector):
         host_start = pos - sum(im.nbytes for im in host.values())
         pixels = torch.empty(max(pos, 1), dtype=torch.uint8, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        dec = list(infos)
+        # JPEG files, then PNG files; status[k] belongs to dec[k]
+        dec = [n for n in infos if infos[n][0] is jpeg] + [n for n in infos if infos[n][0] is png]
         if dec:
             chunks, start, ws = [], 0, 0
             for k, n in enumerate(dec):
-                if k > start and (k - start == JPEG_CHUNK_IMAGES or ws + infos[n].workspace_bytes() > JPEG_CHUNK_WORKSPACE):
+                fmt, info = infos[n]
+                if k > start and (k - start == JPEG_CHUNK_IMAGES or ws + info.workspace_bytes() > JPEG_CHUNK_WORKSPACE
+                                  or fmt is not infos[dec[start]][0]):
                     chunks.append((start, k)); start, ws = k, 0
-                ws += infos[n].workspace_bytes()
+                ws += info.workspace_bytes()
             chunks.append((start, len(dec)))
-            packed = [jpeg.pack([infos[n] for n in dec[a:b]], [datas[n] for n in dec[a:b]], [offsets[n] for n in dec[a:b]])
+            packed = [infos[dec[a]][0].pack([infos[n][1] for n in dec[a:b]], [datas[n] for n in dec[a:b]],
+                                            [offsets[n] for n in dec[a:b]])
                       for a, b in chunks]
             at = np.cumsum([0] + [p[0].nbytes + (-p[0].nbytes) % 16 for p in packed])
             up = torch.empty(int(at[-1]), dtype=torch.uint8, pin_memory=True)
@@ -515,10 +533,11 @@ class MultiPoseDetector(BaseDetector):
             status = torch.empty(len(dec), dtype=torch.int32, device=dev)
             with torch.cuda.device(dev):
                 for (a, b), o in zip(chunks, at):
-                    st = _lib.lib().cpb200_jpeg_decode_batch(src.data_ptr() + int(o), src.data_ptr() + int(o), b - a,
-                                                             work.data_ptr(), work.numel(), pixels.data_ptr(),
-                                                             status.data_ptr() + 4 * a, stream)
-                    _lib.check(st, "jpeg_decode_batch")
+                    name = "jpeg_decode_batch" if infos[dec[a]][0] is jpeg else "png_decode_batch"
+                    st = getattr(_lib.lib(), "cpb200_" + name)(src.data_ptr() + int(o), src.data_ptr() + int(o), b - a,
+                                                              work.data_ptr(), work.numel(), pixels.data_ptr(),
+                                                              status.data_ptr() + 4 * a, stream)
+                    _lib.check(st, name)
         if host:
             staged = torch.empty(pos - host_start, dtype=torch.uint8, pin_memory=True)
             sv = staged.numpy()
@@ -553,11 +572,13 @@ class MultiPoseDetector(BaseDetector):
 
         With ``B200.DEVICE_PREPROCESS`` on (the default) and any path among the inputs, the images are decoded into
         one device buffer first (``_load_images_device``): sequential- and progressive-Huffman JPEG files by
-        ``cpb200_jpeg_decode_batch``, byte for byte as ``cv2.imread``; every other file, and every array, on the
-        host and uploaded into its slot.  The groups then read that buffer in place.  That adds one small
-        device-to-host read of the decode status.  The call then needs device memory for the decoded images (3 bytes
-        per pixel) and one decode chunk's workspace (int16 coefficients and 8-bit planes: 4.5 bytes per pixel at
-        4:2:0, 9 at 4:4:4, at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image needs more)."""
+        ``cpb200_jpeg_decode_batch`` and, from ``PNG_DEVICE_MIN_IMAGES`` PNG files per call on, PNG files (not APNG)
+        by ``cpb200_png_decode_batch``, byte for byte as
+        ``cv2.imread``; every other file, and every array, on the host and uploaded into its slot.  The groups then
+        read that buffer in place.  That adds one small device-to-host read of the decode status.  The call then
+        needs device memory for the decoded images (3 bytes per pixel) and one decode chunk's workspace (JPEG: int16
+        coefficients and 8-bit planes, 4.5 bytes per pixel at 4:2:0, 9 at 4:4:4; PNG: the scanlines, 1 to 8 bytes per
+        pixel; at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image needs more)."""
         import ctypes
         from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch

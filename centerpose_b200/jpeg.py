@@ -71,7 +71,7 @@ class JpegInfo:
         self.restart_interval = 0
 
     def size_after_orientation(self):
-        return (self.w, self.h) if self.orientation >= 5 else (self.h, self.w)
+        return oriented_size(self.h, self.w, self.orientation)
 
     @property
     def mcu(self):
@@ -114,11 +114,23 @@ class JpegScan:
         return bw * bh
 
 
+def oriented_size(h, w, orientation):
+    """(height, width) of an ``h`` x ``w`` image after OpenCV applies EXIF ``orientation`` (5..8 transpose it)."""
+    return (w, h) if orientation >= 5 else (h, w)
+
+
 def _exif_orientation(seg):
     """The orientation tag (0x0112) of IFD0 in an APP1 Exif payload, 1 when absent or unreadable."""
     if len(seg) < 14 or seg[:6] != b"Exif\x00\x00":
         return 1
-    t = seg[6:]
+    return tiff_orientation(seg[6:])
+
+
+def tiff_orientation(t):
+    """The orientation tag (0x0112) of IFD0 in Exif data that starts with its TIFF header (the payload of a PNG eXIf
+    chunk, or of a JPEG APP1 segment after ``Exif\\0\\0``), 1 when absent or unreadable."""
+    if len(t) < 8:
+        return 1
     if t[:2] == b"II":
         order = "<"
     elif t[:2] == b"MM":

@@ -208,6 +208,36 @@ typedef struct cpb200_jpeg_image {
 int cpb200_jpeg_decode_batch(const unsigned char *src, const cpb200_jpeg_image *table, int B, void *workspace,
                              size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
 
+/* One image of cpb200_png_decode_batch (72 bytes, lives in caller-owned DEVICE memory).  Offsets are bytes. */
+typedef struct cpb200_png_image {
+  int64_t src_offset;        /* in `src`: the zlib stream (the IDAT payloads back to back), followed by >= 32 bytes
+                                the decoder may read but ignores */
+  int64_t src_bytes;         /* length of the zlib stream */
+  int64_t palette_offset;    /* colour type 3: in `src`, 256 RGB entries (768 bytes), the ones past PLTE zero */
+  int64_t ws_offset;         /* in `workspace`: the image's scanlines, 16-byte aligned */
+  int64_t ws_bytes;          /* >= the inflated size rounded up to 16, plus 16 */
+  int64_t dst_offset;        /* in `dst`: the decoded HWC uint8 BGR image, rows packed, size after orientation */
+  int32_t h, w;              /* stored size, 1..1000000, h * w <= 2^30 */
+  int32_t color_type;        /* 0 gray, 2 RGB, 3 palette, 4 gray + alpha, 6 RGBA */
+  int32_t depth;             /* bits per sample, legal for the colour type: 1, 2, 4, 8 or 16 */
+  int32_t interlace;         /* 0 none, 1 Adam7 */
+  int32_t orientation;       /* EXIF orientation 1..8 (eXIf chunk), applied as cv2.imread does */
+} cpb200_png_image;
+
+/* cv2.imread(path, IMREAD_COLOR) of PNG files, byte for byte (libpng through OpenCV 4.13: 16-bit samples keep their
+ * high byte, 1/2/4-bit gray is scaled to 8 bits, palette indices past the palette are black, gray is replicated, alpha
+ * is dropped, then OpenCV's EXIF orientation).  B files in one launch: `src` holds each image's zlib stream and
+ * palette, `table` is a DEVICE array of B cpb200_png_image that the caller has checked (the kernels trust it; see
+ * centerpose_b200/png.py), `workspace` holds every image's scanlines (an image whose workspace would end past
+ * `workspace_bytes` is not decoded and gets status 2).  One warp per image inflates its stream (stored, fixed- and
+ * dynamic-Huffman blocks), one warp per image then undoes the scanline filters over 32 rows at a time and checks the
+ * Adler-32, and the output pass expands the samples over the whole launch.  status[b] (DEVICE int array) is 0 when
+ * image b decoded, 1 when its stream was bad (zlib header, block type, Huffman code, a distance before the start of
+ * the data or past the window, more or less data than the image holds, data ending early, Adler-32, a filter type
+ * above 4); the image's `dst` slot is then left unwritten, other images are unaffected.  1 <= B <= 65535. */
+int cpb200_png_decode_batch(const unsigned char *src, const cpb200_png_image *table, int B, void *workspace,
+                            size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)
