@@ -14,7 +14,7 @@ Data (``_data``, seeded by the record's call):
            result equals the float64 reference bit for bit.  Needs CPB200_RZ_COMP=0 when the plan is built, so that
            acc_scale is a pure power of two.
 
-Tolerances (those of tests/test_net_gpu.py, tests/test_split_gpu.py and tests/test_hardnet_gpu.py):
+Tolerances (the op tests' bounds, tests/util.py::check_op; bf16 here is a max-norm, where check_op's is relative L2):
   fp32   : |err| <= 2e-4 max|ref|;  DCN 5e-4 (test_dcn_op_matches_oracle: the sampling positions come from the fp32
            offset conv, whose summation order differs from the reference's)
   bf16   : |err| <= 1e-2 max|ref|;  DCN relative L2 <= 2e-2

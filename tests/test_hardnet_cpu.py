@@ -19,7 +19,7 @@ def _sha(*arrays):
     return h.hexdigest()
 
 
-def _model():
+def _fresh_model():
     from centerpose_b200.config import default_cfg
     from centerpose_b200.model import create_model
     cfg = default_cfg("hardnet")
@@ -33,7 +33,7 @@ def test_hardnet_oracle_matches_reference_golden(tag):
     from oracle.init_recipe import conditioned_state_dict, synth_images
     g = np.load(os.path.join(GOLD, f"hardnet_{tag}.npz"))
     B, H, W = [int(v) for v in g["shape"]]
-    m, _ = _model()
+    m, _ = _fresh_model()
     sd = conditioned_state_dict(m.state_dict(), 317)
     x = synth_images(B, H, W, 317)
     assert _sha(x.numpy()) == str(g["x_sha"])
@@ -47,7 +47,7 @@ def test_hardnet_state_dict_matches_reference():
     """438 entries (69 ConvLayers x (conv weight + 5 BatchNorm entries) + 24 head tensors); the conditioned weights'
     sha equals the golden's, which pins every key name and shape (the recipe draws in sorted-key order)."""
     from oracle.init_recipe import conditioned_state_dict
-    m, _ = _model()
+    m, _ = _fresh_model()
     own = m.state_dict()
     sd = conditioned_state_dict(own, 317)
     assert len(sd) == 438
@@ -76,7 +76,7 @@ def test_hardnet_plan_census():
     """fp32 lowering of the whole network on the CPU: every op reads at most four inputs, every input slab is a multiple
     of 16 channels, the heads run at stride 4, four 2x2 average pools and one resize per up-path slab (1 + 5 + 5 + 3)."""
     from centerpose_b200.plan import OP_AVGPOOL2, OP_CONV, OP_RESIZE_BILINEAR, OP_STEM
-    m, _ = _model()
+    m, _ = _fresh_model()
     m.set_precision("fp32")
     plan = m._plan(2, 128, 160, torch.device("cpu"))
     census = Counter(o.type for o in plan.ops)
@@ -99,7 +99,7 @@ def test_hardnet_split_plan_has_no_fp32_island_at_512():
     """fp16x2 at 512x512: the stride-2 stem takes the space-to-depth route, every conv is tensor-core eligible and the
     pool / resize ops run on the split planes, so the program holds no CONVERT op."""
     from centerpose_b200.plan import OP_CONV, OP_CONVERT
-    m, _ = _model()
+    m, _ = _fresh_model()
     m.set_precision("fp16x2")
     plan = m._plan(1, 512, 512, torch.device("cpu"))
     assert sum(o.type == OP_CONVERT for o in plan.ops) == 0
@@ -107,7 +107,7 @@ def test_hardnet_split_plan_has_no_fp32_island_at_512():
 
 
 def test_hardnet_default_cfg_builds():
-    m, cfg = _model()
+    m, cfg = _fresh_model()
     assert cfg.MODEL.HEAD_CONV == 256 and cfg.MODEL.INTERMEDIATE_CHANNEL == 48
     assert m.head_model.hm._modules["0"].weight.shape == (256, 48, 3, 3)
 
@@ -117,7 +117,7 @@ def test_hardnet_checkpoint_roundtrip_reference_format(tmp_path, capsys):
     prefix) loads through load_model with no missing and no dropped keys."""
     from centerpose_b200.model import load_model, save_model
     from oracle.init_recipe import conditioned_state_dict
-    m, cfg = _model()
+    m, cfg = _fresh_model()
     p = str(tmp_path / "hardnet.pth")
     save_model(p, 11, m)
     ck = torch.load(p, weights_only=False)
@@ -125,7 +125,7 @@ def test_hardnet_checkpoint_roundtrip_reference_format(tmp_path, capsys):
     sd = conditioned_state_dict(ck["state_dict"], 5)
     torch.save({"epoch": 11, "state_dict": {"module." + k: v for k, v in sd.items()}}, p)
     capsys.readouterr()
-    m2 = load_model(_model()[0], p)
+    m2 = load_model(_fresh_model()[0], p)
     out = capsys.readouterr().out
     assert "No param" not in out and "Drop parameter" not in out and "Skip loading" not in out, out
     for k, v in m2.state_dict().items():

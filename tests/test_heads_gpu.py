@@ -4,20 +4,16 @@ import pytest
 import torch
 
 from centerpose_b200 import plan as plan_mod
-from centerpose_b200.config import default_cfg
-from centerpose_b200.model import create_model
-from centerpose_b200.synth import conditioned_state_dict, synth_images
+from centerpose_b200.synth import synth_images
+from tests.util import model
 
 DEV = torch.device("cuda:0")
 _MODELS = {}
 
 
-def _model(arch):
+def _cached_model(arch):
     if arch not in _MODELS:
-        cfg = default_cfg(arch)
-        m = create_model(cfg.MODEL.NAME, cfg.MODEL.HEAD_CONV, cfg)
-        m.load_state_dict(conditioned_state_dict(m.state_dict(), 317))
-        _MODELS[arch] = m.to(DEV)
+        _MODELS[arch] = model(arch, "fp32")[0]
     return _MODELS[arch]
 
 
@@ -39,7 +35,7 @@ def _forward(m, xs, precision, fused, monkeypatch):
 @pytest.mark.parametrize("precision", ["fp16x2", "bf16x2", "bf16"])
 @pytest.mark.parametrize("B,H,W", [(1, 512, 512), (3, 512, 512), (1, 96, 160), (3, 96, 160)])
 def test_fused_heads_bit_identical(precision, B, H, W, monkeypatch):
-    m = _model("dla_34")
+    m = _cached_model("dla_34")
     xs = [synth_images(B, H, W, 317 + k).to(DEV) for k in range(2)]
     got = _forward(m, xs, precision, True, monkeypatch)
     want = _forward(m, xs, precision, False, monkeypatch)
@@ -52,7 +48,7 @@ def test_fused_heads_bit_identical(precision, B, H, W, monkeypatch):
 @pytest.mark.parametrize("precision", ["fp16x2", "bf16"])
 def test_fused_heads_bit_identical_mobilenetv3(precision, monkeypatch):
     """32-channel head input: 32-wide K slab with the 64-byte swizzle"""
-    m = _model("mobilenetv3")
+    m = _cached_model("mobilenetv3")
     xs = [synth_images(2, 96, 160, 317).to(DEV)]
     got = _forward(m, xs, precision, True, monkeypatch)
     want = _forward(m, xs, precision, False, monkeypatch)

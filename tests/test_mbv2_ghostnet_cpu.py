@@ -21,7 +21,7 @@ def _sha(*arrays):
     return h.hexdigest()
 
 
-def _model(arch, name=None):
+def _fresh_model(arch, name=None):
     from centerpose_b200.config import default_cfg
     from centerpose_b200.model import create_model
     cfg = default_cfg(arch)
@@ -41,7 +41,7 @@ def test_oracle_matches_reference_golden(arch, tag):
     g = np.load(os.path.join(GOLD, f"{tag}.npz"))
     B, H, W = [int(v) for v in g["shape"]]
     st, fst = int(g["stride"]), int(g["feat_stride"])
-    m, _ = _model(arch)
+    m, _ = _fresh_model(arch)
     sd = conditioned_state_dict(m.state_dict(), 317)
     assert _sha(*[sd[k].numpy() for k in sorted(sd) if sd[k].is_floating_point()]) == str(g["sd_sha"])
     x = synth_images(B, H, W, 317)
@@ -65,7 +65,7 @@ def test_state_dict_matches_reference(arch):
     from oracle.init_recipe import conditioned_state_dict
     from oracle.ref_harness import reference_available
     yaml, n_backbone = ARCHS[arch]
-    m, _ = _model(arch)
+    m, _ = _fresh_model(arch)
     own = m.state_dict()
     assert sum(k.startswith("backbone_model.") for k in own) == n_backbone and len(own) == n_backbone + 24
     tag = "mbv2_512" if arch == "mobilenetv2" else "ghostnet_512"
@@ -98,8 +98,8 @@ def test_create_model_accepts_any_suffix(name):
     """create_model no longer raises KeyError; like the reference, the _N suffix does not change the network
     (MobileNetV2 is always width 0.5)."""
     arch = name.split("_")[0]
-    m, cfg = _model(arch, name)
-    ref, _ = _model(arch)
+    m, cfg = _fresh_model(arch, name)
+    ref, _ = _fresh_model(arch)
     assert [(k, v.shape) for k, v in m.state_dict().items()] == [(k, v.shape) for k, v in ref.state_dict().items()]
     assert cfg.MODEL.HEAD_CONV == 256
     assert cfg.MODEL.INTERMEDIATE_CHANNEL == (24 if arch == "mobilenetv2" else 160)
@@ -107,7 +107,7 @@ def test_create_model_accepts_any_suffix(name):
 
 def test_unknown_backbone_message_lists_the_new_ones():
     with pytest.raises(KeyError, match="mobilenetv2, ghostnet"):
-        _model("dla_34", "efficientdet")
+        _fresh_model("dla_34", "efficientdet")
 
 
 def test_fold_bn_eps():
@@ -125,7 +125,7 @@ def test_fold_bn_eps():
 
 
 def _plan(arch, precision, B, H, W):
-    m, _ = _model(arch)
+    m, _ = _fresh_model(arch)
     m.set_precision(precision)
     return m._plan(B, H, W, torch.device("cpu"))
 
@@ -196,13 +196,13 @@ def test_checkpoint_roundtrip_reference_format(arch, tmp_path, capsys):
     with no missing and no dropped keys."""
     from centerpose_b200.model import load_model, save_model
     from oracle.init_recipe import conditioned_state_dict
-    m, _ = _model(arch)
+    m, _ = _fresh_model(arch)
     p = str(tmp_path / f"{arch}.pth")
     save_model(p, 3, m)
     sd = conditioned_state_dict(torch.load(p, weights_only=False)["state_dict"], 9)
     torch.save({"epoch": 3, "state_dict": {"module." + k: v for k, v in sd.items()}}, p)
     capsys.readouterr()
-    m2 = load_model(_model(arch)[0], p)
+    m2 = load_model(_fresh_model(arch)[0], p)
     out = capsys.readouterr().out
     assert "No param" not in out and "Drop parameter" not in out and "Skip loading" not in out, out
     for k, v in m2.state_dict().items():

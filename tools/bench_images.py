@@ -34,7 +34,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-from tools.bench_hardnet import gpu_info  # noqa: E402
+from tools.bench_backbones import gpu_info  # noqa: E402
 
 SIZES = [(480, 640), (640, 480), (427, 640)]     # (h, w)
 

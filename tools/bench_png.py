@@ -39,7 +39,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-from tools.bench_hardnet import gpu_info  # noqa: E402
+from tools.bench_backbones import gpu_info  # noqa: E402
 from tools.bench_images import SIZES, detector  # noqa: E402
 from tests.test_jpeg_cpu import make_image  # noqa: E402
 from tests.test_png_cpu import write_png  # noqa: E402
