@@ -18,7 +18,8 @@ from __future__ import annotations
 
 import ctypes
 import os
-from typing import List, Optional, Sequence
+from dataclasses import dataclass
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -103,13 +104,11 @@ class HeadStruct(ctypes.Structure):
 
 class Sym:
     """Symbolic activation tensor (NHWC unless kind says otherwise)."""
-    __slots__ = ("C", "H", "W", "kind", "name", "_buf", "producer", "_last_use", "fixed", "parent", "ch_off", "_f32", "_sp", "keep")
+    __slots__ = ("C", "H", "W", "kind", "name", "_buf", "fixed", "parent", "ch_off", "_f32", "_sp", "keep")
 
     def __init__(self, C, H, W, kind="act", name="", parent=None, ch_off=0):
         self.C, self.H, self.W, self.kind, self.name = C, H, W, kind, name
         self._buf = None         # torch tensor once allocated
-        self.producer = -1
-        self._last_use = -1
         self.fixed = False       # externally provided storage (network input / outputs)
         self.parent = parent     # channel slice [ch_off, ch_off + C) of `parent` (shares its storage)
         self.ch_off = ch_off
@@ -117,7 +116,7 @@ class Sym:
         self._sp = None
         self.keep = False        # PlanBuilder.keep_result(): never pruned, buffer never recycled (tests / diagnostics read it)
 
-    # a slice lives in its parent's buffer and keeps the parent alive
+    # a slice lives in its parent's buffer and keeps the parent alive (liveness is tracked on Plan._root)
     @property
     def buf(self):
         return self.parent.buf if self.parent is not None else self._buf
@@ -127,24 +126,54 @@ class Sym:
         self._buf = v
 
     @property
-    def last_use(self):
-        return self.parent.last_use if self.parent is not None else self._last_use
-
-    @last_use.setter
-    def last_use(self, v):
-        if self.parent is not None:
-            self.parent.last_use = v
-        else:
-            self._last_use = v
-
-    @property
     def pitch(self):
         return self.parent.C if self.parent is not None else self.C
 
 
-class _PendingOp:
-    def __init__(self, **kw):
-        self.__dict__.update(kw)
+@dataclass(eq=False)
+class Op:
+    """One op of the program, over symbolic tensors; ``Plan`` turns it into a ``cpb200_op``.  ``res`` and ``aux`` fill
+    the header's fields of those names: CONV's residual is ``res``; SCALE_ADD's gate is ``res`` and its skip ``aux``;
+    DCN's offset/mask tensor and the DWDECONV_ADD / UPSAMPLE_ADD skip are ``aux``.  ``out_map`` = (Hd, Wd, sy, sx, oy,
+    ox) and ``HoWo`` place the result in ``dst``; by default it fills all of ``dst``."""
+    type: int
+    dtype: int                                   # cpb200_op.act_dtype
+    srcs: List[Sym]
+    dst: Sym
+    cout: int
+    flags: int = 0
+    k: Tuple[int, int] = (1, 1)
+    stride: int = 1
+    pad: Tuple[int, int] = (0, 0)
+    weight: Optional[torch.Tensor] = None
+    bias: Optional[torch.Tensor] = None
+    res: Optional[Sym] = None
+    aux: Optional[Sym] = None
+    aux_pitch: int = 0
+    acc_scale: float = 1.0
+    out_ch_off: int = 0
+    out_map: Optional[Tuple[int, int, int, int, int, int]] = None
+    HoWo: Optional[Tuple[int, int]] = None
+    w_raw: Optional[torch.Tensor] = None         # the unpacked (Co, Ci, kh, kw) weight of a conv / DCN
+    heads: Optional[List[Tuple["Op", "Op"]]] = None      # OP_HEADS: the (3x3, 1x1) conv pairs it replaces
+
+    def __post_init__(self):
+        if self.out_map is None:
+            self.out_map = (self.dst.H, self.dst.W, 1, 1, 0, 0)
+        if self.HoWo is None:
+            self.HoWo = (self.dst.H, self.dst.W)
+
+    def operands(self) -> List[Sym]:
+        """every activation the op reads"""
+        return [*self.srcs, *(s for s in (self.res, self.aux) if s is not None)]
+
+
+def _swizzle_chunks(blk: torch.Tensor, key: torch.Tensor) -> torch.Tensor:
+    """blk [..., row n, 16-byte chunk j, element] -> the same rows with chunk j stored at chunk j ^ key[n]: the
+    shared-memory swizzles of the tensor-core stems' B operand (csrc/net_stem_tc.cu)"""
+    j = torch.arange(blk.shape[-2], device=blk.device)
+    idx = (j.view(1, -1, 1) ^ key.view(-1, 1, 1)).expand(blk.shape)
+    return torch.zeros(blk.shape, dtype=blk.dtype, device=blk.device).scatter_(-2, idx, blk.contiguous())
 
 
 def fold_bn(w: torch.Tensor, b: Optional[torch.Tensor], bn: Optional[dict], eps: float = BN_EPS):
@@ -170,7 +199,7 @@ class PlanBuilder:
         self.split = precision in ("bf16x2", "fp16x2")
         self.torch16 = torch.float16 if precision == "fp16x2" else torch.bfloat16
         self.torch_act = torch.float32 if precision == "fp32" else self.torch16
-        self.ops: List[_PendingOp] = []
+        self.ops: List[Op] = []
         self.keep: List[torch.Tensor] = []      # weights / biases kept alive
         self.syms: List[Sym] = []
         # tensor-core (wgmma) path: 16-bit operands only; tc=False forces the SIMT kernels (bf16: debugging)
@@ -203,13 +232,7 @@ class PlanBuilder:
 
     def keep_result(self, s: Sym) -> Sym:
         """mark an intermediate as a program result: its producer is not pruned and its buffer is not recycled."""
-        self._root_of(s).keep = True
-        return s
-
-    @staticmethod
-    def _root_of(s: Sym) -> Sym:
-        while s.parent is not None:
-            s = s.parent
+        Plan._root(s).keep = True
         return s
 
     def output(self, C, H, W, name):
@@ -223,14 +246,10 @@ class PlanBuilder:
         if x is None or not self.split or x.kind != "act":
             return x
         if x.parent is not None:
-            pf = self._to_f32(x.parent)
-            v = Sym(x.C, x.H, x.W, "actf32", parent=pf, ch_off=x.ch_off)
-            v.producer = pf.producer
-            return v
+            return Sym(x.C, x.H, x.W, "actf32", parent=self._to_f32(x.parent), ch_off=x.ch_off)
         if x._f32 is None:
             y = self._sym(x.C, x.H, x.W, "actf32", x.name + ".f32")
-            self._emit(_PendingOp(type=OP_CONVERT, flags=FLAG_TO_F32, k=(1, 1), stride=1, pad=(0, 0), weight=None, bias=None,
-                                  cout=x.C, dtype=self.act_dtype), [x], y)
+            self.ops.append(Op(OP_CONVERT, self.act_dtype, [x], y, x.C, flags=FLAG_TO_F32))
             x._f32 = y; y._sp = x
         return x._f32
 
@@ -240,8 +259,7 @@ class PlanBuilder:
             return y
         if y._sp is None:
             x = self._sym(y.C, y.H, y.W, "act", y.name + ".sp")
-            self._emit(_PendingOp(type=OP_CONVERT, flags=0, k=(1, 1), stride=1, pad=(0, 0), weight=None, bias=None,
-                                  cout=y.C, dtype=self.act_dtype), [y], x)
+            self.ops.append(Op(OP_CONVERT, self.act_dtype, [y], x, y.C))
             y._sp = x; x._f32 = y
         return y._sp
 
@@ -249,19 +267,14 @@ class PlanBuilder:
         """output of an op that runs on fp32 in split mode (kind 'actf32'), an ordinary activation otherwise."""
         return self._sym(C, H, W, "actf32" if self.split else "act")
 
-    def _emit(self, op: _PendingOp, srcs: Sequence[Sym], dst: Sym, extra: Sequence[Optional[Sym]] = ()):
-        if not hasattr(op, "dtype"):
-            op.dtype = self.act_dtype
-        if not hasattr(op, "acc_scale"):
-            op.acc_scale = 1.0
-        idx = len(self.ops)
-        for s in list(srcs) + [e for e in extra if e is not None]:
-            s.last_use = max(s.last_use, idx)
-        if dst.producer < 0:
-            dst.producer = idx
-        dst.last_use = max(dst.last_use, idx)
-        op.srcs, op.dst, op.extra = list(srcs), dst, list(extra)
-        self.ops.append(op)
+    def _storage(self, kind: str) -> Tuple[int, int, torch.dtype]:
+        """How a tensor of this kind is stored: (bytes per NHWC element slot, bytes per element inside one plane, torch
+        dtype of a plane).  Split activations are two 16-bit planes, hi then lo."""
+        if kind in ("f32", "actf32") or self.act_dtype == F32:
+            return 4, 4, torch.float32
+        if kind != "act":
+            raise KeyError(kind)
+        return (4, 2, self.torch16) if self.split else (2, 2, torch.bfloat16)
 
     def _dev(self, t: torch.Tensor, dtype=torch.float32):
         t = t.detach().to(device=self.device, dtype=dtype).contiguous()
@@ -277,10 +290,10 @@ class PlanBuilder:
         p[:, :, :co] = w.permute(2, 3, 1, 0).reshape(kh * kw, ci, co)
         return self._dev(p)
 
-    def _pack_conv_tc(self, w: torch.Tensor, bk: int):
+    def _pack_conv_tc(self, w: torch.Tensor, bk: int) -> Tuple[torch.Tensor, float]:
         """(Co,Ci,kh,kw) fp32 -> wgmma layout [kh*kw][Ci/bk][Co_pad16][bk] bf16 (K-major B operand, slab-major:
         the rows of one (tap, K-slab) block are contiguous, so a TMA weight box is one dense run of memory instead of
-        Co rows strided by Ci).  bk = the kernels' K-slab width."""
+        Co rows strided by Ci), and the factor the weights were multiplied by.  bk = the kernels' K-slab width."""
         co, ci, kh, kw = w.shape
         assert ci % bk == 0
         cop = (co + 15) // 16 * 16
@@ -289,12 +302,14 @@ class PlanBuilder:
         if self.split:
             # [plane][tap][slab][Co_pad][bk]: hi plane then lo plane; fp16 planes carry the weights times a power of two
             # (pow2_scale) whose inverse the kernel applies to the accumulator (cpb200_op.acc_scale)
-            self._last_scale = pow2_scale(w) if self.torch16 == torch.float16 else 1.0
-            t = split_planes(p * self._last_scale, self.torch16).to(self.device)
-            self.keep.append(t)
-            return t
-        self._last_scale = 1.0
-        return self._dev(p, torch.bfloat16)
+            scale = pow2_scale(w) if self.torch16 == torch.float16 else 1.0
+            return self._dev(split_planes(p * scale, self.torch16), self.torch16), scale
+        return self._dev(p, torch.bfloat16), 1.0
+
+    def _acc_scale(self, k_total: int, scale: float) -> float:
+        """cpb200_op.acc_scale of a tensor-core op that sums k_total products over weights packed times ``scale``: split
+        precisions undo the scale and compensate the accumulator's rounding toward zero (rz_compensation)."""
+        return rz_compensation(self.precision, k_total) / scale if self.split else 1.0
 
     @staticmethod
     def _tc_bk(srcs) -> int:
@@ -309,9 +324,7 @@ class PlanBuilder:
         """View of channels [off, off+c) of an NHWC activation (no copy): readable by conv ops through the op's
         ``src_pitch`` field.  Used to feed the six head 1x1 convs from ONE fused hidden tensor."""
         assert x.parent is None and x.kind == "act" and 0 <= off and off + c <= x.C and off % 16 == 0 and c % 16 == 0
-        v = Sym(c, x.H, x.W, "act", parent=x, ch_off=off)
-        v.producer = x.producer
-        return v
+        return Sym(c, x.H, x.W, "act", parent=x, ch_off=off)
 
     def _pack_stem_tc(self, w: torch.Tensor):
         """(N,3,7,7) fp32 -> the 128-byte-swizzled K-major B operand image of csrc/net_stem_tc.cu:
@@ -322,39 +335,25 @@ class PlanBuilder:
         wk[..., :7] = w.float()
         wk = torch.nn.functional.pad(wk.reshape(N, 168), (0, 24))                   # (N, 192)
         blk = wk.reshape(N, 3, 8, 8).permute(1, 0, 2, 3)                            # [slab][n][chunk j][e]
-        n_idx = torch.arange(N, device=w.device).view(1, N, 1, 1).expand(3, N, 8, 8)
-        j_idx = torch.arange(8, device=w.device).view(1, 1, 8, 1).expand(3, N, 8, 8)
-        img = torch.zeros(3, N, 8, 8, dtype=torch.float32, device=w.device)
-        img.scatter_(2, (j_idx ^ (n_idx & 7)), blk.contiguous())
-        return self._dev(img, torch.bfloat16)
+        return self._dev(_swizzle_chunks(blk, torch.arange(N, device=w.device) & 7), torch.bfloat16)
 
-    def _pack_stem_tc_h(self, w: torch.Tensor):
+    def _pack_stem_tc_h(self, w: torch.Tensor) -> Tuple[torch.Tensor, float]:
         """(N,3,7,7) fp32 -> B operand image of the stride-1 tensor-core stem (stem_tc_h_kernel): one block per
         horizontal tap s of N rows x 64 bytes, k = c*7 + r (21 real of 32), 64-byte swizzle: 16-byte chunk j of
-        row n stored at chunk j ^ ((n >> 1) & 3) (tap blocks are multiples of 1024 bytes)."""
+        row n stored at chunk j ^ ((n >> 1) & 3) (tap blocks are multiples of 1024 bytes); and the factor the weights
+        were multiplied by."""
         N = w.shape[0]
         wk = torch.zeros(7, N, 32, dtype=torch.float32, device=w.device)                # [s][n][k]
         wk[:, :, :21] = w.float().permute(3, 0, 1, 2).reshape(7, N, 21)
         blk = wk.reshape(7, N, 4, 8)                                                     # [s][n][chunk j][e]
-        n_idx = torch.arange(N, device=w.device).view(1, N, 1, 1).expand(7, N, 4, 8)
-        j_idx = torch.arange(4, device=w.device).view(1, 1, 4, 1).expand(7, N, 4, 8)
-        img = torch.zeros(7, N, 4, 8, dtype=torch.float32, device=w.device)
+        key = (torch.arange(N, device=w.device) >> 1) & 3
         if self.split:
             # per tap [hi tile (N rows) | lo tile (N rows)]; row n' = plane * N + n of the 2N-row block is swizzled with
             # (n' >> 1) & 3 == (n >> 1) & 3 (N is a multiple of 8)
-            self._last_scale = pow2_scale(w) if self.torch16 == torch.float16 else 1.0
-            planes = split_planes(blk * self._last_scale, self.torch16).float()       # (2, 7, N, 4, 8)
-            out = torch.zeros(7, 2, N, 4, 8, dtype=torch.float32, device=w.device)
-            for pl in range(2):
-                tmp = torch.zeros(7, N, 4, 8, dtype=torch.float32, device=w.device)
-                tmp.scatter_(2, (j_idx ^ ((n_idx >> 1) & 3)), planes[pl].contiguous())
-                out[:, pl] = tmp
-            t = out.to(self.torch16).to(self.device).contiguous()
-            self.keep.append(t)
-            return t
-        self._last_scale = 1.0
-        img.scatter_(2, (j_idx ^ ((n_idx >> 1) & 3)), blk.contiguous())
-        return self._dev(img, torch.bfloat16)
+            scale = pow2_scale(w) if self.torch16 == torch.float16 else 1.0
+            planes = split_planes(blk * scale, self.torch16)                             # (2, 7, N, 4, 8)
+            return self._dev(_swizzle_chunks(planes, key).transpose(0, 1).contiguous(), self.torch16), scale
+        return self._dev(_swizzle_chunks(blk, key), torch.bfloat16), 1.0
 
     def _tc_ok(self, srcs, co, kh, kw, stride, out, out_map, Wo):
         return (self.use_tc and stride in (1, 2) and Wo >= 8
@@ -378,7 +377,7 @@ class PlanBuilder:
             # q = -1..0 (a 3x3 conv, pad 1).  It then runs on the split tensor-core halo kernel instead of a CUDA-core
             # fp32 island (ResNet-50 B=16: 954 us + a CONVERT pass).
             z = self._sym(16, x.H // 2, x.W // 2)
-            self._emit(_PendingOp(type=OP_S2D, flags=0, k=(2, 2), stride=2, pad=(0, 0), weight=None, bias=None, cout=16), [x], z)
+            self.ops.append(Op(OP_S2D, self.act_dtype, [x], z, 16, k=(2, 2), stride=2))
             k2 = (k + 1) // 2 + 1
             p2 = k2 // 2
             w2 = torch.zeros(co, 16, k2, k2, dtype=torch.float32, device=w.device)
@@ -396,17 +395,14 @@ class PlanBuilder:
                 and not (self.split and stride != 1)):
             # tensor-core stem with the im2col done in shared memory (csrc/net_stem_tc.cu); split precisions: stride 1 only
             y = self._sym(co, Ho, Wo)
-            wp = self._pack_stem_tc_h(w) if stride == 1 else self._pack_stem_tc(w)
-            self._emit(_PendingOp(type=OP_STEM, flags=flags | FLAG_TC, k=(k, k), stride=stride, pad=(pad, pad),
-                                  weight=wp, bias=self._dev(b), cout=co,
-                                  acc_scale=(rz_compensation(self.precision, 7 * 32) / getattr(self, "_last_scale", 1.0))
-                                  if (stride == 1 and self.split) else 1.0), [x], y)
+            wp, scale = self._pack_stem_tc_h(w) if stride == 1 else (self._pack_stem_tc(w), 1.0)
+            self.ops.append(Op(OP_STEM, self.act_dtype, [x], y, co, flags=flags | FLAG_TC, k=(k, k), stride=stride,
+                               pad=(pad, pad), weight=wp, bias=self._dev(b), acc_scale=self._acc_scale(7 * 32, scale)))
             return y
         y = self._island_sym(co, Ho, Wo)
         wp = self._dev(w.permute(2, 3, 1, 0).reshape(k * k * ci, co))
-        self._emit(_PendingOp(type=OP_STEM, flags=flags, k=(k, k), stride=stride,
-                              pad=(pad, pad), weight=wp, bias=self._dev(b), cout=co,
-                              dtype=F32 if self.split else self.act_dtype), [x], y)
+        self.ops.append(Op(OP_STEM, F32 if self.split else self.act_dtype, [x], y, co, flags=flags, k=(k, k),
+                           stride=stride, pad=(pad, pad), weight=wp, bias=self._dev(b)))
         return self._to_split(y)
 
     def conv(self, srcs: Sequence[Sym], w, b, stride=1, pad=0, relu=False, res: Optional[Sym] = None,
@@ -444,13 +440,13 @@ class PlanBuilder:
             y = dst if dst is not None else self._sym(co, Hd, Wd)
         if tc:
             flags |= FLAG_TC
-        wp = self._pack_conv_tc(w, self._tc_bk(srcs)) if tc else self._pack_conv(w)
-        self._emit(_PendingOp(type=OP_CONV, flags=flags, k=(kh, kw), stride=stride, pad=(ph, pw),
-                              weight=wp, bias=self._dev(b), cout=co, ch_off=ch_off,
-                              out_map=(Hd, Wd, sy, sx, oy, ox), HoWo=(Ho, Wo), w_raw=w,
-                              dtype=F32 if island else self.act_dtype,
-                              acc_scale=(rz_compensation(self.precision, kh * kw * ci) / self._last_scale) if (tc and self.split) else 1.0),
-                   srcs, y, [res])
+            wp, scale = self._pack_conv_tc(w, self._tc_bk(srcs))
+            acc_scale = self._acc_scale(kh * kw * ci, scale)
+        else:
+            wp, acc_scale = self._pack_conv(w), 1.0
+        self.ops.append(Op(OP_CONV, F32 if island else self.act_dtype, list(srcs), y, co, flags=flags, k=(kh, kw),
+                           stride=stride, pad=(ph, pw), weight=wp, bias=self._dev(b), res=res, acc_scale=acc_scale,
+                           out_ch_off=ch_off, out_map=(Hd, Wd, sy, sx, oy, ox), HoWo=(Ho, Wo), w_raw=w))
         if island and out == "act" and _island_dst is None:
             return self._to_split(y)
         return y
@@ -472,26 +468,25 @@ class PlanBuilder:
                           pad_hw=(1 - a, 1 - bb), out_map=(Ho, Wo, 2, 2, a, bb, x.H, x.W))
         return self._to_split(y) if island else y
 
-    def _eltwise(self, op: _PendingOp, x: Sym, C, H, W, extra=(), gate: Optional[Sym] = None, f32_out=False) -> Sym:
-        """Emit an element-wise op (csrc/net_simt.cu: run_eltwise).  fp32 / bf16 run it natively.  Split precisions run
-        it on the planes (SpC / SpM handles) when every activation operand is a whole split tensor; there the SCALE_ADD
-        ``gate`` is read as fp32 and ``f32_out`` (AVGPOOL) writes an fp32 result.  Otherwise it runs on fp32 between
-        CONVERT ops (an fp32 island).  ``extra`` and ``gate`` become the op's extra operands, gate first."""
-        if self.split and all(s is None or (s.kind == "act" and s.parent is None) for s in [x, *extra]) \
+    def _eltwise(self, op_type: int, x: Sym, C, H, W, aux: Optional[Sym] = None, gate: Optional[Sym] = None,
+                 f32_out=False, **fields) -> Sym:
+        """Emit an element-wise op (csrc/net_simt.cu: run_eltwise) of C output channels; ``fields`` are the rest of its
+        Op.  fp32 / bf16 run it natively.  Split precisions run it on the planes (SpC / SpM handles) when every
+        activation operand is a whole split tensor; there the SCALE_ADD ``gate`` (the op's ``res``) is read as fp32 and
+        ``f32_out`` (AVGPOOL) writes an fp32 result.  Otherwise it runs on fp32 between CONVERT ops (an fp32 island)."""
+        if self.split and all(s is None or (s.kind == "act" and s.parent is None) for s in (x, aux)) \
                 and (gate is None or gate.parent is None):
             y = self._sym(C, H, W, "actf32" if f32_out else "act")
-            self._emit(op, [x], y, ([self._to_f32(gate)] if gate is not None else []) + list(extra))
+            self.ops.append(Op(op_type, self.act_dtype, [x], y, C, res=self._to_f32(gate), aux=aux, **fields))
             return self._to_split(y)
-        if self.split:
-            op.dtype = F32
         y = self._island_sym(C, H, W)
-        self._emit(op, [self._to_f32(x)], y, [self._to_f32(e) for e in ([gate] if gate is not None else []) + list(extra)])
+        self.ops.append(Op(op_type, F32 if self.split else self.act_dtype, [self._to_f32(x)], y, C,
+                           res=self._to_f32(gate), aux=self._to_f32(aux), **fields))
         return self._to_split(y)
 
     def maxpool(self, x: Sym, k=2, stride=2, pad=0):
         Ho = (x.H + 2 * pad - k) // stride + 1; Wo = (x.W + 2 * pad - k) // stride + 1
-        return self._eltwise(_PendingOp(type=OP_MAXPOOL, flags=0, k=(k, k), stride=stride, pad=(pad, pad),
-                                        weight=None, bias=None, cout=x.C), x, x.C, Ho, Wo)
+        return self._eltwise(OP_MAXPOOL, x, x.C, Ho, Wo, k=(k, k), stride=stride, pad=(pad, pad))
 
     def up_add(self, x: Sym, skip: Optional[Sym], w, *, b=None, act=None, stride=None, pad=None):
         """depthwise ConvTranspose2d weight (C,1,2f,2f), stride f, pad f//2, + skip.
@@ -503,8 +498,9 @@ class PlanBuilder:
         assert b is not None or act is None, "an activation needs the bias form"
         Ho = (x.H - 1) * f - 2 * p + k; Wo = (x.W - 1) * f - 2 * p + k
         wp = self._dev(w.float().reshape(C, k * k).t())          # [k*k][C]
-        return self._eltwise(_PendingOp(type=OP_DWDECONV_ADD, flags=_ACT_FLAG[act], k=(k, k), stride=f, pad=(p, p),
-                                        weight=wp, bias=None if b is None else self._dev(b), cout=C), x, C, Ho, Wo, [skip])
+        return self._eltwise(OP_DWDECONV_ADD, x, C, Ho, Wo, aux=skip, aux_pitch=skip.C if skip is not None else 0,
+                             flags=_ACT_FLAG[act], k=(k, k), stride=f, pad=(p, p), weight=wp,
+                             bias=None if b is None else self._dev(b))
 
     def dwconv(self, x: Sym, w, b, stride=1, act=None):
         """depthwise conv, w (C,1,k,k) BN-folded, pad k//2   (mobilenetv3.py:124-127)."""
@@ -512,35 +508,31 @@ class PlanBuilder:
         assert C == x.C
         Ho = (x.H + 2 * (k // 2) - k) // stride + 1; Wo = (x.W + 2 * (k // 2) - k) // stride + 1
         wp = self._dev(w.float().reshape(C, k * k).t())          # [k*k][C]
-        return self._eltwise(_PendingOp(type=OP_DWCONV, flags=_ACT_FLAG[act], k=(k, k), stride=stride, pad=(k // 2, k // 2),
-                                        weight=wp, bias=self._dev(b), cout=C), x, C, Ho, Wo)
+        return self._eltwise(OP_DWCONV, x, C, Ho, Wo, flags=_ACT_FLAG[act], k=(k, k), stride=stride,
+                             pad=(k // 2, k // 2), weight=wp, bias=self._dev(b))
 
     def avgpool(self, x: Sym):
         """global average pool -> (C, 1, 1)   (mobilenetv3.py:100).  Split mode: planes in, fp32 out (the 1x1-map SE convs
         that follow run on fp32 anyway)."""
-        return self._eltwise(_PendingOp(type=OP_AVGPOOL, flags=0, k=(x.H, x.W), stride=1, pad=(0, 0), weight=None, bias=None,
-                                        cout=x.C), x, x.C, 1, 1, f32_out=True)
+        return self._eltwise(OP_AVGPOOL, x, x.C, 1, 1, f32_out=True, k=(x.H, x.W))
 
     def scale_add(self, x: Sym, gate: Sym, skip: Optional[Sym] = None):
         """x * gate[b, c] (+ skip)   (mobilenetv3.py:111,146).  Split mode: x / skip / result are planes, the gate is fp32."""
         assert gate.C == x.C and gate.H == 1 and gate.W == 1
-        return self._eltwise(_PendingOp(type=OP_SCALE_ADD, flags=0, k=(1, 1), stride=1, pad=(0, 0), weight=None, bias=None,
-                                        cout=x.C), x, x.C, x.H, x.W, [skip], gate=gate)
+        return self._eltwise(OP_SCALE_ADD, x, x.C, x.H, x.W, aux=skip, gate=gate)
 
     def upsample_add(self, x: Sym, skip: Optional[Sym], f: int, relu=False):
         """nearest-neighbour upsample x f of ``x`` (+ skip)(+ReLU)   (pose_higher_hrnet.py:186-187,224-232)."""
-        return self._eltwise(_PendingOp(type=OP_UPSAMPLE_ADD, flags=FLAG_RELU if relu else 0, k=(1, 1), stride=f, pad=(0, 0),
-                                        weight=None, bias=None, cout=x.C), x, x.C, x.H * f, x.W * f, [skip])
+        return self._eltwise(OP_UPSAMPLE_ADD, x, x.C, x.H * f, x.W * f, aux=skip,
+                             aux_pitch=skip.C if skip is not None else 0, flags=FLAG_RELU if relu else 0, stride=f)
 
     def avgpool2(self, x: Sym):
         """2x2 / stride-2 average pool, floor mode   (hardnet.py:141 nn.AvgPool2d(2, 2))."""
-        return self._eltwise(_PendingOp(type=OP_AVGPOOL2, flags=0, k=(2, 2), stride=2, pad=(0, 0), weight=None, bias=None,
-                                        cout=x.C), x, x.C, x.H // 2, x.W // 2)
+        return self._eltwise(OP_AVGPOOL2, x, x.C, x.H // 2, x.W // 2, k=(2, 2), stride=2)
 
     def resize_bilinear(self, x: Sym, Ho: int, Wo: int):
         """bilinear resize to (Ho, Wo) with align_corners=True   (hardnet.py:95-100, TransitionUp)."""
-        return self._eltwise(_PendingOp(type=OP_RESIZE_BILINEAR, flags=0, k=(1, 1), stride=1, pad=(0, 0), weight=None,
-                                        bias=None, cout=x.C), x, x.C, Ho, Wo)
+        return self._eltwise(OP_RESIZE_BILINEAR, x, x.C, Ho, Wo)
 
     def dcn(self, x: Sym, w, b, om_w, om_b, relu=True):
         """DCN module (dcn_v2.py:117-127) with BN already folded into (w, b)."""
@@ -553,33 +545,19 @@ class PlanBuilder:
         island = self.split and not tc
         xin = self._to_f32(x) if island else x
         y = self._sym(co, x.H, x.W, "actf32" if island else "act")
-        wp = self._pack_conv_tc(w, 64) if tc else self._pack_conv(w)
-        self._emit(_PendingOp(type=OP_DCN, flags=(FLAG_RELU if relu else 0) | (FLAG_TC if tc else 0), k=(3, 3),
-                              stride=1, pad=(1, 1), weight=wp, bias=self._dev(b), cout=co, w_raw=w,
-                              dtype=F32 if island else self.act_dtype,
-                              acc_scale=(rz_compensation(self.precision, 9 * x.C) / self._last_scale) if (tc and self.split) else 1.0),
-                   [xin], y, [om])
+        if tc:
+            wp, scale = self._pack_conv_tc(w, 64)
+            acc_scale = self._acc_scale(9 * x.C, scale)
+        else:
+            wp, acc_scale = self._pack_conv(w), 1.0
+        self.ops.append(Op(OP_DCN, F32 if island else self.act_dtype, [xin], y, co,
+                           flags=(FLAG_RELU if relu else 0) | (FLAG_TC if tc else 0), k=(3, 3), pad=(1, 1), weight=wp,
+                           bias=self._dev(b), aux=om, aux_pitch=om.C, acc_scale=acc_scale, w_raw=w))
         return self._to_split(y) if island else y
 
     # ---- finalisation -----------------------------------------------------------------------
     def build(self) -> "Plan":
         return Plan(self)
-
-
-def _esize(pb: "PlanBuilder", kind: str) -> int:
-    """bytes per ELEMENT SLOT of an NHWC tensor of this kind (split activations: two 16-bit planes)."""
-    if kind in ("f32", "actf32"):
-        return 4
-    if kind == "act":
-        return 4 if (pb.act_dtype == F32 or pb.split) else 2
-    raise KeyError(kind)
-
-
-def _ptr_esize(pb: "PlanBuilder", kind: str) -> int:
-    """bytes per element for pointer arithmetic inside ONE plane (channel-slice offsets)."""
-    if kind in ("f32", "actf32"):
-        return 4
-    return 4 if pb.act_dtype == F32 else 2
 
 
 class Plan:
@@ -599,7 +577,7 @@ class Plan:
         for i, po in enumerate(pb.ops):
             o = self.ops[i]
             o.type = po.type; o.flags = po.flags; o.act_dtype = po.dtype
-            o.acc_scale = float(getattr(po, "acc_scale", 1.0))
+            o.acc_scale = po.acc_scale
             s0 = po.srcs[0]
             o.B, o.H, o.W = pb.B, s0.H, s0.W
             o.nsrc = len(po.srcs)
@@ -608,36 +586,27 @@ class Plan:
                 if s.kind == "nchw_in":
                     self.in_slots.append((i, j))
                 else:
-                    o.src[j] = s.buf.data_ptr() + s.ch_off * _ptr_esize(pb, s.kind)
+                    o.src[j] = s.buf.data_ptr() + s.ch_off * pb._storage(s.kind)[1]
                     o.src_pitch[j] = s.pitch if s.parent is not None else 0
             if po.type == OP_HEADS:
                 self._set_heads(i, o, po)
                 continue
             o.cout = po.cout
             o.kh, o.kw = po.k; o.stride = po.stride; o.pad_h, o.pad_w = po.pad
+            o.Hd, o.Wd, o.out_sy, o.out_sx, o.out_oy, o.out_ox = po.out_map
+            o.Ho, o.Wo = po.HoWo
+            o.out_ch_off = po.out_ch_off
             d = po.dst
-            if po.type == OP_CONV:
-                o.Hd, o.Wd, o.out_sy, o.out_sx, o.out_oy, o.out_ox = po.out_map
-                o.Ho, o.Wo = po.HoWo
-            else:
-                o.Ho, o.Wo, o.Hd, o.Wd = d.H, d.W, d.H, d.W
-                o.out_sy = o.out_sx = 1
-            o.out_ch_off = getattr(po, "ch_off", 0)
             o.out_ch_total = d.C
             if d.kind == "nchw_out":
                 self.out_slots.setdefault(d.name, []).append(i)
             else:
                 o.dst = d.buf.data_ptr()
-            ex = po.extra
-            if po.type == OP_CONV and ex and ex[0] is not None:
-                o.res = ex[0].buf.data_ptr()
-            if po.type in (OP_DCN, OP_DWDECONV_ADD, OP_UPSAMPLE_ADD) and ex and ex[0] is not None:
-                o.aux = ex[0].buf.data_ptr()
-                o.aux_pitch = ex[0].C
-            if po.type == OP_SCALE_ADD:
-                o.res = ex[0].buf.data_ptr()
-                if ex[1] is not None:
-                    o.aux = ex[1].buf.data_ptr()
+            if po.res is not None:
+                o.res = po.res.buf.data_ptr()
+            if po.aux is not None:
+                o.aux = po.aux.buf.data_ptr()
+            o.aux_pitch = po.aux_pitch
             if po.weight is not None:
                 o.weight = po.weight.data_ptr()
             if po.bias is not None:
@@ -649,41 +618,31 @@ class Plan:
 
     @staticmethod
     def _root(s: Sym) -> Sym:
+        """the tensor that owns the storage of ``s`` (a channel slice's parent); liveness is tracked on it"""
         while s.parent is not None:
             s = s.parent
         return s
 
+    def _readers(self, ops: Sequence[Op]) -> Dict[int, List[int]]:
+        """id(root Sym) -> indices of the ops reading it, ascending"""
+        readers = {}
+        for i, po in enumerate(ops):
+            for s in po.operands():
+                readers.setdefault(id(self._root(s)), []).append(i)
+        return readers
+
     def _prune(self, pb: PlanBuilder):
         """Split precisions emit a CONVERT back to planes after every fp32-island op; inside a chain of island ops it is
-        dead.  Drop ops whose result nobody reads (outputs, externals and the program's last op are roots) and recompute
-        the producer / last-use indices the allocator works from."""
+        dead.  Drop ops whose result nobody reads (outputs, externals and the program's last op are roots)."""
         if not pb.split:
             return
         ops = pb.ops
-        consumers = {}                                  # id(root sym) -> op indices reading it
-        for i, po in enumerate(ops):
-            for s in list(po.srcs) + [e for e in po.extra if e is not None]:
-                consumers.setdefault(id(self._root(s)), []).append(i)
+        readers = self._readers(ops)
         live = [False] * len(ops)
         for i in range(len(ops) - 1, -1, -1):
             d = self._root(ops[i].dst)
-            live[i] = i == len(ops) - 1 or d.fixed or d.keep or any(live[c] for c in consumers.get(id(d), ()) if c > i)
+            live[i] = i == len(ops) - 1 or d.fixed or d.keep or any(live[c] for c in readers.get(id(d), ()) if c > i)
         pb.ops = [po for i, po in enumerate(ops) if live[i]]
-        self._reindex(pb)
-
-    def _reindex(self, pb: PlanBuilder):
-        """recompute the producer / last-use indices the allocator works from after ops were removed or merged"""
-        for s in pb.syms:
-            s.producer = -1
-            if s.parent is None:
-                s._last_use = -1
-        for i, po in enumerate(pb.ops):
-            for s in list(po.srcs) + [e for e in po.extra if e is not None]:
-                s.last_use = max(s.last_use, i)
-            d = po.dst
-            if d.producer < 0:
-                d.producer = i
-            d.last_use = max(d.last_use, i)
 
     def _fuse_heads(self, pb: PlanBuilder):
         """Replace (tensor-core 3x3 conv + ReLU -> 1x1 conv with NCHW fp32 output) pairs over one shared input by ONE
@@ -695,15 +654,11 @@ class Plan:
         if not pb.use_tc:
             return
         ops = pb.ops
-        readers = {}                                    # id(root sym) -> op indices reading it
-        for i, po in enumerate(ops):
-            for s in list(po.srcs) + [e for e in po.extra if e is not None]:
-                readers.setdefault(id(self._root(s)), []).append(i)
+        readers = self._readers(ops)
         pairs = []
         for i, a in enumerate(ops):
             if not (a.type == OP_CONV and a.flags == FLAG_TC | FLAG_RELU and a.k == (3, 3) and a.stride == 1
-                    and a.pad == (1, 1) and len(a.srcs) == 1 and not any(e is not None for e in a.extra)
-                    and getattr(a, "ch_off", 0) == 0):
+                    and a.pad == (1, 1) and len(a.srcs) == 1 and a.res is None and a.out_ch_off == 0):
                 continue
             x, h = a.srcs[0], a.dst
             if not (x.kind == "act" and x.parent is None and x.C % 16 == 0 and x.C <= 64 and x.H >= 8 and x.W >= 8
@@ -716,8 +671,8 @@ class Plan:
             b = ops[r[0]]
             d = b.dst
             if not (b.type == OP_CONV and b.flags == FLAG_TC | FLAG_OUT_NCHW_F32 and b.k == (1, 1) and len(b.srcs) == 1
-                    and b.srcs[0] is h and not any(e is not None for e in b.extra) and b.cout <= 48
-                    and d.kind == "nchw_out" and d.C == b.cout and getattr(b, "ch_off", 0) == 0
+                    and b.srcs[0] is h and b.res is None and b.cout <= 48
+                    and d.kind == "nchw_out" and d.C == b.cout and b.out_ch_off == 0
                     and b.out_map == (x.H, x.W, 1, 1, 0, 0) and not readers.get(id(d))):
                 continue
             pairs.append((i, r[0]))
@@ -732,14 +687,12 @@ class Plan:
         w = torch.stack([a.weight for a, _ in heads]).contiguous()       # [head][(plane)][tap][K-slab][hid][bk]
         bias = torch.cat([a.bias for a, _ in heads]).contiguous()
         pb.keep += [w, bias]
-        fused = _PendingOp(type=OP_HEADS, flags=FLAG_TC | FLAG_OUT_NCHW_F32, k=(3, 3), stride=1, pad=(1, 1), weight=w,
-                           bias=bias, cout=sum(b.cout for _, b in heads), dtype=pb.act_dtype, acc_scale=1.0, heads=heads,
-                           srcs=[x0], dst=heads[0][1].dst, extra=[])
+        fused = Op(OP_HEADS, pb.act_dtype, [x0], heads[0][1].dst, sum(b.cout for _, b in heads),
+                   flags=FLAG_TC | FLAG_OUT_NCHW_F32, k=(3, 3), pad=(1, 1), weight=w, bias=bias, heads=heads)
         drop = {k for p in pairs for k in p}
         pb.ops = [fused if k == first else po for k, po in enumerate(ops) if k == first or k not in drop]
-        self._reindex(pb)
 
-    def _set_heads(self, i: int, o: OpStruct, po: _PendingOp):
+    def _set_heads(self, i: int, o: OpStruct, po: Op):
         s0 = po.srcs[0]
         o.cout = po.cout
         o.kh = o.kw = 3; o.stride = 1; o.pad_h = o.pad_w = 1
@@ -751,14 +704,18 @@ class Plan:
             e = tab[k]
             e.hidden, e.cout = a.cout, b.cout
             e.weight, e.bias = b.weight.data_ptr(), b.bias.data_ptr()
-            e.acc_scale3, e.acc_scale1 = float(a.acc_scale), float(b.acc_scale)
+            e.acc_scale3, e.acc_scale1 = a.acc_scale, b.acc_scale
             self.out_slots.setdefault(b.dst.name, []).append((i, k))
         self._head_tables[i] = tab
         o.aux = ctypes.addressof(tab); o.aux_pitch = len(tab)
         o.weight = po.weight.data_ptr(); o.bias = po.bias.data_ptr()
 
     def _allocate(self, pb: PlanBuilder):
-        """Liveness-based buffer reuse: a buffer returns to the pool after its last consumer."""
+        """Liveness-based buffer reuse: a buffer returns to the pool after the last op that reads or writes it."""
+        last_use = {}                                   # id(root sym) -> index of the last op reading or writing it
+        for i, po in enumerate(pb.ops):
+            for s in (*po.operands(), po.dst):
+                last_use[id(self._root(s))] = i
         pool = {}
         release_at = {}
         self.buffers = []
@@ -767,7 +724,7 @@ class Plan:
         for i, po in enumerate(pb.ops):
             d = po.dst
             if not d.fixed and d.buf is None:
-                nbytes = pb.B * d.H * d.W * d.C * _esize(pb, d.kind)
+                nbytes = pb.B * d.H * d.W * d.C * pb._storage(d.kind)[0]
                 cand = [k for k in pool if k >= nbytes and pool[k]]
                 if cand:
                     raw = pool[min(cand)].pop()
@@ -776,7 +733,7 @@ class Plan:
                     self.buffers.append(raw); total += nbytes
                 d.buf = raw
                 if not d.keep:
-                    release_at.setdefault(d.last_use, []).append(d)
+                    release_at.setdefault(last_use[id(d)], []).append(d)
             for s in release_at.pop(i, []):
                 if not no_reuse:
                     pool.setdefault(s.buf.numel(), []).append(s.buf)
@@ -786,15 +743,16 @@ class Plan:
         """An internal NHWC activation (valid until a later op reuses its buffer): a view, or — split precisions —
         the fp32 value hi + lo reassembled from the two planes."""
         pb = self.pb
-        n = pb.B * sym.H * sym.W * sym.C
-        if pb.split and sym.kind == "act":
-            raw = sym.buf if not sym.fixed else sym.buf.view(torch.uint8).view(-1)
-            planes = raw[: 4 * n].view(pb.torch16).view(2, pb.B, sym.H, sym.W, sym.C)
-            return planes[0].float() + planes[1].float()
-        if sym.fixed:
+        split = pb.split and sym.kind == "act"
+        if sym.fixed and not split:
             return sym.buf
-        dt = torch.float32 if (sym.kind in ("f32", "actf32") or pb.act_dtype == F32) else torch.bfloat16
-        return sym.buf[: n * (4 if dt == torch.float32 else 2)].view(dt).view(pb.B, sym.H, sym.W, sym.C)
+        slot, _, dt = pb._storage(sym.kind)
+        raw = sym.buf.view(torch.uint8).view(-1) if sym.fixed else sym.buf
+        t = raw[: pb.B * sym.H * sym.W * sym.C * slot].view(dt)
+        if split:
+            hi, lo = t.view(2, pb.B, sym.H, sym.W, sym.C)
+            return hi.float() + lo.float()
+        return t.view(pb.B, sym.H, sym.W, sym.C)
 
     def bind(self, x: torch.Tensor, outs: dict):
         """Point the program at this call's input and output tensors."""

@@ -140,7 +140,7 @@ def test_plan_lowering_shapes():
     assert abs(gmac_512 - 40.17) < 0.1, gmac_512          # SURVEY: 40.24 incl. 0.067 dead project convs
 
 
-def test_split_plane_host_helpers():
+def test_split_plane_helpers_and_packed_weight_scale():
     """Host side of the split-operand precisions (plan.py): hi = rn16(v), lo = rn16(v - hi) reproduces v to 2^-22 (fp16
     planes) / 2^-16 (bf16 planes); the fp16 weight pre-scale is an exact power of two that keeps the lo plane out of the
     subnormals; packed tensor-core weights keep hi + lo == w * scale; the accumulator compensation is linear in K."""
@@ -169,8 +169,8 @@ def test_split_plane_host_helpers():
     assert 0 < c1 < 1e-5 and abs(c2 - 2 * c1) < 1e-12
     pb = PlanBuilder(1, 32, 32, "fp16x2", torch.device("cpu"))
     w = torch.randn(48, 64, 3, 3, generator=g) * 0.05
-    packed = pb._pack_conv_tc(w, 64)                                                # [plane][tap][slab][Co_pad][bk]
-    sc = pb._last_scale
+    packed, sc = pb._pack_conv_tc(w, 64)                                            # [plane][tap][slab][Co_pad][bk]
+    assert sc == pow2_scale(w) and pb._acc_scale(576, sc) == rz_compensation("fp16x2", 576) / sc
     rec = (packed[0].float() + packed[1].float())[:, 0, :48, :]                     # [tap][Co][Ci]
     ref = (w * sc).permute(2, 3, 0, 1).reshape(9, 48, 64)
     assert (rec - ref).abs().max().item() <= ref.abs().max().item() * 2.0 ** -21

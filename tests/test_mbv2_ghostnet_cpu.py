@@ -130,7 +130,7 @@ def _plan(arch, precision, B, H, W):
     return m._plan(B, H, W, torch.device("cpu"))
 
 
-def test_mobilenetv2_plan_census():
+def test_mobilenetv2_lowering_census():
     """fp32 lowering on the CPU: ReLU6 on the stem, the 16 expand convs and the 17 depthwise convs; the three IDAUp
     steps are DWDECONV_ADD ops in the bias form (k 2, stride 2, pad 0, ReLU, a skip); every activation is a multiple
     of 16 channels; the heads run at stride 4."""
@@ -144,7 +144,7 @@ def test_mobilenetv2_plan_census():
     assert all(o.flags & FLAG_RELU6 for o in ops if o.type in (OP_STEM, OP_DWCONV))
     ups = [o for o in ops if o.type == OP_DWDECONV_ADD]
     assert all(o.k == (2, 2) and o.stride == 2 and o.pad == (0, 0) and o.flags == FLAG_RELU and o.bias is not None
-               and o.extra[0] is not None and o.srcs[0].C == 32 for o in ups)
+               and o.aux is not None and o.srcs[0].C == 32 for o in ups)
     assert [(o.dst.H, o.dst.W) for o in ups] == [(6, 10), (12, 20), (24, 40)]
     assert all(s.C % 16 == 0 for o in ops if o.type != OP_STEM for s in o.srcs)
 
