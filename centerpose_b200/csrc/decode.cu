@@ -531,17 +531,24 @@ __device__ void group_joint(Smem &s, const DecodeParams &p, int b, int j) {
     l = __fsub_rn(cx, hw); t = __fsub_rn(cy, hh); r = __fadd_rn(cx, hw); bt = __fadd_rn(cy, hh);
     const int hk = (K + 1) >> 1;
     const int c0 = half ? hk : 0, c1 = half ? K : hk;
-    // nearest candidate on SQUARED distance (monotone in the reference's sqrt); exact ties ->
-    // the reference's first-minimum over its score-sorted list = higher score, then lower index
+    // nearest candidate on the rounded distance sqrt(dx^2 + dy^2) the reference compares: two different squared
+    // distances can round to the same sqrt, and that is a tie there.  Ties -> the reference's first minimum over its
+    // score-sorted list = higher score, then lower index.  A candidate whose sqrt rounds to <= best_d has a squared
+    // distance at most (1 + 2^-23)^2 times that of the candidate that set best_d, so only squared distances up to
+    // `near` (a 2^-20 margin above it) take the sqrt.
+    float near = INFINITY;
 #pragma unroll 4
     for (int c = c0; c < c1; ++c) {                                                 // :286-289
       const float2 g = s.gxy[c];
       const float dx = __fsub_rn(kx, g.x), dy = __fsub_rn(ky, g.y);
-      const float d = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
-      if (d < best_d) { best_d = d; best_c = c; }
-      else if (d == best_d) {
-        const float sc = s.gs[c], sb = s.gs[best_c];
-        if (sc > sb || (sc == sb && s.gi[c] < s.gi[best_c])) best_c = c;
+      const float q = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+      if (q <= near) {
+        const float d = __fsqrt_rn(q);
+        if (d < best_d) { best_d = d; best_c = c; near = __fmul_rn(q, 1.0f + 0x1p-20f); }
+        else if (d == best_d) {
+          const float sc = s.gs[c], sb = s.gs[best_c];
+          if (sc > sb || (sc == sb && s.gi[c] < s.gi[best_c])) best_c = c;
+        }
       }
     }
     if (half) { s.hd[pidx] = best_d; s.hc[pidx] = best_c; }
@@ -556,7 +563,7 @@ __device__ void group_joint(Smem &s, const DecodeParams &p, int b, int j) {
         if (sc > sb || (sc == sb && s.gi[oc] < s.gi[best_c])) best_c = oc;
       }
     }
-    const float min_dist = __fsqrt_rn(best_d);
+    const float min_dist = best_d;
     const float2 g = s.gxy[best_c];
     const float sx = g.x, sy = g.y, ss = s.gs[best_c];
     const bool rej = (sx < l) || (sx > r) || (sy < t) || (sy > bt) || (ss < p.thresh) ||

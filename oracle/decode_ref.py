@@ -168,7 +168,11 @@ def synth_decode_inputs(B, H, W, seed=317, J=17, kind="smooth", dtype=F32):
           'sparse'  fewer than K positive peaks (zeros get selected)
           'plateau' constant heat-map (every cell ties)
           'lowhp'   all hm_hp <= 0.1 (every joint falls back; col 39+j = -1)
+          'sqrttie', 'sqrttie_swap', 'sqtie', 'thresh'
+                    constructed tie and threshold cases of the keypoint grouping, see :func:`_constructed`
     Returns dict of fp32 NCHW arrays: heat, wh, kps, reg, hm_hp, hp_offset."""
+    if kind in CONSTRUCTED:
+        return _constructed(B, H, W, seed, J, kind)
     rng = np.random.RandomState(seed)
 
     def heatmap(C):
@@ -205,3 +209,55 @@ def synth_decode_inputs(B, H, W, seed=317, J=17, kind="smooth", dtype=F32):
         hm_hp=hm_hp.astype(dtype),
         hp_offset=rng.uniform(0, 1, size=(B, 2, H, W)).astype(dtype),
     )
+
+
+CONSTRUCTED = ("sqrttie", "sqrttie_swap", "sqtie", "thresh")
+
+
+def _constructed(B, H, W, seed, J, kind):
+    """Hand-placed keypoint-grouping cases on a 'smooth' base whose heat maps are cleared (every image the same;
+    needs H, W >= 40).  All placed values are exact fp32.
+
+    'sqrttie'       one person at cell (20,20), joint-0 guess (20.3, 20.0).  Candidate A at cell (20,22), score 0.5,
+                    lands at (22.783405, 20.632195); candidate B at cell (20,18), score 0.6, at (17.816463, 20.631685).
+                    Their squared distances 6.5669756 (A) and 6.566976 (B) are adjacent floats with the same fp32
+                    sqrt: the reference's dist.min() takes B, the first of its score-sorted list.
+    'sqrttie_swap'  the same with the scores swapped: A (0.6, the higher flat index) is first in score order.
+    'sqtie'         exactly equal squared distances (dx = +-2 on joint 0, dy = +-2 on joint 1): the higher score
+                    wins, on joint 0 from the higher flat index, on joint 1 from the lower one.
+    'thresh'        four people; on every joint each person has a candidate of exactly fp32(0.1) two cells from its
+                    guess (masked: the reference keeps scores > 0.1) and one of nextafter(0.1, 1) four rows away
+                    (kept, and within 0.3 * box size), each an isolated 3x3 maximum.  Joint J-1 has only the 0.1
+                    candidates, so it has no candidate at all.
+    """
+    assert H >= 40 and W >= 40, "constructed decode kinds need a map of at least 40x40"
+    d = synth_decode_inputs(B, H, W, seed, J, "smooth")
+    heat, hm_hp, wh, kps, reg, off = d["heat"], d["hm_hp"], d["wh"], d["kps"], d["reg"], d["hp_offset"]
+    heat[:] = 0
+    hm_hp[:] = 0
+    f = F32
+    if kind in ("sqrttie", "sqrttie_swap"):
+        sa, sb = (f(0.5), f(0.6)) if kind == "sqrttie" else (f(0.6), f(0.5))
+        heat[:, 0, 20, 20] = f(0.9)
+        wh[:, :, 20, 20] = f(30)
+        kps[:, 0, 20, 20] = f(0.3); kps[:, 1, 20, 20] = f(0.0)
+        hm_hp[:, 0, 20, 22] = sa; off[:, 0, 20, 22] = f(0.7834044); off[:, 1, 20, 22] = f(0.6321947)
+        hm_hp[:, 0, 20, 18] = sb; off[:, 0, 20, 18] = f(-0.18353653); off[:, 1, 20, 18] = f(0.63168526)
+    elif kind == "sqtie":
+        heat[:, 0, 20, 20] = f(0.9)
+        wh[:, :, 20, 20] = f(30)
+        kps[:, 0:2, 20, 20] = (f(0.5), f(0.0))            # joint 0 guess (20.5, 20.0)
+        hm_hp[:, 0, 20, 18] = f(0.5); off[:, :, 20, 18] = (f(0.5), f(0.0))      # (18.5, 20.0)
+        hm_hp[:, 0, 20, 23] = f(0.6); off[:, :, 20, 23] = (f(-0.5), f(0.0))     # (22.5, 20.0)
+        kps[:, 2:4, 20, 20] = (f(0.0), f(0.5))            # joint 1 guess (20.0, 20.5)
+        hm_hp[:, 1, 18, 20] = f(0.7); off[:, :, 18, 20] = (f(0.0), f(0.5))      # (20.0, 18.5)
+        hm_hp[:, 1, 23, 20] = f(0.4); off[:, :, 23, 20] = (f(0.0), f(-0.5))     # (20.0, 22.5)
+    elif kind == "thresh":
+        t, t_up = f(0.1), np.nextafter(f(0.1), f(1))
+        for (y, x), s in zip(((8, 8), (8, 28), (26, 8), (26, 28)), (0.9, 0.8, 0.7, 0.6)):
+            heat[:, 0, y, x] = f(s)
+            wh[:, :, y, x] = f(16); reg[:, :, y, x] = f(0.5)
+            kps[:, :, y, x] = 0                            # every joint's guess is the cell (x, y)
+            hm_hp[:, :, y, x + 2] = t; off[:, :, y, x + 2] = f(0.5)       # (x + 2.5, y + 0.5): masked
+            hm_hp[:, :J - 1, y + 4, x] = t_up; off[:, :, y + 4, x] = f(0.5)   # (x + 0.5, y + 4.5): kept
+    return d

@@ -42,6 +42,11 @@ DECODE_CASES = [
     ("sparse_1x64x64", 1, 64, 64, 100, "sparse", 11, True, True),
     ("lowhp_1x64x64", 1, 64, 64, 100, "lowhp", 12, True, True),
     ("uniform_1x20x12_k40_fewpeaks", 1, 20, 12, 40, "uniform", 13, True, True),
+    # constructed grouping cases (decode_ref._constructed): nearest-candidate ties and the 0.1 keypoint threshold
+    ("sqrttie_1x40x40", 1, 40, 40, 10, "sqrttie", 0, True, True),
+    ("sqrttie_swap_1x40x40", 1, 40, 40, 10, "sqrttie_swap", 0, True, True),
+    ("sqtie_1x40x40", 1, 40, 40, 10, "sqtie", 0, True, True),
+    ("thresh_1x40x40", 1, 40, 40, 10, "thresh", 0, True, True),
 ]
 
 
@@ -65,7 +70,7 @@ def gen_decode(ns):
         # rows whose centre score is > 0 are tie-free by construction -> bit-exact
         pos = ref[:, :, 4] > 0
         assert np.array_equal(mine[pos], ref[pos]), f"decode oracle != reference on {name}"
-        if kind not in ("sparse", "plateau") and "fewpeaks" not in name:
+        if kind not in ("sparse", "plateau") + decode_ref.CONSTRUCTED and "fewpeaks" not in name:
             assert pos.all(), name
         np.savez_compressed(os.path.join(GOLD, f"decode_{name}.npz"), det=ref,
                             meta=np.array([B, H, W, K, seed, int(use_reg), int(use_off)]),
