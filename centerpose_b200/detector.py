@@ -282,9 +282,9 @@ def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda
     return buf, {"o_rsz": o_rsz, "o_aff": o_aff, "o_idx": o_idx, "o_img": o_img, "scratch": scratch}
 
 
-# run_images decodes JPEG and PNG files on the device in launches of at most this many images, whose workspace (JPEG
-# coefficients and planes, PNG scanlines; reused from launch to launch) stays below JPEG_CHUNK_WORKSPACE bytes unless
-# one image needs more
+# run_images decodes JPEG, PNG and WebP files on the device in launches of at most this many images, whose workspace
+# (JPEG coefficients and planes, PNG scanlines, WebP coefficients and planes; reused from launch to launch) stays below
+# JPEG_CHUNK_WORKSPACE bytes unless one image needs more
 JPEG_CHUNK_IMAGES = 256
 JPEG_CHUNK_WORKSPACE = 512 << 20
 # PNG files go to the device only when a call holds at least this many of them.  The inflate is serial within a file,
@@ -292,6 +292,11 @@ JPEG_CHUNK_WORKSPACE = 512 << 20
 # cv2.imread takes 9-17 ms per file on one host thread; below this count the host decode is faster
 # (tools/bench_png.py)
 PNG_DEVICE_MIN_IMAGES = 16
+# Lossy WebP files likewise go to the device only from this many per call on.  The entropy decode is serial within a
+# file, so one launch takes about as long for one file as for 256 (51-59 ms at quality 75, 128-136 ms at 95, 640x480
+# files on one H100).  run_images from quality-75 files with the device decode against cv2.imread: 0.30x for one file,
+# 1.03x for 8, 1.6x for 16, 3.0x for 256 (tools/bench_webp.py)
+WEBP_DEVICE_MIN_IMAGES = 16
 
 
 def _swap_pairs(C, pairs, device):
@@ -466,15 +471,16 @@ class MultiPoseDetector(BaseDetector):
         """Every input of ``run_images`` in one device buffer of packed HWC uint8 BGR images.  Returns
         ``(views, offsets, buffer)``: per input a (h, w, 3) view of its slot and the slot's byte offset.
 
-        The files' headers are parsed first (``jpeg.parse``, ``png.parse``), so every size is known before any pixel
-        exists.  The files the device can decode, with their tables, go up in one pinned buffer and are decoded by
-        ``cpb200_jpeg_decode_batch`` and ``cpb200_png_decode_batch`` in chunks of at most ``JPEG_CHUNK_IMAGES``
-        images that reuse one workspace; PNG files only when the call holds at least ``PNG_DEVICE_MIN_IMAGES`` of them,
-        since one PNG launch costs about as much as a dozen host decodes.  The other files (``cv2.imread``) and the
-        arrays take the host path, and
+        The files' headers are parsed first (``jpeg.parse``, ``png.parse``, ``webp.parse``), so every size is known
+        before any pixel exists.  The files the device can decode, with their tables, go up in one pinned buffer and
+        are decoded by each format module's ``KERNEL`` (``cpb200_jpeg_decode_batch``, ``cpb200_png_decode_batch``,
+        ``cpb200_webp_decode_batch``) in chunks of at most ``JPEG_CHUNK_IMAGES`` images that reuse one workspace; PNG
+        files only when the call holds at least ``PNG_DEVICE_MIN_IMAGES`` of them, since one PNG launch costs about as
+        much as a dozen host decodes, and lossy WebP files from ``WEBP_DEVICE_MIN_IMAGES`` on.  The other files
+        (``cv2.imread``) and the arrays take the host path, and
         their pixels go up in one copy into slots after the decoded ones.  One read of the decode status follows; a
         file whose compressed data the device found bad is read by ``cv2.imread`` and copied into its slot."""
-        from . import _lib, jpeg, png
+        from . import _lib, jpeg, png, webp
         dev = torch.device("cuda")
         datas, infos, host = {}, {}, {}
         for n, src in enumerate(images):
@@ -486,7 +492,7 @@ class MultiPoseDetector(BaseDetector):
                     data = f.read()
             except OSError:
                 raise FileNotFoundError(src)
-            fmt = png if data[:8] == png.SIGNATURE else jpeg
+            fmt = png if data[:8] == png.SIGNATURE else webp if webp.is_webp(data) else jpeg
             try:
                 info = fmt.parse(data, src)
             except ValueError:
@@ -495,11 +501,12 @@ class MultiPoseDetector(BaseDetector):
                 datas[n], infos[n] = data, (fmt, info)
             else:
                 host[n] = self._load_checked(n, src)
-        pngs = [n for n in infos if infos[n][0] is png]
-        if len(pngs) < PNG_DEVICE_MIN_IMAGES:
-            for n in pngs:                                    # cv2.imread is faster for a handful of PNG files
-                del infos[n], datas[n]
-                host[n] = self._load_checked(n, images[n])
+        for fmt, least in ((png, PNG_DEVICE_MIN_IMAGES), (webp, WEBP_DEVICE_MIN_IMAGES)):
+            files = [n for n in infos if infos[n][0] is fmt]
+            if len(files) < least:
+                for n in files:                               # cv2.imread is faster for a handful of these files
+                    del infos[n], datas[n]
+                    host[n] = self._load_checked(n, images[n])
         shape = {n: (info.oh, info.ow, 3) for n, (_, info) in infos.items()}
         shape.update({n: im.shape for n, im in host.items()})
         offsets, pos = {}, 0
@@ -509,8 +516,8 @@ class MultiPoseDetector(BaseDetector):
         host_start = pos - sum(im.nbytes for im in host.values())
         pixels = torch.empty(max(pos, 1), dtype=torch.uint8, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        # JPEG files, then PNG files; status[k] belongs to dec[k]
-        dec = [n for n in infos if infos[n][0] is jpeg] + [n for n in infos if infos[n][0] is png]
+        # JPEG files, then PNG files, then WebP files; status[k] belongs to dec[k]
+        dec = [n for fmt in (jpeg, png, webp) for n in infos if infos[n][0] is fmt]
         if dec:
             chunks, start, ws = [], 0, 0
             for k, n in enumerate(dec):
@@ -533,7 +540,7 @@ class MultiPoseDetector(BaseDetector):
             status = torch.empty(len(dec), dtype=torch.int32, device=dev)
             with torch.cuda.device(dev):
                 for (a, b), o in zip(chunks, at):
-                    name = "jpeg_decode_batch" if infos[dec[a]][0] is jpeg else "png_decode_batch"
+                    name = infos[dec[a]][0].KERNEL
                     st = getattr(_lib.lib(), "cpb200_" + name)(src.data_ptr() + int(o), src.data_ptr() + int(o), b - a,
                                                               work.data_ptr(), work.numel(), pixels.data_ptr(),
                                                               status.data_ptr() + 4 * a, stream)
@@ -572,13 +579,15 @@ class MultiPoseDetector(BaseDetector):
 
         With ``B200.DEVICE_PREPROCESS`` on (the default) and any path among the inputs, the images are decoded into
         one device buffer first (``_load_images_device``): sequential- and progressive-Huffman JPEG files by
-        ``cpb200_jpeg_decode_batch`` and, from ``PNG_DEVICE_MIN_IMAGES`` PNG files per call on, PNG files (not APNG)
-        by ``cpb200_png_decode_batch``, byte for byte as
+        ``cpb200_jpeg_decode_batch``, from ``PNG_DEVICE_MIN_IMAGES`` PNG files per call on, PNG files (not APNG)
+        by ``cpb200_png_decode_batch``, and from ``WEBP_DEVICE_MIN_IMAGES`` on, lossy WebP files (not lossless, alpha
+        or animated ones) by ``cpb200_webp_decode_batch``, byte for byte as
         ``cv2.imread``; every other file, and every array, on the host and uploaded into its slot.  The groups then
         read that buffer in place.  That adds one small device-to-host read of the decode status.  The call then
         needs device memory for the decoded images (3 bytes per pixel) and one decode chunk's workspace (JPEG: int16
         coefficients and 8-bit planes, 4.5 bytes per pixel at 4:2:0, 9 at 4:4:4; PNG: the scanlines, 1 to 8 bytes per
-        pixel; at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image needs more)."""
+        pixel; WebP: 4.6 bytes per pixel of whole macroblocks; at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image
+        needs more)."""
         import ctypes
         from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch

@@ -24,6 +24,8 @@ from __future__ import annotations
 
 import numpy as np
 
+# the C ABI entry point that decodes a launch packed by pack()
+KERNEL = "jpeg_decode_batch"
 # zigzag index -> natural (row-major) index, T.81 figure A.6
 ZIGZAG = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13,
                    6, 7, 14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38,

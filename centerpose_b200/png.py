@@ -27,6 +27,8 @@ import numpy as np
 from .jpeg import oriented_size, tiff_orientation
 
 SIGNATURE = b"\x89PNG\r\n\x1a\n"
+# the C ABI entry point that decodes a launch packed by pack()
+KERNEL = "png_decode_batch"
 # bit depths libpng accepts per colour type (PNG spec 11.2.2)
 DEPTHS = {0: (1, 2, 4, 8, 16), 2: (8, 16), 3: (1, 2, 4, 8), 4: (8, 16), 6: (8, 16)}
 CHANNELS = {0: 1, 2: 3, 3: 1, 4: 2, 6: 4}

@@ -238,6 +238,33 @@ typedef struct cpb200_png_image {
 int cpb200_png_decode_batch(const unsigned char *src, const cpb200_png_image *table, int B, void *workspace,
                             size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
 
+/* One image of cpb200_webp_decode_batch (56 bytes, lives in caller-owned DEVICE memory).  Offsets are bytes. */
+typedef struct cpb200_webp_image {
+  int64_t src_offset;        /* in `src`: the file from its VP8 payload (the frame tag) to its end, followed by >= 32
+                                bytes the decoder may read but ignores */
+  int64_t src_bytes;         /* length of that data; the last token partition runs to its end, as in libwebp */
+  int64_t ws_offset;         /* in `workspace`: the image's macroblock data and planes, 16-byte aligned */
+  int64_t ws_bytes;          /* >= 16 + 1184 * (number of 16x16 macroblocks) */
+  int64_t dst_offset;        /* in `dst`: the decoded HWC uint8 BGR image, rows packed, size after orientation */
+  int32_t h, w;              /* frame size from the key-frame header, 1..16383 */
+  int32_t orientation;       /* EXIF orientation 1..8 (the first EXIF chunk of a VP8X file), applied as cv2.imread does */
+  int32_t pad;
+} cpb200_webp_image;
+
+/* cv2.imread(path, IMREAD_COLOR) of lossy WebP files (one VP8 key frame, RFC 6386), byte for byte (libwebp through
+ * OpenCV 4.13: "fancy" 4:2:0 upsampling and libwebp's fixed-point YUV -> BGR, then OpenCV's EXIF orientation).  B
+ * files in one launch: `src` holds each image's VP8 data, `table` is a DEVICE array of B cpb200_webp_image that the
+ * caller has checked (the kernels trust it; see centerpose_b200/webp.py: the frame tag is a shown key frame, the
+ * first partition fits), `workspace` holds every image's coefficients and planes (an image whose workspace would end
+ * past `workspace_bytes` is not decoded and gets status 2).  One warp per image decodes the bool-coded header, modes
+ * and tokens (serial within an image), one CTA per image then reconstructs and loop-filters its macroblocks along
+ * diagonal wavefronts, and the output pass converts to BGR over the whole launch.  status[b] (DEVICE int array) is 0
+ * when image b decoded, 1 when its stream was bad (a partition that runs out of data where libwebp's does, partition
+ * sizes that do not fit); the image's `dst` slot is then left unwritten, other images are unaffected.
+ * 1 <= B <= 65535. */
+int cpb200_webp_decode_batch(const unsigned char *src, const cpb200_webp_image *table, int B, void *workspace,
+                             size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)
