@@ -192,8 +192,7 @@ __global__ void __launch_bounds__(HD_THREADS, 1) heads_tc_kernel(const __grid_co
               const uint64_t bd = dB + (w_lo14 + (uint32_t)sb * wstep);
               const uint64_t adh = ah0 + toff, adl = al0 + toff;
               wg_fence();
-              for (int k = 0; k < ksteps; ++k)
-                mma_step<HD_CHUNK, P>(acc, acc2, adh, adl, bd, bd + wtile, k, k == 0 ? accf : 1u, bf);
+              mma_stage<HD_CHUNK, P>(acc, acc2, adh, adl, bd, bd + wtile, ksteps, accf, bf);
               accf = 1u;
               wg_commit();
               wg_wait<1>();

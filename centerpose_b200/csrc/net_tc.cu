@@ -20,7 +20,7 @@
 // with full/empty mbarriers feeds the tensor cores, and a stage is released as soon as the MMAs of the NEXT stage are queued.
 //
 // Split-operand precisions (P = 2, CPB200_BF16X2 / CPB200_F16X2, see tc_common.cuh): a stage is
-// [A_hi | A_lo | W_hi | W_lo]; per K step the consumers issue the three products of tc::mma_step.  The DCN gather blends the four corners of BOTH planes in fp32 and re-splits the sample.
+// [A_hi | A_lo | W_hi | W_lo]; per stage the consumers issue the three products of every K step (tc::mma_stage).  The DCN gather blends the four corners of BOTH planes in fp32 and re-splits the sample.
 #include <type_traits>
 #include "tc_common.cuh"
 #include <mutex>
@@ -370,8 +370,7 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
         const uint64_t sd = dT + (base14 + (uint32_t)stage * sstep);
         const uint64_t ad = sd + aoff, bd = sd + boff;
         wg_fence();
-        for (int k = 0; k < ksteps; ++k)
-          mma_step<BN, P>(acc, acc2, ad, ad + aplane, bd, bd + bplane, k, (kb > 0 || k > 0) ? 1u : 0u, bf);
+        mma_stage<BN, P>(acc, acc2, ad, ad + aplane, bd, bd + bplane, ksteps, kb > 0 ? 1u : 0u, bf);
         wg_commit();
         wg_wait<1>();                                      // the previous stage's MMAs have retired: release it
         if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);

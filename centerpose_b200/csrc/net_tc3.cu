@@ -19,7 +19,7 @@
 //
 // Split-operand precisions (P = 2, act_dtype CPB200_BF16X2 / CPB200_F16X2; tc_common.cuh): activations and weights arrive
 // as hi / lo 16-bit planes.  The halo ring is plane-granular (the planes of a slab are two consecutive stages, TMA batch
-// coordinate n and n + B); a weight stage holds the hi tile immediately followed by the lo tile (tc::mma_step,
+// coordinate n and n + B); a weight stage holds the hi tile immediately followed by the lo tile (tc::mma_stage,
 // tc::epilogue_pair).
 #include <type_traits>
 #include "tc_common.cuh"
@@ -178,8 +178,7 @@ __global__ void __launch_bounds__(C3_THREADS, 1) conv3x3_tc_kernel(const __grid_
           }
           const uint64_t adh = ah0 + toff, adl = al0 + toff;
           wg_fence();
-          for (int k = 0; k < ksteps; ++k)
-            mma_step<BN, P>(acc, acc2, adh, adl, bd, bd + btile, k, k == 0 ? accf : 1u, bf);
+          mma_stage<BN, P>(acc, acc2, adh, adl, bd, bd + btile, ksteps, accf, bf);
           accf = 1u;
           wg_commit();
           wg_wait<1>();

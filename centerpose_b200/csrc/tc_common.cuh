@@ -154,6 +154,38 @@ __device__ __forceinline__ void mma_step(float *acc, float *acc2, uint64_t a_hi,
     wgmma_k16<N>(acc2, a_lo + 2 * k, w_hi + 2 * k, 1u, bf);
   }
 }
+// All `ksteps` (1, 2 or 4: a K slab of 16, 32 or 64 channels) K steps of one stage; `first` applies to step 0, the later
+// steps accumulate.  The operand type and the step count are fixed once per stage, so the stage is straight-line code:
+// with a branch between two wgmma (the fp16 / bf16 choice per instruction, or a run-time step loop), ptxas fences every
+// wgmma off from the next, with a warpgroup arrive and a scoreboard wait group each.  P = 2 issues the stage's
+// A_hi x W_hi products back to back into acc, then its cross terms into acc2, step by step: every accumulator element
+// sees the same products in the same order as with mma_step per K step.
+template <int N, int P, uint32_t BF, int KS>
+__device__ __forceinline__ void mma_stage_t(float *acc, float *acc2, uint64_t a_hi, uint64_t a_lo, uint64_t w_hi,
+                                            uint64_t w_lo, uint32_t first) {
+#pragma unroll
+  for (int k = 0; k < KS; ++k) wgmma_k16<N>(acc, a_hi + 2 * k, w_hi + 2 * k, k == 0 ? first : 1u, BF);
+  if constexpr (P == 2) {
+#pragma unroll
+    for (int k = 0; k < KS; ++k) {
+      wgmma_k16<N>(acc2, a_hi + 2 * k, w_lo + 2 * k, k == 0 ? first : 1u, BF);
+      wgmma_k16<N>(acc2, a_lo + 2 * k, w_hi + 2 * k, 1u, BF);
+    }
+  }
+}
+template <int N, int P, uint32_t BF>
+__device__ __forceinline__ void mma_stage_bf(float *acc, float *acc2, uint64_t a_hi, uint64_t a_lo, uint64_t w_hi, uint64_t w_lo,
+                                             int ksteps, uint32_t first) {
+  if (ksteps == 4) mma_stage_t<N, P, BF, 4>(acc, acc2, a_hi, a_lo, w_hi, w_lo, first);
+  else if (ksteps == 2) mma_stage_t<N, P, BF, 2>(acc, acc2, a_hi, a_lo, w_hi, w_lo, first);
+  else mma_stage_t<N, P, BF, 1>(acc, acc2, a_hi, a_lo, w_hi, w_lo, first);
+}
+template <int N, int P>
+__device__ __forceinline__ void mma_stage(float *acc, float *acc2, uint64_t a_hi, uint64_t a_lo, uint64_t w_hi, uint64_t w_lo,
+                                          int ksteps, uint32_t first, uint32_t bf) {
+  if (P == 1 || bf) mma_stage_bf<N, P, 1u>(acc, acc2, a_hi, a_lo, w_hi, w_lo, ksteps, first);
+  else mma_stage_bf<N, P, 0u>(acc, acc2, a_hi, a_lo, w_hi, w_lo, ksteps, first);
+}
 // the same with the A fragments in registers (wgmma_rs_k16)
 template <int N, int P>
 __device__ __forceinline__ void mma_step_rs(float *acc, float *acc2, const uint32_t (&a_hi)[4], const uint32_t (&a_lo)[4],
