@@ -48,6 +48,21 @@ inline int check_launch(const char *what, K *kernel) {
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// cv2's ApplyExifOrientation as an index mapping: pixel (oy, ox) of the oriented image is stored pixel (sy, sx) of the
+// h x w image (transpose for 5..8, then flips)
+__device__ __forceinline__ void exif_source(int o, int oy, int ox, int h, int w, int &sy, int &sx) {
+  switch (o) {
+    case 2: sy = oy; sx = w - 1 - ox; break;
+    case 3: sy = h - 1 - oy; sx = w - 1 - ox; break;
+    case 4: sy = h - 1 - oy; sx = ox; break;
+    case 5: sy = ox; sx = oy; break;
+    case 6: sy = h - 1 - ox; sx = oy; break;
+    case 7: sy = h - 1 - ox; sx = w - 1 - oy; break;
+    case 8: sy = ox; sx = w - 1 - oy; break;
+    default: sy = oy; sx = ox; break;
+  }
+}
+
 #define CPB_ACT_MASK (CPB200_FLAG_RELU | CPB200_FLAG_HSWISH | CPB200_FLAG_HSIGMOID | CPB200_FLAG_RELU6 | CPB200_FLAG_CLIP01)
 // Epilogue non-linearity selected by the op flags (at most one of RELU / HSWISH / HSIGMOID / RELU6 / CLIP01).  hswish
 // and hsigmoid keep the reference's operation order x * relu6(x + 3) / 6 (mobilenetv3.py:84-93).  ReLU6 and the hard

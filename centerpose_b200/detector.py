@@ -283,7 +283,8 @@ def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda
 
 
 # run_images decodes JPEG, PNG and WebP files on the device in launches of at most this many images, whose workspace
-# (JPEG coefficients and planes, PNG scanlines, WebP coefficients and planes; reused from launch to launch) stays below
+# (JPEG coefficients and planes, PNG scanlines, WebP coefficients and planes, lossless WebP ARGB planes and prefix
+# codes; reused from launch to launch) stays below
 # JPEG_CHUNK_WORKSPACE bytes unless one image needs more
 JPEG_CHUNK_IMAGES = 256
 JPEG_CHUNK_WORKSPACE = 512 << 20
@@ -297,6 +298,10 @@ PNG_DEVICE_MIN_IMAGES = 16
 # files on one H100).  run_images from quality-75 files with the device decode against cv2.imread: 0.30x for one file,
 # 1.03x for 8, 1.6x for 16, 3.0x for 256 (tools/bench_webp.py)
 WEBP_DEVICE_MIN_IMAGES = 16
+# Lossless WebP files likewise go to the device only from this many per call on.  One launch takes 135-158 ms whether
+# it holds one 640x480 file or 256 (cv2.imencode defaults, one H100).  run_images with the device decode against
+# cv2.imread: 0.11x for one file, 1.0x for 16, 1.34x for 24, 1.9x for 48, 2.9x for 256 (tools/bench_webp.py --lossless)
+WEBP_LOSSLESS_DEVICE_MIN_IMAGES = 24
 
 
 def _swap_pairs(C, pairs, device):
@@ -471,16 +476,19 @@ class MultiPoseDetector(BaseDetector):
         """Every input of ``run_images`` in one device buffer of packed HWC uint8 BGR images.  Returns
         ``(views, offsets, buffer)``: per input a (h, w, 3) view of its slot and the slot's byte offset.
 
-        The files' headers are parsed first (``jpeg.parse``, ``png.parse``, ``webp.parse``), so every size is known
-        before any pixel exists.  The files the device can decode, with their tables, go up in one pinned buffer and
-        are decoded by each format module's ``KERNEL`` (``cpb200_jpeg_decode_batch``, ``cpb200_png_decode_batch``,
-        ``cpb200_webp_decode_batch``) in chunks of at most ``JPEG_CHUNK_IMAGES`` images that reuse one workspace; PNG
-        files only when the call holds at least ``PNG_DEVICE_MIN_IMAGES`` of them, since one PNG launch costs about as
-        much as a dozen host decodes, and lossy WebP files from ``WEBP_DEVICE_MIN_IMAGES`` on.  The other files
+        The files' headers are parsed first (``jpeg.parse``, ``png.parse``, ``webp.parse``, and
+        ``webp_lossless.parse`` for the files ``webp.parse`` declines as lossless), so every size is known before any
+        pixel exists.  The files the device can decode, with their tables, go up in one pinned buffer and are decoded
+        by each format module's ``KERNEL`` (``cpb200_jpeg_decode_batch``, ``cpb200_png_decode_batch``,
+        ``cpb200_webp_decode_batch``, ``cpb200_webp_lossless_decode_batch``) in chunks of at most ``JPEG_CHUNK_IMAGES``
+        images that reuse one workspace; PNG files only when the call holds at least ``PNG_DEVICE_MIN_IMAGES`` of them,
+        since one PNG launch costs about as much as a dozen host decodes, lossy WebP files from
+        ``WEBP_DEVICE_MIN_IMAGES`` on and lossless ones from ``WEBP_LOSSLESS_DEVICE_MIN_IMAGES`` on.  The other files
         (``cv2.imread``) and the arrays take the host path, and
         their pixels go up in one copy into slots after the decoded ones.  One read of the decode status follows; a
-        file whose compressed data the device found bad is read by ``cv2.imread`` and copied into its slot."""
-        from . import _lib, jpeg, png, webp
+        file whose compressed data the device found bad, or a lossless file over the device's prefix-code group
+        budget, is read by ``cv2.imread`` and copied into its slot."""
+        from . import _lib, jpeg, png, webp, webp_lossless
         dev = torch.device("cuda")
         datas, infos, host = {}, {}, {}
         for n, src in enumerate(images):
@@ -495,13 +503,16 @@ class MultiPoseDetector(BaseDetector):
             fmt = png if data[:8] == png.SIGNATURE else webp if webp.is_webp(data) else jpeg
             try:
                 info = fmt.parse(data, src)
+                if fmt is webp and info.reason.startswith("lossless"):
+                    fmt, info = webp_lossless, webp_lossless.parse(data, src)
             except ValueError:
                 info = None
             if info is not None and (info.eligible or getattr(info, "progressive", None)):
                 datas[n], infos[n] = data, (fmt, info)
             else:
                 host[n] = self._load_checked(n, src)
-        for fmt, least in ((png, PNG_DEVICE_MIN_IMAGES), (webp, WEBP_DEVICE_MIN_IMAGES)):
+        for fmt, least in ((png, PNG_DEVICE_MIN_IMAGES), (webp, WEBP_DEVICE_MIN_IMAGES),
+                           (webp_lossless, WEBP_LOSSLESS_DEVICE_MIN_IMAGES)):
             files = [n for n in infos if infos[n][0] is fmt]
             if len(files) < least:
                 for n in files:                               # cv2.imread is faster for a handful of these files
@@ -516,8 +527,8 @@ class MultiPoseDetector(BaseDetector):
         host_start = pos - sum(im.nbytes for im in host.values())
         pixels = torch.empty(max(pos, 1), dtype=torch.uint8, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        # JPEG files, then PNG files, then WebP files; status[k] belongs to dec[k]
-        dec = [n for fmt in (jpeg, png, webp) for n in infos if infos[n][0] is fmt]
+        # JPEG files, then PNG files, then lossy and lossless WebP files; status[k] belongs to dec[k]
+        dec = [n for fmt in (jpeg, png, webp, webp_lossless) for n in infos if infos[n][0] is fmt]
         if dec:
             chunks, start, ws = [], 0, 0
             for k, n in enumerate(dec):
@@ -580,14 +591,15 @@ class MultiPoseDetector(BaseDetector):
         With ``B200.DEVICE_PREPROCESS`` on (the default) and any path among the inputs, the images are decoded into
         one device buffer first (``_load_images_device``): sequential- and progressive-Huffman JPEG files by
         ``cpb200_jpeg_decode_batch``, from ``PNG_DEVICE_MIN_IMAGES`` PNG files per call on, PNG files (not APNG)
-        by ``cpb200_png_decode_batch``, and from ``WEBP_DEVICE_MIN_IMAGES`` on, lossy WebP files (not lossless, alpha
-        or animated ones) by ``cpb200_webp_decode_batch``, byte for byte as
+        by ``cpb200_png_decode_batch``, from ``WEBP_DEVICE_MIN_IMAGES`` on, lossy WebP files (not alpha or animated
+        ones) by ``cpb200_webp_decode_batch``, and from ``WEBP_LOSSLESS_DEVICE_MIN_IMAGES`` on, lossless WebP files
+        by ``cpb200_webp_lossless_decode_batch``, byte for byte as
         ``cv2.imread``; every other file, and every array, on the host and uploaded into its slot.  The groups then
         read that buffer in place.  That adds one small device-to-host read of the decode status.  The call then
         needs device memory for the decoded images (3 bytes per pixel) and one decode chunk's workspace (JPEG: int16
         coefficients and 8-bit planes, 4.5 bytes per pixel at 4:2:0, 9 at 4:4:4; PNG: the scanlines, 1 to 8 bytes per
-        pixel; WebP: 4.6 bytes per pixel of whole macroblocks; at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image
-        needs more)."""
+        pixel; WebP: 4.6 bytes per pixel of whole macroblocks; lossless WebP: about 8.8 bytes per pixel plus 575 KB
+        of prefix codes per file; at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image needs more)."""
         import ctypes
         from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch

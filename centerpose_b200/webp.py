@@ -97,68 +97,107 @@ def _frame_header(d, pos, ln, name):
     return part0, w, h
 
 
-def parse(data, name="image"):
-    """Chunks of one file (bytes or a uint8 array).  Returns a ``WebpInfo``; raises ``ValueError`` naming ``name``
-    when the file is not a WebP file the parser can read."""
-    d = data.tobytes() if isinstance(data, np.ndarray) else bytes(data)
+class Chunks:
+    """What ``walk`` found in a file's RIFF chunk list: ``riff`` its RIFF size, ``flags`` and ``canvas`` (w, h) of the
+    ``VP8X`` chunk (``canvas`` None in the simple container), ``image`` the FourCC of the first ``VP8 `` / ``VP8L``
+    chunk with its payload offset ``body`` and length ``length``, ``exif`` the first ``EXIF`` payload, and whether a
+    ``VP8L`` (``lossless``), ``ALPH`` (``alpha``) or ``ANIM`` / ``ANMF`` (``anim``) chunk was seen.  ``tail_error`` says
+    why the walk stopped at a bad chunk after the image chunk, which libwebp never reads."""
+
+    def __init__(self, riff):
+        self.riff, self.flags, self.canvas, self.exif = riff, 0, None, None
+        self.image, self.body, self.length = None, None, 0
+        self.lossless = self.alpha = self.anim = False
+        self.tail_error = None
+
+    def animated(self):
+        return self.anim or bool(self.flags & VP8X_ANIMATION)
+
+    def orientation(self):
+        """The EXIF orientation cv2.imread applies: only when ``VP8X`` flags EXIF, from a bare TIFF header (an
+        "Exif\\0\\0" prefix is ignored), and not when a bad chunk follows the image (cv2.imread then reads the
+        image without its metadata)."""
+        if self.canvas is not None and self.flags & VP8X_EXIF and self.exif is not None and self.tail_error is None:
+            return tiff_orientation(self.exif)
+        return 1
+
+
+def walk(d, name):
+    """The chunk list of file bytes ``d`` (the simple container ends at its image chunk, as libwebp reads it).  Raises
+    ``ValueError`` naming ``name`` where cv2.imread refuses the container: no RIFF / WEBP signature, a chunk past the
+    end or a bad ``VP8X`` chunk before the image chunk, a first chunk other than ``VP8X``, ``VP8 `` or ``VP8L``.  The
+    same faults after the image chunk end the walk with ``tail_error`` set."""
     n = len(d)
     if n < 12 or not is_webp(d):
         raise ValueError("%s: not a WebP file (no RIFF / WEBP signature)" % name)
-    info = WebpInfo()
-    info.size = n
-    riff = struct.unpack_from("<I", d, 4)[0]
-    end = min(n, riff + 8)
-    pos, first, flags, canvas, exif = 12, True, 0, None, None
-    alpha = anim = lossless = False
+    c = Chunks(struct.unpack_from("<I", d, 4)[0])
+    end = min(n, c.riff + 8)
+    pos, first = 12, True
     while pos + 8 <= end:
         ctype, ln = d[pos:pos + 4], struct.unpack_from("<I", d, pos + 4)[0]
         body = pos + 8
+        err = None
         if body + ln > end:
-            raise ValueError("%s: chunk %r of %d bytes runs past the end of the file" % (name, ctype, ln))
+            err = "%s: chunk %r of %d bytes runs past the end of the file" % (name, ctype, ln)
+        elif ctype == b"VP8X" and (not first or ln != 10):
+            err = "%s: bad VP8X chunk" % name
+        if err is not None:
+            if c.image is None:
+                raise ValueError(err)
+            c.tail_error = err
+            break
         if first and ctype not in (b"VP8X", b"VP8 ", b"VP8L"):
             # without VP8X, libwebp reads the first chunk as the image bitstream, and cv2.imread fails
             raise ValueError("%s: first chunk %r is neither VP8X nor an image" % (name, ctype))
         if ctype == b"VP8X":
-            if not first or ln != 10:
-                raise ValueError("%s: bad VP8X chunk" % name)
-            flags = d[body]
-            canvas = (1 + int.from_bytes(d[body + 4:body + 7], "little"),
-                      1 + int.from_bytes(d[body + 7:body + 10], "little"))
-        elif ctype == b"VP8 ":
-            if info.vp8 is None:
-                _, info.w, info.h = _frame_header(d, body, ln, name)
-                info.vp8 = body
-                if canvas is None:                    # the simple container: nothing after the image is read
+            c.flags = d[body]
+            c.canvas = (1 + int.from_bytes(d[body + 4:body + 7], "little"),
+                        1 + int.from_bytes(d[body + 7:body + 10], "little"))
+        elif ctype in (b"VP8 ", b"VP8L"):
+            c.lossless |= ctype == b"VP8L"
+            if c.image is None:
+                c.image, c.body, c.length = ctype, body, ln
+                if c.canvas is None:                  # the simple container: nothing after the image is read
                     break
-        elif ctype == b"VP8L":
-            lossless = True
-            break
         elif ctype == b"ALPH":
-            alpha = True
+            c.alpha = True
         elif ctype in (b"ANIM", b"ANMF"):
-            anim = True
+            c.anim = True
         elif ctype == b"EXIF":
-            if exif is None:
-                exif = d[body:body + ln]              # cv2.imread reads the first EXIF chunk
+            if c.exif is None:
+                c.exif = d[body:body + ln]            # cv2.imread reads the first EXIF chunk
         first = False
         pos = body + ln + (ln & 1)
-    if lossless:
+    return c
+
+
+def parse(data, name="image"):
+    """Chunks of one file (bytes or a uint8 array).  Returns a ``WebpInfo``; raises ``ValueError`` naming ``name``
+    when the file is not a WebP file the parser can read."""
+    d = data.tobytes() if isinstance(data, np.ndarray) else bytes(data)
+    c = walk(d, name)
+    info = WebpInfo()
+    info.size = len(d)
+    if c.lossless:
         info.reason = "lossless WebP (VP8L)"
         return info
-    if anim or flags & VP8X_ANIMATION:
+    if c.tail_error:
+        raise ValueError(c.tail_error)
+    if c.animated():
         info.reason = "animated WebP"
         return info
-    if info.vp8 is None:
+    if c.image is None:
         raise ValueError("%s: no VP8 image chunk" % name)
-    if canvas is not None and canvas != (info.w, info.h):
-        raise ValueError("%s: VP8X canvas %dx%d differs from the %dx%d frame" % (name, *canvas, info.w, info.h))
-    if canvas is not None and flags & VP8X_EXIF and exif is not None:
-        info.orientation = tiff_orientation(exif)     # a bare TIFF header; cv2.imread ignores an "Exif\0\0" prefix
+    _, info.w, info.h = _frame_header(d, c.body, c.length, name)
+    info.vp8 = c.body
+    if c.canvas is not None and c.canvas != (info.w, info.h):
+        raise ValueError("%s: VP8X canvas %dx%d differs from the %dx%d frame" % (name, *c.canvas, info.w, info.h))
+    info.orientation = c.orientation()
     info.oh, info.ow = oriented_size(info.h, info.w, info.orientation)
-    if alpha:
+    if c.alpha:
         info.reason = "WebP with an alpha channel (ALPH)"
-    elif riff + 8 != n:
-        info.reason = "RIFF size %d disagrees with the file's %d bytes" % (riff, n)
+    elif c.riff + 8 != info.size:
+        info.reason = "RIFF size %d disagrees with the file's %d bytes" % (c.riff, info.size)
     else:
         info.eligible = True
     return info

@@ -265,6 +265,39 @@ typedef struct cpb200_webp_image {
 int cpb200_webp_decode_batch(const unsigned char *src, const cpb200_webp_image *table, int B, void *workspace,
                              size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
 
+/* Prefix-code groups a lossless WebP image may use on the device; each costs 8992 bytes of its workspace. */
+#define CPB200_WEBP_LOSSLESS_MAX_GROUPS 64
+
+/* One image of cpb200_webp_lossless_decode_batch (56 bytes, lives in caller-owned DEVICE memory).  Offsets are
+ * bytes. */
+typedef struct cpb200_webp_lossless_image {
+  int64_t src_offset;        /* in `src`: the file from its VP8L payload (the 0x2f signature) to its end, followed by
+                                >= 32 zero bytes the decoder may read but ignores */
+  int64_t src_bytes;         /* length of that data; libwebp reads the bitstream to the end of the data it is given */
+  int64_t ws_offset;         /* in `workspace`: the image's ARGB planes, sub-images and prefix codes, 16-byte aligned */
+  int64_t ws_bytes;          /* >= centerpose_b200/webp_lossless.py workspace_bytes(w, h) */
+  int64_t dst_offset;        /* in `dst`: the decoded HWC uint8 BGR image, rows packed, size after orientation */
+  int32_t h, w;              /* image size from the VP8L header, 1..16384 */
+  int32_t orientation;       /* EXIF orientation 1..8 (the first EXIF chunk of a VP8X file), applied as cv2.imread does */
+  int32_t pad;
+} cpb200_webp_lossless_image;
+
+/* cv2.imread(path, IMREAD_COLOR) of lossless WebP files (VP8L, RFC 9649), byte for byte (libwebp through OpenCV
+ * 4.13: the ARGB image with its alpha dropped, then OpenCV's EXIF orientation).  B files in one launch: `src` holds
+ * each image's VP8L data, `table` is a DEVICE array of B cpb200_webp_lossless_image that the caller has checked (the
+ * kernels trust it; see centerpose_b200/webp_lossless.py: the signature and version of the header, the size),
+ * `workspace` holds every image's planes and codes.  One thread per image decodes the transforms, sub-images,
+ * prefix codes and the LZ77 / colour-cache coded pixels (serial within an image), one CTA per image then undoes the
+ * transforms, and the output pass converts to BGR over the whole launch.  status[b] (DEVICE int array) is 0 when
+ * image b decoded, 1 when its stream was bad where libwebp's is (a code-length set that is empty, incomplete or
+ * over-subscribed, a repeat or max_symbol past the alphabet, a transform seen twice, colour-cache bits outside 1..11,
+ * a backward reference outside the image, more bits read than the data holds), 2 when its entropy image uses more
+ * than CPB200_WEBP_LOSSLESS_MAX_GROUPS prefix-code groups or its workspace would end past `workspace_bytes`; the
+ * image's `dst` slot is then left unwritten, other images are unaffected.  1 <= B <= 65535. */
+int cpb200_webp_lossless_decode_batch(const unsigned char *src, const cpb200_webp_lossless_image *table, int B,
+                                      void *workspace, size_t workspace_bytes, unsigned char *dst, int *status,
+                                      void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)

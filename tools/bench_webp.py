@@ -1,13 +1,15 @@
 """Device WebP decode throughput on one GPU: ``cpb200_webp_decode_batch`` against ``cv2.imdecode``, and
 ``run_images`` from lossy WebP files with the device decode against the host ``cv2.imread`` (``DEVICE_PREPROCESS:
-false``).
+false``).  With ``--lossless``, the same for ``cpb200_webp_lossless_decode_batch`` and lossless files.
 
     python tools/bench_webp.py [--images 256] [--batches 1,16,32,64,128,256] [--counts 1,4,16,64,256] [--rounds 3]
-                               [--out DIR] [--precision fp16x2]
+                               [--out DIR] [--precision fp16x2] [--lossless]
 
 The images are seeded gradients with noise (``tests/test_jpeg_cpu.make_image``) at COCO-like sizes, 640x480, 480x640
 and 640x427 in turn, written lossy by ``cv2.imencode`` at quality 75 and at quality 95.  Each set goes to ``--out`` (a
-temporary directory by default).
+temporary directory by default).  With ``--lossless`` there is one set, written by ``cv2.imencode`` with no parameters
+(lossless), and the result also gives the largest number of prefix-code groups a file uses (``tests/vp8l_model``),
+against the device budget ``webp_lossless.MAX_GROUPS``.
 
 1. Decode alone, per set and per batch size in ``--batches``.  Device: the kernels of one ``cpb200_webp_decode_batch``
    over the first ``batch`` images (CUDA events, median of ``--rounds`` launches after a warm-up launch).  Host:
@@ -46,12 +48,13 @@ from tests.test_jpeg_cpu import make_image  # noqa: E402
 
 
 def _files(quality, n, out):
+    """n files at ``quality``, or lossless ones (cv2.imencode's default) for quality None."""
     datas, paths = [], []
     for i in range(n):
         h, w = SIZES[i % len(SIZES)]
         im = make_image(h, w, "smooth_noise", 1000 + i)
-        data = cv2.imencode(".webp", im, [cv2.IMWRITE_WEBP_QUALITY, quality])[1].tobytes()
-        p = os.path.join(out, "q%d_%04d.webp" % (quality, i))
+        data = cv2.imencode(".webp", im, [] if quality is None else [cv2.IMWRITE_WEBP_QUALITY, quality])[1].tobytes()
+        p = os.path.join(out, "%s_%04d.webp" % ("lossless" if quality is None else "q%d" % quality, i))
         with open(p, "wb") as f:
             f.write(data)
         datas.append(data)
@@ -59,18 +62,18 @@ def _files(quality, n, out):
     return datas, paths
 
 
-def _decode_alone(datas, batches, rounds):
-    from centerpose_b200 import _lib, webp
+def _decode_alone(datas, batches, rounds, fmt):
+    from centerpose_b200 import _lib
     decode = lambda d: cv2.imdecode(np.frombuffer(d, np.uint8), cv2.IMREAD_COLOR)
     res = {"compressed_mb": round(sum(len(d) for d in datas) / 1e6, 3), "device": {}}
     exact = 0
     for B in batches:
         sub = datas[:B]
         t0 = time.perf_counter()
-        infos = [webp.parse(d) for d in sub]
+        infos = [fmt.parse(d) for d in sub]
         sizes = [i.oh * i.ow * 3 for i in infos]
         offs = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-        buf, ws_bytes = webp.pack(infos, sub, offs[:-1])
+        buf, ws_bytes = fmt.pack(infos, sub, offs[:-1])
         t_host = time.perf_counter() - t0
         src = torch.from_numpy(buf).cuda()
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda")
@@ -79,9 +82,9 @@ def _decode_alone(datas, batches, rounds):
         stream = torch.cuda.current_stream().cuda_stream
 
         def launch():
-            _lib.check(_lib.lib().cpb200_webp_decode_batch(src.data_ptr(), src.data_ptr(), len(sub), ws.data_ptr(),
-                                                           ws_bytes, dst.data_ptr(), status.data_ptr(), stream),
-                       "webp_decode_batch")
+            _lib.check(getattr(_lib.lib(), "cpb200_" + fmt.KERNEL)(src.data_ptr(), src.data_ptr(), len(sub),
+                                                                   ws.data_ptr(), ws_bytes, dst.data_ptr(),
+                                                                   status.data_ptr(), stream), fmt.KERNEL)
 
         launch()
         torch.cuda.synchronize()
@@ -123,6 +126,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", default=None, help="directory for the WebP files (default: a temporary one)")
     ap.add_argument("--precision", default="fp16x2")
+    ap.add_argument("--lossless", action="store_true", help="lossless files and cpb200_webp_lossless_decode_batch")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise RuntimeError("tools/bench_webp.py needs a CUDA device (there is no CPU path to time)")
@@ -131,17 +135,25 @@ def main():
     os.makedirs(out, exist_ok=True)
     batches = sorted({min(int(b), args.images) for b in args.batches.split(",")})
     hw_before = gpu_info(0)
-    sets, decode = {}, {}
-    for quality in (75, 95):
-        sets[quality] = _files(quality, args.images, out)
-        decode["q%d" % quality] = _decode_alone(sets[quality][0], batches, args.rounds)
+    from centerpose_b200 import webp, webp_lossless
+    sets, decode, extra = {}, {}, {}
+    for quality in (None,) if args.lossless else (75, 95):
+        key = "lossless" if quality is None else "q%d" % quality
+        sets[key] = _files(quality, args.images, out)
+        decode[key] = _decode_alone(sets[key][0], batches, args.rounds, webp_lossless if args.lossless else webp)
+    if args.lossless:
+        from tests import vp8l_model
+        extra["max_groups"] = max(vp8l_model.groups(d[webp_lossless.parse(d).vp8l:]) for d in sets["lossless"][0])
+        extra["group_budget"] = webp_lossless.MAX_GROUPS
 
     from centerpose_b200 import detector as detector_mod
     det = detector("dla_34", args.precision)
     detector_mod.WEBP_DEVICE_MIN_IMAGES = 1
+    detector_mod.WEBP_LOSSLESS_DEVICE_MIN_IMAGES = 1
     e2e = {}
+    e2e_set = "lossless" if args.lossless else "q75"
     for n in sorted({min(int(c), args.images) for c in args.counts.split(",")}):
-        paths = sets[75][1][:n]
+        paths = sets[e2e_set][1][:n]
 
         def run(device):
             det.device_preprocess = device
@@ -162,9 +174,10 @@ def main():
                   "rows_identical": all(np.array_equal(a, b) for a, b in zip(rows[True], rows[False]))}
     det.device_preprocess = True
     result = {
-        "metric": "lossy WebP decode images/s (device kernels vs cv2.imdecode) and run_images images/s from files",
-        "images": args.images, "sizes_hw": SIZES, "host_cores": os.cpu_count(), "decode": decode,
-        "run_images_set": "q75", "run_images": e2e,
+        "metric": "%s WebP decode images/s (device kernels vs cv2.imdecode) and run_images images/s from files"
+                  % ("lossless" if args.lossless else "lossy"),
+        "images": args.images, "sizes_hw": SIZES, "host_cores": os.cpu_count(), "decode": decode, **extra,
+        "run_images_set": e2e_set, "run_images": e2e,
         "precision": args.precision,
         "gpu_before": hw_before, "gpu_after": gpu_info(0),
     }
