@@ -66,6 +66,8 @@ def lib() -> ctypes.CDLL:
     L.cpb200_webp_lossless_decode_batch.restype = ctypes.c_int
     L.cpb200_webp_lossless_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                                     ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    L.cpb200_render_poses_batch.restype = ctypes.c_int
+    L.cpb200_render_poses_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 7
     L.cpb200_soft_nms_39.restype = ctypes.c_int
     L.cpb200_soft_nms_39.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                      ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]

@@ -11,7 +11,9 @@ Differences that are additive only:
     ``flip_lr`` / ``flip_lr_off`` round-trip through numpy (``lib/models/utils.py:30-47``);
   * ``run_batch`` (new): many pre-processed images per call — the reference API is single-image;
   * ``run_images`` (new): ``run()`` for a list of raw images, batched on the device, with the reference's
-    test-time flip / multi-scale / soft-NMS settings.
+    test-time flip / multi-scale / soft-NMS settings, and optionally the drawn images;
+  * ``show_results`` / ``render_poses`` draw the detections on the device (csrc/render.cu), byte for byte as the
+    reference's Debugger; ``debug()`` (the DEBUG >= 2 heat-map views) is not provided.
 """
 from __future__ import annotations
 
@@ -408,7 +410,33 @@ class MultiPoseDetector(BaseDetector):
         raise NotImplementedError("visual debugging (lib/utils/debugger.py) is outside the GPU hot path")
 
     def show_results(self, debugger, image, results):
-        raise NotImplementedError("visualisation (lib/utils/debugger.py) is outside the GPU hot path")
+        """multi_pose.py:96-107: draws every row above ``TEST.VIS_THRESH`` on a copy of ``image`` with the device
+        renderer (``render_poses``) into ``self.debug_imgs['multi_pose']``, then shows it as the reference's
+        ``Debugger.show_all_imgs`` does.  Without a cv2 GUI backend (opencv-python-headless) the display is skipped.
+        ``debugger`` is unused (the reference passes its Debugger; ``run()`` passes None)."""
+        self.debug_imgs = {"multi_pose": self.render_poses([image], [results])[0]}
+        try:
+            for name, img in self.debug_imgs.items():
+                cv2.imshow(name, img)
+            if cv2.waitKey(0 if self.pause else 1) == 27:
+                import sys
+                sys.exit(0)
+        except cv2.error:
+            pass                                                  # no GUI backend in this cv2 build
+
+    def render_poses(self, images, results):
+        """Additive: the image ``show_results`` draws, for many images at once.  ``images`` are BGR uint8 HWC arrays,
+        ``results[i]`` the ``(N_i, 56)`` rows of image i (as ``run_images`` returns them).  Returns one new annotated
+        array per image, byte for byte the reference Debugger's ``imgs['multi_pose']`` (``DEBUG_THEME`` 'white' or
+        any other theme).  One upload of the images and tables, one ``cpb200_render_poses_batch``, one copy back."""
+        from . import render
+        images = [self._load_checked(n, im) for n, im in enumerate(images)]
+        if not images:
+            return []
+        shapes = [im.shape[:2] for im in images]
+        ops = render.build(shapes, results, float(self.cfg.TEST.VIS_THRESH), self.cfg.DEBUG_THEME)
+        pixels, offsets = render.launch(ops, images=images)
+        return render.download(pixels, offsets, shapes)
 
     # -- additive: batched / device-resident paths ------------------------------------------------
     def merge_outputs_device(self, detections, nms=None, return_keep=False):
@@ -574,7 +602,7 @@ class MultiPoseDetector(BaseDetector):
         return views, [offsets[n] for n in range(len(images))], pixels
 
     @torch.no_grad()
-    def run_images(self, images, max_batch=32):
+    def run_images(self, images, max_batch=32, return_images=False):
         """Additive: ``run()`` for many images at once, with the reference's test-time settings (``FLIP_TEST``,
         ``TEST_SCALES``, ``FIX_RES``, ``NMS``; what tools/evaluate.py runs).  ``images`` is a list of BGR uint8 HWC
         arrays or image paths.  Returns one float32 ``(N_i, 56)`` array per image, in input order, equal to
@@ -599,7 +627,13 @@ class MultiPoseDetector(BaseDetector):
         needs device memory for the decoded images (3 bytes per pixel) and one decode chunk's workspace (JPEG: int16
         coefficients and 8-bit planes, 4.5 bytes per pixel at 4:2:0, 9 at 4:4:4; PNG: the scanlines, 1 to 8 bytes per
         pixel; WebP: 4.6 bytes per pixel of whole macroblocks; lossless WebP: about 8.8 bytes per pixel plus 575 KB
-        of prefix codes per file; at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image needs more)."""
+        of prefix codes per file; at most ``JPEG_CHUNK_WORKSPACE`` bytes unless one image needs more).
+
+        With ``return_images=True`` it returns ``(rows, drawn)``: the same rows, and per image the ``render_poses``
+        image of its rows (what ``show_results`` draws).  The images are then all in one device buffer (the decoded
+        files where the device decode put them, the arrays uploaded once into slots after them), the groups read them
+        there, and ``cpb200_render_poses_batch`` draws on them in place after the rows are known, followed by one
+        device-to-host copy of the drawn images."""
         import ctypes
         from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch
@@ -608,10 +642,14 @@ class MultiPoseDetector(BaseDetector):
         offsets = None
         if self.device_preprocess and any(isinstance(src, str) for src in images):
             loaded, offsets, pixels_dev = self._load_images_device(images)
+        elif return_images:
+            # every image in one device buffer, so that the drawing needs no second upload
+            loaded, offsets, pixels_dev = self._load_images_device(
+                [self._load_checked(n, src) for n, src in enumerate(images)])
         else:
             loaded = [self._load_checked(n, src) for n, src in enumerate(images)]
         if not loaded:
-            return []
+            return ([], []) if return_images else []
         cfg = self.cfg
         dev = torch.device("cuda")
         stream = torch.cuda.current_stream(dev).cuda_stream
@@ -669,7 +707,14 @@ class MultiPoseDetector(BaseDetector):
         if cfg.TEST.NMS or S > 1:
             soft_nms_39_cuda_batch(rows, Nt=0.5, method=2)
         out = rows.cpu().numpy()
-        return [out[i] for i in range(len(loaded))]
+        rows_out = [out[i] for i in range(len(loaded))]
+        if not return_images:
+            return rows_out
+        from . import render
+        shapes = [tuple(im.shape[:2]) for im in loaded]
+        ops = render.build(shapes, rows_out, float(cfg.TEST.VIS_THRESH), cfg.DEBUG_THEME)
+        render.launch(ops, pixels=pixels_dev, offsets=offsets)
+        return rows_out, render.download(pixels_dev, offsets, shapes)
 
 
 detector_factory = {"multi_pose": MultiPoseDetector}     # detector_factory.py:5-7

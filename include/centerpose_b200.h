@@ -298,6 +298,58 @@ int cpb200_webp_lossless_decode_batch(const unsigned char *src, const cpb200_web
                                       void *workspace, size_t workspace_bytes, unsigned char *dst, int *status,
                                       void *stream);
 
+/* Pose drawing (csrc/render.cu, centerpose_b200/render.py builds the tables).  One image of
+ * cpb200_render_poses_batch (40 bytes, DEVICE memory).  Offsets are bytes. */
+typedef struct cpb200_render_image {
+  int64_t offset;            /* in `pixels`: the HWC uint8 BGR image, rows packed, drawn in place */
+  int64_t ws_offset;         /* in `workspace`: h * w bytes of limb marks, then its limbs' span rows; 8-byte aligned */
+  int32_t h, w;
+  int32_t person_begin, person_count;   /* its drawn persons in `persons`, in drawing order */
+  int32_t limb_begin, limb_count;       /* its persons' limbs in `limbs` (contiguous) */
+} cpb200_render_image;
+
+#define CPB200_RENDER_JOINTS 17
+#define CPB200_RENDER_MAX_LIMBS 18
+
+/* One drawn person (224 bytes).  Coordinates are int32 as the reference truncates them. */
+typedef struct cpb200_render_person {
+  int32_t box[4];            /* x1, y1, x2, y2: the thickness-2 rectangle */
+  int32_t label[4];          /* x1, y1, x2, y2: the filled label rectangle */
+  int32_t text_x, text_y;    /* the label text's origin */
+  int32_t text_begin, text_count;       /* its pixels in `text_px`, each inside the image */
+  uint8_t color[4];          /* B, G, R of the rectangles; [3] unused */
+  int32_t joints;            /* bit j: a radius-2 white disc at joint j */
+  int32_t limb_begin, limb_count;       /* its limbs in `limbs`, in the reference's edge order, <= 18 */
+  int32_t fold_box[4];       /* x0, y0, x1, y1: image pixels its limbs can cover (x1 < x0: none) */
+  int32_t joint_x[CPB200_RENDER_JOINTS], joint_y[CPB200_RENDER_JOINTS];
+  int32_t pad[2];
+} cpb200_render_person;
+
+/* One limb polygon (24 bytes): cv2.fillConvexPoly(canvas, verts, white, LINE_8, 0) of its vertices. */
+typedef struct cpb200_render_limb {
+  int32_t vert_begin, vert_count;       /* (x, y) int32 pairs in `verts` */
+  int32_t row0, row1;        /* image rows its spans may cover (row1 < row0: none) */
+  int64_t rows_offset;       /* in `workspace`: (row1 - row0 + 1) int32 (lo, hi) pairs, written by the kernel */
+} cpb200_render_limb;
+
+/* One pixel of a label text (8 bytes): the pixel at (text_x + dx, text_y + dy) becomes luts[lut + v] for each of its
+ * channels' value v (cv2.putText's anti-aliased black text changes a channel as a function of that channel alone). */
+typedef struct cpb200_render_text_px {
+  int16_t dx, dy;
+  int32_t lut;
+} cpb200_render_text_px;
+
+/* What MultiPoseDetector.show_results draws (the reference's Debugger.add_coco_bbox + add_coco_hp for every row above
+ * VIS_THRESH), byte for byte as cv2 4.13 draws it, on B images in place.  One CTA per image walks its persons in
+ * order: the box, the label box, the label text, the joint discs, then the limb polygons, each limb's
+ * addWeighted(img, 0.8, canvas, 0.2, 0) folded into one pass over the pixels the limbs cover.  `workspace` holds
+ * every image's marks and span rows (see cpb200_render_image).  The tables are trusted: centerpose_b200/render.py
+ * builds them.  1 <= B <= 65535. */
+int cpb200_render_poses_batch(unsigned char *pixels, const cpb200_render_image *images, int B,
+                              const cpb200_render_person *persons, const cpb200_render_limb *limbs,
+                              const int32_t *verts, const cpb200_render_text_px *text_px, const unsigned char *luts,
+                              void *workspace, void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)
