@@ -68,6 +68,9 @@ def lib() -> ctypes.CDLL:
                                                     ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     L.cpb200_render_poses_batch.restype = ctypes.c_int
     L.cpb200_render_poses_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 7
+    L.cpb200_heatmap_views_batch.restype = ctypes.c_int
+    L.cpb200_heatmap_views_batch.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.POINTER(ctypes.c_float)] * 3 + \
+        [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     L.cpb200_soft_nms_39.restype = ctypes.c_int
     L.cpb200_soft_nms_39.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                      ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]

@@ -63,6 +63,54 @@ __device__ __forceinline__ void exif_source(int o, int oy, int ox, int h, int w,
   }
 }
 
+// ---- cv2.resize INTER_LINEAR on 8-bit images, one output pixel ----
+// Bit-exact with OpenCV's fixed-point linear resize (resize.cpp, resizeGeneric_ with HResizeLinear / VResizeLinear and
+// the SIMD vertical pass): per output coordinate d, f = float((d + 0.5) * scale - 0.5) with scale = 1 / (out / in) in
+// double, i = floor(f), f -= i, a0 = rint((1 - f) * 2048), a1 = 2048 - a0.  Columns clamp the coefficient at the
+// border (i < 0 or i >= in - 1: i = clamp, f = 0); rows do not: the weights stay, each of the two source rows is
+// clipped to [0, in - 1] on its own (this is what makes the first and last rows of an upscale differ from a clamped
+// coefficient).  Horizontal pass exact in int32, h = s[i] * a0 + s[i + 1] * a1 (< 2^19); vertical pass as the 16-bit
+// SIMD code does it, t = ((h0 >> 4) * b0 >> 16) + ((h1 >> 4) * b1 >> 16), out = (t + 2) >> 2.
+
+// source index and 11-bit weight of the left / upper tap for output coordinate d; the float steps use explicit
+// round-to-nearest intrinsics so nvcc cannot contract them into FMAs (the host computes them unfused)
+__device__ __forceinline__ int resize_tap(int d, double scale, int &a0) {
+  float f = (float)__dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5);
+  const float fi = floorf(f);
+  f = __fsub_rn(f, fi);
+  a0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
+  return (int)fi;
+}
+
+// the 1 / (out / in) scale of one axis
+__device__ __forceinline__ double resize_scale(int out, int in) { return __ddiv_rn(1.0, __ddiv_rn((double)out, (double)in)); }
+
+// the two source columns (x0, x1), rows (y0, y1) and weights (a0, b0) of output pixel (x, y) when an h x w image is
+// resized with scales (sx, sy)
+struct LinearTaps {
+  int x0, x1, y0, y1, a0, b0;
+};
+
+__device__ __forceinline__ LinearTaps linear_taps(int x, int y, int h, int w, double sx, double sy) {
+  LinearTaps t;
+  t.x0 = resize_tap(x, sx, t.a0);
+  if (t.x0 < 0) { t.x0 = 0; t.a0 = 2048; }
+  if (t.x0 >= w - 1) { t.x0 = w - 1; t.a0 = 2048; }
+  t.x1 = min(t.x0 + 1, w - 1);
+  const int yt = resize_tap(y, sy, t.b0);
+  t.y0 = min(max(yt, 0), h - 1);
+  t.y1 = min(max(yt + 1, 0), h - 1);
+  return t;
+}
+
+// one channel of the output pixel from its four source values s<row><col> at (y0|y1, x0|x1)
+__device__ __forceinline__ unsigned char linear_mix(int s00, int s01, int s10, int s11, const LinearTaps &t) {
+  const int h0 = s00 * t.a0 + s01 * (2048 - t.a0);
+  const int h1 = s10 * t.a0 + s11 * (2048 - t.a0);
+  const int v = (((h0 >> 4) * t.b0) >> 16) + (((h1 >> 4) * (2048 - t.b0)) >> 16);
+  return (unsigned char)min(max((v + 2) >> 2, 0), 255);
+}
+
 #define CPB_ACT_MASK (CPB200_FLAG_RELU | CPB200_FLAG_HSWISH | CPB200_FLAG_HSIGMOID | CPB200_FLAG_RELU6 | CPB200_FLAG_CLIP01)
 // Epilogue non-linearity selected by the op flags (at most one of RELU / HSWISH / HSIGMOID / RELU6 / CLIP01).  hswish
 // and hsigmoid keep the reference's operation order x * relu6(x + 3) / 6 (mobilenetv3.py:84-93).  ReLU6 and the hard

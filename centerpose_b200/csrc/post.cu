@@ -298,26 +298,10 @@ extern "C" int cpb200_pre_process_batch(const unsigned char *imgs, const cpb200_
 
 // ---- device resize: cv2.resize(img, (new_w, new_h)), INTER_LINEAR, 8-bit, 3 channels ----
 // Replaces the first line of BaseDetector.pre_process at a test scale != 1 (lib/detectors/base_detector.py:33-34).
-// Bit-exact with OpenCV's fixed-point linear resize (resize.cpp, resizeGeneric_ with HResizeLinear / VResizeLinear and
-// the SIMD vertical pass): per output coordinate d, f = float((d + 0.5) * scale - 0.5) with scale = 1 / (out / in) in
-// double, i = floor(f), f -= i, a0 = rint((1 - f) * 2048), a1 = 2048 - a0.  Columns clamp the coefficient at the
-// border (i < 0 or i >= in - 1: i = clamp, f = 0); rows do not: the weights stay, each of the two source rows is
-// clipped to [0, in - 1] on its own (this is what makes the first and last rows of an upscale differ from a clamped
-// coefficient).  Horizontal pass exact in int32, h = s[i] * a0 + s[i + 1] * a1 (< 2^19); vertical pass as the 16-bit
-// SIMD code does it, t = ((h0 >> 4) * b0 >> 16) + ((h1 >> 4) * b1 >> 16), out = (t + 2) >> 2.
+// The per-pixel arithmetic is cpb::linear_taps / cpb::linear_mix (common.cuh).
 namespace {
 
 static_assert(sizeof(cpb200_resize_image) == 32, "cpb200_resize_image layout is part of the C ABI");
-
-// source index and 11-bit weight of the left / upper tap for output coordinate d; the float steps use explicit
-// round-to-nearest intrinsics so nvcc cannot contract them into FMAs (the host computes them unfused)
-__device__ __forceinline__ int resize_tap(int d, double scale, int &a0) {
-  float f = (float)__dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5);
-  const float fi = floorf(f);
-  f = __fsub_rn(f, fi);
-  a0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
-  return (int)fi;
-}
 
 // grid (pixel blocks, image): blockIdx.y selects the image; one thread per output pixel (its 3 channels), the blocks
 // of one image stride over its new_h * new_w pixels in row-major order, so a warp writes 96 contiguous bytes
@@ -327,27 +311,15 @@ __global__ void __launch_bounds__(256) resize_linear_u8_kernel(const unsigned ch
   const cpb200_resize_image e = table[blockIdx.y];
   const unsigned char *img = src + e.src_offset;
   unsigned char *out = dst + e.dst_offset;
-  const double sx = __ddiv_rn(1.0, __ddiv_rn((double)e.new_w, (double)e.w));
-  const double sy = __ddiv_rn(1.0, __ddiv_rn((double)e.new_h, (double)e.h));
+  const double sx = cpb::resize_scale(e.new_w, e.w), sy = cpb::resize_scale(e.new_h, e.h);
   const int total = e.new_h * e.new_w;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int x = i % e.new_w, y = i / e.new_w;
-    int a0, b0;
-    int x0 = resize_tap(x, sx, a0);
-    if (x0 < 0) { x0 = 0; a0 = 2048; }
-    if (x0 >= e.w - 1) { x0 = e.w - 1; a0 = 2048; }
-    const int x1 = min(x0 + 1, e.w - 1), a1 = 2048 - a0;
-    const int yt = resize_tap(y, sy, b0), b1 = 2048 - b0;
-    const int y0 = min(max(yt, 0), e.h - 1), y1 = min(max(yt + 1, 0), e.h - 1);
-    const unsigned char *r0 = img + (size_t)y0 * e.w * 3, *r1 = img + (size_t)y1 * e.w * 3;
+    const cpb::LinearTaps t = cpb::linear_taps(i % e.new_w, i / e.new_w, e.h, e.w, sx, sy);
+    const unsigned char *r0 = img + (size_t)t.y0 * e.w * 3, *r1 = img + (size_t)t.y1 * e.w * 3;
     unsigned char *o = out + (size_t)i * 3;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const int h0 = r0[x0 * 3 + c] * a0 + r0[x1 * 3 + c] * a1;
-      const int h1 = r1[x0 * 3 + c] * a0 + r1[x1 * 3 + c] * a1;
-      const int t = (((h0 >> 4) * b0) >> 16) + (((h1 >> 4) * b1) >> 16);
-      o[c] = (unsigned char)min(max((t + 2) >> 2, 0), 255);
-    }
+    for (int c = 0; c < 3; ++c)
+      o[c] = cpb::linear_mix(r0[t.x0 * 3 + c], r0[t.x1 * 3 + c], r1[t.x0 * 3 + c], r1[t.x1 * 3 + c], t);
   }
 }
 

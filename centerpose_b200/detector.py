@@ -11,9 +11,11 @@ Differences that are additive only:
     ``flip_lr`` / ``flip_lr_off`` round-trip through numpy (``lib/models/utils.py:30-47``);
   * ``run_batch`` (new): many pre-processed images per call — the reference API is single-image;
   * ``run_images`` (new): ``run()`` for a list of raw images, batched on the device, with the reference's
-    test-time flip / multi-scale / soft-NMS settings, and optionally the drawn images;
-  * ``show_results`` / ``render_poses`` draw the detections on the device (csrc/render.cu), byte for byte as the
-    reference's Debugger; ``debug()`` (the DEBUG >= 2 heat-map views) is not provided.
+    test-time flip / multi-scale / soft-NMS settings, and optionally the drawn images and the heat-map views;
+  * ``show_results`` / ``render_poses`` draw the detections on the device (csrc/render.cu), and ``debug()`` (DEBUG >= 2)
+    blends the predicted heat maps onto the network input on the device (csrc/heatmaps.cu), byte for byte as the
+    reference's Debugger.  ``debug()`` reads ``output[0]`` / ``output[4]`` and ``cfg.LOSS.HM_HP`` where the
+    reference's ``output['hm']`` / ``self.LOSS.HM_HP`` would raise (INTEGRATION.md).
 """
 from __future__ import annotations
 
@@ -48,6 +50,7 @@ class BaseDetector(object):
         self.scales = cfg.TEST.TEST_SCALES
         self.cfg = cfg
         self.pause = True
+        self.debug_imgs = {}        # the Debugger's imgs: what DEBUG >= 1 shows, refilled by every run()
         if int(cfg.TEST.TOPK) > 128 or int(cfg.TEST.TOPK) < 1:
             # the fused decode kernel keeps K candidates per channel on chip (CPB200_DECODE_MAX_K, include/centerpose_b200.h);
             # the reference accepts any TOPK (lib/models/decode.py:235) — say so here instead of failing at the first image
@@ -165,6 +168,7 @@ class BaseDetector(object):
         'net', 'dec', 'post', 'merge'}`` (seconds, CUDA-synchronised like the reference's timers)."""
         clock = {k: 0.0 for k in ("load", "pre", "net", "dec", "post", "merge", "tot")}
         sync = torch.cuda.synchronize
+        self.debug_imgs = {}        # the reference makes a new Debugger per call
         t_start = time.time()
         image, prepared = self._load(image_or_path_or_tensor)
         t_prev = time.time()
@@ -407,14 +411,23 @@ class MultiPoseDetector(BaseDetector):
         return results.tolist()
 
     def debug(self, debugger, images, dets, output, scale=1):
-        raise NotImplementedError("visual debugging (lib/utils/debugger.py) is outside the GPU hot path")
+        """multi_pose.py:82-94: ``self.debug_imgs['pred_hm']`` and ``['pred_hmhp']``, the centre and keypoint heat maps
+        of ``output`` (as ``process()`` leaves them) blended onto the de-normalized network input ``images[0]``, made
+        on the device (``heatmaps.views``: one launch table, three kernels, one copy back).  ``debugger`` and
+        ``dets`` are unused (the reference scales ``dets`` and then drops them).  ``HM_HP: false`` never gets here:
+        the decode raises first."""
+        from . import heatmaps
+        self.debug_imgs.update(heatmaps.views([images[0].contiguous()], [output[0][0].contiguous()],
+                                              [output[4][0].contiguous()], self.cfg.MODEL.DOWN_RATIO,
+                                              self.cfg.DEBUG_THEME, self.mean, self.std)[0])
 
     def show_results(self, debugger, image, results):
         """multi_pose.py:96-107: draws every row above ``TEST.VIS_THRESH`` on a copy of ``image`` with the device
-        renderer (``render_poses``) into ``self.debug_imgs['multi_pose']``, then shows it as the reference's
+        renderer (``render_poses``) into ``self.debug_imgs['multi_pose']``, then shows every entry of
+        ``self.debug_imgs`` in insertion order (with DEBUG >= 2 the heat-map views first) as the reference's
         ``Debugger.show_all_imgs`` does.  Without a cv2 GUI backend (opencv-python-headless) the display is skipped.
         ``debugger`` is unused (the reference passes its Debugger; ``run()`` passes None)."""
-        self.debug_imgs = {"multi_pose": self.render_poses([image], [results])[0]}
+        self.debug_imgs["multi_pose"] = self.render_poses([image], [results])[0]
         try:
             for name, img in self.debug_imgs.items():
                 cv2.imshow(name, img)
@@ -602,7 +615,7 @@ class MultiPoseDetector(BaseDetector):
         return views, [offsets[n] for n in range(len(images))], pixels
 
     @torch.no_grad()
-    def run_images(self, images, max_batch=32, return_images=False):
+    def run_images(self, images, max_batch=32, return_images=False, return_heatmaps=False):
         """Additive: ``run()`` for many images at once, with the reference's test-time settings (``FLIP_TEST``,
         ``TEST_SCALES``, ``FIX_RES``, ``NMS``; what tools/evaluate.py runs).  ``images`` is a list of BGR uint8 HWC
         arrays or image paths.  Returns one float32 ``(N_i, 56)`` array per image, in input order, equal to
@@ -633,7 +646,13 @@ class MultiPoseDetector(BaseDetector):
         image of its rows (what ``show_results`` draws).  The images are then all in one device buffer (the decoded
         files where the device decode put them, the arrays uploaded once into slots after them), the groups read them
         there, and ``cpb200_render_poses_batch`` draws on them in place after the rows are known, followed by one
-        device-to-host copy of the drawn images."""
+        device-to-host copy of the drawn images.
+
+        With ``return_heatmaps=True`` it also returns per image the ``{'pred_hm', 'pred_hmhp'}`` views ``run()`` with
+        DEBUG 2 leaves in ``debug_imgs``: ``(rows, views)``, or ``(rows, drawn, views)`` with ``return_images``.  They
+        come from each image's last test scale, as ``run()`` keeps the last scale's views.  Every group at that scale
+        makes its images' views with one ``cpb200_heatmap_views_batch`` after its decode (the maps get ``process()``'s
+        in-place logistic first), into one device buffer that one device-to-host copy brings back."""
         import ctypes
         from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch
@@ -649,7 +668,7 @@ class MultiPoseDetector(BaseDetector):
         else:
             loaded = [self._load_checked(n, src) for n, src in enumerate(images)]
         if not loaded:
-            return ([], []) if return_images else []
+            return ([],) * (1 + bool(return_images) + bool(return_heatmaps)) if return_images or return_heatmaps else []
         cfg = self.cfg
         dev = torch.device("cuda")
         stream = torch.cuda.current_stream(dev).cuda_stream
@@ -665,6 +684,11 @@ class MultiPoseDetector(BaseDetector):
                 items.append((i, (new_h, new_w), trans_input, meta))
                 keys.append((si, inp_h, inp_w))
         rows = torch.empty((len(loaded), S * K, 56), dtype=torch.float32, device=dev)
+        if return_heatmaps:
+            from . import heatmaps
+            view_shapes = [keys[i * S + S - 1][1:] for i in range(len(loaded))]
+            view_at = np.cumsum([0] + [heatmaps.view_bytes(H, W) for H, W in view_shapes]).tolist()
+            views_dev = torch.empty(max(view_at[-1], 1), dtype=torch.uint8, device=dev)
         for (si, inp_h, inp_w), idx in group_by_shape(keys, max_batch):
             B = len(idx)
             # one pinned buffer, one upload of the raw images with their tables (pack_group)
@@ -703,18 +727,39 @@ class MultiPoseDetector(BaseDetector):
                 dets = multi_pose_decode(hm, wh, hps, reg=reg, hm_hp=hm_hp, hp_offset=hp_offset, K=K, affine=aff)
             else:
                 dets = self._decode_heads(outputs, affine=aff)
+                if return_heatmaps and si == S - 1:
+                    # the decode read the logits; the views take the maps as process() leaves them
+                    sigmoid_(outputs[0])
+                    if not cfg.LOSS.MSE_LOSS:
+                        sigmoid_(outputs[4])
             rows[dst, si * K:(si + 1) * K] = dets
+            if return_heatmaps and si == S - 1:
+                step = 2 if flip else 1
+                hm, hm_hp = outputs[0], outputs[4]
+                n_img = [items[j][0] for j in idx]
+                heatmaps.check([inp[b * step] for b in range(B)], [hm[b * step] for b in range(B)],
+                               [hm_hp[b * step] for b in range(B)], cfg.MODEL.DOWN_RATIO)
+                table, _, ws = heatmaps.layout(
+                    [(inp[b * step].data_ptr(), hm[b * step].data_ptr(), hm_hp[b * step].data_ptr()) for b in range(B)],
+                    [(inp_h, inp_w, hm.shape[2], hm.shape[3], hm_hp.shape[1])] * B, cfg.MODEL.DOWN_RATIO,
+                    [view_at[i] for i in n_img])
+                heatmaps.launch(table, ws, cfg.DEBUG_THEME, self.mean, self.std, views_dev)
         if cfg.TEST.NMS or S > 1:
             soft_nms_39_cuda_batch(rows, Nt=0.5, method=2)
         out = rows.cpu().numpy()
         rows_out = [out[i] for i in range(len(loaded))]
-        if not return_images:
+        if not (return_images or return_heatmaps):
             return rows_out
-        from . import render
-        shapes = [tuple(im.shape[:2]) for im in loaded]
-        ops = render.build(shapes, rows_out, float(cfg.TEST.VIS_THRESH), cfg.DEBUG_THEME)
-        render.launch(ops, pixels=pixels_dev, offsets=offsets)
-        return rows_out, render.download(pixels_dev, offsets, shapes)
+        res = (rows_out,)
+        if return_images:
+            from . import render
+            shapes = [tuple(im.shape[:2]) for im in loaded]
+            ops = render.build(shapes, rows_out, float(cfg.TEST.VIS_THRESH), cfg.DEBUG_THEME)
+            render.launch(ops, pixels=pixels_dev, offsets=offsets)
+            res += (render.download(pixels_dev, offsets, shapes),)
+        if return_heatmaps:
+            res += (heatmaps.download(views_dev, view_at[:-1], view_shapes),)
+        return res
 
 
 detector_factory = {"multi_pose": MultiPoseDetector}     # detector_factory.py:5-7

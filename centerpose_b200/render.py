@@ -19,6 +19,10 @@ import torch
 EDGES = ((0, 1), (0, 2), (1, 3), (2, 4), (3, 5), (4, 6), (5, 6), (5, 7), (7, 9), (6, 8), (8, 10), (5, 11), (6, 12),
          (11, 12), (11, 13), (13, 15), (12, 14), (14, 16))
 JOINTS = 17
+# the colour (BGR) of each joint's heat map in the Debugger's 'pred_hmhp' view (its colors_hp), in joint order
+JOINT_COLORS = ((255, 0, 255), (255, 0, 0), (0, 0, 255), (255, 0, 0), (0, 0, 255), (255, 0, 0), (0, 0, 255),
+                (255, 0, 0), (0, 0, 255), (255, 0, 0), (0, 0, 255), (255, 0, 0), (0, 0, 255), (255, 0, 0), (0, 0, 255),
+                (255, 0, 0), (0, 0, 255))
 STICK_WIDTH = 2
 FONT = cv2.FONT_HERSHEY_SIMPLEX
 # the box and label colour of class 0 (BGR): the 'white' theme draws the inverted, clipped last colour of the

@@ -350,6 +350,33 @@ int cpb200_render_poses_batch(unsigned char *pixels, const cpb200_render_image *
                               const int32_t *verts, const cpb200_render_text_px *text_px, const unsigned char *luts,
                               void *workspace, void *stream);
 
+/* Heat-map views (csrc/heatmaps.cu, centerpose_b200/heatmaps.py builds the table).  One image of
+ * cpb200_heatmap_views_batch (64 bytes, DEVICE memory).  The three sources are device addresses, so one table can
+ * take images from several forward batches and every other image of a flip-test batch. */
+typedef struct cpb200_heatmap_image {
+  const float *input;        /* its (3, H, W) normalized network input */
+  const float *hm;           /* its (1, h, w) centre heat map */
+  const float *hm_hp;        /* its (C, h, w) keypoint heat maps */
+  int64_t out_offset;        /* in `out`: the (H, W, 3) uint8 BGR pred_hm view, then the pred_hmhp view */
+  int64_t ws_offset;         /* in `workspace`: 2 * (h * w + H * W) * 3 bytes */
+  int32_t H, W, h, w;        /* H = h * dr, W = w * dr; H * W < 2^31 */
+  int32_t C, dr;             /* 1 <= C <= CPB200_HEATMAP_MAX_C, dr >= 1 */
+} cpb200_heatmap_image;
+
+#define CPB200_HEATMAP_MAX_C 17
+
+/* The reference's Debugger views of MultiPoseDetector.debug (DEBUG >= 2): gen_colormap of `hm` blended onto the
+ * de-normalized input as 'pred_hm', gen_colormap_hp of `hm_hp` as 'pred_hmhp' (add_blend_img, trans 0.7), byte for
+ * byte.  Per view: the colour map max_c(map[c] * colour[c]) cast to uint8 as numpy casts, cv2.resize'd to
+ * (h * dr, w * dr) (so a non-square map comes out transposed), inverted with the 'white' theme, resized back to
+ * (W, H) unless already that size, and blended in float64 with clip(((x * std + mean) * 255), 0, 255) as uint8.
+ * Three launches for B images of any sizes: colour maps, first resize, second resize and blend.  `colors` is a HOST
+ * array of (1 + CPB200_HEATMAP_MAX_C) x 3 floats, the hm colour then the keypoint colours, with the theme applied;
+ * `mean` / `stdv` HOST arrays of 3 floats; `white` != 0 inverts the resized colour map.  The table is trusted:
+ * centerpose_b200/heatmaps.py checks it.  1 <= B <= 65535. */
+int cpb200_heatmap_views_batch(const cpb200_heatmap_image *table, int B, const float *colors, const float *mean,
+                               const float *stdv, int white, unsigned char *out, unsigned char *workspace, void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)
