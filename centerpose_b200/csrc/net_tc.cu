@@ -520,6 +520,9 @@ int tap_prepare(const cpb200_op &op, Prepared **out) {
   const long long src_plane = (long long)op.B * op.H * op.W * op.cin[0];
   if (dcn && P == 2 && src_plane * 4 >= (1LL << 32))
     return fail(CPB200_ERR_ARG, "tc: split-precision DCN input must stay below 4 GiB (32-bit gather offsets)");
+  // the bf16 gather builds its corner offsets in elements as signed ints: B*H*W*Cin must stay below 2^31
+  if (dcn && P == 1 && src_plane >= (1LL << 31))
+    return fail(CPB200_ERR_ARG, "tc: bf16 DCN input must stay below 2^31 elements (32-bit gather offsets)");
   int BN = bn_for(op.cout, P);
   // DCN: the gather warps leave 120 registers per thread, so a consumer holds at most 64 accumulator registers
   if (dcn && BN > 128 / P) BN = 128 / P;

@@ -166,7 +166,8 @@ class Case:
     reason: str
     B: int = 1
     error: Optional[str] = None                # an expected CPB200_ERR_ARG: a fragment of its message
-    randn_only: bool = False                   # no integer-exact leg (set for DCN, hswish / hsigmoid, pools, resize)
+    randn_only: bool = False                   # no integer-exact leg (hswish / hsigmoid, pools over 2^k-free sizes)
+    claims: FrozenSet[str] = frozenset()       # DCN: what its "int" data reaches (tests/test_dcn_cases_cpu.py)
 
     def precisions(self):
         out = []
@@ -195,8 +196,9 @@ def _fs(*ks):
 CASES = []
 
 
-def add(method, routes, reason, B=1, error=None, randn_only=False, **kw):
-    CASES.append(Case(record(method, **kw), {k: frozenset(v) for k, v in routes.items()}, reason, B, error, randn_only))
+def add(method, routes, reason, B=1, error=None, randn_only=False, claims=(), **kw):
+    CASES.append(Case(record(method, **kw), {k: frozenset(v) for k, v in routes.items()}, reason, B, error, randn_only,
+                      frozenset(claims)))
 
 
 def island(*ks):
@@ -305,8 +307,21 @@ for co in (16, 27, 48):
          reason=f"CUDA-core conv, cout {co} (tile {k_simt('float', co)})")
 
 # ---- DCN ----
-def dcn(cin, cout, H, W, routes, reason, B=1):
-    add("dcn", routes, reason, B=B, randn_only=True, x=sym(cin, H, W), w=tensor(cout, cin, 3, 3), b=tensor(cout),
+# Every DCN case runs three legs: dyadic data (exact sampling positions, exact result), "coord" data (exact positions,
+# real-valued samples, conv bounds) and randn data.  ``claims`` name what a case's dyadic data reaches, as
+# tests/test_dcn_cases_cpu.py computes it from the data in float64:
+#   "all-pairs"   every (h-class, w-class) pair of sampling classes (DCN_CLASSES) on a tap whose mask is not 0
+#   "beyond-tile" samples inside the map displaced by more than the tensor-core tile: one with |dh| > TH, one with
+#                 |dw| > TW
+#   "beyond-map"  a displacement larger than the map: |dh| > H or |dw| > W
+#   "masks"       each mask value (0, 0.5, 1) on at least two taps
+#   "last-pixel"  B >= 2 and a sample of the last image that reads its last row and column with a nonzero weight
+DCN_CLASSES = ("p <= -1", "-1 < p < 0", "integer p in [0, S-1]", "fractional p in (0, S-1)", "S-1 < p < S", "p >= S")
+DCN_CLAIMS = ("all-pairs", "beyond-tile", "beyond-map", "masks", "last-pixel")
+
+
+def dcn(cin, cout, H, W, routes, reason, B=1, claims=()):
+    add("dcn", routes, reason, B=B, claims=claims, x=sym(cin, H, W), w=tensor(cout, cin, 3, 3), b=tensor(cout),
         om_w=tensor(27, cin, 3, 3), om_b=tensor(27))
 
 
@@ -329,6 +344,7 @@ dcn(64, 16, 9, 9, {"bf16-simt": {k_simt("bf16", 32), k_simt("bf16", 16, True)}, 
     reason="DCN cout 16 on the CUDA-core kernel (bf16 with tc=False)")
 dcn(64, 32, 9, 9, {"bf16-simt": {k_simt("bf16", 32), k_simt("bf16", 32, True)}}, reason="bf16 CUDA-core DCN, cout 32")
 dcn(64, 64, 9, 9, {"bf16-simt": {k_simt("bf16", 32), k_simt("bf16", 64, True)}}, reason="bf16 CUDA-core DCN, cout 64")
+
 
 # ---- stems ----
 def stem(co, k, stride, H, W, routes, reason, B=1, error=None, act=None):
@@ -413,16 +429,53 @@ elt("maxpool", lambda fm: k_elt("maxpool_kernel", fm), "3x3 / stride 2 / pad 1, 
 for f, skip, relu in ((2, True, True), (4, False, False), (8, True, False), (4, True, True), (8, False, True)):
     elt("upsample_add", lambda fm: k_elt("upsample_add_kernel", fm), f"nearest upsample x{f}, skip {skip}, relu {relu}",
         x=sym(32, 5, 7), skip=sym(32, 5 * f, 7 * f) if skip else None, f=f, relu=relu)
-for H, W in ((1, 1), (7, 7), (96, 160)):
+def avgpool(H, W):
+    pow2 = (H * W) & (H * W - 1) == 0                   # a mean over 2^k integers is exact
     elt("avgpool", lambda fm: {f"avgpool_kernel<{FMT[fm][0]},{'float*' if fm == 'x2' else FMT[fm][1]}>"} |
-        ({CVT_OUT} if fm == "x2" else set()), f"global average pool over {H}x{W}", randn_only=True, x=sym(64, H, W))
+        ({CVT_OUT} if fm == "x2" else set()), f"global average pool over {H}x{W}", randn_only=not pow2, x=sym(64, H, W))
+
+
+for H, W in ((1, 1), (7, 7), (96, 160)):
+    avgpool(H, W)
 for skip in (True, False):
     elt("scale_add", lambda fm: {f"scale_add_kernel<{FMT[fm][0]},{'float*' if fm == 'x2' else FMT[fm][1]},{FMT[fm][1]}>"} |
         ({CVT_IN} if fm == "x2" else set()), f"SE gate, skip {skip}", x=sym(48, 9, 11), gate=sym(48, 1, 1),
         skip=sym(48, 9, 11) if skip else None)
-elt("avgpool2", lambda fm: k_elt("avgpool2_kernel", fm), "2x2 average pool, odd sizes", randn_only=True, x=sym(32, 17, 23))
+elt("avgpool2", lambda fm: k_elt("avgpool2_kernel", fm), "2x2 average pool, odd sizes", x=sym(32, 17, 23))
 elt("resize_bilinear", lambda fm: k_elt("resize_bilinear_kernel", fm), "align-corners bilinear 9x11 -> 17x23",
     randn_only=True, x=sym(32, 9, 11), Ho=17, Wo=23)
+
+# ---- cases added after the ones above (appended, so that a case keeps its index in CASES) ----
+avgpool(8, 8)
+avgpool(16, 32)
+elt("resize_bilinear", lambda fm: k_elt("resize_bilinear_kernel", fm),
+    "align-corners bilinear 9x11 -> 17x21: ratio 1/2 both ways, exact on integers", x=sym(32, 9, 11), Ho=17, Wo=21)
+
+# constructed sampling: every class pair, displacements past a tile and past the map, B = 2 (the rowb = n * H base)
+_ALL = ("all-pairs", "masks", "last-pixel")
+dcn(64, 48, 13, 11, {"fp32": _dcn_simt("float", 64, 48), "bf16": {k_c3(32, 1), k_tc(64, 1, True)},
+                     "x2": {k_c3(32, 2), k_tc(64, 2, True)}, "bf16-simt": {k_simt("bf16", 32), k_simt("bf16", 48, True)}},
+    B=2, claims=_ALL + ("beyond-map",),
+    reason="DCN TW 8 x TH 16, partial tiles both ways (13 x 11), cout 48: partial 64 tile")
+dcn(128, 96, 11, 23, {"fp32": _dcn_simt("float", 128, 96), "bf16": {k_c3(32, 1), k_tc(128, 1, True)},
+                      "x2": {k_c3(32, 2), k_tc(64, 2, True)}},
+    B=2, claims=_ALL + ("beyond-map",),
+    reason="DCN TW 16 x TH 8, partial tiles both ways (11 x 23), cin 128 (two K slabs), cout 96: partial 128 tile (bf16), "
+           "64 + partial 32 (split)")
+dcn(256, 32, 9, 17, {"fp32": _dcn_simt("float", 256, 32), "bf16": {k_c3(32, 1), k_tc(32, 1, True)},
+                     "x2": {k_c3(32, 2), k_tc(32, 2, True)}, "bf16-simt": {k_simt("bf16", 32), k_simt("bf16", 32, True)}},
+    B=2, claims=_ALL + ("beyond-map",), reason="DCN cin 256 (four K slabs), cout 32, TW 16 with one extra column")
+dcn(64, 16, 10, 9, {"fp32": _dcn_simt("float", 64, 16), "bf16": {k_c3(32, 1), k_simt("bf16", 16, True)},
+                    "x2": island(k_c3(32, 2), k_simt("float", 16, True))},
+    B=2, claims=_ALL + ("beyond-map",),
+    reason="DCN cout 16: tensor-core offset conv, CUDA-core DCN (an fp32 island in the split precisions)")
+dcn(64, 64, 9, 6, {"fp32": _dcn_simt("float", 64, 64), "bf16": {k_simt("bf16", 32), k_simt("bf16", 64, True)},
+                   "x2": island(k_simt("float", 32), k_simt("float", 64, True))},
+    B=2, claims=_ALL + ("beyond-map",), reason="DCN W = 6 < 8: the split fp32 island, every class pair")
+dcn(64, 128, 96, 128, {"bf16": {k_c3(32, 1), k_tc(128, 1, True)}, "x2": {k_c3(32, 2), k_tc(64, 2, True)}},
+    B=3, claims=_ALL + ("beyond-tile",),
+    reason="DCN 288 tiles (bf16) / 576 (split) > 2 x 132 SMs: the persistent loop wraps and the next unit's corner "
+           "loads cross a tile boundary")
 
 
 # ---- fused heads (Plan._fuse_heads -> heads_tc_kernel): n x (3x3 + ReLU -> 1x1 NCHW) over one input ----

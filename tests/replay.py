@@ -12,7 +12,20 @@ Data (``_data``, seeded by the record's call):
            value is an integer of magnitude <= INT_NNZ + 5 (<= 256), so fp32, bf16 and fp16 hold each one exactly, even
            after fp16x2's 2^12 weight pre-scale (sums stay below 2^24 * 2^12 in steps of 2^12), the lo plane is 0 and the
            result equals the float64 reference bit for bit.  Needs CPB200_RZ_COMP=0 when the plan is built, so that
-           acc_scale is a pure power of two.
+           acc_scale is a pure power of two.  The pools and the resize are exact on it too: means over 4 or 2^k pixels,
+           and align-corners ratios of 1/2.
+           DCN (_dcn_int): dyadic data.  x and the DCN weights / bias as above; the offset rows of om_w are sparse
+           multiples of 1/4 with |w| <= 4 (exact in bf16, and under fp16x2's 2^12 pre-scale) and om_b's offsets
+           multiples of 1/4, so every sampling position is a multiple of 1/4, exact in fp32 on every route; the mask
+           rows of om_w are zero and the mask logits (om_b) exactly 0 or +-200, a mask of 0.5 or exactly 0 / 1 on every
+           route.  Corner weights are multiples of 1/16, samples multiples of 1/32 with |s| <= 1 (at most 6 significant
+           bits: the packed bf16 blend of the bf16 kernel is exact) and every output a multiple of 1/32 below 2^10 (15
+           bits): the tensor-core sums and both split planes are exact, and each route equals the float64 reference as
+           the output format stores it (_as_stored).
+  "coord": a real-valued DCN with exact sampling positions (_dcn_coord).  x randn (bf16-rounded for bf16) except
+           COORD_CH channels of small integers, which are the only channels the offset rows of om_w read (multiples of
+           1/4, so with CPB200_RZ_COMP=0 the positions are exact and vary over space); mask rows randn.  Judged by the
+           conv bounds (TOL), not the DCN's relative-L2 ones: only the arithmetic of the samples and the GEMM is left.
 
 Tolerances (the op tests' bounds, tests/util.py::check_op; bf16 here is a max-norm, where check_op's is relative L2):
   fp32   : |err| <= 2e-4 max|ref|;  DCN 5e-4 (test_dcn_op_matches_oracle: the sampling positions come from the fp32
@@ -21,8 +34,9 @@ Tolerances (the op tests' bounds, tests/util.py::check_op; bf16 here is a max-no
   bf16x2 : |err| <= 3e-4 max|ref|
   fp16x2 : |err| <= 1e-5 max|ref|
   split DCN: relative L2 <= 4 tol and |err| <= 40 tol max|ref|  (a sample within rounding of a pixel boundary flips corners)
+  DCN on "coord" data: the conv bounds above (TOL)
   max-pool: exact on the values the input planes hold.
-  "int" data: exact, element by element.
+  "int" data: exact, element by element (against the reference as the output format stores it, RNE).
 
 Guards.  Every check stays inside memory the test allocated.
   * Output canary: the final op(s) of the call write into [guard | output (both planes) | guard], all pre-filled with
@@ -47,7 +61,10 @@ BIASES = {"b", "om_b"}
 RELU_INPUTS = {"conv": "srcs", "deconv_k4s2": "x", "dcn": "x"}
 INT_NNZ = 96                                     # nonzeros per output channel of an integer-exact weight
 # methods whose result is a sum of products of the inputs, weights and biases: "int" data makes them exact
-INT_EXACT = {"conv", "stem", "deconv_k4s2", "maxpool", "up_add", "dwconv", "scale_add", "upsample_add"}
+INT_EXACT = {"conv", "stem", "deconv_k4s2", "maxpool", "up_add", "dwconv", "scale_add", "upsample_add", "avgpool",
+             "avgpool2", "resize_bilinear", "dcn"}
+MASK_LOGIT = (200.0, 0.0, -200.0)                # DCN "int" mask logits: sigmoid 1, 0.5 and 0 on every route
+COORD_CH = 2                                     # DCN "coord": integer channels the offset rows read
 
 
 def _is_sym(d):
@@ -69,9 +86,88 @@ def _ternary(shape, g, nnz_per_row=None):
     return torch.zeros(shape[0], n).scatter_(1, keep, sign).reshape(shape)
 
 
+def _quarters(shape, g, nnz, top=16):
+    """sparse multiples of 1/4 with |w| <= top / 4: at most ``nnz`` nonzeros in each row of dim 0"""
+    n = 1
+    for s in shape[1:]:
+        n *= s
+    keep = torch.rand(shape[0], n, generator=g).argsort(1)[:, :nnz]
+    q = torch.randint(1, top + 1, keep.shape, generator=g).float() / 4
+    q *= torch.randint(0, 2, keep.shape, generator=g).float() * 2 - 1
+    return torch.zeros(shape[0], n).scatter_(1, keep, q).reshape(shape)
+
+
+def _dcn_int(rec, g, B):
+    """dyadic DCN data (module docstring, "int").  Tap t's mask logit is MASK_LOGIT[(t + seed) % 3] (neighbouring taps
+    differ).  Five of the six taps whose mask is not 0 are "near" taps: their offsets read only x channel 0, which is
+    constant over each image (-1, 0, 1, -1, ...), so a near tap samples every pixel at one (dh, dw) per image, chosen
+    so that its first sample row / column starts at a position of _DCN_START.  Over two images the five near taps take
+    all nine (row start, column start) kinds of _DCN_START in turn, whose class sets (kernel_routes.DCN_CLASSES: p <= -1,
+    (-1, 0), integer, fractional, (S-1, S), >= S) cross to every (h-class, w-class) pair.  The other taps read eight
+    (channel, tap) entries of x with weights k/4, |k| <= 16, around a bias in [-6, 6]: positions that vary over the
+    map, up to 38 pixels away."""
+    x = rec.arg("x")
+    C, H, W = x[1], x[2], x[3]
+    co = rec.arg("w")[1][0]
+    xs = _ternary((B, C, H, W), g)
+    xs[:, 0] = (torch.arange(B) % 3 - 1).float().view(B, 1, 1)
+    out = {"x": xs, "w": _ternary((co, C, 3, 3), g, INT_NNZ), "b": torch.randint(-4, 5, (co,), generator=g).float()}
+    logits = [MASK_LOGIT[(t + rec.seed) % 3] for t in range(9)]
+    near = [t for t in range(9) if logits[t] != MASK_LOGIT[2]][:5]
+    om_w = torch.zeros(27, C, 3, 3)
+    om_b = torch.zeros(27)
+    kinds = [(h, w) for h in _DCN_START for w in _DCN_START]
+    for t in range(9):
+        if t not in near:
+            om_w[2 * t:2 * t + 2] = _quarters((2, C, 3, 3), g, 8)
+            om_b[2 * t:2 * t + 2] = torch.randint(-24, 25, (2,), generator=g).float() / 4
+            continue
+        k = near.index(t)
+        d = []                                         # (dh, dw) of image 0 (x channel 0 = -1) and image 1 (= 0)
+        for n in (0, 1):
+            kh, kw = kinds[(5 * n + k) % 9]
+            d.append((_DCN_START[kh][k % 2] - (t // 3 - 1), _DCN_START[kw][(k + n) % 2] - (t % 3 - 1)))
+        for axis in (0, 1):
+            om_b[2 * t + axis] = d[1][axis]
+            om_w[2 * t + axis, 0, 1, 1] = d[1][axis] - d[0][axis]
+    om_b[18:] = torch.tensor(logits)
+    out["om_w"], out["om_b"] = om_w, om_b
+    return out
+
+
+# first sample position of a near tap's row or column (tap offset included), by kind: its classes on a map of size S
+_DCN_START = {"below": (-1.25, -1.75),    # p <= -1, (-1, 0), fractional
+              "above": (1.5, 1.25),       # fractional, (S-1, S), >= S
+              "whole": (-1.0, 1.0)}       # p = -1, integers / integers, p = S
+
+
+def _dcn_coord(rec, g, B, bf):
+    """real-valued DCN data with exact sampling positions (module docstring, "coord")"""
+    x = rec.arg("x")
+    C, H, W = x[1], x[2], x[3]
+    co = rec.arg("w")[1][0]
+    rnd = (lambda t: t.bfloat16().float()) if bf else (lambda t: t)
+    xs = torch.randn(B, C, H, W, generator=g)
+    xs[:, :COORD_CH] = torch.randint(-3, 4, (B, COORD_CH, H, W), generator=g).float()
+    om_w = torch.zeros(27, C, 3, 3)
+    om_w[:18, :COORD_CH] = _quarters((18, COORD_CH, 3, 3), g, 4, top=8)
+    om_w[18:] = rnd(torch.randn(9, C, 3, 3, generator=g) / (9 * C) ** 0.5)
+    om_b = torch.zeros(27)
+    om_b[:18] = torch.randint(-8, 9, (18,), generator=g).float() / 4
+    om_b[18:] = torch.randn(9, generator=g)
+    return {"x": rnd(xs), "w": rnd(torch.randn(co, C, 3, 3, generator=g) / (9 * C) ** 0.5),
+            "b": torch.randn(co, generator=g), "om_w": om_w, "om_b": om_b}
+
+
 def _data(rec, variant, B=2):
-    """float32 CPU tensors for every tensor / Sym argument of ``rec`` (NCHW for Syms)."""
+    """float32 CPU tensors for every tensor / Sym argument of ``rec`` (NCHW for Syms).  "coord" / "coord-bf16": DCN
+    only (the latter bf16-rounded)."""
     g = torch.Generator().manual_seed(rec.seed)
+    if variant in ("coord", "coord-bf16"):
+        assert rec.method == "dcn", rec.method
+        return _dcn_coord(rec, g, B, variant == "coord-bf16")
+    if variant == "int" and rec.method == "dcn":
+        return _dcn_int(rec, g, B)
     if variant == "int":
         out = {}
         for name, d in rec.args:
@@ -252,17 +348,32 @@ def _replay(rec, precision, data, guard_from_end=0, B=2, tc=None, run=None):
     return got.cpu(), problems
 
 
-def _judge(rec, precision, got, ref, exact=False):
-    """-> (err / max|ref|, within bound, description)"""
+def _as_stored(rec, precision, ref):
+    """``ref`` rounded (RNE) to the format ``rec``'s result is stored in: fp32 (fp32 precision, fp32 / NCHW conv outputs,
+    the split global average pool), bf16, or the sum of the two split planes"""
+    from centerpose_b200.plan import split_planes
+    f32 = precision == "fp32" or dict(rec.args).get("out", "act") != "act" or \
+        (rec.method == "avgpool" and precision in ("bf16x2", "fp16x2"))
+    if f32:
+        return ref.float().double()
+    if precision == "bf16":
+        return ref.float().bfloat16().double()
+    return split_planes(ref.float(), torch.float16 if precision == "fp16x2" else torch.bfloat16).double().sum(0)
+
+
+def _judge(rec, precision, got, ref, exact=False, positions_exact=False):
+    """-> (err / max|ref|, within bound, description).  positions_exact: a DCN on "coord" data, held to the conv bounds."""
     scale = ref.abs().max().item() + 1e-30
     diff = (got - ref).nan_to_num(float("inf")).abs()
     ratio = diff.max().item() / scale
     tol = TOL[precision]
     if exact:
-        bad = int((diff != 0).sum())
+        bad = int((got != _as_stored(rec, precision, ref)).sum())
         return ratio, bad == 0, f"exact: {bad} elements differ"
     if rec.method == "maxpool":
         return ratio, ratio == 0.0, "exact"
+    if positions_exact:
+        return ratio, ratio <= tol, f"tol {tol:.0e} (exact positions)"
     if rec.method == "dcn" and precision != "fp32":
         rel = ((got - ref).norm() / ref.norm()).item()
         if precision == "bf16":

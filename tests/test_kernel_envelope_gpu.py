@@ -6,7 +6,10 @@ Each case runs twice where it can:
     every precision, so a dropped, doubled or shifted tap, K slab, tile row / column, padding error or wrong channel
     offset fails whatever the format's rounding (CPB200_RZ_COMP=0 at plan build: acc_scale a pure power of two);
   * randn data under the per-precision bounds of the layer replay (rounding, the hi / lo split, the RZ compensation).
-    DCN, hswish / hsigmoid, average pools and resize take this leg only.
+    hswish / hsigmoid and the global average pools over sizes that are not powers of two take this leg only.
+DCN cases take the exact leg on dyadic data (exact sampling positions; the result equals the reference as the output
+format rounds it) and a third, "coord" leg between the two: real-valued samples at exact positions, held to the conv
+bounds, so a split gather that loses the lo plane fails where the DCN's own loose randn bounds would pass it.
 The first leg also runs with the library's route log on: the set of kernels the program launched must equal the case's
 route set.
 """
@@ -72,12 +75,14 @@ def test_route(idx, pkey, monkeypatch):
                     run=lambda plan, st: _launched(plan, st, names))
         assert names == set(), names
         return
-    legs = (["int"] if case.exact else []) + ["bf16" if precision == "bf16" else "f32"]
+    bf = precision == "bf16"
+    coord = ["coord-bf16" if bf else "coord"] if case.rec.method == "dcn" else []
+    legs = (["int"] if case.exact else []) + coord + ["bf16" if bf else "f32"]
     failures = []
     for leg in legs:
         data = _data(case.rec, leg, case.B)
         with monkeypatch.context() as mp:
-            if leg == "int":
+            if leg == "int" or leg in coord:
                 mp.setenv("CPB200_RZ_COMP", "0")
             got, problems = _replay(case.rec, precision, data, B=case.B, tc=tc,
                                     run=(lambda plan, st: _launched(plan, st, names)) if leg == legs[0] else None)
@@ -89,7 +94,7 @@ def test_route(idx, pkey, monkeypatch):
             ref = _reference(case.rec, data, {"x": _stored(pb, data["x"])})
         else:
             ref = _reference(case.rec, data)
-        ratio, ok, how = _judge(case.rec, precision, got, ref, exact=leg == "int")
+        ratio, ok, how = _judge(case.rec, precision, got, ref, exact=leg == "int", positions_exact=leg in coord)
         if leg != "int":
             _note(pkey, ratio, case.label())
         if problems or not ok:

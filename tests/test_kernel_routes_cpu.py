@@ -16,9 +16,6 @@ from tests.replay import _is_sym, _is_syms
 CPU = torch.device("cpu")
 TC_KERNELS = ("conv_tc_kernel<", "conv3x3_tc_kernel<", "conv_sp_kernel<", "stem_tc_kernel<", "stem_tc_h_kernel<",
               "heads_tc_kernel<")
-# routes whose every case is judged on randn data only (no integer-exact leg exists for their arithmetic)
-RANDN_ONLY = re.compile(r"^(conv_tc_kernel<\d+,true|conv_simt_kernel<\w+,\d+,\d+,true|avgpool_kernel|avgpool2_kernel|"
-                        r"resize_bilinear_kernel)")
 
 
 def _precision(p):
@@ -66,7 +63,7 @@ def test_kernel_key_reads_both_demanglings():
 
 
 def test_every_route_has_a_case():
-    """... and an integer-exact one, except for the routes whose arithmetic has no exact form"""
+    """... and an exact one"""
     declared, exact = set(), set()
     for c in CASES:
         for p in c.routes:
@@ -79,8 +76,8 @@ def test_every_route_has_a_case():
             exact |= hc.routes[p]
     assert declared <= set(ROUTES), sorted(declared - set(ROUTES))
     assert set(ROUTES) <= declared, sorted(set(ROUTES) - declared)
-    missing = sorted(r for r in ROUTES if r not in exact and not RANDN_ONLY.match(r))
-    assert not missing, f"routes without an integer-exact case: {missing}"
+    missing = sorted(r for r in ROUTES if r not in exact)
+    assert not missing, f"routes without an exact case: {missing}"
     assert not set(UNREACHABLE) & set(ROUTES)
 
 

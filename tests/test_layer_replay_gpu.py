@@ -11,6 +11,10 @@ inputs randn (bf16-rounded in bf16); the split precisions replay every conv, den
 post-ReLU |randn| inputs, the statistics plan.RZ_BETA was measured with.  Weights randn / sqrt(fan_in), bias and residual
 randn, DCN offset weights with gain 1.5 (as tests/test_split_gpu.py::test_dcn_split).
 
+Every DCN is replayed twice more, with CPB200_RZ_COMP=0 at plan build (tests/replay.py): on dyadic data, where it must
+equal the float64 reference element by element as the output format stores it, and on "coord" data (exact sampling
+positions, real-valued samples), held to the conv bounds below rather than the DCN's.
+
 Tolerances (those of tests/test_net_gpu.py, tests/test_split_gpu.py and tests/test_hardnet_gpu.py):
   fp32   : |err| <= 2e-4 max|ref|;  DCN 5e-4 (test_dcn_op_matches_oracle: the sampling positions come from the fp32
            offset conv, whose summation order differs from the reference's)
@@ -76,7 +80,7 @@ def test_guards_notice_stray_writes_and_reads(precision):
 
 
 @pytest.mark.parametrize("arch,precision", [(a, p) for a in ARCHS for p in PRECS])
-def test_layer_replay(arch, precision):
+def test_layer_replay(arch, precision, monkeypatch):
     t0 = time.time()
     recs = signatures(arch, precision)
     split = precision in ("bf16x2", "fp16x2")
@@ -85,12 +89,18 @@ def test_layer_replay(arch, precision):
         variants = ["bf16"] if precision == "bf16" else ["f32"]
         if split and rec.method in RELU_INPUTS:
             variants.append("relu")
+        exact_pos = {"int", "coord", "coord-bf16"}
+        if rec.method == "dcn":
+            variants += ["int", "coord-bf16" if precision == "bf16" else "coord"]
         for variant in variants:
             n += 1
             label = f"{rec.label()} [{variant} inputs]"
             data = _data(rec, variant)
             try:
-                got, problems = _replay(rec, precision, data)
+                with monkeypatch.context() as mp:
+                    if variant in exact_pos:
+                        mp.setenv("CPB200_RZ_COMP", "0")
+                    got, problems = _replay(rec, precision, data)
             except Exception as e:                          # an op the library rejects is a finding too
                 failures.append(f"{label}: {type(e).__name__}: {e}")
                 continue
@@ -98,11 +108,12 @@ def test_layer_replay(arch, precision):
                 from centerpose_b200.plan import PlanBuilder
                 pb = PlanBuilder(B, 1, 1, precision, torch.device("cpu"))
                 ref = _reference(rec, data, {"x": _stored(pb, data["x"])})
-            elif variant == "bf16":
+            elif variant in ("bf16", "coord-bf16"):
                 ref = _reference(rec, data)
             else:
                 ref = _cached_reference(arch, rec, variant, data)
-            ratio, ok, how = _judge(rec, precision, got, ref)
+            ratio, ok, how = _judge(rec, precision, got, ref, exact=variant == "int",
+                                    positions_exact=variant in ("coord", "coord-bf16"))
             if ratio > worst[0]:
                 worst = (ratio, label)
             if problems or not ok:
