@@ -60,6 +60,9 @@ def lib() -> ctypes.CDLL:
     L.cpb200_png_decode_batch.restype = ctypes.c_int
     L.cpb200_png_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    L.cpb200_png_encode_batch.restype = ctypes.c_int
+    L.cpb200_png_encode_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     L.cpb200_webp_decode_batch.restype = ctypes.c_int
     L.cpb200_webp_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]

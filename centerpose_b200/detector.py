@@ -615,7 +615,7 @@ class MultiPoseDetector(BaseDetector):
         return views, [offsets[n] for n in range(len(images))], pixels
 
     @torch.no_grad()
-    def run_images(self, images, max_batch=32, return_images=False, return_heatmaps=False):
+    def run_images(self, images, max_batch=32, return_images=False, return_heatmaps=False, encode_png=False):
         """Additive: ``run()`` for many images at once, with the reference's test-time settings (``FLIP_TEST``,
         ``TEST_SCALES``, ``FIX_RES``, ``NMS``; what tools/evaluate.py runs).  ``images`` is a list of BGR uint8 HWC
         arrays or image paths.  Returns one float32 ``(N_i, 56)`` array per image, in input order, equal to
@@ -652,7 +652,14 @@ class MultiPoseDetector(BaseDetector):
         DEBUG 2 leaves in ``debug_imgs``: ``(rows, views)``, or ``(rows, drawn, views)`` with ``return_images``.  They
         come from each image's last test scale, as ``run()`` keeps the last scale's views.  Every group at that scale
         makes its images' views with one ``cpb200_heatmap_views_batch`` after its decode (the maps get ``process()``'s
-        in-place logistic first), into one device buffer that one device-to-host copy brings back."""
+        in-place logistic first), into one device buffer that one device-to-host copy brings back.
+
+        With ``encode_png=True`` the drawn images and the views come back as PNG files, ``bytes`` equal to
+        ``cv2.imencode('.png', image)[1].tobytes()`` (what the reference's ``Debugger.save_img`` writes), instead of
+        arrays: one ``cpb200_png_encode_batch`` encodes them where they are on the device, and the files are copied
+        back in place of the images.  It needs ``return_images`` or ``return_heatmaps``."""
+        if encode_png and not (return_images or return_heatmaps):
+            raise ValueError("run_images: encode_png=True needs return_images=True or return_heatmaps=True")
         import ctypes
         from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch
@@ -756,9 +763,27 @@ class MultiPoseDetector(BaseDetector):
             shapes = [tuple(im.shape[:2]) for im in loaded]
             ops = render.build(shapes, rows_out, float(cfg.TEST.VIS_THRESH), cfg.DEBUG_THEME)
             render.launch(ops, pixels=pixels_dev, offsets=offsets)
-            res += (render.download(pixels_dev, offsets, shapes),)
-        if return_heatmaps:
+            if not encode_png:
+                res += (render.download(pixels_dev, offsets, shapes),)
+        if return_heatmaps and not encode_png:
             res += (heatmaps.download(views_dev, view_at[:-1], view_shapes),)
+        if encode_png:
+            # the drawn images, then each image's two views, encoded in one launch where they are
+            from . import png
+            at, sh = [], []
+            if return_images:
+                at += [pixels_dev.data_ptr() + offsets[n] for n in range(len(loaded))]
+                sh += shapes
+            if return_heatmaps:
+                for o, (H, W) in zip(view_at[:-1], view_shapes):
+                    at += [views_dev.data_ptr() + o, views_dev.data_ptr() + o + H * W * 3]
+                    sh += [(H, W)] * 2
+            files = png.encode_at(at, sh, [3 * w for _, w in sh], dev)
+            if return_images:
+                res += (files[:len(loaded)],)
+                files = files[len(loaded):]
+            if return_heatmaps:
+                res += ([dict(zip(heatmaps.VIEWS, files[2 * i:2 * i + 2])) for i in range(len(loaded))],)
         return res
 
 

@@ -17,6 +17,10 @@ The device takes bit depths 1/2/4/8/16 in colour types 0/2/3/4/6, interlaced (Ad
 The kernels trust the table, so every size and offset read from the file is checked here; a file the parser cannot
 read (bad signature or CRC, truncated, a bad or oversize IHDR, an unknown critical chunk, IDAT chunks that are not
 consecutive, a missing or duplicate palette) raises ``ValueError`` naming the image.  ``cv2.imread`` refuses those files too.
+
+The other direction, ``cv2.imencode('.png', img)`` byte for byte on the device (``cpb200_png_encode_batch``,
+``csrc/png_encode.cu``): ``encode(images)`` returns the files of BGR uint8 host arrays or CUDA tensors, and
+``encode_layout`` / ``encode_launch`` encode images already on the device where they are.
 """
 from __future__ import annotations
 
@@ -203,3 +207,163 @@ def pack(infos, datas, dst_offsets, alloc=lambda n: np.empty(n, np.uint8)):
             hv[p:p + 768] = 0
             hv[p:p + len(info.palette)] = np.frombuffer(info.palette, np.uint8)
     return buf, ws
+
+
+# ---- encoding: cv2.imencode('.png', img) on the device ----
+#
+# OpenCV 4.13 writes a BGR uint8 image through libpng with the Sub filter (None on one-pixel rows), zlib level 1,
+# strategy Z_RLE and memLevel 8, so the file is fixed by the pixels.  zlib's _tr_flush_block may only store a block
+# whose start is still in the window; here it always is when storing could win.  Up to 16 KiB of scanlines the window
+# holds all of them (libpng sizes it so, and zlib slides only past 2 * window - 262 bytes).  Past that a block's start
+# leaves the 32 KiB window only if the block covers more than 32506 bytes with at most 16383 symbols, and then its
+# static coding, which bounds zlib's estimate, costs at most 9 bits per literal and 4 bits per matched byte: under 8
+# bits per byte, so storing (8 bits per byte plus 4 bytes) never wins and the rule never decides.
+
+ENCODE_KERNEL = "png_encode_batch"
+# struct cpb200_png_encode_image (include/centerpose_b200.h)
+ENCODE_IMAGE = np.dtype([("src", "<u8"), ("pitch", "<i8"), ("filt_offset", "<i8"), ("sym_offset", "<i8"),
+                         ("tile_offset", "<i8"), ("block_offset", "<i8"), ("state_offset", "<i8"), ("z_offset", "<i8"),
+                         ("z_bytes", "<i8"), ("h", "<i4"), ("w", "<i4"), ("tile0", "<i4"), ("block0", "<i4"),
+                         ("chunk0", "<i4"), ("pad", "<i4")])
+assert ENCODE_IMAGE.itemsize == 96
+# CPB200_PNG_ENCODE_TILE / _TILE_REC / _BLOCK_REC / _STATE_REC
+ENCODE_TILE, TILE_REC, BLOCK_REC, STATE_REC = 4096, 32, 1088, 64
+# zlib's symbol buffer at memLevel 8 (lit_bufsize - 1) and libpng's IDAT size
+BLOCK_SYMBOLS = 16383
+IDAT_BYTES = 8192
+
+
+def filtered_size(h, w):
+    """Bytes of the scanlines libpng deflates: per row a filter-type byte and 3 * w samples."""
+    return h * (1 + 3 * w)
+
+
+def deflate_bound(n):
+    """zlib's deflateBound of n bytes with the zlib wrapper, in the conservative form it uses for parameters other
+    than its defaults (libpng lowers windowBits for small images)."""
+    return n + ((n + 7) >> 3) + ((n + 63) >> 6) + 5 + 6
+
+
+def encode_bound(h, w):
+    """An upper bound of the PNG file size of an h x w image: signature, IHDR, the bound zlib stream in IDAT chunks,
+    IEND."""
+    zb = deflate_bound(filtered_size(h, w))
+    return 8 + 25 + 12 * -(-zb // IDAT_BYTES) + zb + 12
+
+
+def encode_layout(sources, shapes, pitches):
+    """The launch table of images at device addresses ``sources`` with ``(h, w)`` ``shapes`` and row ``pitches`` in
+    bytes.  Returns ``(table, (tiles, blocks, chunks), workspace_bytes, out_bytes)``: the slot counts of the launch,
+    the workspace it needs and the output bytes that hold every file (the sum of ``encode_bound``)."""
+    table = np.zeros(len(shapes), ENCODE_IMAGE)
+    up = lambda x, a: x + (-x) % a
+    ws = tiles = blocks = chunks = out = 0
+    for e, src, (h, w), pitch in zip(table, sources, shapes, pitches):
+        n = filtered_size(h, w)
+        if not (h >= 1 and w >= 1 and pitch >= 3 * w and n < 2 ** 31):
+            raise ValueError("png.encode: a %dx%d image with row pitch %d cannot be encoded" % (h, w, pitch))
+        e["src"], e["pitch"], e["h"], e["w"] = src, pitch, h, w
+        nt, nb = -(-n // ENCODE_TILE), n // BLOCK_SYMBOLS + 1
+        e["filt_offset"] = ws
+        e["sym_offset"] = ws = up(ws + n, 16)
+        e["tile_offset"] = ws = up(ws + 2 * n, 16)
+        e["block_offset"] = ws = ws + nt * TILE_REC
+        e["state_offset"] = ws = ws + nb * BLOCK_REC
+        e["z_offset"] = ws = up(ws + STATE_REC, 16)
+        e["z_bytes"] = up(deflate_bound(n) + 8, 16)
+        ws += int(e["z_bytes"])
+        e["tile0"], e["block0"], e["chunk0"] = tiles, blocks, chunks
+        tiles, blocks, chunks = tiles + nt, blocks + nb, chunks + -(-int(e["z_bytes"]) // IDAT_BYTES)
+        out += encode_bound(h, w)
+    if len(table) > 65535 or chunks >= 2 ** 31:
+        raise ValueError("png.encode: %d images exceed one launch" % len(table))
+    return table, (tiles, blocks, chunks), max(ws, 16), max(out, 1)
+
+
+def encode_launch(table, counts, workspace_bytes, out, sizes):
+    """One upload of ``table`` and one ``cpb200_png_encode_batch`` on the current stream: the files back to back from
+    byte 0 of the uint8 CUDA tensor ``out``, their sizes into the int64 CUDA tensor ``sizes``."""
+    import torch
+    from . import _lib
+    dev = out.device
+    host = torch.from_numpy(table.view(np.uint8).reshape(-1).copy()).pin_memory()
+    buf = host.to(dev, non_blocking=True)
+    ws = torch.empty(workspace_bytes, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        st = _lib.lib().cpb200_png_encode_batch(buf.data_ptr(), len(table), *counts, ws.data_ptr(), out.data_ptr(),
+                                                sizes.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(st, ENCODE_KERNEL)
+
+
+def download_files(out, sizes):
+    """One read of the sizes and one copy of the packed files: one ``bytes`` per image."""
+    sz = sizes.cpu().numpy()
+    ends = np.cumsum(sz)
+    data = out[:int(ends[-1])].cpu().numpy().tobytes()
+    return [data[e - s:e] for s, e in zip(sz.tolist(), ends.tolist())]
+
+
+def encode(images):
+    """``cv2.imencode('.png', img)[1].tobytes()`` of each BGR uint8 ``(H, W, 3)`` image, a host array or a CUDA tensor,
+    on the device: one upload of the host arrays, one launch, one read of the sizes and one copy of the files.  A CUDA
+    tensor is read where it is when its pixels are packed (strides (pitch, 3, 1)).  Anything else raises
+    ``ValueError`` before any launch."""
+    import torch
+    images = list(images)
+    dev = None
+    for i, im in enumerate(images):
+        if isinstance(im, torch.Tensor):
+            if not im.is_cuda:
+                raise ValueError("png.encode: image %d is a CPU tensor; pass a numpy array or a CUDA tensor" % i)
+            dev = dev or im.device
+            if im.device != dev:
+                raise ValueError("png.encode: image %d is on %s, image 0 on %s" % (i, im.device, dev))
+            dtype, shape = im.dtype, tuple(im.shape)
+            ok = dtype == torch.uint8
+        elif isinstance(im, np.ndarray):
+            dtype, shape = im.dtype, im.shape
+            ok = dtype == np.uint8
+        else:
+            raise ValueError("png.encode: image %d is a %s, not an array or a CUDA tensor" % (i, type(im).__name__))
+        if not ok or len(shape) != 3 or shape[2] != 3 or shape[0] < 1 or shape[1] < 1:
+            raise ValueError("png.encode: image %d is %s %s; only non-empty uint8 (H, W, 3) images are encoded"
+                             % (i, dtype, shape))
+    if not images:
+        return []
+    dev = dev or torch.device("cuda", torch.cuda.current_device())
+    host_at = {}
+    nbytes = 0
+    for i, im in enumerate(images):
+        if isinstance(im, np.ndarray):
+            host_at[i] = nbytes
+            nbytes += im.size
+    keep, sources, pitches = [], [], []
+    if host_at:
+        host = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
+        hv = host.numpy()
+        for i, o in host_at.items():
+            hv[o:o + images[i].size] = images[i].reshape(-1)
+        up = host.to(dev, non_blocking=True)
+        keep.append(up)
+    for i, im in enumerate(images):
+        if i in host_at:
+            sources.append(up.data_ptr() + host_at[i])
+            pitches.append(3 * im.shape[1])
+            continue
+        if not (im.stride(2) == 1 and im.stride(1) == 3 and im.stride(0) >= 3 * im.shape[1]):
+            im = im.contiguous()
+            keep.append(im)
+        sources.append(im.data_ptr())
+        pitches.append(im.stride(0))
+    return encode_at(sources, [tuple(im.shape[:2]) for im in images], pitches, dev)
+
+
+def encode_at(sources, shapes, pitches, device):
+    """The PNG files of images already on ``device`` at addresses ``sources`` with ``(h, w)`` ``shapes`` and row
+    ``pitches``: one launch, one read of the sizes, one copy of the files."""
+    import torch
+    table, counts, ws, out_bytes = encode_layout(sources, shapes, pitches)
+    out = torch.empty(out_bytes, dtype=torch.uint8, device=device)
+    sizes = torch.empty(len(shapes), dtype=torch.int64, device=device)
+    encode_launch(table, counts, ws, out, sizes)
+    return download_files(out, sizes)

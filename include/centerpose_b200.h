@@ -238,6 +238,46 @@ typedef struct cpb200_png_image {
 int cpb200_png_decode_batch(const unsigned char *src, const cpb200_png_image *table, int B, void *workspace,
                             size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
 
+/* PNG encoding (csrc/png_encode.cu, centerpose_b200/png.py lays out the table).  Workspace records: scanline bytes per
+ * tile, and the bytes of one tile, one deflate block and one image's state. */
+#define CPB200_PNG_ENCODE_TILE 4096
+#define CPB200_PNG_ENCODE_TILE_REC 32
+#define CPB200_PNG_ENCODE_BLOCK_REC 1088
+#define CPB200_PNG_ENCODE_STATE_REC 64
+
+/* One image of cpb200_png_encode_batch (96 bytes, lives in caller-owned DEVICE memory).  Offsets are bytes into
+ * `workspace`; slots are indices into the launch's tiles, deflate blocks and IDAT chunks, ascending with the image. */
+typedef struct cpb200_png_encode_image {
+  const unsigned char *src;  /* DEVICE address of pixel (0, 0): BGR uint8, 3 bytes per pixel, read only */
+  int64_t pitch;             /* bytes from one row to the next, >= 3 * w */
+  int64_t filt_offset;       /* the filtered scanlines: N = h * (1 + 3 * w) bytes, N < 2^31 */
+  int64_t sym_offset;        /* N uint16 symbols, 2-byte aligned */
+  int64_t tile_offset;       /* ceil(N / CPB200_PNG_ENCODE_TILE) tile records, 8-byte aligned */
+  int64_t block_offset;      /* N / 16383 + 1 block records, 8-byte aligned */
+  int64_t state_offset;      /* one state record, 8-byte aligned */
+  int64_t z_offset;          /* the zlib stream, 16-byte aligned */
+  int64_t z_bytes;           /* a multiple of 16, >= zlib's deflateBound(N) + 8 */
+  int32_t h, w;              /* >= 1 */
+  int32_t tile0;             /* the image's first tile slot; it has ceil(N / CPB200_PNG_ENCODE_TILE) */
+  int32_t block0;            /* its first deflate-block slot; it has N / 16383 + 1 */
+  int32_t chunk0;            /* its first IDAT-chunk slot; it has ceil(z_bytes / 8192) */
+  int32_t pad;
+} cpb200_png_encode_image;
+
+/* cv2.imencode('.png', img) of BGR uint8 images, byte for byte (OpenCV 4.13 through libpng: Sub filter, None on
+ * one-pixel rows, BGR -> RGB, zlib level 1 with strategy Z_RLE and memLevel 8, libpng's smaller window and header for
+ * at most 16 KiB of scanlines, IDAT chunks of 8192 bytes, no other chunks).  B images in one launch, none of them
+ * allocated or waited for: `table` is a DEVICE array of B cpb200_png_encode_image that the caller has checked (the
+ * kernels trust it; see centerpose_b200/png.py), `tiles` / `blocks` / `chunks` the slot counts of the launch (the
+ * last image's first slot plus its count).  The files are written back to back in input order from out[0] and
+ * sizes[b] (DEVICE int64 array) receives file b's size; `out` must hold the sum of the images' bounds
+ * (centerpose_b200/png.py encode_bound) and nothing past the files' total is written.  Per 4096-byte tile: the
+ * filter and the runs of equal bytes (deflate_rle's parse is closed form per run), per deflate block: zlib's trees
+ * and block choice, per image: the bit offsets, then per block the codes and per IDAT chunk the CRC-32.
+ * 1 <= B <= 65535. */
+int cpb200_png_encode_batch(const cpb200_png_encode_image *table, int B, int tiles, int blocks, int chunks,
+                            void *workspace, unsigned char *out, int64_t *sizes, void *stream);
+
 /* One image of cpb200_webp_decode_batch (56 bytes, lives in caller-owned DEVICE memory).  Offsets are bytes. */
 typedef struct cpb200_webp_image {
   int64_t src_offset;        /* in `src`: the file from its VP8 payload (the frame tag) to its end, followed by >= 32
