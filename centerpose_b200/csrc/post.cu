@@ -86,7 +86,8 @@ __global__ void __launch_bounds__(NMS_T) soft_nms_kernel(float *boxes, int N0, f
       float v = s_val[0]; int ix = s_idx[0];
       for (int w = 1; w < NMS_T / 32; ++w)
         if (s_val[w] > v || (s_val[w] == v && s_idx[w] < ix)) { v = s_val[w]; ix = s_idx[w]; }
-      // a NaN-free input always yields ix in [i,N); the reference starts from maxpos = i
+      // a NaN-free input always yields ix in [i,N); the reference starts from maxpos = i.  Scores are NaN-free by
+      // premise (centerpose_b200/soft_nms.py): a NaN never wins here, not even at i
       s_maxpos = (ix == 0x7fffffff) ? i : ix;
     }
     __syncthreads();
@@ -242,8 +243,12 @@ __global__ void __launch_bounds__(256) pre_process_kernel(const PreArgs a) {
   const int total = a.OH * a.OW;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int x = i % a.OW, y = i / a.OW;
-    const long long adelta = llrint(m0 * (double)x * 1024.0), bdelta = llrint(m3 * (double)x * 1024.0);
-    const long long X0 = llrint((m1 * (double)y + m2) * 1024.0) + 16, Y0 = llrint((m4 * (double)y + m5) * 1024.0) + 16;
+    // cv2 rounds m1*y, then the sum: an FMA would round once and, where the sum lands on a half-unit of 1/1024, can
+    // make llrint pick the other integer (tests/post_cases.py tie_x_row, tie_y_row)
+    const long long adelta = llrint(__dmul_rn(__dmul_rn(m0, (double)x), 1024.0));
+    const long long bdelta = llrint(__dmul_rn(__dmul_rn(m3, (double)x), 1024.0));
+    const long long X0 = llrint(__dmul_rn(__dadd_rn(__dmul_rn(m1, (double)y), m2), 1024.0)) + 16;
+    const long long Y0 = llrint(__dmul_rn(__dadd_rn(__dmul_rn(m4, (double)y), m5), 1024.0)) + 16;
     const long long X = (X0 + adelta) >> 5, Y = (Y0 + bdelta) >> 5;
     long long sxl = X >> 5, syl = Y >> 5;
     sxl = sxl < -32768 ? -32768 : (sxl > 32767 ? 32767 : sxl);       // saturate_cast<short>

@@ -6,7 +6,9 @@ Faithful to the reference's quirks because callers consume the mutated array, no
 ``keep`` list (``lib/detectors/multi_pose.py:76-78``): columns 0..38 travel with a row when it is
 moved, the 17 keypoint-score columns 39..55 never move (``nms.pyx:214-217``); a row whose score
 falls below ``threshold`` gets columns 0..4 overwritten by the last live row and columns 5..38
-swapped with it (``:257-268``); all arithmetic is C ``float``.
+swapped with it (``:257-268``); all arithmetic is C ``float``.  Scores must be NaN-free (the detector's are sigmoids
+of finite logits): ``np.argmax`` takes the first NaN, the reference's strict ``<`` scan never takes one unless it
+starts on it, and the device kernel never takes one.
 N <= 100 x scales, O(N^2) on the host exactly as in the reference.  The device version is ``cpb200_soft_nms_39``
 (``csrc/post.cu``; ``detector.merge_outputs_device`` / ``run_batch_fused(nms=True)`` use it, ``run_images`` its batched
 form ``cpb200_soft_nms_39_batch``); this port serves

@@ -235,6 +235,31 @@ def gen_soft_nms(ns=None):
     print("soft_nms_39: port == compiled reference on 24 cases (keep lists equal, scores within 1 ulp)")
 
 
+def gen_soft_nms_cases(ns=None):
+    """The reference's own Cython ``soft_nms_39`` (oracle/build_ref.py) on the constructed soft-NMS cases of
+    tests/post_cases.py; the inputs are rebuilt from the cases, so only their sha256 is stored."""
+    from oracle.build_ref import load
+    from tests import post_cases as pc
+    from tests.test_post_cases_cpu import assert_matches_cython
+    nms = load()
+    assert nms is not None, "reference tree absent"
+    store = {}
+    for case in pc.NMS_CASES:
+        rows = case.build()
+        out = rows.copy()
+        keep = len(nms.soft_nms_39(out, **case.params()))
+        store[f"out_{case.label}"] = out
+        store[f"keep_{case.label}"] = np.array(keep)
+        store[f"sha_{case.label}"] = np.array(pc.digest(rows))
+    for case in pc.NMS_CASES:                  # pin: the port agrees with what was just stored
+        port = case.build()
+        k = pc.soft_nms_literal(port, **case.params())
+        assert_matches_cython(port, k, store, case)
+    np.savez_compressed(os.path.join(GOLD, "soft_nms_cases.npz"), **store)
+    print(f"soft_nms_39: {len(pc.NMS_CASES)} constructed cases, port == compiled reference (keeps and moves exact, "
+          "scores within 1 ulp)")
+
+
 def gen_post(ns):
     rng = np.random.RandomState(3)
     dets = rng.uniform(0, 128, size=(1, 100, 56)).astype(np.float32)
@@ -278,6 +303,7 @@ def main():
     gen_hrnet(ns)
     gen_mbv3(ns)
     gen_soft_nms(ns)
+    gen_soft_nms_cases(ns)
     print("golden fixtures written to", GOLD)
 
 
