@@ -80,6 +80,14 @@ def lib() -> ctypes.CDLL:
     L.cpb200_soft_nms_39_batch.restype = ctypes.c_int
     L.cpb200_soft_nms_39_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
                                            ctypes.c_float, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+    L.cpb200_coco_kp_eval_workspace_bytes.restype = ctypes.c_size_t
+    L.cpb200_coco_kp_eval_workspace_bytes.argtypes = [ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int64]
+    L.cpb200_coco_kp_oks.restype = ctypes.c_int
+    L.cpb200_coco_kp_oks.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+                                     ctypes.c_int, ctypes.c_int, ctypes.c_int64] + [ctypes.c_void_p] * 4
+    L.cpb200_coco_kp_eval.restype = ctypes.c_int
+    L.cpb200_coco_kp_eval.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
+                                      ctypes.c_int, ctypes.c_int, ctypes.c_int64] + [ctypes.c_void_p] * 6
     _lib = L
     return L
 

@@ -23,7 +23,9 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-Xcompiler", "-fPIC", "-std=c++17", "-O3", "-lineinfo"] + ARCH
 # NVVM's -O3 pipeline for sm_90 takes tens of minutes on net_simt.cu's stem_kernel (seconds for other targets); -O1
 # compiles the file in about 10 s.  The bandwidth-bound max-pool and depthwise-deconv kernels are in net_eltwise.cu, at -O3.
-FILE_FLAGS = {"net_simt.cu": ["-Xcicc", "-O1"]}
+FILE_FLAGS = {"net_simt.cu": ["-Xcicc", "-O1"],
+              # the COCO evaluation reproduces numpy's float64 results bit for bit: no product may become an FMA
+              "coco_eval.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

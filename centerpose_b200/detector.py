@@ -614,6 +614,18 @@ class MultiPoseDetector(BaseDetector):
         views = [pixels[offsets[n]:offsets[n] + int(np.prod(shape[n]))].view(shape[n]) for n in range(len(images))]
         return views, [offsets[n] for n in range(len(images))], pixels
 
+    def run_eval(self, images, image_ids, gt, max_batch=32):
+        """Additive: tools/evaluate.py's loop and ``dataset.run_eval`` (coco_hp.py:97-107) in one call.  Runs
+        ``run_images(images, max_batch)``, evaluates the rows of ``images[i]`` as image ``image_ids[i]`` against ``gt``
+        (a ``coco_eval.KeypointEval``, or what it takes: a ``person_keypoints_*.json`` path, its dict, or an object
+        with a ``.dataset`` dict) on the device, prints the summary and returns ``stats[0]`` (AP at OKS .50:.95)."""
+        from .coco_eval import KeypointEval
+        ev = gt if isinstance(gt, KeypointEval) else KeypointEval(gt)
+        if len(image_ids) != len(images):
+            raise ValueError("run_eval: %d image ids for %d images" % (len(image_ids), len(images)))
+        ev.evaluate((list(image_ids), self.run_images(images, max_batch=max_batch)))
+        return ev.summarize()[0]
+
     @torch.no_grad()
     def run_images(self, images, max_batch=32, return_images=False, return_heatmaps=False, encode_png=False):
         """Additive: ``run()`` for many images at once, with the reference's test-time settings (``FLIP_TEST``,

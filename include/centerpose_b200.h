@@ -417,6 +417,66 @@ typedef struct cpb200_heatmap_image {
 int cpb200_heatmap_views_batch(const cpb200_heatmap_image *table, int B, const float *colors, const float *mean,
                                const float *stdv, int white, unsigned char *out, unsigned char *workspace, void *stream);
 
+/* COCO keypoint evaluation (csrc/coco_eval.cu, centerpose_b200/coco_eval.py builds the tables): pycocotools'
+ * COCOeval(gt, gt.loadRes(results), "keypoints") with the default Params (maxDets 20; area ranges all, medium,
+ * large) on detection rows as tools/evaluate.py formats them, every value in float64 as numpy computes it.
+ *
+ * One image of the evaluated image ids (32 bytes, DEVICE memory), in sorted image id order. */
+typedef struct cpb200_coco_kp_image {
+  int64_t det_begin;         /* its first row in `rows`; its rows are consecutive, in results order */
+  int32_t det_count;
+  int32_t keep_begin;        /* its min(det_count, 20) kept detections start here (packed in image order) */
+  int32_t gt_begin, gt_count;           /* its ground truths in `gts`, in annotation-file order */
+  int64_t oks_offset;        /* in the OKS array: its min(det_count, 20) x gt_count matrix, row-major */
+} cpb200_coco_kp_image;
+
+#define CPB200_COCO_KP_JOINTS 17
+#define CPB200_COCO_KP_MAX_DETS 20
+#define CPB200_COCO_KP_T 10        /* IoU (OKS) thresholds */
+#define CPB200_COCO_KP_R 101       /* recall thresholds */
+#define CPB200_COCO_KP_A 3         /* area ranges */
+
+/* One ground-truth annotation (336 bytes, DEVICE memory). */
+typedef struct cpb200_coco_kp_gt {
+  double x[CPB200_COCO_KP_JOINTS], y[CPB200_COCO_KP_JOINTS];
+  double area;
+  double bbox[4];            /* x, y, w, h */
+  int64_t id;                /* a matched detection with id == 0 counts as unmatched, as in COCOeval.accumulate */
+  int32_t iscrowd;           /* int(iscrowd): a crowd can be matched more than once */
+  int32_t ignore;            /* iscrowd or num_keypoints == 0 (COCOeval._prepare) */
+  int32_t visible;           /* bit j: v_j > 0 */
+  int32_t pad;
+} cpb200_coco_kp_gt;
+
+/* The numpy-computed constants of Params(iouType="keypoints") (HOST memory, passed by value to the kernels). */
+typedef struct cpb200_coco_kp_params {
+  double iou_thrs[CPB200_COCO_KP_T];    /* np.linspace(.5, .95, 10) */
+  double rec_thrs[CPB200_COCO_KP_R];    /* np.linspace(0, 1, 101) */
+  double vars[CPB200_COCO_KP_JOINTS];   /* (kpt_oks_sigmas * 2) ** 2 */
+  double area_rng[CPB200_COCO_KP_A][2];
+} cpb200_coco_kp_params;
+
+/* Workspace of cpb200_coco_kp_eval / cpb200_coco_kp_oks for `n_images` images, `n_rows` rows, `n_gts` ground
+ * truths, `n_keep` kept detections (the sum of min(det_count, 20)) and `n_oks` OKS entries. */
+size_t cpb200_coco_kp_eval_workspace_bytes(int n_images, int64_t n_rows, int n_gts, int n_keep, int64_t n_oks);
+
+/* The OKS matrices of COCOeval.computeOks alone, into `oks` (DEVICE, n_oks doubles at each image's oks_offset): per
+ * image its detections stable-sorted by -score (scores and keypoints rounded as '{:.2f}' formats them), the first 20
+ * against its ground truths in file order.  `rows` is the DEVICE (n_rows, 56) float32 detection rows.  The tables are
+ * trusted: centerpose_b200/coco_eval.py builds them.  No allocation, no host sync. */
+int cpb200_coco_kp_oks(const cpb200_coco_kp_image *images, int n_images, const float *rows, int64_t n_rows,
+                       const cpb200_coco_kp_gt *gts, int n_gts, int n_keep, int64_t n_oks,
+                       const cpb200_coco_kp_params *params, double *oks, void *workspace, void *stream);
+
+/* evaluate() and accumulate(): writes COCOeval.eval's `precision` and `scores` ([10][101][1][3][1] doubles) and
+ * `recall` ([10][1][3][1]) to DEVICE memory.  Five steps on `stream`: detection prep per image, OKS per
+ * (detection, ground truth), the greedy match per (image, area range, threshold), one stable sort of every kept
+ * detection by -score, and the precision / recall scans per (area range, threshold). */
+int cpb200_coco_kp_eval(const cpb200_coco_kp_image *images, int n_images, const float *rows, int64_t n_rows,
+                        const cpb200_coco_kp_gt *gts, int n_gts, int n_keep, int64_t n_oks,
+                        const cpb200_coco_kp_params *params, double *precision, double *recall, double *scores,
+                        void *workspace, void *stream);
+
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
  * swap-with-last walk; columns 0..38 travel with a row, 39..55 stay).  *keep_count (device int, may be NULL)
