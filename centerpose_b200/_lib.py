@@ -13,6 +13,23 @@ LIBPATH = os.path.join(_HERE, "lib", "libcenterpose_b200.so")
 
 _lib = None
 
+
+class Targets(ctypes.Structure):
+    """``cpb200_multi_pose_targets``: the device addresses of the eleven target arrays."""
+    _fields_ = [(n, ctypes.c_void_p) for n in ("hm", "hm_hp", "wh", "reg", "ind", "reg_mask", "hps", "hps_mask",
+                                               "hp_offset", "hp_ind", "hp_mask")]
+
+
+class Heads(ctypes.Structure):
+    """``cpb200_multi_pose_heads``: the device addresses of the six head maps."""
+    _fields_ = [(n, ctypes.c_void_p) for n in ("hm", "wh", "hps", "reg", "hm_hp", "hp_offset")]
+
+
+class LossCfg(ctypes.Structure):
+    """``cpb200_multi_pose_loss_cfg``."""
+    _fields_ = [(n, ctypes.c_float) for n in ("hm_weight", "wh_weight", "off_weight", "hp_weight", "hm_hp_weight")] + \
+               [(n, ctypes.c_int32) for n in ("hm_hp", "reg_offset", "reg_hp_offset")]
+
 c_float_p = ctypes.c_void_p   # raw device addresses are passed as integers
 
 
@@ -88,6 +105,20 @@ def lib() -> ctypes.CDLL:
     L.cpb200_coco_kp_eval.restype = ctypes.c_int
     L.cpb200_coco_kp_eval.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
                                       ctypes.c_int, ctypes.c_int, ctypes.c_int64] + [ctypes.c_void_p] * 6
+    L.cpb200_pre_process_batch_f32.restype = ctypes.c_int
+    L.cpb200_pre_process_batch_f32.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                               ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_float),
+                                               ctypes.POINTER(ctypes.c_float), ctypes.c_void_p]
+    L.cpb200_multi_pose_targets_batch.restype = ctypes.c_int
+    L.cpb200_multi_pose_targets_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                                  Targets, ctypes.c_void_p]
+    L.cpb200_multi_pose_loss_workspace_bytes.restype = ctypes.c_size_t
+    L.cpb200_multi_pose_loss_workspace_bytes.argtypes = [ctypes.c_int]
+    L.cpb200_multi_pose_loss_batch.restype = ctypes.c_int
+    L.cpb200_multi_pose_loss_batch.argtypes = [Heads, Targets, ctypes.c_int, ctypes.c_int, ctypes.POINTER(LossCfg),
+                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    L.cpb200_gaussian_radius.restype = ctypes.c_int
+    L.cpb200_gaussian_radius.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
     _lib = L
     return L
 

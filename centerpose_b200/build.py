@@ -25,7 +25,9 @@ NVCC_FLAGS = ["-Xcompiler", "-fPIC", "-std=c++17", "-O3", "-lineinfo"] + ARCH
 # compiles the file in about 10 s.  The bandwidth-bound max-pool and depthwise-deconv kernels are in net_eltwise.cu, at -O3.
 FILE_FLAGS = {"net_simt.cu": ["-Xcicc", "-O1"],
               # the COCO evaluation reproduces numpy's float64 results bit for bit: no product may become an FMA
-              "coco_eval.cu": ["-fmad=false"]}
+              "coco_eval.cu": ["-fmad=false"],
+              # the validation targets reproduce numpy's float64 box and radius arithmetic bit for bit, likewise
+              "targets.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

@@ -192,6 +192,9 @@ class KeypointEval:
         for i in self.img_ids:
             self.gt_range[i] = (len(ordered), len(per_image[i]))
             ordered += per_image[i]
+        # coco.getImgIds(imgIds, catIds): the images with an annotation of the category (crowds count), what the
+        # reference's COCOHP dataset iterates
+        self.cat_img_ids = [i for i in self.img_ids if per_image[i]]
         self.device = torch.device("cuda") if device is None else torch.device(device)
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())

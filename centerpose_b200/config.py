@@ -52,8 +52,10 @@ _DEFAULT = {
     "MODEL": {"NAME": "dla_34", "HEADS_NAME": "keypoint", "HEADS_NUM": [1, 2, 34, 2, 17, 2],
               "HEAD_CONV": 256, "INTERMEDIATE_CHANNEL": 64, "DOWN_RATIO": 4, "NUM_CLASSES": 1,
               "INPUT_H": 512, "INPUT_W": 512, "INPUT_RES": 512, "OUTPUT_RES": 128, "PAD": 31,
-              "NUM_KEYPOINTS": 17, "INIT_WEIGHTS": False, "PRETRAINED": ""},
-    "LOSS": {"HM_HP": True, "MSE_LOSS": False, "REG_OFFSET": True, "REG_HP_OFFSET": True, "REG_BBOX": True},
+              "NUM_KEYPOINTS": 17, "INIT_WEIGHTS": False, "PRETRAINED": "", "NUM_STACKS": 1},
+    "LOSS": {"HM_HP": True, "MSE_LOSS": False, "REG_OFFSET": True, "REG_HP_OFFSET": True, "REG_BBOX": True,
+             "HM_WEIGHT": 1., "WH_WEIGHT": 0.1, "OFF_WEIGHT": 1., "HP_WEIGHT": 1., "HM_HP_WEIGHT": 1., "REG_LOSS": "l1",
+             "DENSE_HP": False},
     "DATASET": {"MEAN": [0.408, 0.447, 0.470], "STD": [0.289, 0.274, 0.278]},
     "TEST": {"MODEL_PATH": "", "TASK": "multi_pose", "FLIP_TEST": False, "TEST_SCALES": [1],
              "TOPK": 100, "NMS": False, "FIX_RES": True, "VIS_THRESH": 0.3},

@@ -203,7 +203,8 @@ extern "C" int cpb200_soft_nms_39_batch(float *boxes, int B, int N, float sigma,
 // remapBilinear): the 2x3 matrix is inverted in double exactly as cv2 does, source coordinates are 10-bit fixed
 // point (AB_SCALE = 1024, round_delta = 16) reduced to 5 fractional bits, the four bilinear weights are the
 // integers (32-fx)(32-fy)*32 ... that sum to 2^15, result = (sum + 2^14) >> 15; then ((u/255 - mean)/std) is
-// evaluated in double and rounded to float like numpy does for `(inp / 255. - mean) / std`.astype(float32).
+// evaluated in double and rounded to float like numpy does for `(inp / 255. - mean) / std`.astype(float32).  With
+// f32 set it is the training dataset's `(inp.astype(float32) / 255. - mean32) / std32`, every step rounded to float.
 namespace {
 
 static_assert(sizeof(cpb200_pre_image) == 64, "cpb200_pre_image layout is part of the C ABI");
@@ -213,7 +214,7 @@ struct PreArgs {
   const cpb200_pre_image *table;   // B entries on the device, or NULL: `one` describes the only image
   cpb200_pre_image one;
   float *out;                      // (B or 2B, 3, OH, OW) fp32
-  int OH, OW, flip;
+  int OH, OW, flip, f32;
   float mean[3], stdv[3];
 };
 
@@ -263,7 +264,8 @@ __global__ void __launch_bounds__(256) pre_process_kernel(const PreArgs a) {
       const int v10 = (y1 && x0) ? p00[(size_t)w * 3 + c] : 0, v11 = (y1 && x1) ? p00[(size_t)w * 3 + 3 + c] : 0;
       int u = (v00 * w0 + v01 * w1 + v10 * w2 + v11 * w3 + (1 << 14)) >> 15;
       u = u < 0 ? 0 : (u > 255 ? 255 : u);
-      const float f = (float)(((double)u / 255.0 - (double)a.mean[c]) / (double)a.stdv[c]);
+      const float f = a.f32 ? __fdiv_rn(__fsub_rn(__fdiv_rn((float)u, 255.f), a.mean[c]), a.stdv[c])
+                            : (float)(((double)u / 255.0 - (double)a.mean[c]) / (double)a.stdv[c]);
       out[((size_t)c * a.OH + y) * a.OW + x] = f;
       if (a.flip) out[((size_t)(3 + c) * a.OH + y) * a.OW + (a.OW - 1 - x)] = f;
     }
@@ -298,6 +300,17 @@ extern "C" int cpb200_pre_process_batch(const unsigned char *imgs, const cpb200_
   if ((long long)out_h * out_w > (1LL << 30)) return cpb::fail(CPB200_ERR_ARG, "pre_process_batch: output too large");
   PreArgs a = {};
   a.imgs = imgs; a.table = table; a.out = out; a.OH = out_h; a.OW = out_w; a.flip = flip ? 1 : 0;
+  return pre_process_launch(a, B, mean, stdv, stream);
+}
+
+extern "C" int cpb200_pre_process_batch_f32(const unsigned char *imgs, const cpb200_pre_image *table, int B, float *out,
+                                            int out_h, int out_w, const float *mean, const float *stdv, void *stream) {
+  if (!imgs || !table || !out || !mean || !stdv || B <= 0 || out_h <= 0 || out_w <= 0)
+    return cpb::fail(CPB200_ERR_ARG, "pre_process_batch_f32: bad arguments");
+  if (B > 65535) return cpb::fail(CPB200_ERR_ARG, "pre_process_batch_f32: B = %d images exceed one launch (max 65535)", B);
+  if ((long long)out_h * out_w > (1LL << 30)) return cpb::fail(CPB200_ERR_ARG, "pre_process_batch_f32: output too large");
+  PreArgs a = {};
+  a.imgs = imgs; a.table = table; a.out = out; a.OH = out_h; a.OW = out_w; a.f32 = 1;
   return pre_process_launch(a, B, mean, stdv, stream);
 }
 

@@ -1,0 +1,329 @@
+// Multi-pose training targets and MultiPoseLoss for the reference's validation pass (cpb200_multi_pose_targets_batch,
+// cpb200_multi_pose_loss_batch, cpb200_gaussian_radius).
+//
+// The targets are what MultiPoseDataset.__getitem__ returns for the val split (no augmentation: rot 0, no flip), bit
+// for bit.  The file is built with -fmad=false so that no product is contracted into an FMA; the one FMA the
+// reference's np.dot performs is written out with __fma_rn.
+//
+//   targets_kernel  one CTA per (image, object slot): the slot's annotation (the k-th non-crowd one in file order),
+//                   its box, radius, centre and joints into the sparse targets, then the CTA stamps the object's
+//                   Gaussians into hm and hm_hp with atomic maxima (every draw is a max, so the order is free)
+//   focal_kernel    one CTA per (image, heat-map channel): _neg_loss's positive / negative sums and positive count
+//   loss_kernel     one warp per image: the regression losses and the weighted total, from the focal partials
+#include "common.cuh"
+
+namespace {
+
+static_assert(sizeof(cpb200_val_image) == 64, "cpb200_val_image layout is part of the C ABI");
+static_assert(sizeof(cpb200_coco_kp_gt) == 336, "cpb200_coco_kp_gt layout is part of the C ABI");
+
+constexpr int J = CPB200_COCO_KP_JOINTS;
+constexpr int M = CPB200_MAX_OBJS;
+constexpr int kStampThreads = 256;
+
+// gaussian_radius((h, w), min_overlap=0.7) of lib/utils/image.py in double, left to right as Python evaluates it
+// (the file has no FMA contraction): (1 - 0.7) is 0.30000000000000004, 4 * 0.7 is 2.8, -2 * 0.7 is -1.4
+__device__ __host__ inline double gaussian_radius(int height, int width) {
+  const double mo = 0.7, omo = 1.0 - 0.7, hw = (double)(height + width), wh = (double)width * (double)height;
+  const double c1 = wh * omo / (1.0 + mo);
+  const double r1 = (hw + sqrt(hw * hw - 4.0 * c1)) / 2.0;
+  const double b2 = 2.0 * hw, c2 = omo * (double)width * (double)height;
+  const double r2 = (b2 + sqrt(b2 * b2 - 16.0 * c2)) / 2.0;
+  const double a3 = 4.0 * mo, b3 = -2.0 * mo * hw, c3 = (mo - 1.0) * (double)width * (double)height;
+  const double r3 = (b3 + sqrt(b3 * b3 - 4.0 * a3 * c3)) / 2.0;
+  return fmin(r1, fmin(r2, r3));
+}
+
+__device__ inline int radius_of(int height, int width) {
+  const double r = gaussian_radius(height, width);
+  return r > 0 ? (int)r : 0;                      // max(0, int(r)): int() truncates toward zero
+}
+
+// affine_transform(pt, t): np.dot(t, float32([x, y, 1])) in float64, rounded to float32 where it is stored
+__device__ inline float affine_x(const double *t, float x, float y) {
+  return (float)__dadd_rn(__fma_rn(t[0], (double)x, __dmul_rn(t[1], (double)y)), t[2]);
+}
+
+// float32(gaussian2D((2r+1, 2r+1), sigma=(2r+1)/6)[r + dy, r + dx]); the reference's eps * max cut never fires
+__device__ inline float gauss(int dx, int dy, double sigma) {
+  const double e = -(double)(dx * dx + dy * dy) / (2.0 * sigma * sigma);
+  return (float)exp(e);
+}
+
+struct Stamp {
+  int x, y, r;
+  int map;                           // -1: hm, else the hm_hp channel
+};
+
+struct TargetArgs {
+  const cpb200_val_image *images;
+  const cpb200_coco_kp_gt *gts;
+  cpb200_multi_pose_targets out;
+  int R;
+};
+
+__global__ void __launch_bounds__(kStampThreads) targets_kernel(const TargetArgs a) {
+  const int k = blockIdx.x, b = blockIdx.y, R = a.R;
+  const cpb200_val_image im = a.images[b];
+  __shared__ int s_ann, s_n;
+  __shared__ Stamp s_st[1 + J];
+  // the k-th annotation with iscrowd != 1, in file order (warp 0 counts with ballots)
+  if (threadIdx.x < 32) {
+    int seen = 0, found = -1;
+    for (int base = 0; base < im.gt_count && found < 0; base += 32) {
+      const int i = base + (int)threadIdx.x;
+      const bool keep = i < im.gt_count && a.gts[im.gt_begin + i].iscrowd != 1;
+      const unsigned m = __ballot_sync(0xffffffffu, keep);
+      const int n = __popc(m);
+      if (seen + n > k) {
+        unsigned mm = m;
+        for (int q = 0; q < k - seen; ++q) mm &= mm - 1;     // drop the set bits below the one wanted
+        found = base + __ffs(mm) - 1;
+      }
+      seen += n;
+    }
+    if (threadIdx.x == 0) { s_ann = found; s_n = 0; }
+  }
+  __syncthreads();
+  if (s_ann < 0) return;
+  if (threadIdx.x == 0) {
+    const cpb200_coco_kp_gt &g = a.gts[im.gt_begin + s_ann];
+    const double *t = im.trans_output;
+    const float hi = (float)(R - 1);
+    // float32([x, y, x + w, y + h]), corners through trans_output, clipped to [0, R - 1]
+    float bb[4] = {(float)g.bbox[0], (float)g.bbox[1], (float)(g.bbox[0] + g.bbox[2]), (float)(g.bbox[1] + g.bbox[3])};
+    for (int c = 0; c < 4; c += 2) {
+      const float x = bb[c], y = bb[c + 1];
+      bb[c] = affine_x(t, x, y);
+      bb[c + 1] = affine_x(t + 3, x, y);
+    }
+    for (int c = 0; c < 4; ++c) bb[c] = fminf(fmaxf(bb[c], 0.f), hi);
+    const float h = __fsub_rn(bb[3], bb[1]), w = __fsub_rn(bb[2], bb[0]);
+    if (h > 0 && w > 0) {
+      const int r = radius_of((int)ceilf(h), (int)ceilf(w));
+      const float cx = __fdiv_rn(__fadd_rn(bb[0], bb[2]), 2.f), cy = __fdiv_rn(__fadd_rn(bb[1], bb[3]), 2.f);
+      const int ix = (int)cx, iy = (int)cy;
+      const size_t o = (size_t)b * M + k;
+      a.out.wh[2 * o] = w;
+      a.out.wh[2 * o + 1] = h;
+      a.out.ind[o] = (int64_t)iy * R + ix;
+      a.out.reg[2 * o] = __fsub_rn(cx, (float)ix);
+      a.out.reg[2 * o + 1] = __fsub_rn(cy, (float)iy);
+      // num_kpts == 0: reg_mask 0, and hm[ct] = 0.9999, which this object's own stamp (1.0 at ct) always overwrites
+      a.out.reg_mask[o] = g.visible != 0;
+      int n = 0;
+      s_st[n++] = Stamp{ix, iy, r, -1};
+      for (int j = 0; j < J; ++j) {
+        if (!((g.visible >> j) & 1)) continue;
+        const float x = (float)g.x[j], y = (float)g.y[j];
+        const float px = affine_x(t, x, y), py = affine_x(t + 3, x, y);
+        if (!(px >= 0 && px < (float)R && py >= 0 && py < (float)R)) continue;
+        const int qx = (int)px, qy = (int)py;
+        const size_t p = o * J + j;
+        a.out.hps[2 * p] = __fsub_rn(px, (float)ix);
+        a.out.hps[2 * p + 1] = __fsub_rn(py, (float)iy);
+        a.out.hps_mask[2 * p] = a.out.hps_mask[2 * p + 1] = 1;
+        a.out.hp_offset[2 * p] = __fsub_rn(px, (float)qx);
+        a.out.hp_offset[2 * p + 1] = __fsub_rn(py, (float)qy);
+        a.out.hp_ind[p] = (int64_t)qy * R + qx;
+        a.out.hp_mask[p] = 1;
+        s_st[n++] = Stamp{qx, qy, r, j};
+      }
+      s_n = n;
+    }
+  }
+  __syncthreads();
+  // draw_umich_gaussian: the window [x - min(x, r), x + min(R - x, r + 1)) x [same in y]; values are >= 0, so their
+  // float bit patterns order as ints and atomicMax on them is np.maximum
+  for (int s = 0; s < s_n; ++s) {
+    const Stamp st = s_st[s];
+    const int x0 = st.x - min(st.x, st.r), x1 = st.x + min(R - st.x, st.r + 1);
+    const int y0 = st.y - min(st.y, st.r), y1 = st.y + min(R - st.y, st.r + 1);
+    const int W = x1 - x0, n = W * (y1 - y0);
+    const double sigma = (double)(2 * st.r + 1) / 6.0;
+    float *map = st.map < 0 ? a.out.hm + (size_t)b * R * R : a.out.hm_hp + ((size_t)b * J + st.map) * R * R;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const int x = x0 + i % W, y = y0 + i / W;
+      atomicMax(reinterpret_cast<int *>(map + (size_t)y * R + x), __float_as_int(gauss(x - st.x, y - st.y, sigma)));
+    }
+  }
+}
+
+__global__ void radius_kernel(const int *hw, int n, int *radius) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) radius[i] = radius_of(hw[2 * i], hw[2 * i + 1]);
+}
+
+// ---- MultiPoseLoss ----
+
+// _sigmoid then _neg_loss's two terms for one element, in float32 and in the order torch evaluates them; both terms are
+// taken and multiplied by their indicator, so a non-finite logit poisons both sums as it does in the reference
+struct Focal { double pos, neg, npos; };
+
+__device__ inline void focal_term(float logit, float gt, Focal &f) {
+  float p = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-logit)));
+  p = p != p ? p : fminf(fmaxf(p, 1e-4f), 0.9999f);          // torch.clamp keeps NaN
+  const float pi = gt == 1.f ? 1.f : 0.f, ni = gt < 1.f ? 1.f : 0.f;
+  const float q = __fsub_rn(1.f, p), w = __fsub_rn(1.f, gt), w2 = __fmul_rn(w, w);
+  f.pos += (double)__fmul_rn(__fmul_rn(logf(p), __fmul_rn(q, q)), pi);
+  f.neg += (double)__fmul_rn(__fmul_rn(__fmul_rn(logf(q), __fmul_rn(p, p)), __fmul_rn(w2, w2)), ni);
+  f.npos += (double)pi;
+}
+
+__device__ inline double block_sum(double v, double *red) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  double s = 0;
+  if (threadIdx.x == 0)
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += red[i];
+  return s;
+}
+
+// grid (1 + J, B): channel 0 is hm, 1..J the hm_hp channels; partial[(b * (1 + J) + c) * 3 + {pos, neg, npos}]
+__global__ void __launch_bounds__(256) focal_kernel(const float *hm, const float *hm_hp, const float *t_hm,
+                                                    const float *t_hm_hp, int R, double *partial) {
+  const int c = blockIdx.x, b = blockIdx.y, n = R * R;
+  const float *x = c == 0 ? hm + (size_t)b * n : hm_hp + ((size_t)b * J + c - 1) * n;
+  const float *g = c == 0 ? t_hm + (size_t)b * n : t_hm_hp + ((size_t)b * J + c - 1) * n;
+  Focal f = {0, 0, 0};
+  for (int i = threadIdx.x; i < n; i += blockDim.x) focal_term(x[i], g[i], f);
+  __shared__ double red[8];
+  double *out = partial + ((size_t)b * (1 + J) + c) * 3;
+  const double pos = block_sum(f.pos, red), neg = block_sum(f.neg, red), npos = block_sum(f.npos, red);
+  if (threadIdx.x == 0) { out[0] = pos; out[1] = neg; out[2] = npos; }
+}
+
+__device__ inline float focal_loss(const double *p, int channels) {
+  double pos = 0, neg = 0, npos = 0;
+  for (int c = 0; c < channels; ++c) { pos += p[3 * c]; neg += p[3 * c + 1]; npos += p[3 * c + 2]; }
+  return (float)(npos == 0 ? -neg : -(pos + neg) / npos);
+}
+
+// sum |pred * m - t * m| / (sum(m) + 1e-4) over `n` entries of `dim` values, pred gathered at ind (RegL1Loss,
+// RegWeightedL1Loss); a warp-wide float64 sum, the mask count + 1e-4 in float32 as torch adds it
+template <typename MaskT>
+__device__ inline float l1_loss(const float *map, int R, const int64_t *ind, const MaskT *mask, bool per_value,
+                                const float *t, int n, int dim) {
+  double s = 0, cnt = 0;
+  const size_t plane = (size_t)R * R;
+  for (int i = threadIdx.x & 31; i < n * dim; i += 32) {
+    const int k = i / dim, c = i % dim;
+    const float m = per_value ? (float)mask[i] : (float)mask[k];
+    const float pr = map[c * plane + ind[k]];
+    s += (double)fabsf(__fsub_rn(__fmul_rn(pr, m), __fmul_rn(t[i], m)));
+    cnt += m;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    s += __shfl_xor_sync(0xffffffffu, s, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  return (float)(s / (double)__fadd_rn((float)cnt, 1e-4f));
+}
+
+struct LossArgs {
+  cpb200_multi_pose_heads heads;
+  cpb200_multi_pose_targets t;
+  int B, R;
+  cpb200_multi_pose_loss_cfg cfg;
+  const double *partial;
+  float *stats;
+};
+
+__global__ void loss_kernel(const LossArgs a) {
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= a.B) return;
+  const int R = a.R;
+  const size_t plane = (size_t)R * R;
+  const cpb200_multi_pose_loss_cfg &c = a.cfg;
+  const double *p = a.partial + (size_t)b * (1 + J) * 3;
+  const int64_t *ind = a.t.ind + (size_t)b * M;
+  const unsigned char *reg_mask = a.t.reg_mask + (size_t)b * M;
+  const float hm_loss = focal_loss(p, 1);
+  const float hp_loss = l1_loss(a.heads.hps + (size_t)b * 2 * J * plane, R, ind, a.t.hps_mask + (size_t)b * M * 2 * J,
+                                true, a.t.hps + (size_t)b * M * 2 * J, M, 2 * J);
+  float wh_loss = 0, off_loss = 0, hp_offset_loss = 0, hm_hp_loss = 0;
+  if (c.wh_weight > 0)
+    wh_loss = l1_loss(a.heads.wh + (size_t)b * 2 * plane, R, ind, reg_mask, false, a.t.wh + (size_t)b * M * 2, M, 2);
+  if (c.reg_offset && c.off_weight > 0)
+    off_loss = l1_loss(a.heads.reg + (size_t)b * 2 * plane, R, ind, reg_mask, false, a.t.reg + (size_t)b * M * 2, M, 2);
+  if (c.reg_hp_offset && c.off_weight > 0)
+    hp_offset_loss = l1_loss(a.heads.hp_offset + (size_t)b * 2 * plane, R, a.t.hp_ind + (size_t)b * M * J,
+                             a.t.hp_mask + (size_t)b * M * J, false, a.t.hp_offset + (size_t)b * M * J * 2, M * J, 2);
+  if (c.hm_hp && c.hm_hp_weight > 0) hm_hp_loss = focal_loss(p + 3, J);
+  // loss = HM_WEIGHT * hm + WH_WEIGHT * wh + OFF_WEIGHT * off + HP_WEIGHT * hp + HM_HP_WEIGHT * hm_hp
+  //        + OFF_WEIGHT * hp_offset, in float32, left to right
+  float loss = __fmul_rn(c.hm_weight, hm_loss);
+  loss = __fadd_rn(loss, __fmul_rn(c.wh_weight, wh_loss));
+  loss = __fadd_rn(loss, __fmul_rn(c.off_weight, off_loss));
+  loss = __fadd_rn(loss, __fmul_rn(c.hp_weight, hp_loss));
+  loss = __fadd_rn(loss, __fmul_rn(c.hm_hp_weight, hm_hp_loss));
+  loss = __fadd_rn(loss, __fmul_rn(c.off_weight, hp_offset_loss));
+  if ((threadIdx.x & 31) == 0) {
+    float *o = a.stats + (size_t)b * CPB200_LOSS_STATS;
+    o[0] = loss; o[1] = hm_loss; o[2] = hp_loss; o[3] = hm_hp_loss; o[4] = hp_offset_loss; o[5] = wh_loss;
+    o[6] = off_loss;
+  }
+}
+
+bool targets_complete(const cpb200_multi_pose_targets &t) {
+  return t.hm && t.hm_hp && t.wh && t.reg && t.ind && t.reg_mask && t.hps && t.hps_mask && t.hp_offset && t.hp_ind &&
+         t.hp_mask;
+}
+
+}  // namespace
+
+extern "C" int cpb200_multi_pose_targets_batch(const cpb200_val_image *images, int B, const cpb200_coco_kp_gt *gts,
+                                               int R, cpb200_multi_pose_targets out, void *stream) {
+  if (!images || B < 1 || !gts || R < 1 || !targets_complete(out))
+    return cpb::fail(CPB200_ERR_ARG, "multi_pose_targets_batch: bad arguments");
+  if (B > 65535) return cpb::fail(CPB200_ERR_ARG, "multi_pose_targets_batch: B = %d images exceed one launch", B);
+  if ((long long)R * R * J >= (1LL << 31)) return cpb::fail(CPB200_ERR_ARG, "multi_pose_targets_batch: R = %d too large", R);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t plane = (size_t)R * R, bm = (size_t)B * M;
+  // the reference's np.zeros: every slot and pixel no object writes stays 0
+  CPB_CUDA(cudaMemsetAsync(out.hm, 0, sizeof(float) * B * plane, s));
+  CPB_CUDA(cudaMemsetAsync(out.hm_hp, 0, sizeof(float) * B * J * plane, s));
+  CPB_CUDA(cudaMemsetAsync(out.wh, 0, sizeof(float) * bm * 2, s));
+  CPB_CUDA(cudaMemsetAsync(out.reg, 0, sizeof(float) * bm * 2, s));
+  CPB_CUDA(cudaMemsetAsync(out.ind, 0, sizeof(int64_t) * bm, s));
+  CPB_CUDA(cudaMemsetAsync(out.reg_mask, 0, bm, s));
+  CPB_CUDA(cudaMemsetAsync(out.hps, 0, sizeof(float) * bm * 2 * J, s));
+  CPB_CUDA(cudaMemsetAsync(out.hps_mask, 0, bm * 2 * J, s));
+  CPB_CUDA(cudaMemsetAsync(out.hp_offset, 0, sizeof(float) * bm * J * 2, s));
+  CPB_CUDA(cudaMemsetAsync(out.hp_ind, 0, sizeof(int64_t) * bm * J, s));
+  CPB_CUDA(cudaMemsetAsync(out.hp_mask, 0, sizeof(int64_t) * bm * J, s));
+  TargetArgs a = {images, gts, out, R};
+  targets_kernel<<<dim3(M, (unsigned)B), kStampThreads, 0, s>>>(a);
+  return cpb::check_launch("targets_kernel");
+}
+
+extern "C" size_t cpb200_multi_pose_loss_workspace_bytes(int B) {
+  return sizeof(double) * 3 * (1 + J) * (size_t)(B > 0 ? B : 0);
+}
+
+extern "C" int cpb200_multi_pose_loss_batch(cpb200_multi_pose_heads heads, cpb200_multi_pose_targets targets, int B,
+                                            int R, const cpb200_multi_pose_loss_cfg *cfg, float *stats,
+                                            void *workspace, void *stream) {
+  if (!heads.hm || !heads.wh || !heads.hps || !heads.reg || !heads.hm_hp || !heads.hp_offset ||
+      !targets_complete(targets) || B < 1 || R < 1 || !cfg || !stats || !workspace)
+    return cpb::fail(CPB200_ERR_ARG, "multi_pose_loss_batch: bad arguments");
+  if (B > 65535) return cpb::fail(CPB200_ERR_ARG, "multi_pose_loss_batch: B = %d images exceed one launch", B);
+  if ((long long)R * R * 2 * J >= (1LL << 31)) return cpb::fail(CPB200_ERR_ARG, "multi_pose_loss_batch: R = %d too large", R);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  double *partial = static_cast<double *>(workspace);
+  focal_kernel<<<dim3(1 + J, (unsigned)B), 256, 0, s>>>(heads.hm, heads.hm_hp, targets.hm, targets.hm_hp, R, partial);
+  if (int st = cpb::check_launch("focal_kernel")) return st;
+  LossArgs a = {heads, targets, B, R, *cfg, partial, stats};
+  loss_kernel<<<(unsigned)((B + 3) / 4), 128, 0, s>>>(a);
+  return cpb::check_launch("loss_kernel");
+}
+
+extern "C" int cpb200_gaussian_radius(const int *hw, int n, int *radius, void *stream) {
+  if (!hw || !radius || n < 0) return cpb::fail(CPB200_ERR_ARG, "gaussian_radius: bad arguments");
+  if (n == 0) return CPB200_OK;
+  radius_kernel<<<(unsigned)((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(hw, n, radius);
+  return cpb::check_launch("radius_kernel");
+}

@@ -627,6 +627,85 @@ class MultiPoseDetector(BaseDetector):
         return ev.summarize()[0]
 
     @torch.no_grad()
+    def run_val(self, images, image_ids, gt, max_batch=32):
+        """Additive: tools/train.py's validation pass, ``trainer.val`` (``BaseTrainer.run_epoch('val')`` over the val
+        split's ``MultiPoseDataset``), on the device.  ``images[i]`` (a path or a BGR uint8 array, loaded as
+        ``run_images`` loads them) is image ``image_ids[i]`` of ``gt`` (a ``coco_eval.KeypointEval`` or what it takes).
+        Returns ``(log_dict_val, preds)`` as ``trainer.val`` does:
+
+        * ``log_dict_val``: the seven ``MultiPoseLoss`` stats averaged over the images as ``AverageMeter`` averages
+          batches of one (a float64 sum of the float32 per-image stats, in image order, over the count), and
+          ``'time'``, the elapsed minutes;
+        * ``preds``: ``{image_id: {1: (TOPK, 56) float32 rows}}``, every decoded row in original-image pixels as
+          ``save_result`` leaves them (no threshold, no soft-NMS); ``gt.evaluate(preds)`` is ``dataset.run_eval``.
+
+        Per batch of at most ``max_batch`` images: the dataset's warp to ``INPUT_RES`` with its float32 normalisation
+        (``cpb200_pre_process_batch_f32``), the forward, the targets (``val.targets``), the loss (``val.loss``) and the
+        decode with the back-projection fused; one copy of the stats and rows at the end.  ``KeypointEval.cat_img_ids``
+        lists the images the reference's val split holds.  Raises ``NotImplementedError`` for the settings
+        ``val.check_cfg`` refuses."""
+        import ctypes
+        from . import _lib, val
+        from .coco_eval import KeypointEval
+        t_start = time.time()
+        cfg = self.cfg
+        ev = gt if isinstance(gt, KeypointEval) else KeypointEval(gt)
+        val.check_cfg(cfg, ev)
+        if len(image_ids) != len(images):
+            raise ValueError("run_val: %d image ids for %d images" % (len(image_ids), len(images)))
+        if int(max_batch) < 1:
+            raise ValueError("run_val: max_batch must be >= 1, got %r" % (max_batch,))
+        for i in image_ids:
+            if i not in ev.gt_range:
+                raise ValueError("run_val: image id %r is not in the ground truth" % (i,))
+        n = len(images)
+        if n == 0:
+            log = {k: 0 for k in val.STATS}
+            log["time"] = (time.time() - t_start) / 60.
+            return log, {}
+        loaded, offsets, pixels = self._load_images_device(images)
+        dev = torch.device("cuda")
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        res, R, K = int(cfg.MODEL.INPUT_RES), int(cfg.MODEL.OUTPUT_RES), int(cfg.TEST.TOPK)
+        mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
+        std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
+        stats = torch.empty((n, len(val.STATS)), dtype=torch.float32, device=dev)
+        rows = torch.empty((n, K, 56), dtype=torch.float32, device=dev)
+        for a in range(0, n, int(max_batch)):
+            idx = list(range(a, min(n, a + int(max_batch))))
+            B = len(idx)
+            shapes = [tuple(loaded[i].shape[0:2]) for i in idx]
+            trans, metas = [], []
+            for h, w in shapes:
+                c, s = val.center_scale(h, w)
+                trans.append(get_affine_transform(c, s, 0, [res, res]))
+                metas.append({"c": c, "s": s, "out_height": R, "out_width": R})
+            host, at = pack_group([loaded[i] for i in idx], shapes, trans, affine_for_meta(metas).numpy(), idx,
+                                  alloc=lambda nb: torch.empty(nb, dtype=torch.uint8, pin_memory=True),
+                                  src_offsets=[offsets[i] for i in idx])
+            buf = host.to(dev, non_blocking=True)
+            aff = buf[at["o_aff"]:at["o_aff"] + B * 24].view(torch.float32).view(B, 6)
+            inp = torch.empty((B, 3, res, res), dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                st = _lib.lib().cpb200_pre_process_batch_f32(pixels.data_ptr(), buf.data_ptr(), B, inp.data_ptr(),
+                                                             res, res, mean, std, stream)
+            _lib.check(st, "pre_process_batch_f32")
+            outputs = self.model(inp)
+            tg = val.targets(ev, [image_ids[i] for i in idx], shapes, cfg)
+            stats[a:a + B] = val.loss(outputs, tg, cfg)
+            rows[a:a + B] = self._decode_heads(outputs, affine=aff)
+        host_stats, host_rows = stats.cpu().numpy(), rows.cpu().numpy()
+        log = {}
+        for j, k in enumerate(val.STATS):
+            total = 0
+            for v in host_stats[:, j]:
+                total += float(v)
+            log[k] = total / n
+        log["time"] = (time.time() - t_start) / 60.
+        preds = {image_ids[i]: {1: host_rows[i]} for i in range(n)}
+        return log, preds
+
+    @torch.no_grad()
     def run_images(self, images, max_batch=32, return_images=False, return_heatmaps=False, encode_png=False):
         """Additive: ``run()`` for many images at once, with the reference's test-time settings (``FLIP_TEST``,
         ``TEST_SCALES``, ``FIX_RES``, ``NMS``; what tools/evaluate.py runs).  ``images`` is a list of BGR uint8 HWC

@@ -126,6 +126,11 @@ typedef struct cpb200_pre_image {
 int cpb200_pre_process_batch(const unsigned char *imgs, const cpb200_pre_image *table, int B, float *out, int out_h,
                              int out_w, const float *mean, const float *stdv, int flip, void *stream);
 
+/* cpb200_pre_process_batch with the training dataset's normalisation (lib/datasets/multi_pose.py):
+ * `(u.astype(float32) / 255. - mean) / std`, every step in fp32, and no mirrored copy.  out is (B,3,out_h,out_w). */
+int cpb200_pre_process_batch_f32(const unsigned char *imgs, const cpb200_pre_image *table, int B, float *out,
+                                 int out_h, int out_w, const float *mean, const float *stdv, void *stream);
+
 /* One image of cpb200_resize_linear_u8_batch (32 bytes, lives in caller-owned DEVICE memory).  All sizes >= 1. */
 typedef struct cpb200_resize_image {
   int64_t src_offset;        /* byte offset of the source image's first pixel in `src` */
@@ -476,6 +481,67 @@ int cpb200_coco_kp_eval(const cpb200_coco_kp_image *images, int n_images, const 
                         const cpb200_coco_kp_gt *gts, int n_gts, int n_keep, int64_t n_oks,
                         const cpb200_coco_kp_params *params, double *precision, double *recall, double *scores,
                         void *workspace, void *stream);
+
+/* Multi-pose training targets and loss (csrc/targets.cu, centerpose_b200/val.py builds the tables): what the
+ * reference's validation pass (tools/train.py, trainer.val) computes per image.  MultiPoseDataset.__getitem__'s
+ * targets for the val split (lib/datasets/multi_pose.py, no augmentation) bit for bit, and MultiPoseLoss.forward's
+ * seven stats with float64 sums.
+ *
+ * One image (64 bytes, DEVICE memory). */
+typedef struct cpb200_val_image {
+  int32_t gt_begin, gt_count;          /* its annotations in `gts` (cpb200_coco_kp_gt), in annotation-file order */
+  int32_t pad[2];
+  double trans_output[6];              /* get_affine_transform(c, s, 0, [R, R]), row-major */
+} cpb200_val_image;
+
+#define CPB200_MAX_OBJS 32             /* the dataset's max_objs */
+#define CPB200_LOSS_STATS 7            /* loss, hm_loss, hp_loss, hm_hp_loss, hp_offset_loss, wh_loss, off_loss */
+
+/* The dataset's targets for B images, all DEVICE memory, J = 17 joints, M = CPB200_MAX_OBJS. */
+typedef struct cpb200_multi_pose_targets {
+  float *hm;                 /* (B,1,R,R) */
+  float *hm_hp;              /* (B,J,R,R) */
+  float *wh, *reg;           /* (B,M,2) */
+  int64_t *ind;              /* (B,M) */
+  uint8_t *reg_mask;         /* (B,M) */
+  float *hps;                /* (B,M,2J) */
+  uint8_t *hps_mask;         /* (B,M,2J) */
+  float *hp_offset;          /* (B,M*J,2) */
+  int64_t *hp_ind, *hp_mask; /* (B,M*J) */
+} cpb200_multi_pose_targets;
+
+/* Builds every target of B images in one launch: slot k of an image is its k-th annotation with iscrowd != 1 (the
+ * first M), boxes and joints go through trans_output as np.dot does, the Gaussians are draw_umich_gaussian's, and
+ * slots and pixels nothing writes are 0.  `gts` is the ground-truth table of coco_eval.KeypointEval.  The tables
+ * are trusted.  1 <= B <= 65535. */
+int cpb200_multi_pose_targets_batch(const cpb200_val_image *images, int B, const cpb200_coco_kp_gt *gts, int R,
+                                    cpb200_multi_pose_targets out, void *stream);
+
+/* The six head maps of B images as the forward leaves them (DEVICE, (B,C,R,R) fp32; hm and hm_hp are logits). */
+typedef struct cpb200_multi_pose_heads {
+  const float *hm, *wh, *hps, *reg, *hm_hp, *hp_offset;
+} cpb200_multi_pose_heads;
+
+/* The LOSS settings MultiPoseLoss reads (HOST memory). */
+typedef struct cpb200_multi_pose_loss_cfg {
+  float hm_weight, wh_weight, off_weight, hp_weight, hm_hp_weight;
+  int32_t hm_hp, reg_offset, reg_hp_offset;      /* LOSS.HM_HP, REG_OFFSET, REG_HP_OFFSET */
+} cpb200_multi_pose_loss_cfg;
+
+/* Workspace of cpb200_multi_pose_loss_batch for B images. */
+size_t cpb200_multi_pose_loss_workspace_bytes(int B);
+
+/* MultiPoseLoss.forward (lib/trains/multi_pose.py; FocalLoss on the clamped logistic, RegWeightedL1Loss for hps,
+ * RegL1Loss for wh, reg and hp_offset) per image: stats (DEVICE, (B, CPB200_LOSS_STATS) fp32) in the order of
+ * CPB200_LOSS_STATS.  Each image is its own batch of one: the focal loss is normalised by the image's positive
+ * count.  Sums are float64, each stat is rounded to fp32 once; the weighted total is fp32, left to right.
+ * 1 <= B <= 65535. */
+int cpb200_multi_pose_loss_batch(cpb200_multi_pose_heads heads, cpb200_multi_pose_targets targets, int B, int R,
+                                 const cpb200_multi_pose_loss_cfg *cfg, float *stats, void *workspace, void *stream);
+
+/* max(0, int(gaussian_radius((h, w)))) of lib/utils/image.py for n (h, w) int pairs (DEVICE memory), as the targets
+ * kernel computes it.  For tests. */
+int cpb200_gaussian_radius(const int *hw, int n, int *radius, void *stream);
 
 /* soft_nms_39 (lib/external/nms.pyx:172-275) on a DEVICE (N,56) fp32 array, in place, same semantics as the
  * reference's Cython routine (score decay: 0 hard / 1 linear / 2 gaussian; rows below `threshold` are removed by the
