@@ -181,9 +181,8 @@ class Case:
 
     @property
     def exact(self):
-        from tests.replay import INT_EXACT
-        act = dict(self.rec.args).get("act")
-        return not self.randn_only and self.rec.method in INT_EXACT and act not in ("hswish", "hsigmoid")
+        from tests.replay import int_exact
+        return not self.randn_only and int_exact(self.rec)
 
     def label(self):
         return f"{self.rec.label()} B={self.B}: {self.reason}"

@@ -19,7 +19,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-ARCHS = ["dla_34", "res_50", "hrnet", "mobilenetv3", "hardnet"]
+ARCHS = ["dla_34", "res_50", "hrnet", "mobilenetv3", "hardnet", "mobilenetv2", "ghostnet"]
 
 # public PlanBuilder methods that emit no op: symbols, views and finalisation.  Every other public method is recorded.
 NOT_LAYERS = {"input", "output", "external", "keep_result", "channel_slice", "build"}
@@ -168,11 +168,21 @@ def census(arch: str, precision: str, B: int, H: int, W: int) -> Tuple[Record, .
     return tuple(dict.fromkeys(lower_recorded(arch, precision, B, H, W).records))
 
 
+def signatures(arch: str, precision: str) -> List[Record]:
+    """the calls the op-level replay runs: the census at 128x160, plus the 512x512 calls whose signature (spatial size
+    ignored) the 128x160 census does not hold"""
+    base = census(arch, precision, 1, 128, 160)
+    seen = {r.shapeless for r in base}
+    extra = [r for r in census(arch, precision, 1, 512, 512) if r.shapeless not in seen]
+    return list(base) + list(dict.fromkeys(extra))
+
+
 # ---------------------------------------------------------------------------------------- float64 references (NCHW)
 def _act(y, act=None, relu=False):
     from oracle.mobilenet_ref import hsigmoid, hswish
     if act:
-        return {"relu": F.relu, "hswish": hswish, "hsigmoid": hsigmoid}[act](y)
+        return {"relu": F.relu, "hswish": hswish, "hsigmoid": hsigmoid, "relu6": lambda t: t.clamp(0, 6),
+                "clip01": lambda t: t.clamp(0, 1)}[act](y)
     return F.relu(y) if relu else y
 
 
@@ -197,9 +207,12 @@ def _ref_deconv(a):
 
 
 def _ref_up_add(a):
+    # PlanBuilder.up_add: act(conv_transpose2d(x, w, b, stride f, pad p, groups C)) + skip, f = stride or k // 2,
+    # p = pad or f // 2
     C, _, k, _ = a["w"].shape
-    f = k // 2
-    y = F.conv_transpose2d(a["x"], a["w"], None, stride=f, padding=f // 2, groups=C)
+    f = k // 2 if a["stride"] is None else a["stride"]
+    p = f // 2 if a["pad"] is None else a["pad"]
+    y = _act(F.conv_transpose2d(a["x"], a["w"], a["b"], stride=f, padding=p, groups=C), a["act"])
     return y + a["skip"] if a["skip"] is not None else y
 
 

@@ -12,8 +12,8 @@ Data (``_data``, seeded by the record's call):
            value is an integer of magnitude <= INT_NNZ + 5 (<= 256), so fp32, bf16 and fp16 hold each one exactly, even
            after fp16x2's 2^12 weight pre-scale (sums stay below 2^24 * 2^12 in steps of 2^12), the lo plane is 0 and the
            result equals the float64 reference bit for bit.  Needs CPB200_RZ_COMP=0 when the plan is built, so that
-           acc_scale is a pure power of two.  The pools and the resize are exact on it too: means over 4 or 2^k pixels,
-           and align-corners ratios of 1/2.
+           acc_scale is a pure power of two.  The pools and the resize are exact on it where ``int_exact`` says so:
+           means over 4 or 2^k pixels, and align-corners resizes whose weights are dyadic.
            DCN (_dcn_int): dyadic data.  x and the DCN weights / bias as above; the offset rows of om_w are sparse
            multiples of 1/4 with |w| <= 4 (exact in bf16, and under fp16x2's 2^12 pre-scale) and om_b's offsets
            multiples of 1/4, so every sampling position is a multiple of 1/4, exact in fp32 on every route; the mask
@@ -47,6 +47,8 @@ Guards.  Every check stays inside memory the test allocated.
     the output: as NaN, or, where the ReLU epilogue or the fp16 saturation absorbs the NaN, as an error far above the
     bound.
 """
+import math
+
 import torch
 
 from tests.layer_census import REFERENCES
@@ -65,6 +67,22 @@ INT_EXACT = {"conv", "stem", "deconv_k4s2", "maxpool", "up_add", "dwconv", "scal
              "avgpool2", "resize_bilinear", "dcn"}
 MASK_LOGIT = (200.0, 0.0, -200.0)                # DCN "int" mask logits: sigmoid 1, 0.5 and 0 on every route
 COORD_CH = 2                                     # DCN "coord": integer channels the offset rows read
+
+
+def int_exact(rec):
+    """whether ``rec`` has an exact leg on "int" data: a method of INT_EXACT without the h-swish / h-sigmoid activations
+    (their /6 is not dyadic), an average pool over 2^k pixels, and an align-corners resize whose weights are dyadic:
+    (Ho-1) / gcd(H-1, Ho-1) and the same ratio for W powers of two"""
+    if rec.method not in INT_EXACT or dict(rec.args).get("act") in ("hswish", "hsigmoid"):
+        return False
+    if rec.method == "avgpool":
+        _, _, H, W, _, _, _ = rec.arg("x")
+        return (H * W) & (H * W - 1) == 0
+    if rec.method == "resize_bilinear":
+        _, _, H, W, _, _, _ = rec.arg("x")
+        steps = [(o - 1) // math.gcd(i - 1, o - 1) for i, o in ((H, rec.arg("Ho")), (W, rec.arg("Wo")))]
+        return all(s & (s - 1) == 0 for s in steps)
+    return True
 
 
 def _is_sym(d):

@@ -1,19 +1,22 @@
-"""Op-level replay of every layer the five lowerings and the head produce (tests/layer_census.py), in all four
+"""Op-level replay of every layer the seven lowerings and the head produce (tests/layer_census.py), in all four
 precisions, against a float64 torch evaluation of the same operation.
 
-Which calls: the census of each arch at 128x160, replayed at the recorded spatial size, plus the 512x512 calls whose
-signature (spatial size ignored) the 128x160 census does not hold.  B = 2, so the split kernels' "lo plane = batch
-n + B" addressing is exercised.  Each call runs in a program of its own (the call's ops, plus the CONVERT ops an fp32
-island adds around them).
+Which calls: layer_census.signatures, the census of each arch at 128x160, replayed at the recorded spatial size, plus
+the 512x512 calls whose signature (spatial size ignored) the 128x160 census does not hold.  B = 2, so the split
+kernels' "lo plane = batch n + B" addressing is exercised.  Each call runs in a program of its own (the call's ops, plus
+the CONVERT ops an fp32 island adds around them).
 
 Data (seeded by the record's call, so fp32 / bf16x2 / fp16x2 replay the same numbers and share one reference):
 inputs randn (bf16-rounded in bf16); the split precisions replay every conv, dense deconv and DCN a second time with
 post-ReLU |randn| inputs, the statistics plan.RZ_BETA was measured with.  Weights randn / sqrt(fan_in), bias and residual
 randn, DCN offset weights with gain 1.5 (as tests/test_split_gpu.py::test_dcn_split).
 
-Every DCN is replayed twice more, with CPB200_RZ_COMP=0 at plan build (tests/replay.py): on dyadic data, where it must
-equal the float64 reference element by element as the output format stores it, and on "coord" data (exact sampling
-positions, real-valued samples), held to the conv bounds below rather than the DCN's.
+Every call with an integer-exact leg (tests/replay.py: int_exact; all but the h-swish / h-sigmoid layers, average pools
+over sizes that are not 2^k and resizes with non-dyadic weights) is replayed once more on "int" data, with
+CPB200_RZ_COMP=0 at plan build, and must equal the float64 reference element by element as the output format stores
+it: the ReLU6 / clip01 clamps are reached on both sides there (tests/test_layer_census_cpu.py).  The DCNs' "int" data is
+dyadic, and every DCN is replayed on "coord" data too (exact sampling positions, real-valued samples), held to the conv
+bounds below rather than the DCN's.
 
 Tolerances (those of tests/test_net_gpu.py, tests/test_split_gpu.py and tests/test_hardnet_gpu.py):
   fp32   : |err| <= 2e-4 max|ref|;  DCN 5e-4 (test_dcn_op_matches_oracle: the sampling positions come from the fp32
@@ -24,6 +27,7 @@ Tolerances (those of tests/test_net_gpu.py, tests/test_split_gpu.py and tests/te
   split DCN: relative L2 <= 4 tol and |err| <= 40 tol max|ref|  (a sample within rounding of a pixel boundary flips corners)
   max-pool: exact on the values the input planes hold.  upsample_add always adds a skip here, whose sum is rounded
            (fp32, or re-split into planes), so it is held to the precision's bound.
+  "int" data: exact, element by element (against the reference as the output format stores it, RNE).
 
 Guards and data: tests/replay.py.
 """
@@ -32,20 +36,13 @@ import time
 import pytest
 import torch
 
-from tests.layer_census import ARCHS, census
-from tests.replay import RELU_INPUTS, _data, _judge, _reference, _replay, _stored
+from tests.layer_census import ARCHS, signatures
+from tests.replay import RELU_INPUTS, _data, _judge, _reference, _replay, _stored, int_exact
 
 pytestmark = pytest.mark.gpu
 B = 2
 # fp32 / bf16x2 / fp16x2 replay identical data: keep them together so that they share the float64 references
 PRECS = ["fp32", "bf16x2", "fp16x2", "bf16"]
-
-
-def signatures(arch, precision):
-    base = census(arch, precision, 1, 128, 160)
-    seen = {r.shapeless for r in base}
-    extra = [r for r in census(arch, precision, 1, 512, 512) if r.shapeless not in seen]
-    return list(base) + list(dict.fromkeys(extra))
 
 
 _REF_CACHE = {"arch": None, "refs": {}}
@@ -90,8 +87,10 @@ def test_layer_replay(arch, precision, monkeypatch):
         if split and rec.method in RELU_INPUTS:
             variants.append("relu")
         exact_pos = {"int", "coord", "coord-bf16"}
+        if int_exact(rec):
+            variants.append("int")
         if rec.method == "dcn":
-            variants += ["int", "coord-bf16" if precision == "bf16" else "coord"]
+            variants.append("coord-bf16" if precision == "bf16" else "coord")
         for variant in variants:
             n += 1
             label = f"{rec.label()} [{variant} inputs]"
