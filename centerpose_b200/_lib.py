@@ -117,6 +117,16 @@ def lib() -> ctypes.CDLL:
     L.cpb200_multi_pose_loss_batch.restype = ctypes.c_int
     L.cpb200_multi_pose_loss_batch.argtypes = [Heads, Targets, ctypes.c_int, ctypes.c_int, ctypes.POINTER(LossCfg),
                                                ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    L.cpb200_multi_pose_targets_train_batch.restype = ctypes.c_int
+    L.cpb200_multi_pose_targets_train_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                                        Targets, ctypes.c_void_p]
+    L.cpb200_train_augment_workspace_bytes.restype = ctypes.c_size_t
+    L.cpb200_train_augment_workspace_bytes.argtypes = [ctypes.c_int, ctypes.c_int]
+    L.cpb200_train_augment_batch.restype = ctypes.c_int
+    L.cpb200_train_augment_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                             ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),
+                                             ctypes.POINTER(ctypes.c_float), ctypes.c_void_p, ctypes.c_void_p,
+                                             ctypes.c_size_t, ctypes.c_void_p]
     L.cpb200_gaussian_radius.restype = ctypes.c_int
     L.cpb200_gaussian_radius.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
     _lib = L

@@ -27,7 +27,9 @@ FILE_FLAGS = {"net_simt.cu": ["-Xcicc", "-O1"],
               # the COCO evaluation reproduces numpy's float64 results bit for bit: no product may become an FMA
               "coco_eval.cu": ["-fmad=false"],
               # the validation targets reproduce numpy's float64 box and radius arithmetic bit for bit, likewise
-              "targets.cu": ["-fmad=false"]}
+              "targets.cu": ["-fmad=false"],
+              # the training input reproduces color_aug's float32 steps, each rounded on its own
+              "augment.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

@@ -56,7 +56,10 @@ _DEFAULT = {
     "LOSS": {"HM_HP": True, "MSE_LOSS": False, "REG_OFFSET": True, "REG_HP_OFFSET": True, "REG_BBOX": True,
              "HM_WEIGHT": 1., "WH_WEIGHT": 0.1, "OFF_WEIGHT": 1., "HP_WEIGHT": 1., "HM_HP_WEIGHT": 1., "REG_LOSS": "l1",
              "DENSE_HP": False},
-    "DATASET": {"MEAN": [0.408, 0.447, 0.470], "STD": [0.289, 0.274, 0.278]},
+    "DATASET": {"MEAN": [0.408, 0.447, 0.470], "STD": [0.289, 0.274, 0.278],
+                # the train split's augmentation (lib/config/default.py)
+                "RANDOM_CROP": True, "SHIFT": 0.1, "SCALE": 0.4, "ROTATE": 0., "AUG_ROT": 0., "FLIP": 0.5,
+                "NO_COLOR_AUG": False},
     "TEST": {"MODEL_PATH": "", "TASK": "multi_pose", "FLIP_TEST": False, "TEST_SCALES": [1],
              "TOPK": 100, "NMS": False, "FIX_RES": True, "VIS_THRESH": 0.3},
     # additive (not in the reference): activation precision of the CUDA backbone

@@ -111,6 +111,50 @@ __device__ __forceinline__ unsigned char linear_mix(int s00, int s01, int s10, i
   return (unsigned char)min(max((v + 2) >> 2, 0), 255);
 }
 
+// ---- cv2.warpAffine INTER_LINEAR on 8-bit images, constant-0 border, one output pixel ----
+// Bit-exact with OpenCV's imgwarp.cpp (WarpAffineInvoker + remapBilinear): the 2x3 matrix is inverted in double
+// exactly as cv2 does, source coordinates are 10-bit fixed point (AB_SCALE = 1024, round_delta = 16) reduced to 5
+// fractional bits, the four bilinear weights are the integers (32-fx)(32-fy)*32 ... that sum to 2^15, and the result
+// is (sum + 2^14) >> 15.
+
+// cv2::warpAffine without WARP_INVERSE_MAP inverts the forward matrix t like this, in double on the host; the explicit
+// round-to-nearest operations keep nvcc from contracting them into FMAs, so the inverse m is the host's bit for bit
+__device__ __forceinline__ void warp_inverse(const double *t, double *m) {
+  double D = __dsub_rn(__dmul_rn(t[0], t[4]), __dmul_rn(t[1], t[3]));
+  D = D != 0 ? __ddiv_rn(1.0, D) : 0;
+  m[0] = __dmul_rn(t[4], D); m[4] = __dmul_rn(t[0], D); m[1] = __dmul_rn(t[1], -D); m[3] = __dmul_rn(t[3], -D);
+  m[2] = __dsub_rn(__dmul_rn(-m[0], t[2]), __dmul_rn(m[1], t[5]));
+  m[5] = __dsub_rn(__dmul_rn(-m[3], t[2]), __dmul_rn(m[4], t[5]));
+}
+
+// the three channels u[] of output pixel (x, y) of the h x w HWC image `img` warped by the inverse matrix m; with
+// `mirror` the source is img[:, ::-1] (source column sx is stored column w - 1 - sx)
+__device__ __forceinline__ void warp_linear_u8(const unsigned char *img, int h, int w, const double *m, int x, int y,
+                                               bool mirror, int u[3]) {
+  // cv2 rounds m1*y, then the sum: an FMA would round once and, where the sum lands on a half-unit of 1/1024, can
+  // make llrint pick the other integer (tests/post_cases.py tie_x_row, tie_y_row)
+  const long long adelta = llrint(__dmul_rn(__dmul_rn(m[0], (double)x), 1024.0));
+  const long long bdelta = llrint(__dmul_rn(__dmul_rn(m[3], (double)x), 1024.0));
+  const long long X0 = llrint(__dmul_rn(__dadd_rn(__dmul_rn(m[1], (double)y), m[2]), 1024.0)) + 16;
+  const long long Y0 = llrint(__dmul_rn(__dadd_rn(__dmul_rn(m[4], (double)y), m[5]), 1024.0)) + 16;
+  const long long X = (X0 + adelta) >> 5, Y = (Y0 + bdelta) >> 5;
+  long long sxl = X >> 5, syl = Y >> 5;
+  sxl = sxl < -32768 ? -32768 : (sxl > 32767 ? 32767 : sxl);       // saturate_cast<short>
+  syl = syl < -32768 ? -32768 : (syl > 32767 ? 32767 : syl);
+  const int sx = (int)sxl, sy = (int)syl, fx = (int)(X & 31), fy = (int)(Y & 31);
+  const int w0 = (32 - fx) * (32 - fy) * 32, w1 = fx * (32 - fy) * 32, w2 = (32 - fx) * fy * 32, w3 = fx * fy * 32;
+  const bool y0 = sy >= 0 && sy < h, y1 = sy + 1 >= 0 && sy + 1 < h, x0 = sx >= 0 && sx < w, x1 = sx + 1 >= 0 && sx + 1 < w;
+  const unsigned char *p00 = img + ((long long)sy * w + (mirror ? w - 1 - sx : sx)) * 3;
+  const int dx = mirror ? -3 : 3;                                    // the next source column's byte step
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int v00 = (y0 && x0) ? p00[c] : 0, v01 = (y0 && x1) ? p00[dx + c] : 0;
+    const int v10 = (y1 && x0) ? p00[(size_t)w * 3 + c] : 0, v11 = (y1 && x1) ? p00[(size_t)w * 3 + dx + c] : 0;
+    const int s = (v00 * w0 + v01 * w1 + v10 * w2 + v11 * w3 + (1 << 14)) >> 15;
+    u[c] = s < 0 ? 0 : (s > 255 ? 255 : s);
+  }
+}
+
 #define CPB_ACT_MASK (CPB200_FLAG_RELU | CPB200_FLAG_HSWISH | CPB200_FLAG_HSIGMOID | CPB200_FLAG_RELU6 | CPB200_FLAG_CLIP01)
 // Epilogue non-linearity selected by the op flags (at most one of RELU / HSWISH / HSIGMOID / RELU6 / CLIP01).  hswish
 // and hsigmoid keep the reference's operation order x * relu6(x + 3) / 6 (mobilenetv3.py:84-93).  ReLU6 and the hard

@@ -232,40 +232,19 @@ __global__ void __launch_bounds__(256) pre_process_kernel(const PreArgs a) {
 #pragma unroll
     for (int k = 0; k < 6; ++k) t[k] = a.one.trans_input[k];
   }
-  // cv2::warpAffine without WARP_INVERSE_MAP inverts the matrix like this (imgwarp.cpp), in double on the host; the
-  // explicit round-to-nearest operations keep nvcc from contracting them into FMAs, so the inverse is the host's bit for bit
-  double D = __dsub_rn(__dmul_rn(t[0], t[4]), __dmul_rn(t[1], t[3]));
-  D = D != 0 ? __ddiv_rn(1.0, D) : 0;
-  const double m0 = __dmul_rn(t[4], D), m4 = __dmul_rn(t[0], D), m1 = __dmul_rn(t[1], -D), m3 = __dmul_rn(t[3], -D);
-  const double m2 = __dsub_rn(__dmul_rn(-m0, t[2]), __dmul_rn(m1, t[5]));
-  const double m5 = __dsub_rn(__dmul_rn(-m3, t[2]), __dmul_rn(m4, t[5]));
+  double m[6];
+  cpb::warp_inverse(t, m);
   const unsigned char *img = a.imgs + off;
   float *out = a.out + (size_t)(a.flip ? 2 * b : b) * 3 * a.OH * a.OW;
   const int total = a.OH * a.OW;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int x = i % a.OW, y = i / a.OW;
-    // cv2 rounds m1*y, then the sum: an FMA would round once and, where the sum lands on a half-unit of 1/1024, can
-    // make llrint pick the other integer (tests/post_cases.py tie_x_row, tie_y_row)
-    const long long adelta = llrint(__dmul_rn(__dmul_rn(m0, (double)x), 1024.0));
-    const long long bdelta = llrint(__dmul_rn(__dmul_rn(m3, (double)x), 1024.0));
-    const long long X0 = llrint(__dmul_rn(__dadd_rn(__dmul_rn(m1, (double)y), m2), 1024.0)) + 16;
-    const long long Y0 = llrint(__dmul_rn(__dadd_rn(__dmul_rn(m4, (double)y), m5), 1024.0)) + 16;
-    const long long X = (X0 + adelta) >> 5, Y = (Y0 + bdelta) >> 5;
-    long long sxl = X >> 5, syl = Y >> 5;
-    sxl = sxl < -32768 ? -32768 : (sxl > 32767 ? 32767 : sxl);       // saturate_cast<short>
-    syl = syl < -32768 ? -32768 : (syl > 32767 ? 32767 : syl);
-    const int sx = (int)sxl, sy = (int)syl, fx = (int)(X & 31), fy = (int)(Y & 31);
-    const int w0 = (32 - fx) * (32 - fy) * 32, w1 = fx * (32 - fy) * 32, w2 = (32 - fx) * fy * 32, w3 = fx * fy * 32;
-    const bool y0 = sy >= 0 && sy < h, y1 = sy + 1 >= 0 && sy + 1 < h, x0 = sx >= 0 && sx < w, x1 = sx + 1 >= 0 && sx + 1 < w;
-    const unsigned char *p00 = img + ((long long)sy * w + sx) * 3;
+    int u[3];
+    cpb::warp_linear_u8(img, h, w, m, x, y, false, u);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const int v00 = (y0 && x0) ? p00[c] : 0, v01 = (y0 && x1) ? p00[3 + c] : 0;
-      const int v10 = (y1 && x0) ? p00[(size_t)w * 3 + c] : 0, v11 = (y1 && x1) ? p00[(size_t)w * 3 + 3 + c] : 0;
-      int u = (v00 * w0 + v01 * w1 + v10 * w2 + v11 * w3 + (1 << 14)) >> 15;
-      u = u < 0 ? 0 : (u > 255 ? 255 : u);
-      const float f = a.f32 ? __fdiv_rn(__fsub_rn(__fdiv_rn((float)u, 255.f), a.mean[c]), a.stdv[c])
-                            : (float)(((double)u / 255.0 - (double)a.mean[c]) / (double)a.stdv[c]);
+      const float f = a.f32 ? __fdiv_rn(__fsub_rn(__fdiv_rn((float)u[c], 255.f), a.mean[c]), a.stdv[c])
+                            : (float)(((double)u[c] / 255.0 - (double)a.mean[c]) / (double)a.stdv[c]);
       out[((size_t)c * a.OH + y) * a.OW + x] = f;
       if (a.flip) out[((size_t)(3 + c) * a.OH + y) * a.OW + (a.OW - 1 - x)] = f;
     }

@@ -1,8 +1,8 @@
 // Multi-pose training targets and MultiPoseLoss for the reference's validation pass (cpb200_multi_pose_targets_batch,
 // cpb200_multi_pose_loss_batch, cpb200_gaussian_radius).
 //
-// The targets are what MultiPoseDataset.__getitem__ returns for the val split (no augmentation: rot 0, no flip), bit
-// for bit.  The file is built with -fmad=false so that no product is contracted into an FMA; the one FMA the
+// The targets are what MultiPoseDataset.__getitem__ returns, bit for bit: for the val split (no augmentation: rot 0,
+// no flip, one matrix) and for the train split's augmented draws (cpb200_multi_pose_targets_train_batch).  The file is built with -fmad=false so that no product is contracted into an FMA; the one FMA the
 // reference's np.dot performs is written out with __fma_rn.
 //
 //   targets_kernel  one CTA per (image, object slot): the slot's annotation (the k-th non-crowd one in file order),
@@ -15,6 +15,7 @@
 namespace {
 
 static_assert(sizeof(cpb200_val_image) == 64, "cpb200_val_image layout is part of the C ABI");
+static_assert(sizeof(cpb200_train_image) == 240, "cpb200_train_image layout is part of the C ABI");
 static_assert(sizeof(cpb200_coco_kp_gt) == 336, "cpb200_coco_kp_gt layout is part of the C ABI");
 
 constexpr int J = CPB200_COCO_KP_JOINTS;
@@ -55,18 +56,43 @@ struct Stamp {
   int map;                           // -1: hm, else the hm_hp channel
 };
 
+// What the targets kernel reads of one image.  The val split's entry is the case without flip or rotation whose
+// joints go through the box matrix.
+struct ImageView {
+  int gt_begin, gt_count, flip, rot;
+  float width;                       // the image width, for the flip
+  const double *t, *t_rot;           // trans_output (boxes) and trans_output_rot (joints)
+};
+
+__device__ inline ImageView view(const cpb200_val_image &e) {
+  return ImageView{e.gt_begin, e.gt_count, 0, 0, 0.f, e.trans_output, e.trans_output};
+}
+
+__device__ inline ImageView view(const cpb200_train_image &e) {
+  return ImageView{e.gt_begin, e.gt_count, e.flip, e.rot, (float)e.w, e.trans_output, e.trans_output_rot};
+}
+
+// the dataset's flip_idx pairs (1, 2), (3, 4), ..., (15, 16): after a flip joint j holds the annotation's joint
+__device__ inline int flip_partner(int j) { return j == 0 ? 0 : (j & 1 ? j + 1 : j - 1); }
+
+template <typename Image>
 struct TargetArgs {
-  const cpb200_val_image *images;
+  const Image *images;
   const cpb200_coco_kp_gt *gts;
   cpb200_multi_pose_targets out;
   int R;
 };
 
-__global__ void __launch_bounds__(kStampThreads) targets_kernel(const TargetArgs a) {
+template <typename Image>
+__global__ void __launch_bounds__(kStampThreads) targets_kernel(const TargetArgs<Image> a) {
   const int k = blockIdx.x, b = blockIdx.y, R = a.R;
-  const cpb200_val_image im = a.images[b];
+  const Image e = a.images[b];
+  const ImageView im = view(e);
   __shared__ int s_ann, s_n;
   __shared__ Stamp s_st[1 + J];
+  // rot != 0: hm = hm * 0 + 0.9999 after every object, so no object stamps it and slot 0's CTA fills it
+  if (im.rot && k == 0)
+    for (int i = threadIdx.x; i < R * R; i += blockDim.x) a.out.hm[(size_t)b * R * R + i] = 0.9999f;
   // the k-th annotation with iscrowd != 1, in file order (warp 0 counts with ballots)
   if (threadIdx.x < 32) {
     int seen = 0, found = -1;
@@ -88,10 +114,16 @@ __global__ void __launch_bounds__(kStampThreads) targets_kernel(const TargetArgs
   if (s_ann < 0) return;
   if (threadIdx.x == 0) {
     const cpb200_coco_kp_gt &g = a.gts[im.gt_begin + s_ann];
-    const double *t = im.trans_output;
+    const double *t = im.t;
     const float hi = (float)(R - 1);
-    // float32([x, y, x + w, y + h]), corners through trans_output, clipped to [0, R - 1]
+    // float32([x, y, x + w, y + h]); flipped: bbox[[0, 2]] = width - bbox[[2, 0]] - 1 in float32; corners through
+    // trans_output, clipped to [0, R - 1]
     float bb[4] = {(float)g.bbox[0], (float)g.bbox[1], (float)(g.bbox[0] + g.bbox[2]), (float)(g.bbox[1] + g.bbox[3])};
+    if (im.flip) {
+      const float x0 = bb[0];
+      bb[0] = __fsub_rn(__fsub_rn(im.width, bb[2]), 1.f);
+      bb[2] = __fsub_rn(__fsub_rn(im.width, x0), 1.f);
+    }
     for (int c = 0; c < 4; c += 2) {
       const float x = bb[c], y = bb[c + 1];
       bb[c] = affine_x(t, x, y);
@@ -99,7 +131,8 @@ __global__ void __launch_bounds__(kStampThreads) targets_kernel(const TargetArgs
     }
     for (int c = 0; c < 4; ++c) bb[c] = fminf(fmaxf(bb[c], 0.f), hi);
     const float h = __fsub_rn(bb[3], bb[1]), w = __fsub_rn(bb[2], bb[0]);
-    if (h > 0 && w > 0) {
+    // with rot != 0 every object is drawn, a degenerate box too (its radius is 0)
+    if ((h > 0 && w > 0) || im.rot) {
       const int r = radius_of((int)ceilf(h), (int)ceilf(w));
       const float cx = __fdiv_rn(__fadd_rn(bb[0], bb[2]), 2.f), cy = __fdiv_rn(__fadd_rn(bb[1], bb[3]), 2.f);
       const int ix = (int)cx, iy = (int)cy;
@@ -109,20 +142,26 @@ __global__ void __launch_bounds__(kStampThreads) targets_kernel(const TargetArgs
       a.out.ind[o] = (int64_t)iy * R + ix;
       a.out.reg[2 * o] = __fsub_rn(cx, (float)ix);
       a.out.reg[2 * o + 1] = __fsub_rn(cy, (float)iy);
-      // num_kpts == 0: reg_mask 0, and hm[ct] = 0.9999, which this object's own stamp (1.0 at ct) always overwrites
-      a.out.reg_mask[o] = g.visible != 0;
+      // num_kpts == 0: reg_mask 0, and hm[ct] = 0.9999, which this object's own stamp (1.0 at ct) always overwrites;
+      // rot != 0 zeroes reg_mask and hps_mask afterwards
+      a.out.reg_mask[o] = g.visible != 0 && !im.rot;
       int n = 0;
-      s_st[n++] = Stamp{ix, iy, r, -1};
+      if (!im.rot) s_st[n++] = Stamp{ix, iy, r, -1};
+      const double *tr = im.t_rot;
       for (int j = 0; j < J; ++j) {
-        if (!((g.visible >> j) & 1)) continue;
-        const float x = (float)g.x[j], y = (float)g.y[j];
-        const float px = affine_x(t, x, y), py = affine_x(t + 3, x, y);
+        // flipped: pts[:, 0] = width - pts[:, 0] - 1 in float32, then the flip_idx rows (v included) swap
+        const int src = im.flip ? flip_partner(j) : j;
+        if (!((g.visible >> src) & 1)) continue;
+        float x = (float)g.x[src];
+        const float y = (float)g.y[src];
+        if (im.flip) x = __fsub_rn(__fsub_rn(im.width, x), 1.f);
+        const float px = affine_x(tr, x, y), py = affine_x(tr + 3, x, y);
         if (!(px >= 0 && px < (float)R && py >= 0 && py < (float)R)) continue;
         const int qx = (int)px, qy = (int)py;
         const size_t p = o * J + j;
         a.out.hps[2 * p] = __fsub_rn(px, (float)ix);
         a.out.hps[2 * p + 1] = __fsub_rn(py, (float)iy);
-        a.out.hps_mask[2 * p] = a.out.hps_mask[2 * p + 1] = 1;
+        a.out.hps_mask[2 * p] = a.out.hps_mask[2 * p + 1] = !im.rot;
         a.out.hp_offset[2 * p] = __fsub_rn(px, (float)qx);
         a.out.hp_offset[2 * p + 1] = __fsub_rn(py, (float)qy);
         a.out.hp_ind[p] = (int64_t)qy * R + qx;
@@ -273,14 +312,12 @@ bool targets_complete(const cpb200_multi_pose_targets &t) {
          t.hp_mask;
 }
 
-}  // namespace
-
-extern "C" int cpb200_multi_pose_targets_batch(const cpb200_val_image *images, int B, const cpb200_coco_kp_gt *gts,
-                                               int R, cpb200_multi_pose_targets out, void *stream) {
-  if (!images || B < 1 || !gts || R < 1 || !targets_complete(out))
-    return cpb::fail(CPB200_ERR_ARG, "multi_pose_targets_batch: bad arguments");
-  if (B > 65535) return cpb::fail(CPB200_ERR_ARG, "multi_pose_targets_batch: B = %d images exceed one launch", B);
-  if ((long long)R * R * J >= (1LL << 31)) return cpb::fail(CPB200_ERR_ARG, "multi_pose_targets_batch: R = %d too large", R);
+template <typename Image>
+int targets_launch(const Image *images, int B, const cpb200_coco_kp_gt *gts, int R, cpb200_multi_pose_targets out,
+                   void *stream, const char *what) {
+  if (!images || B < 1 || !gts || R < 1 || !targets_complete(out)) return cpb::fail(CPB200_ERR_ARG, "%s: bad arguments", what);
+  if (B > 65535) return cpb::fail(CPB200_ERR_ARG, "%s: B = %d images exceed one launch", what, B);
+  if ((long long)R * R * J >= (1LL << 31)) return cpb::fail(CPB200_ERR_ARG, "%s: R = %d too large", what, R);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t plane = (size_t)R * R, bm = (size_t)B * M;
   // the reference's np.zeros: every slot and pixel no object writes stays 0
@@ -295,9 +332,22 @@ extern "C" int cpb200_multi_pose_targets_batch(const cpb200_val_image *images, i
   CPB_CUDA(cudaMemsetAsync(out.hp_offset, 0, sizeof(float) * bm * J * 2, s));
   CPB_CUDA(cudaMemsetAsync(out.hp_ind, 0, sizeof(int64_t) * bm * J, s));
   CPB_CUDA(cudaMemsetAsync(out.hp_mask, 0, sizeof(int64_t) * bm * J, s));
-  TargetArgs a = {images, gts, out, R};
-  targets_kernel<<<dim3(M, (unsigned)B), kStampThreads, 0, s>>>(a);
+  TargetArgs<Image> a = {images, gts, out, R};
+  targets_kernel<Image><<<dim3(M, (unsigned)B), kStampThreads, 0, s>>>(a);
   return cpb::check_launch("targets_kernel");
+}
+
+}  // namespace
+
+extern "C" int cpb200_multi_pose_targets_batch(const cpb200_val_image *images, int B, const cpb200_coco_kp_gt *gts,
+                                               int R, cpb200_multi_pose_targets out, void *stream) {
+  return targets_launch(images, B, gts, R, out, stream, "multi_pose_targets_batch");
+}
+
+extern "C" int cpb200_multi_pose_targets_train_batch(const cpb200_train_image *images, int B,
+                                                     const cpb200_coco_kp_gt *gts, int R,
+                                                     cpb200_multi_pose_targets out, void *stream) {
+  return targets_launch(images, B, gts, R, out, stream, "multi_pose_targets_train_batch");
 }
 
 extern "C" size_t cpb200_multi_pose_loss_workspace_bytes(int B) {

@@ -310,6 +310,125 @@ WEBP_DEVICE_MIN_IMAGES = 16
 WEBP_LOSSLESS_DEVICE_MIN_IMAGES = 24
 
 
+def load_checked(n, src):
+    """Input ``n`` of ``run_images`` as a BGR uint8 HWC array (a path through ``cv2.imread``)."""
+    if not isinstance(src, (np.ndarray, str)):
+        raise ValueError("run_images: image %d is a %s, expected a BGR uint8 HWC array or a path"
+                         % (n, type(src).__name__))
+    if isinstance(src, np.ndarray):
+        image = src
+    else:
+        image = cv2.imread(src)
+        if image is None:
+            raise FileNotFoundError(src)
+    if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+        raise ValueError("run_images: image %d must be uint8 (H, W, 3), got %s %s" % (n, image.dtype, image.shape))
+    return image
+
+
+def load_images_device(images):
+    """Every input of ``run_images`` (a path or a BGR uint8 HWC array) in one device buffer of packed HWC uint8 BGR
+    images.  It needs no model: ``train_data.TrainData`` loads its images with it too.  Returns ``(views, offsets,
+    buffer)``: per input a (h, w, 3) view of its slot and the slot's byte offset.
+
+    The files' headers are parsed first (``jpeg.parse``, ``png.parse``, ``webp.parse``, and
+    ``webp_lossless.parse`` for the files ``webp.parse`` declines as lossless), so every size is known before any
+    pixel exists.  The files the device can decode, with their tables, go up in one pinned buffer and are decoded
+    by each format module's ``KERNEL`` (``cpb200_jpeg_decode_batch``, ``cpb200_png_decode_batch``,
+    ``cpb200_webp_decode_batch``, ``cpb200_webp_lossless_decode_batch``) in chunks of at most ``JPEG_CHUNK_IMAGES``
+    images that reuse one workspace; PNG files only when the call holds at least ``PNG_DEVICE_MIN_IMAGES`` of them,
+    since one PNG launch costs about as much as a dozen host decodes, lossy WebP files from
+    ``WEBP_DEVICE_MIN_IMAGES`` on and lossless ones from ``WEBP_LOSSLESS_DEVICE_MIN_IMAGES`` on.  The other files
+    (``cv2.imread``) and the arrays take the host path, and
+    their pixels go up in one copy into slots after the decoded ones.  One read of the decode status follows; a
+    file whose compressed data the device found bad, or a lossless file over the device's prefix-code group
+    budget, is read by ``cv2.imread`` and copied into its slot."""
+    from . import _lib, jpeg, png, webp, webp_lossless
+    dev = torch.device("cuda")
+    datas, infos, host = {}, {}, {}
+    for n, src in enumerate(images):
+        if not isinstance(src, str):
+            host[n] = load_checked(n, src)
+            continue
+        try:
+            with open(src, "rb") as f:
+                data = f.read()
+        except OSError:
+            raise FileNotFoundError(src)
+        fmt = png if data[:8] == png.SIGNATURE else webp if webp.is_webp(data) else jpeg
+        try:
+            info = fmt.parse(data, src)
+            if fmt is webp and info.reason.startswith("lossless"):
+                fmt, info = webp_lossless, webp_lossless.parse(data, src)
+        except ValueError:
+            info = None
+        if info is not None and (info.eligible or getattr(info, "progressive", None)):
+            datas[n], infos[n] = data, (fmt, info)
+        else:
+            host[n] = load_checked(n, src)
+    for fmt, least in ((png, PNG_DEVICE_MIN_IMAGES), (webp, WEBP_DEVICE_MIN_IMAGES),
+                       (webp_lossless, WEBP_LOSSLESS_DEVICE_MIN_IMAGES)):
+        files = [n for n in infos if infos[n][0] is fmt]
+        if len(files) < least:
+            for n in files:                               # cv2.imread is faster for a handful of these files
+                del infos[n], datas[n]
+                host[n] = load_checked(n, images[n])
+    shape = {n: (info.oh, info.ow, 3) for n, (_, info) in infos.items()}
+    shape.update({n: im.shape for n, im in host.items()})
+    offsets, pos = {}, 0
+    for n in list(infos) + list(host):                   # decoded slots first, then the host ones in one run
+        offsets[n] = pos
+        pos += int(np.prod(shape[n]))
+    host_start = pos - sum(im.nbytes for im in host.values())
+    pixels = torch.empty(max(pos, 1), dtype=torch.uint8, device=dev)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    # JPEG files, then PNG files, then lossy and lossless WebP files; status[k] belongs to dec[k]
+    dec = [n for fmt in (jpeg, png, webp, webp_lossless) for n in infos if infos[n][0] is fmt]
+    if dec:
+        chunks, start, ws = [], 0, 0
+        for k, n in enumerate(dec):
+            fmt, info = infos[n]
+            if k > start and (k - start == JPEG_CHUNK_IMAGES or ws + info.workspace_bytes() > JPEG_CHUNK_WORKSPACE
+                              or fmt is not infos[dec[start]][0]):
+                chunks.append((start, k)); start, ws = k, 0
+            ws += info.workspace_bytes()
+        chunks.append((start, len(dec)))
+        packed = [infos[dec[a]][0].pack([infos[n][1] for n in dec[a:b]], [datas[n] for n in dec[a:b]],
+                                        [offsets[n] for n in dec[a:b]])
+                  for a, b in chunks]
+        at = np.cumsum([0] + [p[0].nbytes + (-p[0].nbytes) % 16 for p in packed])
+        up = torch.empty(int(at[-1]), dtype=torch.uint8, pin_memory=True)
+        uv = up.numpy()
+        for (b, _), o in zip(packed, at):
+            uv[o:o + b.nbytes] = b
+        src = up.to(dev, non_blocking=True)
+        work = torch.empty(max(p[1] for p in packed), dtype=torch.uint8, device=dev)
+        status = torch.empty(len(dec), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            for (a, b), o in zip(chunks, at):
+                name = infos[dec[a]][0].KERNEL
+                st = getattr(_lib.lib(), "cpb200_" + name)(src.data_ptr() + int(o), src.data_ptr() + int(o), b - a,
+                                                          work.data_ptr(), work.numel(), pixels.data_ptr(),
+                                                          status.data_ptr() + 4 * a, stream)
+                _lib.check(st, name)
+    if host:
+        staged = torch.empty(pos - host_start, dtype=torch.uint8, pin_memory=True)
+        sv = staged.numpy()
+        for n, im in host.items():
+            sv[offsets[n] - host_start:offsets[n] - host_start + im.nbytes] = np.ascontiguousarray(im).reshape(-1)
+        pixels[host_start:pos].copy_(staged, non_blocking=True)
+    if dec:
+        for k in np.flatnonzero(status.cpu().numpy()):
+            n = dec[k]
+            image = load_checked(n, images[n])
+            if image.shape != shape[n]:
+                raise RuntimeError("run_images: %s decodes to %s on the host, its header says %s"
+                                   % (images[n], image.shape, shape[n]))
+            pixels[offsets[n]:offsets[n] + image.nbytes].copy_(torch.from_numpy(image.reshape(-1)))
+    views = [pixels[offsets[n]:offsets[n] + int(np.prod(shape[n]))].view(shape[n]) for n in range(len(images))]
+    return views, [offsets[n] for n in range(len(images))], pixels
+
+
 def _swap_pairs(C, pairs, device):
     idx = list(range(C))
     for a, b in pairs:
@@ -443,7 +562,7 @@ class MultiPoseDetector(BaseDetector):
         array per image, byte for byte the reference Debugger's ``imgs['multi_pose']`` (``DEBUG_THEME`` 'white' or
         any other theme).  One upload of the images and tables, one ``cpb200_render_poses_batch``, one copy back."""
         from . import render
-        images = [self._load_checked(n, im) for n, im in enumerate(images)]
+        images = [load_checked(n, im) for n, im in enumerate(images)]
         if not images:
             return []
         shapes = [im.shape[:2] for im in images]
@@ -503,117 +622,6 @@ class MultiPoseDetector(BaseDetector):
         Returns the merged ``(N, 56)`` rows (numpy) in original-image pixels, like ``run()['results'][1]``."""
         return self.run_images([image])[0]
 
-    def _load_checked(self, n, src):
-        """Input ``n`` of ``run_images`` as a BGR uint8 HWC array (a path through ``cv2.imread``)."""
-        if not isinstance(src, (np.ndarray, str)):
-            raise ValueError("run_images: image %d is a %s, expected a BGR uint8 HWC array or a path"
-                             % (n, type(src).__name__))
-        image = self._load(src)[0]
-        if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
-            raise ValueError("run_images: image %d must be uint8 (H, W, 3), got %s %s" % (n, image.dtype, image.shape))
-        return image
-
-    def _load_images_device(self, images):
-        """Every input of ``run_images`` in one device buffer of packed HWC uint8 BGR images.  Returns
-        ``(views, offsets, buffer)``: per input a (h, w, 3) view of its slot and the slot's byte offset.
-
-        The files' headers are parsed first (``jpeg.parse``, ``png.parse``, ``webp.parse``, and
-        ``webp_lossless.parse`` for the files ``webp.parse`` declines as lossless), so every size is known before any
-        pixel exists.  The files the device can decode, with their tables, go up in one pinned buffer and are decoded
-        by each format module's ``KERNEL`` (``cpb200_jpeg_decode_batch``, ``cpb200_png_decode_batch``,
-        ``cpb200_webp_decode_batch``, ``cpb200_webp_lossless_decode_batch``) in chunks of at most ``JPEG_CHUNK_IMAGES``
-        images that reuse one workspace; PNG files only when the call holds at least ``PNG_DEVICE_MIN_IMAGES`` of them,
-        since one PNG launch costs about as much as a dozen host decodes, lossy WebP files from
-        ``WEBP_DEVICE_MIN_IMAGES`` on and lossless ones from ``WEBP_LOSSLESS_DEVICE_MIN_IMAGES`` on.  The other files
-        (``cv2.imread``) and the arrays take the host path, and
-        their pixels go up in one copy into slots after the decoded ones.  One read of the decode status follows; a
-        file whose compressed data the device found bad, or a lossless file over the device's prefix-code group
-        budget, is read by ``cv2.imread`` and copied into its slot."""
-        from . import _lib, jpeg, png, webp, webp_lossless
-        dev = torch.device("cuda")
-        datas, infos, host = {}, {}, {}
-        for n, src in enumerate(images):
-            if not isinstance(src, str):
-                host[n] = self._load_checked(n, src)
-                continue
-            try:
-                with open(src, "rb") as f:
-                    data = f.read()
-            except OSError:
-                raise FileNotFoundError(src)
-            fmt = png if data[:8] == png.SIGNATURE else webp if webp.is_webp(data) else jpeg
-            try:
-                info = fmt.parse(data, src)
-                if fmt is webp and info.reason.startswith("lossless"):
-                    fmt, info = webp_lossless, webp_lossless.parse(data, src)
-            except ValueError:
-                info = None
-            if info is not None and (info.eligible or getattr(info, "progressive", None)):
-                datas[n], infos[n] = data, (fmt, info)
-            else:
-                host[n] = self._load_checked(n, src)
-        for fmt, least in ((png, PNG_DEVICE_MIN_IMAGES), (webp, WEBP_DEVICE_MIN_IMAGES),
-                           (webp_lossless, WEBP_LOSSLESS_DEVICE_MIN_IMAGES)):
-            files = [n for n in infos if infos[n][0] is fmt]
-            if len(files) < least:
-                for n in files:                               # cv2.imread is faster for a handful of these files
-                    del infos[n], datas[n]
-                    host[n] = self._load_checked(n, images[n])
-        shape = {n: (info.oh, info.ow, 3) for n, (_, info) in infos.items()}
-        shape.update({n: im.shape for n, im in host.items()})
-        offsets, pos = {}, 0
-        for n in list(infos) + list(host):                   # decoded slots first, then the host ones in one run
-            offsets[n] = pos
-            pos += int(np.prod(shape[n]))
-        host_start = pos - sum(im.nbytes for im in host.values())
-        pixels = torch.empty(max(pos, 1), dtype=torch.uint8, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        # JPEG files, then PNG files, then lossy and lossless WebP files; status[k] belongs to dec[k]
-        dec = [n for fmt in (jpeg, png, webp, webp_lossless) for n in infos if infos[n][0] is fmt]
-        if dec:
-            chunks, start, ws = [], 0, 0
-            for k, n in enumerate(dec):
-                fmt, info = infos[n]
-                if k > start and (k - start == JPEG_CHUNK_IMAGES or ws + info.workspace_bytes() > JPEG_CHUNK_WORKSPACE
-                                  or fmt is not infos[dec[start]][0]):
-                    chunks.append((start, k)); start, ws = k, 0
-                ws += info.workspace_bytes()
-            chunks.append((start, len(dec)))
-            packed = [infos[dec[a]][0].pack([infos[n][1] for n in dec[a:b]], [datas[n] for n in dec[a:b]],
-                                            [offsets[n] for n in dec[a:b]])
-                      for a, b in chunks]
-            at = np.cumsum([0] + [p[0].nbytes + (-p[0].nbytes) % 16 for p in packed])
-            up = torch.empty(int(at[-1]), dtype=torch.uint8, pin_memory=True)
-            uv = up.numpy()
-            for (b, _), o in zip(packed, at):
-                uv[o:o + b.nbytes] = b
-            src = up.to(dev, non_blocking=True)
-            work = torch.empty(max(p[1] for p in packed), dtype=torch.uint8, device=dev)
-            status = torch.empty(len(dec), dtype=torch.int32, device=dev)
-            with torch.cuda.device(dev):
-                for (a, b), o in zip(chunks, at):
-                    name = infos[dec[a]][0].KERNEL
-                    st = getattr(_lib.lib(), "cpb200_" + name)(src.data_ptr() + int(o), src.data_ptr() + int(o), b - a,
-                                                              work.data_ptr(), work.numel(), pixels.data_ptr(),
-                                                              status.data_ptr() + 4 * a, stream)
-                    _lib.check(st, name)
-        if host:
-            staged = torch.empty(pos - host_start, dtype=torch.uint8, pin_memory=True)
-            sv = staged.numpy()
-            for n, im in host.items():
-                sv[offsets[n] - host_start:offsets[n] - host_start + im.nbytes] = np.ascontiguousarray(im).reshape(-1)
-            pixels[host_start:pos].copy_(staged, non_blocking=True)
-        if dec:
-            for k in np.flatnonzero(status.cpu().numpy()):
-                n = dec[k]
-                image = self._load_checked(n, images[n])
-                if image.shape != shape[n]:
-                    raise RuntimeError("run_images: %s decodes to %s on the host, its header says %s"
-                                       % (images[n], image.shape, shape[n]))
-                pixels[offsets[n]:offsets[n] + image.nbytes].copy_(torch.from_numpy(image.reshape(-1)))
-        views = [pixels[offsets[n]:offsets[n] + int(np.prod(shape[n]))].view(shape[n]) for n in range(len(images))]
-        return views, [offsets[n] for n in range(len(images))], pixels
-
     def run_eval(self, images, image_ids, gt, max_batch=32):
         """Additive: tools/evaluate.py's loop and ``dataset.run_eval`` (coco_hp.py:97-107) in one call.  Runs
         ``run_images(images, max_batch)``, evaluates the rows of ``images[i]`` as image ``image_ids[i]`` against ``gt``
@@ -663,7 +671,7 @@ class MultiPoseDetector(BaseDetector):
             log = {k: 0 for k in val.STATS}
             log["time"] = (time.time() - t_start) / 60.
             return log, {}
-        loaded, offsets, pixels = self._load_images_device(images)
+        loaded, offsets, pixels = load_images_device(images)
         dev = torch.device("cuda")
         stream = torch.cuda.current_stream(dev).cuda_stream
         res, R, K = int(cfg.MODEL.INPUT_RES), int(cfg.MODEL.OUTPUT_RES), int(cfg.TEST.TOPK)
@@ -721,7 +729,7 @@ class MultiPoseDetector(BaseDetector):
         only host wait is the final device-to-host copy.
 
         With ``B200.DEVICE_PREPROCESS`` on (the default) and any path among the inputs, the images are decoded into
-        one device buffer first (``_load_images_device``): sequential- and progressive-Huffman JPEG files by
+        one device buffer first (``load_images_device``): sequential- and progressive-Huffman JPEG files by
         ``cpb200_jpeg_decode_batch``, from ``PNG_DEVICE_MIN_IMAGES`` PNG files per call on, PNG files (not APNG)
         by ``cpb200_png_decode_batch``, from ``WEBP_DEVICE_MIN_IMAGES`` on, lossy WebP files (not alpha or animated
         ones) by ``cpb200_webp_decode_batch``, and from ``WEBP_LOSSLESS_DEVICE_MIN_IMAGES`` on, lossless WebP files
@@ -758,13 +766,13 @@ class MultiPoseDetector(BaseDetector):
             raise ValueError("run_images: max_batch must be >= 1, got %r" % (max_batch,))
         offsets = None
         if self.device_preprocess and any(isinstance(src, str) for src in images):
-            loaded, offsets, pixels_dev = self._load_images_device(images)
+            loaded, offsets, pixels_dev = load_images_device(images)
         elif return_images:
             # every image in one device buffer, so that the drawing needs no second upload
-            loaded, offsets, pixels_dev = self._load_images_device(
-                [self._load_checked(n, src) for n, src in enumerate(images)])
+            loaded, offsets, pixels_dev = load_images_device(
+                [load_checked(n, src) for n, src in enumerate(images)])
         else:
-            loaded = [self._load_checked(n, src) for n, src in enumerate(images)]
+            loaded = [load_checked(n, src) for n, src in enumerate(images)]
         if not loaded:
             return ([],) * (1 + bool(return_images) + bool(return_heatmaps)) if return_images or return_heatmaps else []
         cfg = self.cfg

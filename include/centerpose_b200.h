@@ -517,6 +517,47 @@ typedef struct cpb200_multi_pose_targets {
 int cpb200_multi_pose_targets_batch(const cpb200_val_image *images, int B, const cpb200_coco_kp_gt *gts, int R,
                                     cpb200_multi_pose_targets out, void *stream);
 
+/* ---- Training split (lib/datasets/multi_pose.py, split 'train'): augmented inputs and targets ----
+ * One image of an augmented batch (240 bytes, DEVICE memory).  The host draws the random parameters in the
+ * reference's order and builds the matrices; the kernels apply them. */
+typedef struct cpb200_train_image {
+  int64_t offset;            /* byte offset of the image's first pixel in `imgs` */
+  int32_t h, w;              /* image size; HWC uint8 BGR, rows packed (pitch 3*w bytes) */
+  int32_t flip;              /* 1: the image is mirrored (img[:, ::-1]), its boxes and joints too */
+  int32_t rot;               /* 1: rot != 0 (hm is 0.9999 everywhere, reg_mask and hps_mask are 0) */
+  int32_t color;             /* 1: color_aug runs (DATASET.NO_COLOR_AUG off) */
+  int32_t order[3];          /* color_aug's shuffled functions: 0 brightness, 1 contrast, 2 saturation */
+  int32_t gt_begin, gt_count;  /* its annotations in `gts` (cpb200_coco_kp_gt), in annotation-file order */
+  float alpha[3];            /* float32(1 + uniform(-0.4, 0.4)) of function order[i] */
+  float beta[3];             /* float32(1 - alpha) of the same draw, rounded from double */
+  double light[3];           /* np.dot(eig_vec, eig_val * normal(scale=0.1, size=3)), added per channel */
+  double trans_input[6];     /* get_affine_transform(c, s, rot, [S, S]), row-major */
+  double trans_output[6];    /* get_affine_transform(c, s, 0, [R, R]): the boxes */
+  double trans_output_rot[6];  /* get_affine_transform(c, s, rot, [R, R]): the joints */
+} cpb200_train_image;
+
+/* Workspace of cpb200_train_augment_batch for B images of S x S. */
+size_t cpb200_train_augment_workspace_bytes(int B, int S);
+
+/* MultiPoseDataset.__getitem__'s 'input' for B images (S = INPUT_RES, S % 4 == 0, S <= 768), bit for bit:
+ * cv2.warpAffine (INTER_LINEAR, constant 0) of img or img[:, ::-1] with trans_input, / 255 in float32, color_aug
+ * (the three blends in the image's order, then lighting) where `color` is set, then (x - mean) / std in float32.
+ * out is (B,3,S,S) fp32.  color_aug's grey mean is numpy's pairwise float32 sum over the S*S grey values: `plan` is a
+ * DEVICE int32 array describing its summation tree for n = S*S (centerpose_b200.train_data.mean_plan):
+ *   [L, D, leaf begins (L + 1), level starts (D + 1), per internal node its two child slots (2 each)],
+ * slots 0..L-1 the leaves, L + k internal node k, children before parents, the root last.  mean / stdv are HOST
+ * arrays of 3 floats.  No allocation, no host wait.  1 <= B <= 65535. */
+int cpb200_train_augment_batch(const unsigned char *imgs, const cpb200_train_image *table, int B, int S,
+                               const int32_t *plan, const float *mean, const float *stdv, float *out,
+                               void *workspace, size_t workspace_bytes, void *stream);
+
+/* cpb200_multi_pose_targets_batch for the training split: the boxes are flipped when `flip` is set (x -> w - x - 1,
+ * left and right joints swapped), the boxes go through trans_output and the joints through trans_output_rot, and
+ * with `rot` every object is drawn and hm, reg_mask and hps_mask are set as the reference sets them.  The val
+ * entry point is this kernel with no flip, rot 0 and one matrix.  1 <= B <= 65535. */
+int cpb200_multi_pose_targets_train_batch(const cpb200_train_image *images, int B, const cpb200_coco_kp_gt *gts,
+                                          int R, cpb200_multi_pose_targets out, void *stream);
+
 /* The six head maps of B images as the forward leaves them (DEVICE, (B,C,R,R) fp32; hm and hm_hp are logits). */
 typedef struct cpb200_multi_pose_heads {
   const float *hm, *wh, *hps, *reg, *hm_hp, *hp_offset;
