@@ -109,23 +109,37 @@ def loss_cfg(cfg):
                         float(c.HM_HP_WEIGHT), int(bool(c.HM_HP)), int(bool(c.REG_OFFSET)), int(bool(c.REG_HP_OFFSET)))
 
 
-def loss(outputs, targets, cfg):
-    """``MultiPoseLoss.forward`` per image on the forward's six head maps ``outputs`` (hm and hm_hp as logits; they
-    are not modified) and ``targets`` (:func:`targets`).  Returns a (B, 7) float32 CUDA tensor, the stats in
-    :data:`STATS` order, as each image's ``loss_stats[l].mean().item()`` would be in a batch of one."""
-    from . import _lib
+def check_loss_inputs(outputs, targets, what, names=None):
+    """The six head maps ``outputs`` as contiguous tensors, after checking that they are CUDA float32 (B, C, R, R) on
+    one device and that the ``targets`` named ``names`` (default: all of :data:`TARGETS`) are contiguous tensors of
+    the dataset's dtypes and shapes on that device.  Raises ``ValueError`` naming ``what`` otherwise."""
     heads = [o.contiguous() for o in outputs]
     hm = heads[0]
     B, R = hm.shape[0], hm.shape[-1]
     for h, c in zip(heads, (1, 2, 2 * J, 2, J, 2)):
         if not h.is_cuda or h.dtype != torch.float32 or tuple(h.shape) != (B, c, R, R) or h.device != hm.device:
-            raise ValueError("val.loss: head maps must be CUDA float32 (B, C, R, R) with C = 1, 2, 34, 2, 17, 2 on one "
-                             "device; got %s" % [(tuple(x.shape), x.dtype) for x in heads])
+            raise ValueError("%s: head maps must be CUDA float32 (B, C, R, R) with C = 1, 2, 34, 2, 17, 2 on one "
+                             "device; got %s" % (what, [(tuple(x.shape), x.dtype) for x in heads]))
     for name, dt, shape in TARGETS:
+        if names is not None and name not in names:
+            continue
+        if name not in targets:
+            raise ValueError("%s: the batch has no target %r" % (what, name))
         t = targets[name]
         if t.dtype != dt or tuple(t.shape) != (B,) + shape(R) or t.device != hm.device or not t.is_contiguous():
-            raise ValueError("val.loss: target %r is %s %s, expected %s %s on %s"
-                             % (name, t.dtype, tuple(t.shape), dt, (B,) + shape(R), hm.device))
+            raise ValueError("%s: target %r is %s %s, expected %s %s on %s"
+                             % (what, name, t.dtype, tuple(t.shape), dt, (B,) + shape(R), hm.device))
+    return heads
+
+
+def loss(outputs, targets, cfg):
+    """``MultiPoseLoss.forward`` per image on the forward's six head maps ``outputs`` (hm and hm_hp as logits; they
+    are not modified) and ``targets`` (:func:`targets`).  Returns a (B, 7) float32 CUDA tensor, the stats in
+    :data:`STATS` order, as each image's ``loss_stats[l].mean().item()`` would be in a batch of one."""
+    from . import _lib
+    heads = check_loss_inputs(outputs, targets, "val.loss")
+    hm = heads[0]
+    B, R = hm.shape[0], hm.shape[-1]
     stats = torch.empty((B, len(STATS)), dtype=torch.float32, device=hm.device)
     L = _lib.lib()
     ws = torch.empty(max(L.cpb200_multi_pose_loss_workspace_bytes(B), 1), dtype=torch.uint8, device=hm.device)

@@ -580,6 +580,31 @@ size_t cpb200_multi_pose_loss_workspace_bytes(int B);
 int cpb200_multi_pose_loss_batch(cpb200_multi_pose_heads heads, cpb200_multi_pose_targets targets, int B, int R,
                                  const cpb200_multi_pose_loss_cfg *cfg, float *stats, void *workspace, void *stream);
 
+/* ---- The trainer's MultiPoseLoss: normalised once over the batch, with its gradient ----
+ * The heads, targets and gradients the LOSS gates leave out may be NULL: reg unless reg_offset, hm_hp unless hm_hp,
+ * hp_offset / hp_ind / hp_mask unless reg_hp_offset (the keys the training batch leaves out), and a head map or
+ * gradient of a term whose weight is not > 0.  1 <= B <= 65535.  Neither direction waits on the host. */
+
+/* Workspace of cpb200_multi_pose_loss_train_batch for B images; the backward reads what the forward leaves in it. */
+size_t cpb200_multi_pose_loss_train_workspace_bytes(int B);
+
+/* MultiPoseLoss.forward on a batch of B images as tools/train.py calls it: _neg_loss's sums and positive count over
+ * the whole (B, C, R, R) map (the num_pos == 0 branch decided on the device), each regression loss divided by the
+ * batch's mask count + 1e-4.  stats (DEVICE, CPB200_LOSS_STATS fp32) in CPB200_LOSS_STATS order; loss (DEVICE, one
+ * fp32) is stats[0].  Sums are float64 in a fixed order, each stat is rounded to fp32 once. */
+int cpb200_multi_pose_loss_train_batch(cpb200_multi_pose_heads heads, cpb200_multi_pose_targets targets, int B, int R,
+                                       const cpb200_multi_pose_loss_cfg *cfg, float *stats, float *loss,
+                                       void *workspace, void *stream);
+
+/* d (grad_loss * loss) / d head of the last cpb200_multi_pose_loss_train_batch on the same arguments and workspace,
+ * written into grads (DEVICE, (B,C,R,R) fp32 like the heads; the struct's maps are written).  grad_loss is DEVICE,
+ * one fp32.  hm and hm_hp: torch's autograd chain of the clamped logistic and _neg_loss, element by element.  The
+ * regression maps: sign(pred * m - t * m) * m * grad_loss * weight / (sum(m) + 1e-4) at each gathered entry, 0
+ * elsewhere; the entries meeting at one pixel are counted, so the result is the same bits on every run. */
+int cpb200_multi_pose_loss_train_backward(cpb200_multi_pose_heads heads, cpb200_multi_pose_targets targets, int B,
+                                          int R, const cpb200_multi_pose_loss_cfg *cfg, const float *grad_loss,
+                                          const void *workspace, cpb200_multi_pose_heads grads, void *stream);
+
 /* max(0, int(gaussian_radius((h, w)))) of lib/utils/image.py for n (h, w) int pairs (DEVICE memory), as the targets
  * kernel computes it.  For tests. */
 int cpb200_gaussian_radius(const int *hw, int n, int *radius, void *stream);
