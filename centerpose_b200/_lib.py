@@ -136,6 +136,13 @@ def lib() -> ctypes.CDLL:
     L.cpb200_multi_pose_loss_train_backward.argtypes = [Heads, Targets, ctypes.c_int, ctypes.c_int,
                                                         ctypes.POINTER(LossCfg), ctypes.c_void_p, ctypes.c_void_p,
                                                         Heads, ctypes.c_void_p]
+    L.cpb200_dcn_train_workspace_bytes.restype = ctypes.c_size_t
+    L.cpb200_dcn_train_workspace_bytes.argtypes = [ctypes.c_int] * 5
+    L.cpb200_dcn_train_forward.restype = ctypes.c_int
+    L.cpb200_dcn_train_forward.argtypes = [ctypes.c_void_p] * 6 + [ctypes.c_int] * 6 + [ctypes.c_void_p]
+    L.cpb200_dcn_train_backward.restype = ctypes.c_int
+    L.cpb200_dcn_train_backward.argtypes = [ctypes.c_void_p] * 10 + [ctypes.c_int] * 6 + \
+        [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
     L.cpb200_gaussian_radius.restype = ctypes.c_int
     L.cpb200_gaussian_radius.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
     _lib = L

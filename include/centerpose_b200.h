@@ -605,6 +605,33 @@ int cpb200_multi_pose_loss_train_backward(cpb200_multi_pose_heads heads, cpb200_
                                           int R, const cpb200_multi_pose_loss_cfg *cfg, const float *grad_loss,
                                           const void *workspace, cpb200_multi_pose_heads grads, void *stream);
 
+/* ---- Modulated deformable convolution (DCNv2) for training: the reference's _ext.dcn_v2_forward / _backward ----
+ * (DCNv2/src/dcn_v2.h:9-79) for 3x3 taps, stride 1, padding 1, dilation 1 and one deformable group, the only
+ * configuration the reference's backbones build.  NCHW fp32: input (B,C,H,W), weight (Co,C,3,3), bias (Co), offset
+ * (B,18,H,W) with channel 2*tap = dh and 2*tap+1 = dw, mask (B,9,H,W) (probabilities), output (B,Co,H,W).
+ * precision CPB200_DCN_TF32X3: tensor cores, each fp32 operand split into two tf32 parts (fp32-faithful over fp32's
+ * normal range); CPB200_DCN_FP32: CUDA-core fp32.  Both take every shape.  Nothing is allocated and nothing waits on
+ * the host.  The forward, grad_offset, grad_mask, grad_weight and grad_bias are the same bits on every run;
+ * grad_input is scattered with fp32 atomics. */
+#define CPB200_DCN_TF32X3 0
+#define CPB200_DCN_FP32 1
+
+/* Workspace of cpb200_dcn_train_backward (the weight gradient's split-K partials, at most 16 MiB); 0 for a bad shape. */
+size_t cpb200_dcn_train_workspace_bytes(int B, int C, int H, int W, int Co);
+
+/* output = bias + W . col(input, offset, mask), the column matrix gathered tile by tile and never stored. */
+int cpb200_dcn_train_forward(const float *input, const float *weight, const float *bias, const float *offset,
+                             const float *mask, float *output, int B, int C, int H, int W, int Co, int precision,
+                             void *stream);
+
+/* The five gradients of dcn_v2_cuda_backward for grad_output (B,Co,H,W): grad_input (zeroed here, then col2im's
+ * scatter), grad_offset and grad_mask (col2im_coord, summed over channels in a fixed order), grad_weight (sum over the
+ * batch of grad_output . columns^T, split over pixels and reduced in split order) and grad_bias. */
+int cpb200_dcn_train_backward(const float *input, const float *weight, const float *offset, const float *mask,
+                              const float *grad_output, float *grad_input, float *grad_offset, float *grad_mask,
+                              float *grad_weight, float *grad_bias, int B, int C, int H, int W, int Co, int precision,
+                              void *workspace, size_t workspace_bytes, void *stream);
+
 /* max(0, int(gaussian_radius((h, w)))) of lib/utils/image.py for n (h, w) int pairs (DEVICE memory), as the targets
  * kernel computes it.  For tests. */
 int cpb200_gaussian_radius(const int *hw, int n, int *radius, void *stream);
