@@ -1,5 +1,10 @@
 """ctypes binding of the C ABI declared in ``include/centerpose_b200.h``.
 
+The header is the only statement of the ABI: ``lib()`` binds ``restype`` and ``argtypes`` of every ``cpb200_*``
+prototype from it when the library loads, and a type the binding does not know fails the load.  ``launch`` makes
+every call that enqueues work on a stream; the queries that take none (``*_workspace_bytes``, ``launch_count``,
+``sizeof_op``, ``prepare_ops``, ``release_ops``) are plain calls on ``lib()``.
+
 The product path has NO CPU fallback: if the shared library is missing this module raises,
 and every op raises ``RuntimeError`` on non-CUDA tensors.
 """
@@ -7,9 +12,13 @@ from __future__ import annotations
 
 import ctypes
 import os
+import re
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIBPATH = os.path.join(_HERE, "lib", "libcenterpose_b200.so")
+HEADER = os.path.join(_HERE, "..", "include", "centerpose_b200.h")
 
 _lib = None
 
@@ -30,7 +39,46 @@ class LossCfg(ctypes.Structure):
     _fields_ = [(n, ctypes.c_float) for n in ("hm_weight", "wh_weight", "off_weight", "hp_weight", "hm_hp_weight")] + \
                [(n, ctypes.c_int32) for n in ("hm_hp", "reg_offset", "reg_hp_offset")]
 
-c_float_p = ctypes.c_void_p   # raw device addresses are passed as integers
+
+# the by-value types of the header; every pointer is bound as c_void_p (device addresses are passed as integers,
+# host arrays as ctypes arrays or byref), a `const char *` return as c_char_p
+_TYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "size_t": ctypes.c_size_t, "float": ctypes.c_float,
+          "double": ctypes.c_double, "unsigned long long": ctypes.c_ulonglong,
+          "cpb200_multi_pose_heads": Heads, "cpb200_multi_pose_targets": Targets}
+_PROTOTYPE = re.compile(r"(.+?)\b(cpb200_\w+)\s*\((.*)\)", re.S)
+
+
+def _ctype(fn: str, decl: str, ret: bool):
+    """The ctypes type of ``fn``'s return type or parameter declaration ``decl``."""
+    words = [w for w in decl.replace("*", " * ").split() if w != "const"]
+    if "*" in words:
+        return ctypes.c_char_p if ret and words == ["char", "*"] else ctypes.c_void_p
+    t = " ".join(words)
+    if ret and t == "void":
+        return None
+    if not ret and t not in _TYPES:
+        t = " ".join(words[:-1])           # drop the parameter's name
+    if t not in _TYPES:
+        raise TypeError(f"{fn}: type {decl.strip()!r} has no ctypes binding (include/centerpose_b200.h)")
+    return _TYPES[t]
+
+
+def signatures(text: str | None = None) -> dict:
+    """``{name: (restype, argtypes)}`` of every ``cpb200_*`` prototype of ``text`` (default: the header).  Reads no
+    library, so it also works where the library is not built."""
+    if text is None:
+        with open(HEADER) as f:
+            text = f.read()
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"^[ \t]*#[^\n]*", " ", text, flags=re.M)
+    sigs = {}
+    for stmt in re.split(r"[;{}]", text):
+        m = _PROTOTYPE.fullmatch(stmt.strip())
+        if m:
+            ret, name, params = m.groups()
+            params = [p for p in params.split(",") if p.strip() not in ("", "void")]
+            sigs[name] = (_ctype(name, ret, True), [_ctype(name, p, False) for p in params])
+    return sigs
 
 
 def lib() -> ctypes.CDLL:
@@ -42,109 +90,9 @@ def lib() -> ctypes.CDLL:
             f"centerpose_b200: CUDA library not built ({LIBPATH} missing). Run "
             "`python -m centerpose_b200.build` (needs nvcc); there is no CPU fallback.")
     L = ctypes.CDLL(LIBPATH)
-    L.cpb200_version.restype = ctypes.c_int
-    L.cpb200_last_error.restype = ctypes.c_char_p
-    L.cpb200_launch_count.restype = ctypes.c_ulonglong
-    L.cpb200_route_log_start.restype = None
-    L.cpb200_route_log_start.argtypes = []
-    L.cpb200_route_log_read.restype = ctypes.c_int
-    L.cpb200_route_log_read.argtypes = [ctypes.c_char_p, ctypes.c_size_t]
-    L.cpb200_decode_workspace_bytes.restype = ctypes.c_size_t
-    L.cpb200_decode_workspace_bytes.argtypes = [ctypes.c_int] * 3
-    L.cpb200_multi_pose_decode.restype = ctypes.c_int
-    L.cpb200_multi_pose_decode.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int] * 6 + \
-        [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
-    L.cpb200_multi_pose_decode_affine.restype = ctypes.c_int
-    L.cpb200_multi_pose_decode_affine.argtypes = [ctypes.c_void_p] * 8 + [ctypes.c_int] * 6 + \
-        [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
-    L.cpb200_sigmoid_inplace.restype = ctypes.c_int
-    L.cpb200_sigmoid_inplace.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
-    L.cpb200_flip_merge.restype = ctypes.c_int
-    L.cpb200_flip_merge.argtypes = [ctypes.c_void_p] * 8 + [ctypes.c_int] * 5 + [ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]
-    L.cpb200_pre_process.restype = ctypes.c_int
-    L.cpb200_pre_process.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_double), ctypes.c_void_p,
-                                     ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
-                                     ctypes.c_int, ctypes.c_void_p]
-    L.cpb200_pre_process_batch.restype = ctypes.c_int
-    L.cpb200_pre_process_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
-                                           ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
-                                           ctypes.c_int, ctypes.c_void_p]
-    L.cpb200_resize_linear_u8_batch.restype = ctypes.c_int
-    L.cpb200_resize_linear_u8_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_jpeg_decode_batch.restype = ctypes.c_int
-    L.cpb200_jpeg_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
-                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_png_decode_batch.restype = ctypes.c_int
-    L.cpb200_png_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
-                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_png_encode_batch.restype = ctypes.c_int
-    L.cpb200_png_encode_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                          ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_webp_decode_batch.restype = ctypes.c_int
-    L.cpb200_webp_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
-                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_webp_lossless_decode_batch.restype = ctypes.c_int
-    L.cpb200_webp_lossless_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
-                                                    ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_render_poses_batch.restype = ctypes.c_int
-    L.cpb200_render_poses_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 7
-    L.cpb200_heatmap_views_batch.restype = ctypes.c_int
-    L.cpb200_heatmap_views_batch.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.POINTER(ctypes.c_float)] * 3 + \
-        [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_soft_nms_39.restype = ctypes.c_int
-    L.cpb200_soft_nms_39.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float,
-                                     ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_soft_nms_39_batch.restype = ctypes.c_int
-    L.cpb200_soft_nms_39_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
-                                           ctypes.c_float, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_coco_kp_eval_workspace_bytes.restype = ctypes.c_size_t
-    L.cpb200_coco_kp_eval_workspace_bytes.argtypes = [ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int64]
-    L.cpb200_coco_kp_oks.restype = ctypes.c_int
-    L.cpb200_coco_kp_oks.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
-                                     ctypes.c_int, ctypes.c_int, ctypes.c_int64] + [ctypes.c_void_p] * 4
-    L.cpb200_coco_kp_eval.restype = ctypes.c_int
-    L.cpb200_coco_kp_eval.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p,
-                                      ctypes.c_int, ctypes.c_int, ctypes.c_int64] + [ctypes.c_void_p] * 6
-    L.cpb200_pre_process_batch_f32.restype = ctypes.c_int
-    L.cpb200_pre_process_batch_f32.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
-                                               ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_float),
-                                               ctypes.POINTER(ctypes.c_float), ctypes.c_void_p]
-    L.cpb200_multi_pose_targets_batch.restype = ctypes.c_int
-    L.cpb200_multi_pose_targets_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
-                                                  Targets, ctypes.c_void_p]
-    L.cpb200_multi_pose_loss_workspace_bytes.restype = ctypes.c_size_t
-    L.cpb200_multi_pose_loss_workspace_bytes.argtypes = [ctypes.c_int]
-    L.cpb200_multi_pose_loss_batch.restype = ctypes.c_int
-    L.cpb200_multi_pose_loss_batch.argtypes = [Heads, Targets, ctypes.c_int, ctypes.c_int, ctypes.POINTER(LossCfg),
-                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.cpb200_multi_pose_targets_train_batch.restype = ctypes.c_int
-    L.cpb200_multi_pose_targets_train_batch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
-                                                        Targets, ctypes.c_void_p]
-    L.cpb200_train_augment_workspace_bytes.restype = ctypes.c_size_t
-    L.cpb200_train_augment_workspace_bytes.argtypes = [ctypes.c_int, ctypes.c_int]
-    L.cpb200_train_augment_batch.restype = ctypes.c_int
-    L.cpb200_train_augment_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
-                                             ctypes.c_void_p, ctypes.POINTER(ctypes.c_float),
-                                             ctypes.POINTER(ctypes.c_float), ctypes.c_void_p, ctypes.c_void_p,
-                                             ctypes.c_size_t, ctypes.c_void_p]
-    L.cpb200_multi_pose_loss_train_workspace_bytes.restype = ctypes.c_size_t
-    L.cpb200_multi_pose_loss_train_workspace_bytes.argtypes = [ctypes.c_int]
-    L.cpb200_multi_pose_loss_train_batch.restype = ctypes.c_int
-    L.cpb200_multi_pose_loss_train_batch.argtypes = [Heads, Targets, ctypes.c_int, ctypes.c_int,
-                                                     ctypes.POINTER(LossCfg)] + [ctypes.c_void_p] * 4
-    L.cpb200_multi_pose_loss_train_backward.restype = ctypes.c_int
-    L.cpb200_multi_pose_loss_train_backward.argtypes = [Heads, Targets, ctypes.c_int, ctypes.c_int,
-                                                        ctypes.POINTER(LossCfg), ctypes.c_void_p, ctypes.c_void_p,
-                                                        Heads, ctypes.c_void_p]
-    L.cpb200_dcn_train_workspace_bytes.restype = ctypes.c_size_t
-    L.cpb200_dcn_train_workspace_bytes.argtypes = [ctypes.c_int] * 5
-    L.cpb200_dcn_train_forward.restype = ctypes.c_int
-    L.cpb200_dcn_train_forward.argtypes = [ctypes.c_void_p] * 6 + [ctypes.c_int] * 6 + [ctypes.c_void_p]
-    L.cpb200_dcn_train_backward.restype = ctypes.c_int
-    L.cpb200_dcn_train_backward.argtypes = [ctypes.c_void_p] * 10 + [ctypes.c_int] * 6 + \
-        [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
-    L.cpb200_gaussian_radius.restype = ctypes.c_int
-    L.cpb200_gaussian_radius.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+    for name, (restype, argtypes) in signatures().items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = L
     return L
 
@@ -153,6 +101,16 @@ def check(status: int, what: str = "centerpose_b200"):
     if status != 0:
         msg = lib().cpb200_last_error().decode("utf-8", "replace")
         raise RuntimeError(f"{what}: {msg} (status {status})")
+
+
+def launch(name: str, device, *args) -> None:
+    """``cpb200_<name>(*args, stream)`` with ``device``'s current stream, inside a device guard.  Tensors are passed as
+    their ``data_ptr()`` and None as NULL; a non-zero status raises ``RuntimeError`` naming the entry point."""
+    fn = getattr(lib(), "cpb200_" + name)
+    args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(device):
+        st = fn(*args, torch.cuda.current_stream(device).cuda_stream)
+    check(st, "cpb200_" + name)
 
 
 def launch_count() -> int:

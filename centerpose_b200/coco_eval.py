@@ -249,12 +249,8 @@ class KeypointEval:
             return {}
         out = torch.empty(max(n_oks, 1), dtype=torch.float64, device=self.device)
         ws = self._workspace(len(evaluated), n_rows, n_keep, n_oks)
-        with torch.cuda.device(self.device):
-            st = _lib.lib().cpb200_coco_kp_oks(up.data_ptr(), len(evaluated), rows.data_ptr(), n_rows,
-                                               self.gts.data_ptr(), self.n_gts, n_keep, n_oks, ctypes.byref(self.params),
-                                               out.data_ptr(), ws.data_ptr(),
-                                               torch.cuda.current_stream(self.device).cuda_stream)
-        _lib.check(st, "coco_kp_oks")
+        _lib.launch("coco_kp_oks", self.device, up, len(evaluated), rows, n_rows, self.gts, self.n_gts, n_keep, n_oks,
+                    ctypes.byref(self.params), out, ws)
         host = out.cpu().numpy()
         res = {}
         for i, e in zip(evaluated, table):
@@ -276,13 +272,8 @@ class KeypointEval:
             out = torch.empty(2 * T * R * A + T * A, dtype=torch.float64, device=self.device)
             ws = self._workspace(len(evaluated), n_rows, n_keep, n_oks)
             p = out.data_ptr()
-            with torch.cuda.device(self.device):
-                st = _lib.lib().cpb200_coco_kp_eval(up.data_ptr(), len(evaluated), rows.data_ptr(), n_rows,
-                                                    self.gts.data_ptr(), self.n_gts, n_keep, n_oks,
-                                                    ctypes.byref(self.params), p, p + 8 * 2 * T * R * A,
-                                                    p + 8 * T * R * A, ws.data_ptr(),
-                                                    torch.cuda.current_stream(self.device).cuda_stream)
-            _lib.check(st, "coco_kp_eval")
+            _lib.launch("coco_kp_eval", self.device, up, len(evaluated), rows, n_rows, self.gts, self.n_gts, n_keep,
+                        n_oks, ctypes.byref(self.params), p, p + 8 * 2 * T * R * A, p + 8 * T * R * A, ws)
             host = out.cpu().numpy()
             precision = host[:T * R * A].reshape(T, R, 1, A, 1).copy()
             scores = host[T * R * A:2 * T * R * A].reshape(T, R, 1, A, 1).copy()

@@ -85,10 +85,6 @@ def _check_shapes(what, input, weight, bias, offset, mask, kernel_h, kernel_w):
     return B, C, H, W, Co
 
 
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
-
-
 def dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w,
                    dilation_h, dilation_w, deformable_group, *, precision="default"):
     """``_ext.dcn_v2_forward``: the (B, Co, H, W) output of the modulated deformable conv."""
@@ -101,10 +97,7 @@ def dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride
     dev = input.device
     x, w, b, o, m = (t.contiguous() for t in (input, weight, bias, offset, mask))
     out = torch.empty((B, Co, H, W), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().cpb200_dcn_train_forward(x.data_ptr(), w.data_ptr(), b.data_ptr(), o.data_ptr(),
-                                                 m.data_ptr(), out.data_ptr(), B, C, H, W, Co, code, _stream(dev))
-    _lib.check(st, "dcn_v2_forward")
+    _lib.launch("dcn_train_forward", dev, x, w, b, o, m, out, B, C, H, W, Co, code)
     return out
 
 
@@ -124,13 +117,8 @@ def dcn_v2_backward(input, weight, bias, offset, mask, grad_output, kernel_h, ke
     x, w, o, m, g = (t.contiguous() for t in (input, weight, offset, mask, grad_output))
     grads = [torch.empty_like(x), torch.empty_like(o), torch.empty_like(m), torch.empty_like(w),
              torch.empty((Co,), dtype=torch.float32, device=dev)]
-    L = _lib.lib()
-    ws = torch.empty(L.cpb200_dcn_train_workspace_bytes(B, C, H, W, Co), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        st = L.cpb200_dcn_train_backward(x.data_ptr(), w.data_ptr(), o.data_ptr(), m.data_ptr(), g.data_ptr(),
-                                         *[t.data_ptr() for t in grads], B, C, H, W, Co, code, ws.data_ptr(),
-                                         ws.numel(), _stream(dev))
-    _lib.check(st, "dcn_v2_backward")
+    ws = torch.empty(_lib.lib().cpb200_dcn_train_workspace_bytes(B, C, H, W, Co), dtype=torch.uint8, device=dev)
+    _lib.launch("dcn_train_backward", dev, x, w, o, m, g, *grads, B, C, H, W, Co, code, ws, ws.numel())
     return grads
 
 

@@ -15,8 +15,8 @@ _ws_cache = {}
 
 
 def _workspace(device, B, J, K):
-    stream = torch.cuda.current_stream(device)
-    key = (device.index, stream.cuda_stream, B, J, K)
+    """The zero-filled decode workspace of (device, current stream, B, J, K) and its cache key."""
+    key = (device.index, torch.cuda.current_stream(device).cuda_stream, B, J, K)
     ws = _ws_cache.get(key)
     if ws is None:
         nbytes = _lib.lib().cpb200_decode_workspace_bytes(B, J, K)
@@ -24,7 +24,7 @@ def _workspace(device, B, J, K):
         if len(_ws_cache) > 64:
             _ws_cache.clear()
         _ws_cache[key] = ws
-    return ws
+    return key, ws
 
 
 def _prep(t, name, shape=None):
@@ -72,24 +72,18 @@ def multi_pose_decode(heat, wh, kps, reg=None, hm_hp=None, hp_offset=None, K=100
     dev = heat.device
     if out is None:
         out = torch.empty((B, K, 5 + 3 * J), dtype=torch.float32, device=dev)
-    ws = _workspace(dev, B, J, K)
-    ptr = lambda t: None if t is None else t.data_ptr()
-    with torch.cuda.device(dev):
-        if affine is None:
-            st = _lib.lib().cpb200_multi_pose_decode(
-                ptr(heat), ptr(wh), ptr(kps), ptr(reg), ptr(hm_hp), ptr(hp_offset), out.data_ptr(),
-                B, H, W, J, K, 1 if apply_sigmoid else 0, ws.data_ptr(), ws.numel(),
-                torch.cuda.current_stream(dev).cuda_stream)
-        else:
-            affine = _prep(affine, "affine", (B, 6))
-            st = _lib.lib().cpb200_multi_pose_decode_affine(
-                ptr(heat), ptr(wh), ptr(kps), ptr(reg), ptr(hm_hp), ptr(hp_offset), affine.data_ptr(),
-                out.data_ptr(), B, H, W, J, K, 1 if apply_sigmoid else 0, ws.data_ptr(), ws.numel(),
-                torch.cuda.current_stream(dev).cuda_stream)
-    if st != 0:
+    key, ws = _workspace(dev, B, J, K)
+    if affine is None:
+        name, extra = "multi_pose_decode", ()
+    else:
+        name, extra = "multi_pose_decode_affine", (_prep(affine, "affine", (B, 6)),)
+    try:
+        _lib.launch(name, dev, heat, wh, kps, reg, hm_hp, hp_offset, *extra, out, B, H, W, J, K,
+                    1 if apply_sigmoid else 0, ws, ws.numel())
+    except RuntimeError:
         # a failed / aborted launch may leave the workspace's pair counters non-zero: never reuse it
-        _ws_cache.pop((dev.index, torch.cuda.current_stream(dev).cuda_stream, B, J, K), None)
-    _lib.check(st, "multi_pose_decode")
+        _ws_cache.pop(key, None)
+        raise
     return out
 
 
@@ -110,10 +104,7 @@ def sigmoid_(x: torch.Tensor) -> torch.Tensor:
     """In-place logistic on a CUDA fp32 tensor (``multi_pose.py:35-37`` ``hm.sigmoid_()``)."""
     if not x.is_cuda or x.dtype != torch.float32 or not x.is_contiguous():
         raise RuntimeError("sigmoid_: contiguous CUDA fp32 tensor required")
-    with torch.cuda.device(x.device):
-        st = _lib.lib().cpb200_sigmoid_inplace(x.data_ptr(), x.numel(),
-                                               torch.cuda.current_stream(x.device).cuda_stream)
-    _lib.check(st, "sigmoid_")
+    _lib.launch("sigmoid_inplace", x.device, x, x.numel())
     return x
 
 
@@ -143,11 +134,6 @@ def flip_merge(hm, wh, hps, hm_hp, flip_idx):
         raise RuntimeError("flip_merge: inconsistent head-map shapes")
     outs = [torch.empty((P,) + tuple(t.shape[1:]), dtype=torch.float32, device=hm.device) for t in tens]
     perm = (ctypes.c_int * J)(*flip_perm(flip_idx, J))
-    with torch.cuda.device(hm.device):
-        st = _lib.lib().cpb200_flip_merge(hm.data_ptr(), wh.data_ptr(), hps.data_ptr(),
-                                          hm_hp.data_ptr() if hm_hp is not None else None,
-                                          outs[0].data_ptr(), outs[1].data_ptr(), outs[2].data_ptr(),
-                                          outs[3].data_ptr() if hm_hp is not None else None,
-                                          P, H, W, J, CH, perm, torch.cuda.current_stream(hm.device).cuda_stream)
-    _lib.check(st, "flip_merge")
+    _lib.launch("flip_merge", hm.device, hm, wh, hps, hm_hp, outs[0], outs[1], outs[2],
+                outs[3] if hm_hp is not None else None, P, H, W, J, CH, perm)
     return outs[0], outs[1], outs[2], (outs[3] if hm_hp is not None else None)

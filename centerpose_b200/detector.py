@@ -113,10 +113,7 @@ class BaseDetector(object):
         host[table.nbytes:] = np.ascontiguousarray(image_u8).reshape(-1)
         buf = torch.from_numpy(host).to(dev)
         out = torch.empty((new_height, new_width, 3), dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = _lib.lib().cpb200_resize_linear_u8_batch(buf.data_ptr() + table.nbytes, buf.data_ptr(), 1, out.data_ptr(),
-                                                          torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(st, "resize_linear_u8_batch")
+        _lib.launch("resize_linear_u8_batch", dev, buf.data_ptr() + table.nbytes, buf, 1, out)
         return out
 
     def _pre_process_device(self, src, trans_input, inp_height, inp_width):
@@ -129,11 +126,8 @@ class BaseDetector(object):
         M = (ctypes.c_double * 6)(*np.asarray(trans_input, np.float64).reshape(-1))
         mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
         std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
-        with torch.cuda.device(dev):
-            st = _lib.lib().cpb200_pre_process(src.data_ptr(), src.shape[0], src.shape[1], M, out.data_ptr(),
-                                               inp_height, inp_width, mean, std, 1 if flip else 0,
-                                               torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(st, "pre_process")
+        _lib.launch("pre_process", dev, src, src.shape[0], src.shape[1], M, out, inp_height, inp_width, mean, std,
+                    1 if flip else 0)
         return out
 
     def process(self, images, return_time=False):
@@ -381,7 +375,6 @@ def load_images_device(images):
         pos += int(np.prod(shape[n]))
     host_start = pos - sum(im.nbytes for im in host.values())
     pixels = torch.empty(max(pos, 1), dtype=torch.uint8, device=dev)
-    stream = torch.cuda.current_stream(dev).cuda_stream
     # JPEG files, then PNG files, then lossy and lossless WebP files; status[k] belongs to dec[k]
     dec = [n for fmt in (jpeg, png, webp, webp_lossless) for n in infos if infos[n][0] is fmt]
     if dec:
@@ -404,13 +397,9 @@ def load_images_device(images):
         src = up.to(dev, non_blocking=True)
         work = torch.empty(max(p[1] for p in packed), dtype=torch.uint8, device=dev)
         status = torch.empty(len(dec), dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            for (a, b), o in zip(chunks, at):
-                name = infos[dec[a]][0].KERNEL
-                st = getattr(_lib.lib(), "cpb200_" + name)(src.data_ptr() + int(o), src.data_ptr() + int(o), b - a,
-                                                          work.data_ptr(), work.numel(), pixels.data_ptr(),
-                                                          status.data_ptr() + 4 * a, stream)
-                _lib.check(st, name)
+        for (a, b), o in zip(chunks, at):
+            _lib.launch(infos[dec[a]][0].KERNEL, dev, src.data_ptr() + int(o), src.data_ptr() + int(o), b - a, work,
+                        work.numel(), pixels, status.data_ptr() + 4 * a)
     if host:
         staged = torch.empty(pos - host_start, dtype=torch.uint8, pin_memory=True)
         sv = staged.numpy()
@@ -673,7 +662,6 @@ class MultiPoseDetector(BaseDetector):
             return log, {}
         loaded, offsets, pixels = load_images_device(images)
         dev = torch.device("cuda")
-        stream = torch.cuda.current_stream(dev).cuda_stream
         res, R, K = int(cfg.MODEL.INPUT_RES), int(cfg.MODEL.OUTPUT_RES), int(cfg.TEST.TOPK)
         mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
         std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
@@ -694,10 +682,7 @@ class MultiPoseDetector(BaseDetector):
             buf = host.to(dev, non_blocking=True)
             aff = buf[at["o_aff"]:at["o_aff"] + B * 24].view(torch.float32).view(B, 6)
             inp = torch.empty((B, 3, res, res), dtype=torch.float32, device=dev)
-            with torch.cuda.device(dev):
-                st = _lib.lib().cpb200_pre_process_batch_f32(pixels.data_ptr(), buf.data_ptr(), B, inp.data_ptr(),
-                                                             res, res, mean, std, stream)
-            _lib.check(st, "pre_process_batch_f32")
+            _lib.launch("pre_process_batch_f32", dev, pixels, buf, B, inp, res, res, mean, std)
             outputs = self.model(inp)
             tg = val.targets(ev, [image_ids[i] for i in idx], shapes, cfg)
             stats[a:a + B] = val.loss(outputs, tg, cfg)
@@ -777,7 +762,6 @@ class MultiPoseDetector(BaseDetector):
             return ([],) * (1 + bool(return_images) + bool(return_heatmaps)) if return_images or return_heatmaps else []
         cfg = self.cfg
         dev = torch.device("cuda")
-        stream = torch.cuda.current_stream(dev).cuda_stream
         flip = bool(cfg.TEST.FLIP_TEST)
         K, S = int(cfg.TEST.TOPK), len(self.scales)
         mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
@@ -810,16 +794,10 @@ class MultiPoseDetector(BaseDetector):
             if at["o_rsz"] is not None:
                 # the scaled images go into a device scratch buffer, where the pre-process table points
                 scratch = torch.empty(at["scratch"], dtype=torch.uint8, device=dev)
-                with torch.cuda.device(dev):
-                    st = _lib.lib().cpb200_resize_linear_u8_batch(pixels, buf.data_ptr() + at["o_rsz"], B,
-                                                                  scratch.data_ptr(), stream)
-                _lib.check(st, "resize_linear_u8_batch")
+                _lib.launch("resize_linear_u8_batch", dev, pixels, buf.data_ptr() + at["o_rsz"], B, scratch)
                 pixels = scratch.data_ptr()
             inp = torch.empty((2 * B if flip else B, 3, inp_h, inp_w), dtype=torch.float32, device=dev)
-            with torch.cuda.device(dev):
-                st = _lib.lib().cpb200_pre_process_batch(pixels, buf.data_ptr(), B, inp.data_ptr(),
-                                                         inp_h, inp_w, mean, std, 1 if flip else 0, stream)
-            _lib.check(st, "pre_process_batch")
+            _lib.launch("pre_process_batch", dev, pixels, buf, B, inp, inp_h, inp_w, mean, std, 1 if flip else 0)
             outputs = self.model(inp)
             if flip:
                 # process()'s gating (multi_pose.py:35-53) on B [image, mirror] pairs

@@ -92,11 +92,7 @@ def launch(table, workspace_bytes, theme, mean, std, out):
     col = (ctypes.c_float * col.size)(*col)
     mean = (ctypes.c_float * 3)(*np.asarray(mean, np.float32).reshape(-1))
     std = (ctypes.c_float * 3)(*np.asarray(std, np.float32).reshape(-1))
-    with torch.cuda.device(dev):
-        st = _lib.lib().cpb200_heatmap_views_batch(buf.data_ptr(), len(table), col, mean, std,
-                                                   1 if theme == "white" else 0, out.data_ptr(), ws.data_ptr(),
-                                                   torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(st, "heatmap_views_batch")
+    _lib.launch("heatmap_views_batch", dev, buf, len(table), col, mean, std, 1 if theme == "white" else 0, out, ws)
 
 
 def download(out, offsets, shapes):

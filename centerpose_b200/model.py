@@ -201,9 +201,8 @@ class BackBoneWithHead(nn.Module):
         plan = self._plan(B, H, W, x.device)
         Ho, Wo = plan.out_shape
         outs = {name: torch.empty((B, c, Ho, Wo), dtype=torch.float32, device=x.device) for name, c in HEADS}
-        with torch.cuda.device(x.device):
-            plan.bind(x, outs)
-            plan.run(torch.cuda.current_stream(x.device).cuda_stream)
+        plan.bind(x, outs)
+        plan.run()
         return [outs[name] for name, _ in HEADS]
 
 

@@ -766,17 +766,23 @@ class Plan:
                 else:
                     self.ops[i].dst = p
 
-    def run(self, stream: int):
+    def run(self, stream: Optional[int] = None):
+        """Enqueue the program on the current stream of the plan's device, or on ``stream`` (a raw ``cudaStream_t``
+        handle of the current device) for callers that hold one."""
         L = _lib.lib()
         if not self._prepared:
-            _lib.check(L.cpb200_prepare_ops(self.ops, self.n), "prepare_ops")
+            _lib.check(L.cpb200_prepare_ops(self.ops, self.n), "cpb200_prepare_ops")
             self._prepared = True
-        _lib.check(L.cpb200_run_ops(self.ops, ctypes.c_int(self.n), ctypes.c_void_p(stream)), "run_ops")
+        if stream is None:
+            _lib.launch("run_ops", self.device, self.ops, self.n)
+        else:
+            _lib.check(L.cpb200_run_ops(self.ops, self.n, stream), "cpb200_run_ops")
 
     def profile_ops(self, stream: int, reps: int = 3):
         """CUDA-event time of every op launched ON ITS OWN (ms, best of ``reps``), after one full run has filled the buffers.
         Serialised launches on whatever the earlier ops left in the (recycled) buffers: per-op SHARES of a step and per-op
-        rates, not a step time.  Returns [(op type, flags, B, Ho, Wo, cout, cin_total, kh, kw, ms)]."""
+        rates, not a step time.  ``stream`` is the device's current stream (the events are recorded there).  Returns
+        [(op type, flags, B, Ho, Wo, cout, cin_total, kh, kw, ms)]."""
         L = _lib.lib()
         self.run(stream)
         ev0 = torch.cuda.Event(enable_timing=True); ev1 = torch.cuda.Event(enable_timing=True)
@@ -788,7 +794,7 @@ class Plan:
             best = None
             for _ in range(reps):
                 ev0.record()
-                _lib.check(L.cpb200_run_ops(one, ctypes.c_int(1), ctypes.c_void_p(stream)), "run_ops")
+                _lib.check(L.cpb200_run_ops(one, 1, stream), "cpb200_run_ops")
                 ev1.record(); ev1.synchronize()
                 t = ev0.elapsed_time(ev1)
                 best = t if best is None or t < best else best

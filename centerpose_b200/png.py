@@ -289,10 +289,7 @@ def encode_launch(table, counts, workspace_bytes, out, sizes):
     host = torch.from_numpy(table.view(np.uint8).reshape(-1).copy()).pin_memory()
     buf = host.to(dev, non_blocking=True)
     ws = torch.empty(workspace_bytes, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        st = _lib.lib().cpb200_png_encode_batch(buf.data_ptr(), len(table), *counts, ws.data_ptr(), out.data_ptr(),
-                                                sizes.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(st, ENCODE_KERNEL)
+    _lib.launch(ENCODE_KERNEL, dev, buf, len(table), *counts, ws, out, sizes)
 
 
 def download_files(out, sizes):

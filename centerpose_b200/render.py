@@ -220,11 +220,8 @@ def launch(ops, pixels=None, offsets=None, images=None):
         pixels = buf[o_img:]
     ws = torch.empty(ops.workspace_bytes, dtype=torch.uint8, device=dev)
     base = buf.data_ptr()
-    with torch.cuda.device(dev):
-        st = _lib.lib().cpb200_render_poses_batch(pixels.data_ptr(), base + at[0], len(table), base + at[1],
-                                                  base + at[2], base + at[3], base + at[4], base + at[5],
-                                                  ws.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(st, "render_poses_batch")
+    _lib.launch("render_poses_batch", dev, pixels, base + at[0], len(table), base + at[1], base + at[2], base + at[3],
+                base + at[4], base + at[5], ws)
     return pixels, offsets
 
 

@@ -67,10 +67,8 @@ def soft_nms_39_cuda(boxes, sigma: float = 0.5, Nt: float = 0.3, threshold: floa
             and boxes.is_contiguous()):
         raise ValueError("soft_nms_39_cuda expects a contiguous CUDA float32 (N, 56) tensor")
     keep = torch.zeros(1, dtype=torch.int32, device=boxes.device)
-    with torch.cuda.device(boxes.device):
-        st = _lib.lib().cpb200_soft_nms_39(boxes.data_ptr(), boxes.shape[0], float(sigma), float(Nt), float(threshold),
-                                           int(method), keep.data_ptr(), torch.cuda.current_stream(boxes.device).cuda_stream)
-    _lib.check(st, "soft_nms_39")
+    _lib.launch("soft_nms_39", boxes.device, boxes, boxes.shape[0], float(sigma), float(Nt), float(threshold),
+                int(method), keep)
     return int(keep.item())
 
 
@@ -84,9 +82,6 @@ def soft_nms_39_cuda_batch(boxes, sigma: float = 0.5, Nt: float = 0.3, threshold
             and boxes.is_contiguous()):
         raise ValueError("soft_nms_39_cuda_batch expects a contiguous CUDA float32 (B, N, 56) tensor")
     keep = torch.empty(boxes.shape[0], dtype=torch.int32, device=boxes.device)
-    with torch.cuda.device(boxes.device):
-        st = _lib.lib().cpb200_soft_nms_39_batch(boxes.data_ptr(), boxes.shape[0], boxes.shape[1], float(sigma), float(Nt),
-                                                 float(threshold), int(method), keep.data_ptr(),
-                                                 torch.cuda.current_stream(boxes.device).cuda_stream)
-    _lib.check(st, "soft_nms_39_batch")
+    _lib.launch("soft_nms_39_batch", boxes.device, boxes, boxes.shape[0], boxes.shape[1], float(sigma), float(Nt),
+                float(threshold), int(method), keep)
     return keep

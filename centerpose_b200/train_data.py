@@ -202,21 +202,13 @@ class TrainData:
         up = host.to(dev, non_blocking=True)
         if self._plan is None or self._plan.device != dev:
             self._plan = torch.from_numpy(mean_plan(S * S)).to(dev)
-        L = _lib.lib()
-        stream = torch.cuda.current_stream(dev).cuda_stream
         inp = torch.empty((B, 3, S, S), dtype=torch.float32, device=dev)
-        ws = torch.empty(L.cpb200_train_augment_workspace_bytes(B, S), dtype=torch.uint8, device=dev)
+        ws = torch.empty(_lib.lib().cpb200_train_augment_workspace_bytes(B, S), dtype=torch.uint8, device=dev)
         mean = (ctypes.c_float * 3)(*np.asarray(cfg.DATASET.MEAN, np.float32))
         std = (ctypes.c_float * 3)(*np.asarray(cfg.DATASET.STD, np.float32))
         tg = {name: torch.empty((B,) + shape(R), dtype=dt, device=dev) for name, dt, shape in val.TARGETS}
-        with torch.cuda.device(dev):
-            st = L.cpb200_train_augment_batch(pixels.data_ptr(), up.data_ptr(), B, S, self._plan.data_ptr(), mean, std,
-                                              inp.data_ptr(), ws.data_ptr(), ws.numel(), stream)
-            _lib.check(st, "train_augment_batch")
-            st = L.cpb200_multi_pose_targets_train_batch(up.data_ptr(), B, ev.gts.data_ptr(), R,
-                                                         val._pointers(_lib.Targets, tg, [n for n, _, _ in val.TARGETS]),
-                                                         stream)
-            _lib.check(st, "multi_pose_targets_train_batch")
+        _lib.launch("train_augment_batch", dev, pixels, up, B, S, self._plan, mean, std, inp, ws, ws.numel())
+        _lib.launch("multi_pose_targets_train_batch", dev, up, B, ev.gts, R, val.targets_struct(tg))
         out = {"input": inp}
         for k in ("hm", "reg_mask", "ind", "wh", "hps", "hps_mask"):
             out[k] = tg[k]

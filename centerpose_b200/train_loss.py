@@ -40,27 +40,17 @@ def head_gates(cfg):
             bool(c.HM_HP) and c.HM_HP_WEIGHT > 0, bool(c.REG_HP_OFFSET) and c.OFF_WEIGHT > 0)
 
 
-def _targets_struct(batch, keys):
-    from . import _lib
-    return _lib.Targets(*[batch[n].data_ptr() if n in keys else None for n, _, _ in val.TARGETS])
-
-
 class _Loss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, loss_cfg, gates, batch, hm, wh, hps, reg, hm_hp, hp_offset):
         from . import _lib
         heads = (hm, wh, hps, reg, hm_hp, hp_offset)
         B, R, dev = hm.shape[0], hm.shape[-1], hm.device
-        L = _lib.lib()
-        ws = torch.empty(L.cpb200_multi_pose_loss_train_workspace_bytes(B), dtype=torch.uint8, device=dev)
+        ws = torch.empty(_lib.lib().cpb200_multi_pose_loss_train_workspace_bytes(B), dtype=torch.uint8, device=dev)
         stats = torch.empty(len(val.STATS), dtype=torch.float32, device=dev)
         loss = torch.empty((), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            st = L.cpb200_multi_pose_loss_train_batch(
-                _lib.Heads(*[h.data_ptr() for h in heads]), _targets_struct(batch, batch.keys()), B, R,
-                ctypes.byref(loss_cfg), stats.data_ptr(), loss.data_ptr(), ws.data_ptr(),
-                torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(st, "multi_pose_loss_train_batch")
+        _lib.launch("multi_pose_loss_train_batch", dev, _lib.Heads(*[h.data_ptr() for h in heads]),
+                    val.targets_struct(batch), B, R, ctypes.byref(loss_cfg), stats, loss, ws)
         ctx.save_for_backward(*heads)
         ctx.loss_cfg, ctx.gates, ctx.batch, ctx.ws = loss_cfg, gates, batch, ws
         ctx.mark_non_differentiable(stats)
@@ -74,13 +64,9 @@ class _Loss(torch.autograd.Function):
         B, R, dev = hm.shape[0], hm.shape[-1], hm.device
         g = grad_loss.to(device=dev, dtype=torch.float32).contiguous()
         grads = [torch.empty_like(h) if on else None for h, on in zip(heads, ctx.gates)]
-        with torch.cuda.device(dev):
-            st = _lib.lib().cpb200_multi_pose_loss_train_backward(
-                _lib.Heads(*[h.data_ptr() for h in heads]), _targets_struct(ctx.batch, ctx.batch.keys()), B, R,
-                ctypes.byref(ctx.loss_cfg), g.data_ptr(), ctx.ws.data_ptr(),
-                _lib.Heads(*[x.data_ptr() if x is not None else None for x in grads]),
-                torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(st, "multi_pose_loss_train_backward")
+        _lib.launch("multi_pose_loss_train_backward", dev, _lib.Heads(*[h.data_ptr() for h in heads]),
+                    val.targets_struct(ctx.batch), B, R, ctypes.byref(ctx.loss_cfg), g, ctx.ws,
+                    _lib.Heads(*[x.data_ptr() if x is not None else None for x in grads]))
         return (None, None, None) + tuple(grads)
 
 

@@ -78,8 +78,11 @@ def image_table(ev, image_ids, shapes, R):
     return t
 
 
-def _pointers(struct, tensors, names):
-    return struct(*[tensors[n].data_ptr() for n in names])
+def targets_struct(tensors):
+    """The ``cpb200_multi_pose_targets`` of the dict ``tensors`` under :data:`TARGETS`' names; a name it lacks is
+    NULL."""
+    from . import _lib
+    return _lib.Targets(*[tensors[n].data_ptr() if n in tensors else None for n, _, _ in TARGETS])
 
 
 def targets(ev, image_ids, shapes, cfg):
@@ -94,11 +97,7 @@ def targets(ev, image_ids, shapes, cfg):
     if B == 0:
         return out
     up = torch.from_numpy(table.view(np.uint8).reshape(-1).copy()).to(ev.device)
-    with torch.cuda.device(ev.device):
-        st = _lib.lib().cpb200_multi_pose_targets_batch(up.data_ptr(), B, ev.gts.data_ptr(), R,
-                                                        _pointers(_lib.Targets, out, [n for n, _, _ in TARGETS]),
-                                                        torch.cuda.current_stream(ev.device).cuda_stream)
-    _lib.check(st, "multi_pose_targets_batch")
+    _lib.launch("multi_pose_targets_batch", ev.device, up, B, ev.gts, R, targets_struct(out))
     return out
 
 
@@ -141,13 +140,8 @@ def loss(outputs, targets, cfg):
     hm = heads[0]
     B, R = hm.shape[0], hm.shape[-1]
     stats = torch.empty((B, len(STATS)), dtype=torch.float32, device=hm.device)
-    L = _lib.lib()
-    ws = torch.empty(max(L.cpb200_multi_pose_loss_workspace_bytes(B), 1), dtype=torch.uint8, device=hm.device)
+    ws = torch.empty(max(_lib.lib().cpb200_multi_pose_loss_workspace_bytes(B), 1), dtype=torch.uint8, device=hm.device)
     cfg_c = loss_cfg(cfg)
-    with torch.cuda.device(hm.device):
-        st = L.cpb200_multi_pose_loss_batch(
-            _lib.Heads(*[h.data_ptr() for h in heads]),
-            _pointers(_lib.Targets, targets, [n for n, _, _ in TARGETS]), B, R, ctypes.byref(cfg_c),
-            stats.data_ptr(), ws.data_ptr(), torch.cuda.current_stream(hm.device).cuda_stream)
-    _lib.check(st, "multi_pose_loss_batch")
+    _lib.launch("multi_pose_loss_batch", hm.device, _lib.Heads(*[h.data_ptr() for h in heads]), targets_struct(targets),
+                B, R, ctypes.byref(cfg_c), stats, ws)
     return stats

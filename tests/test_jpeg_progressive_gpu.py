@@ -8,7 +8,7 @@ import torch
 
 from centerpose_b200 import jpeg
 from tests.test_jpeg_cpu import CONTENTS, QUALITIES, SAMPLINGS, SIZES, cv2_decode, encode, make_image, with_exif
-from tests.test_jpeg_gpu import COCO, _detector, _launch
+from tests.test_jpeg_gpu import COCO, _detector
 from tests.test_jpeg_progressive_cpu import RESTARTS, _sos, penc
 
 pytestmark = pytest.mark.gpu
@@ -27,8 +27,7 @@ def _decode(datas):
     ws = torch.full((ws_bytes,), 0x55, dtype=torch.uint8, device="cuda")      # the kernel must zero the blocks itself
     dst = torch.full((int(offs[-1]) + 256,), 77, dtype=torch.uint8, device="cuda")
     status = torch.full((len(datas),), -1, dtype=torch.int32, device="cuda")
-    _lib.check(_launch(src.data_ptr(), src.data_ptr(), len(datas), ws.data_ptr(), ws_bytes, dst.data_ptr(),
-                       status.data_ptr()), "jpeg_decode_batch")
+    _lib.launch("jpeg_decode_batch", src.device, src, src, len(datas), ws, ws_bytes, dst, status)
     out = dst.cpu().numpy()
     assert (out[offs[-1]:] == 77).all()
     return [out[offs[n]:offs[n + 1]].reshape(i.oh, i.ow, 3) for n, i in enumerate(infos)], status.cpu().numpy()

@@ -44,9 +44,7 @@ def _pre_single(img, t, OH, OW, flip):
     buf, out = _guarded(n)
     M = (ctypes.c_double * 6)(*np.asarray(t, np.float64).reshape(6))
     mean, std = _mean_std()
-    st = _lib.lib().cpb200_pre_process(src.data_ptr(), img.shape[0], img.shape[1], M, out.data_ptr(), OH, OW, mean, std,
-                                       1 if flip else 0, torch.cuda.current_stream().cuda_stream)
-    _lib.check(st, "pre_process")
+    _lib.launch("pre_process", DEV, src, img.shape[0], img.shape[1], M, out, OH, OW, mean, std, 1 if flip else 0)
     torch.cuda.synchronize()
     _check_guards(buf, n)
     return out.view(-1, 3, OH, OW).cpu()
@@ -65,9 +63,7 @@ def _pre_batch(images, trans, OH, OW, flip):
     n = (2 if flip else 1) * len(images) * 3 * OH * OW
     buf, out = _guarded(n)
     mean, std = _mean_std()
-    st = _lib.lib().cpb200_pre_process_batch(pix.data_ptr(), tab.data_ptr(), len(images), out.data_ptr(), OH, OW, mean,
-                                             std, 1 if flip else 0, torch.cuda.current_stream().cuda_stream)
-    _lib.check(st, "pre_process_batch")
+    _lib.launch("pre_process_batch", DEV, pix, tab, len(images), out, OH, OW, mean, std, 1 if flip else 0)
     torch.cuda.synchronize()
     _check_guards(buf, n)
     return out.view(-1, 3, OH, OW).cpu()
@@ -104,10 +100,7 @@ def test_flip_merge_equals_restatement(label):
     P = case.P
     outs = [torch.full((P,) + tuple(m.shape[1:]), CANARY, device=DEV) if m is not None else None for m in dev]
     perm = (ctypes.c_int * case.J)(*case.perm)
-    st = _lib.lib().cpb200_flip_merge(*[m.data_ptr() if m is not None else None for m in dev],
-                                      *[o.data_ptr() if o is not None else None for o in outs],
-                                      P, case.H, case.W, case.J, case.CH, perm, torch.cuda.current_stream().cuda_stream)
-    _lib.check(st, "flip_merge")
+    _lib.launch("flip_merge", DEV, *dev, *outs, P, case.H, case.W, case.J, case.CH, perm)
     for name, g, w in zip(("hm", "wh", "hps", "hm_hp"), outs, want):
         assert (g is None) == (w is None)
         if g is not None:

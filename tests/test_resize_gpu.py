@@ -25,7 +25,7 @@ def _resize_batch(images, new_shapes):
     tab = torch.from_numpy(table.view(np.uint8).copy()).cuda()
     total = sum(h * w * 3 for h, w in new_shapes)
     dst = torch.full((total + 256,), 77, dtype=torch.uint8, device="cuda")
-    _lib.check(_launch(src.data_ptr(), tab.data_ptr(), len(images), dst.data_ptr()), "resize_linear_u8_batch")
+    _lib.launch("resize_linear_u8_batch", dst.device, src, tab, len(images), dst)
     out = dst.cpu().numpy()
     assert (out[total:] == 77).all()
     return [out[e["dst_offset"]:e["dst_offset"] + e["new_h"] * e["new_w"] * 3].reshape(e["new_h"], e["new_w"], 3)

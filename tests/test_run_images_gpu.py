@@ -51,9 +51,7 @@ def _pre_process_batch(det, images, trans, inp_h, inp_w, flip):
     tab = torch.from_numpy(table.view(np.uint8).copy()).cuda()
     out = torch.full(((2 if flip else 1) * len(images), 3, inp_h, inp_w), float("nan"), device="cuda")
     mean = (ctypes.c_float * 3)(*det.mean.reshape(-1)); std = (ctypes.c_float * 3)(*det.std.reshape(-1))
-    st = _lib.lib().cpb200_pre_process_batch(pix.data_ptr(), tab.data_ptr(), len(images), out.data_ptr(), inp_h, inp_w,
-                                             mean, std, 1 if flip else 0, torch.cuda.current_stream().cuda_stream)
-    _lib.check(st, "pre_process_batch")
+    _lib.launch("pre_process_batch", out.device, pix, tab, len(images), out, inp_h, inp_w, mean, std, 1 if flip else 0)
     return out
 
 

@@ -1,9 +1,7 @@
 """CPU tests of the trainer's loss: the torch restatement (oracle/train_loss_ref.py) and the float64 gradient bounds
 against the reference's MultiPoseLoss and backward (tests/golden/train_loss.npz), the settings and inputs
 ``train_loss.MultiPoseLoss`` refuses, and the C-ABI structs the new entry points take."""
-import ctypes
 import os
-import re
 
 import numpy as np
 import pytest
@@ -113,33 +111,3 @@ def test_refuses_bad_inputs():
         crit(th, tb)                                              # CPU heads
     with pytest.raises(ValueError, match="six head maps"):
         crit(th[:5], tb)
-
-
-def _struct_fields(hdr, name):
-    body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (name, name), hdr, re.S).group(1)
-    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-    fields = []
-    for decl in body.split(";"):
-        decl = re.sub(r"\bconst\b", "", decl).strip()
-        if decl:
-            fields += [re.sub(r"[\s*]", "", f) for f in decl.split(None, 1)[1].replace("*", " ").split(",")]
-    return fields
-
-
-def test_c_abi_structs_and_signatures():
-    from centerpose_b200 import _lib
-    hdr = open(os.path.join(ROOT, "include", "centerpose_b200.h")).read()
-    for cls, name in ((_lib.Heads, "cpb200_multi_pose_heads"), (_lib.Targets, "cpb200_multi_pose_targets"),
-                      (_lib.LossCfg, "cpb200_multi_pose_loss_cfg")):
-        assert [f for f, _ in cls._fields_] == _struct_fields(hdr, name), name
-    assert ctypes.sizeof(_lib.Heads) == 6 * 8 and ctypes.sizeof(_lib.Targets) == 11 * 8
-    assert ctypes.sizeof(_lib.LossCfg) == 8 * 4
-    for fn, n in (("cpb200_multi_pose_loss_train_batch", 9), ("cpb200_multi_pose_loss_train_backward", 9),
-                  ("cpb200_multi_pose_loss_train_workspace_bytes", 1)):
-        decl = re.search(r"\b%s\((.*?)\);" % fn, hdr, re.S).group(1)
-        assert len(decl.split(",")) == n, fn
-    if os.path.exists(_lib.LIBPATH):
-        L = _lib.lib()
-        assert len(L.cpb200_multi_pose_loss_train_batch.argtypes) == 9
-        assert len(L.cpb200_multi_pose_loss_train_backward.argtypes) == 9
-        assert L.cpb200_multi_pose_loss_train_workspace_bytes(32) == 8 * 3 * 18 * 32 + 4 * 6

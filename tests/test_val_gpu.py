@@ -50,9 +50,7 @@ def test_radius_exhaustive():
     hw = np.array([(h, w) for h in range(1, 129) for w in range(1, 129)], np.int32)
     d = torch.from_numpy(hw).cuda()
     out = torch.empty(len(hw), dtype=torch.int32, device="cuda")
-    st = _lib.lib().cpb200_gaussian_radius(d.data_ptr(), len(hw), out.data_ptr(),
-                                           torch.cuda.current_stream().cuda_stream)
-    _lib.check(st, "gaussian_radius")
+    _lib.launch("gaussian_radius", d.device, d, len(hw), out)
     want = np.array([val_ref.radius(int(h), int(w)) for h, w in hw], np.int32)
     np.testing.assert_array_equal(out.cpu().numpy(), want)
     assert want.max() == 34
@@ -125,10 +123,8 @@ def test_pre_process_f32_equals_dataset_normalisation():
     out = torch.empty((len(images), 3, res, res), dtype=torch.float32, device="cuda")
     mean = (ctypes.c_float * 3)(*np.float32(cfg.DATASET.MEAN))
     std = (ctypes.c_float * 3)(*np.float32(cfg.DATASET.STD))
-    st = _lib.lib().cpb200_pre_process_batch_f32(buf.data_ptr() + at["o_img"], buf.data_ptr(), len(images),
-                                                 out.data_ptr(), res, res, mean, std,
-                                                 torch.cuda.current_stream().cuda_stream)
-    _lib.check(st, "pre_process_batch_f32")
+    _lib.launch("pre_process_batch_f32", out.device, buf.data_ptr() + at["o_img"], buf, len(images), out, res, res, mean,
+                std)
     got = out.cpu().numpy()
     for n, (im, t) in enumerate(zip(images, trans)):
         want = np.ascontiguousarray(val_ref.inputs(im, t, res, cfg.DATASET.MEAN, cfg.DATASET.STD))

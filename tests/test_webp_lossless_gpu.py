@@ -42,8 +42,7 @@ def _decode(datas):
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda")
     dst = torch.full((int(offs[-1]) + 256,), 77, dtype=torch.uint8, device="cuda")
     status = torch.full((len(datas),), -1, dtype=torch.int32, device="cuda")
-    _lib.check(_launch(src.data_ptr(), src.data_ptr(), len(datas), ws.data_ptr(), ws_bytes, dst.data_ptr(),
-                       status.data_ptr()), "webp_lossless_decode_batch")
+    _lib.launch("webp_lossless_decode_batch", src.device, src, src, len(datas), ws, ws_bytes, dst, status)
     out = dst.cpu().numpy()
     assert (out[offs[-1]:] == 77).all()
     return [out[offs[n]:offs[n + 1]].reshape(i.oh, i.ow, 3) for n, i in enumerate(infos)], status.cpu().numpy()

@@ -33,15 +33,14 @@ def op_bytes(o):
     return 4 * (o.B * o.H * o.W * cin + n_out + extra)
 
 
-def time_op(plan, i, stream, min_ms):
-    L = _lib.lib()
+def time_op(plan, i, min_ms):
     one = ctypes.cast(ctypes.addressof(plan.ops) + i * ctypes.sizeof(P.OpStruct), ctypes.POINTER(P.OpStruct))
     e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
     n = 8
     while True:
         e0.record()
         for _ in range(n):
-            _lib.check(L.cpb200_run_ops(one, ctypes.c_int(1), ctypes.c_void_p(stream)), "run_ops")
+            _lib.launch("run_ops", plan.device, one, 1)
         e1.record(); e1.synchronize()
         ms = e0.elapsed_time(e1)
         if ms >= min_ms:
@@ -71,8 +70,7 @@ def main():
     model = model.to(dev).set_precision(a.precision)
     model(synth_images(a.batch, 512, 512, 317).to(dev))
     plan = model._plan(a.batch, 512, 512, dev)
-    st = torch.cuda.current_stream().cuda_stream
-    plan.run(st)
+    plan.run()
     torch.cuda.synchronize()
     picked = [i for i in range(plan.n) if plan.ops[i].type in CLASS or (i in (1, 2) and plan.ops[i].type == P.OP_CONV)]
     print(f"{a.arch} [{a.precision}] B={a.batch}, {plan.n} ops; share = GB/s over the data-sheet {DATA_SHEET_GBS:.0f} GB/s (not measured peak)")
@@ -80,7 +78,7 @@ def main():
     n_cls = 0
     for i in picked:
         o = plan.ops[i]
-        ms, n = time_op(plan, i, st, a.min_ms)
+        ms, n = time_op(plan, i, a.min_ms)
         by = op_bytes(o)
         gbs = by / ms / 1e6
         cin = sum(o.cin[j] for j in range(o.nsrc))

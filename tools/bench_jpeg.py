@@ -82,12 +82,9 @@ def main():
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda")
     dst = torch.empty(int(offs[-1]), dtype=torch.uint8, device="cuda")
     status = torch.empty(len(datas), dtype=torch.int32, device="cuda")
-    stream = torch.cuda.current_stream().cuda_stream
 
     def launch():
-        _lib.check(_lib.lib().cpb200_jpeg_decode_batch(src.data_ptr(), src.data_ptr(), len(datas), ws.data_ptr(),
-                                                       ws_bytes, dst.data_ptr(), status.data_ptr(), stream),
-                   "jpeg_decode_batch")
+        _lib.launch("jpeg_decode_batch", src.device, src, src, len(datas), ws, ws_bytes, dst, status)
 
     launch()
     torch.cuda.synchronize()

@@ -87,22 +87,19 @@ def kernels_alone(tr, paths, ids, reps=20):
     dev = pixels.device
     up = torch.from_numpy(table.view(np.uint8).reshape(-1).copy()).to(dev)
     plan = torch.from_numpy(train_data.mean_plan(S * S)).to(dev)
-    L = _lib.lib()
     n = len(paths)
     inp = torch.empty((n, 3, S, S), dtype=torch.float32, device=dev)
-    ws = torch.empty(L.cpb200_train_augment_workspace_bytes(n, S), dtype=torch.uint8, device=dev)
+    ws = torch.empty(_lib.lib().cpb200_train_augment_workspace_bytes(n, S), dtype=torch.uint8, device=dev)
     tg = {k: torch.empty((n,) + shape(R), dtype=dt, device=dev) for k, dt, shape in val.TARGETS}
     mean = (ctypes.c_float * 3)(*np.float32(cfg.DATASET.MEAN))
     std = (ctypes.c_float * 3)(*np.float32(cfg.DATASET.STD))
-    stream = torch.cuda.current_stream().cuda_stream
-    ptrs = val._pointers(_lib.Targets, tg, [k for k, _, _ in val.TARGETS])
+    ptrs = val.targets_struct(tg)
 
     def aug():
-        _lib.check(L.cpb200_train_augment_batch(pixels.data_ptr(), up.data_ptr(), n, S, plan.data_ptr(), mean, std,
-                                                inp.data_ptr(), ws.data_ptr(), ws.numel(), stream))
+        _lib.launch("train_augment_batch", dev, pixels, up, n, S, plan, mean, std, inp, ws, ws.numel())
 
     def tgt():
-        _lib.check(L.cpb200_multi_pose_targets_train_batch(up.data_ptr(), n, tr.ev.gts.data_ptr(), R, ptrs, stream))
+        _lib.launch("multi_pose_targets_train_batch", dev, up, n, tr.ev.gts, R, ptrs)
 
     out = {}
     src_bytes = sum(int(np.prod(v.shape)) for v in loaded)

@@ -120,27 +120,23 @@ def compare(dev, ref):
 
 def kernels_alone(cfg, batch, heads, reps):
     from centerpose_b200 import _lib, val
-    from centerpose_b200.train_loss import _targets_struct, target_keys
-    L = _lib.lib()
+    from centerpose_b200.train_loss import target_keys
     B, R = heads[0].shape[0], heads[0].shape[-1]
-    ws = torch.empty(L.cpb200_multi_pose_loss_train_workspace_bytes(B), dtype=torch.uint8, device="cuda")
+    ws = torch.empty(_lib.lib().cpb200_multi_pose_loss_train_workspace_bytes(B), dtype=torch.uint8, device="cuda")
     stats = torch.empty(7, device="cuda")
     loss = torch.empty((), device="cuda")
     one = torch.ones((), device="cuda")
     grads = [torch.empty_like(h) for h in heads]
     hs = _lib.Heads(*[h.data_ptr() for h in heads])
     gs = _lib.Heads(*[g.data_ptr() for g in grads])
-    ts = _targets_struct(batch, target_keys(cfg))
+    ts = val.targets_struct({k: batch[k] for k in target_keys(cfg)})
     lc = val.loss_cfg(cfg)
-    s = torch.cuda.current_stream().cuda_stream
 
     def fwd():
-        _lib.check(L.cpb200_multi_pose_loss_train_batch(hs, ts, B, R, ctypes.byref(lc), stats.data_ptr(),
-                                                        loss.data_ptr(), ws.data_ptr(), s))
+        _lib.launch("multi_pose_loss_train_batch", one.device, hs, ts, B, R, ctypes.byref(lc), stats, loss, ws)
 
     def bwd():
-        _lib.check(L.cpb200_multi_pose_loss_train_backward(hs, ts, B, R, ctypes.byref(lc), one.data_ptr(),
-                                                           ws.data_ptr(), gs, s))
+        _lib.launch("multi_pose_loss_train_backward", one.device, hs, ts, B, R, ctypes.byref(lc), one, ws, gs)
     out = {}
     fwd()
     plane = B * R * R * 4

@@ -74,7 +74,7 @@ def kernel_times(det, ev, ds, cfg, reps=50):
     call (CUDA events around ``reps`` calls of each entry point) and the bytes each moves at least."""
     import ctypes
     from centerpose_b200 import _lib
-    L, stream = _lib.lib(), torch.cuda.current_stream().cuda_stream
+    L = _lib.lib()
     ids = [im["id"] for im in ds["images"][:32]]
     shapes = [(im["height"], im["width"]) for im in ds["images"][:32]]
     R = int(cfg.MODEL.OUTPUT_RES)
@@ -82,18 +82,17 @@ def kernel_times(det, ev, ds, cfg, reps=50):
         outputs = det.model(torch.zeros((32, 3, 512, 512), device="cuda"))
     tg = val.targets(ev, ids, shapes, cfg)
     table = torch.from_numpy(val.image_table(ev, ids, shapes, R).view(np.uint8).reshape(-1).copy()).cuda()
-    ptrs = _lib.Targets(*[tg[k].data_ptr() for k, _, _ in val.TARGETS])
+    ptrs = val.targets_struct(tg)
     heads = _lib.Heads(*[o.data_ptr() for o in outputs])
     lcfg = val.loss_cfg(cfg)
     stats = torch.empty((32, len(val.STATS)), device="cuda")
     ws = torch.empty(L.cpb200_multi_pose_loss_workspace_bytes(32), dtype=torch.uint8, device="cuda")
-    calls = {"targets": lambda: L.cpb200_multi_pose_targets_batch(table.data_ptr(), 32, ev.gts.data_ptr(), R, ptrs,
-                                                                   stream),
-             "loss": lambda: L.cpb200_multi_pose_loss_batch(heads, ptrs, 32, R, ctypes.byref(lcfg), stats.data_ptr(),
-                                                            ws.data_ptr(), stream)}
+    calls = {"targets": lambda: _lib.launch("multi_pose_targets_batch", table.device, table, 32, ev.gts, R, ptrs),
+             "loss": lambda: _lib.launch("multi_pose_loss_batch", table.device, heads, ptrs, 32, R, ctypes.byref(lcfg),
+                                         stats, ws)}
     res = {}
     for name, fn in calls.items():
-        _lib.check(fn(), name)
+        fn()
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         for _ in range(reps):

@@ -79,12 +79,9 @@ def _decode_alone(datas, batches, rounds, fmt):
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda")
         dst = torch.empty(int(offs[-1]), dtype=torch.uint8, device="cuda")
         status = torch.empty(len(sub), dtype=torch.int32, device="cuda")
-        stream = torch.cuda.current_stream().cuda_stream
 
         def launch():
-            _lib.check(getattr(_lib.lib(), "cpb200_" + fmt.KERNEL)(src.data_ptr(), src.data_ptr(), len(sub),
-                                                                   ws.data_ptr(), ws_bytes, dst.data_ptr(),
-                                                                   status.data_ptr(), stream), fmt.KERNEL)
+            _lib.launch(fmt.KERNEL, src.device, src, src, len(sub), ws, ws_bytes, dst, status)
 
         launch()
         torch.cuda.synchronize()

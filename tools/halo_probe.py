@@ -1,5 +1,4 @@
 """Run the wgmma halo-descriptor probe (see csrc/probe.cu) and report which variant is exact."""
-import ctypes
 import json
 import os
 import sys
@@ -11,8 +10,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from centerpose_b200 import _lib
 
 L = _lib.lib()
-L.cpb200_probe_halo.restype = ctypes.c_int
-L.cpb200_probe_halo.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
 g = torch.Generator().manual_seed(1)
 x = torch.randint(-4, 5, (1, 64, 18, 10), generator=g).float()
 w = torch.randint(-2, 3, (64, 64, 3, 3), generator=g).float()

@@ -17,13 +17,12 @@ for act in (None, "relu", "hswish", "hsigmoid"):
     xin = torch.randn(B, hw, hw, ci, generator=g).to(dev, adt)
     y = pb.conv([pb.external(xin)], torch.randn(co, ci, 1, 1, generator=g).to(dev) * 0.05, torch.zeros(co, device=dev), act=act)
     plan = pb.build()
-    st = torch.cuda.current_stream().cuda_stream
     for _ in range(2):
-        plan.run(st)
+        plan.run()
     torch.cuda.synchronize()
     e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(5):
-        plan.run(st)
+        plan.run()
     e1.record(); torch.cuda.synchronize()
     print(f"PROFACT [{prec}] act={act}: {e0.elapsed_time(e1) / 5 * 1e3:.1f} us")

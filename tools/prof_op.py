@@ -101,15 +101,14 @@ def main():
     plan = pb.build()
     outs = {"o": torch.empty(B, 34, 128, 128, device=dev)} if spec[0] == "conv" and spec[2] == 34 else {}
     plan.bind(x if spec[0] == "stem" else torch.zeros(1, device=dev), outs)
-    st = torch.cuda.current_stream().cuda_stream
     which = int(os.environ.get("PROF_OP_INDEX", "-1"))     # dcn: 0 = offset conv, 1 = DCN itself
     for _ in range(2):
-        plan.run(st)
+        plan.run()
     torch.cuda.synchronize()
     e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(reps):
-        plan.run(st)
+        plan.run()
     e1.record(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / reps
     print(f"PROFOP {name} [{prec}]: {ms * 1e3:.1f} us per plan run ({plan.n} ops), {flops / ms / 1e9:.1f} TFLOP/s on the main op's flops")

@@ -1,6 +1,5 @@
 """TMA box-shape throughput (see csrc/probe.cu::probe_tma_kernel): how fast can one SM's TMA unit bring
 boxes of a given shape into shared memory?  Prints GB/s (box bytes, incl. halo over-fetch) and ns per box."""
-import ctypes
 import os
 import sys
 
@@ -10,8 +9,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from centerpose_b200 import _lib
 
 L = _lib.lib()
-L.cpb200_probe_tma.restype = ctypes.c_int
-L.cpb200_probe_tma.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 9 + [ctypes.c_void_p]
 CASES = [
     # C, W, H, N, box_w, box_h, step_w, step_h, stages
     (64, 128, 128, 32, 16, 8, 16, 8, 4), (64, 128, 128, 32, 10, 18, 8, 16, 3), (64, 128, 128, 32, 10, 18, 8, 16, 6),
