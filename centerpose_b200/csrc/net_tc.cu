@@ -21,6 +21,13 @@
 //
 // Split-operand precisions (P = 2, CPB200_BF16X2 / CPB200_F16X2, see tc_common.cuh): a stage is
 // [A_hi | A_lo | W_hi | W_lo]; per stage the consumers issue the three products of every K step (tc::mma_stage).  The DCN gather blends the four corners of BOTH planes in fp32 and re-splits the sample.
+//
+// Pointwise convs (pw_eligible: 1x1 / stride 1 / pad 0 with an NHWC output) run as one 1 x (B*H*W) "image": a tile is 128
+// consecutive pixels of the flattened map (TH 1 x TW 128, one 2-D box per K slab), the ring fills the whole opt-in shared
+// memory so that several tiles of A stay in flight across an epilogue, and the epilogue stores 16 bytes per lane and
+// plane (TcArgs::vec8: tc::quad_rows8 + tc::epilogue_vec8).  The products and the epilogue arithmetic are the same as
+// with 2-D tiles, so the outputs are too; CPB200_NO_PW=1 (read at prepare) keeps these ops on 2-D tiles.
+#include <cstdlib>
 #include <type_traits>
 #include "tc_common.cuh"
 #include <mutex>
@@ -31,6 +38,7 @@ namespace {
 constexpr int CONS_THREADS = 256;      // two consumer warpgroups
 constexpr int TC_THREADS = CONS_THREADS + 32;        // + TMA producer warp
 constexpr int TILE_M = 128;
+constexpr int MAX_STAGES = 16;
 
 struct alignas(64) TcArgs {
   CUtensorMap amap[4];
@@ -59,6 +67,7 @@ struct alignas(64) TcArgs {
   long long dst_plane;            // elements between the hi and lo planes of dst / res
   long long src_plane;            // DCN: elements between the planes of dcn_src
   int wplane;                     // weight blocks (tap x K-slab) per plane
+  unsigned vec8;                  // 16-byte epilogue (pointwise convs: NHWC output, cout % 16 == 0, 16-byte aligned dst / res)
 };
 
 using namespace tc;
@@ -77,9 +86,9 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_bytes = TILE_M * a.BK * 2, b_bytes = BN * a.BK * 2;
   const uint32_t stage_bytes = P * a_bytes + ((P * b_bytes + 1023u) & ~1023u);
-  __shared__ __align__(8) uint64_t bars[2 * 8];
+  __shared__ __align__(8) uint64_t bars[2 * MAX_STAGES];
   __shared__ DcnPrm s_prm[DCN ? DCN_GW : 1][DCN ? 9 : 1][DCN ? DCN_ROWS : 1];
-  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[8]);
+  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[MAX_STAGES]);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == CONS_THREADS) {
@@ -382,6 +391,29 @@ __global__ void __launch_bounds__(DCN ? DCN_THREADS : TC_THREADS, 1) conv_tc_ker
       if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
       int n, h0, w0, nt; decode_tile(tt, n, h0, w0, nt);
       const int n0 = nt * BN;
+      if (a.vec8) {
+        // after quad_rows8, lane q owns row r0 + 8 (q & 1) and 8-column block q >> 1 of each 16-column group
+        const int q = t & 3, row = wg * 64 + frag_row(t, q & 1);
+        const int ho = h0 + row / a.TW, wo = w0 + row % a.TW;
+        const int pix = ho < a.Ho && wo < a.Wo ? (n * a.Hd + ho) * a.Wd + wo : -1;     // < 2^31: pw_eligible
+#pragma unroll
+        for (int g = 0; g < BN / 16; ++g) {
+          float2 v[4];
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {                   // registers 8g + 2u, +1: row r0 + 8 (u & 1), block 2g + (u >> 1)
+            const int r = 8 * g + 2 * u, c = n0 + 16 * g + 8 * (u >> 1) + 2 * (t & 3);
+            const bool hb = a.bias && c < a.cout;         // cout % 16 == 0: c < cout implies c + 1 < cout
+            const float b0 = hb ? __ldg(a.bias + c) : 0.f, b1 = hb ? __ldg(a.bias + c + 1) : 0.f;
+            if constexpr (P == 2) v[u] = make_float2(fmaf(acc[r] + acc2[r], a.acc_scale, b0), fmaf(acc[r + 1] + acc2[r + 1], a.acc_scale, b1));
+            else v[u] = make_float2(acc[r] + b0, acc[r + 1] + b1);
+          }
+          quad_rows8(v, q);
+          const int c = n0 + 16 * g + 8 * (q >> 1);
+          if (pix < 0 || c >= a.cout) continue;
+          epilogue_vec8<P>(v, act, form, a.dst, a.res, (size_t)pix * a.cout_store + c, a.dst_plane, a.fmt);
+        }
+        continue;
+      }
 #pragma unroll
       for (int j = 0; j < BN / 4; ++j) {                   // pairs of adjacent columns of this thread's fragment
         const int row = wg * 64 + frag_row(t, j), nb = n0 + frag_col(t, j);
@@ -498,6 +530,16 @@ int encode_weight_map(CUtensorMap *map, const void *w, uint32_t fmt, int bk, int
 
 namespace cpb {
 
+// CPB200_NO_PW=1 keeps pointwise convs on 2-D tiles (read when the program is prepared): both compute the same bits, so
+// tests and timings can compare them in one process.
+static bool pw_eligible(const cpb200_op &op) {
+  if (const char *e = getenv("CPB200_NO_PW")) if (e[0] == '1') return false;
+  if (op.type != CPB200_OP_CONV || op.kh != 1 || op.kw != 1 || op.stride != 1 || op.pad_h != 0 || op.pad_w != 0) return false;
+  if (op.out_sy != 1 || op.out_sx != 1 || op.out_oy != 0 || op.out_ox != 0 || op.Hd != op.Ho || op.Wd != op.Wo) return false;
+  if (op.H != op.Ho || op.W != op.Wo || (op.flags & CPB200_FLAG_OUT_NCHW_F32) || op.cout % 16) return false;
+  return (long long)op.B * op.Ho * op.Wo < (1LL << 31);
+}
+
 int tap_prepare(const cpb200_op &op, Prepared **out) {
   const bool dcn = op.type == CPB200_OP_DCN;
   if (op.type != CPB200_OP_CONV && !dcn) return fail(CPB200_ERR_ARG, "tc: only CONV / DCN ops run on the tensor-core path");
@@ -523,13 +565,16 @@ int tap_prepare(const cpb200_op &op, Prepared **out) {
   // the bf16 gather builds its corner offsets in elements as signed ints: B*H*W*Cin must stay below 2^31
   if (dcn && P == 1 && src_plane >= (1LL << 31))
     return fail(CPB200_ERR_ARG, "tc: bf16 DCN input must stay below 2^31 elements (32-bit gather offsets)");
+  const bool pw = !dcn && pw_eligible(op);
   int BN = bn_for(op.cout, P);
   // DCN: the gather warps leave 120 registers per thread, so a consumer holds at most 64 accumulator registers
   if (dcn && BN > 128 / P) BN = 128 / P;
   const size_t a_bytes = (size_t)P * TILE_M * bk * 2, b_bytes = ((size_t)P * BN * bk * 2 + 1023) / 1024 * 1024;
-  const size_t budget = dcn ? 176 * 1024 : 200 * 1024;     // the DCN variant keeps 37 KB of sampling parameters in static smem
+  // the DCN variant keeps 37 KB of sampling parameters in static smem; a pointwise conv takes the whole opt-in 227 KB
+  // (less the alignment pad): every stage more is one more K block of A in flight across an epilogue
+  const size_t budget = dcn ? 176 * 1024 : pw ? 226 * 1024 : 200 * 1024;
   int stages = (int)(budget / (a_bytes + b_bytes));
-  if (stages > 8) stages = 8;
+  if (stages > (pw ? MAX_STAGES : 8)) stages = pw ? MAX_STAGES : 8;
   if (dcn && stages > 4) stages = 4;      // leave the rest of the 256 KB to L1: the 9 taps x 4 corners re-read one ~30 KB footprint
   if (stages < 2) return fail(CPB200_ERR_ARG, "tc: tile does not fit shared memory");
 
@@ -544,14 +589,21 @@ int tap_prepare(const cpb200_op &op, Prepared **out) {
   a.kh = op.kh; a.kw = op.kw; a.stride = op.stride; a.pad_h = op.pad_h; a.pad_w = op.pad_w;
   a.B = op.B; a.Ho = op.Ho; a.Wo = op.Wo;
   a.TW = op.Wo >= 16 ? 16 : 8; a.TH = TILE_M / a.TW;
-  a.tiles_h = (op.Ho + a.TH - 1) / a.TH; a.tiles_w = (op.Wo + a.TW - 1) / a.TW;
+  a.Hd = op.Hd; a.Wd = op.Wd;
+  int map_w = op.W, map_h = op.H;
+  if (pw) {                 // one 1 x (B*H*W) image of 1 x 128 tiles
+    a.B = 1; a.Ho = a.Hd = map_h = 1; a.Wo = a.Wd = map_w = op.B * op.Ho * op.Wo;
+    a.TW = TILE_M; a.TH = 1;
+    a.vec8 = 1;
+  }
+  a.tiles_h = (a.Ho + a.TH - 1) / a.TH; a.tiles_w = (a.Wo + a.TW - 1) / a.TW;
   a.dcn_src = static_cast<const __nv_bfloat16 *>(op.src[0]);
   a.H = op.H; a.W = op.W; a.om_pitch = op.aux_pitch > 0 ? op.aux_pitch : 27;
-  a.Hd = op.Hd; a.Wd = op.Wd; a.sy = op.out_sy; a.sx = op.out_sx; a.oy = op.out_oy; a.ox = op.out_ox;
+  a.sy = op.out_sy; a.sx = op.out_sx; a.oy = op.out_oy; a.ox = op.out_ox;
   a.n_tiles = (op.cout + BN - 1) / BN;
   a.cout = op.cout; a.cout_store = op.cout;
   a.out_ch_off = op.out_ch_off; a.out_ch_total = op.out_ch_total;
-  a.total_tiles = op.B * a.tiles_h * a.tiles_w * a.n_tiles;
+  a.total_tiles = a.B * a.tiles_h * a.tiles_w * a.n_tiles;
   a.flags = op.flags;
   a.dst_plane = (long long)op.B * op.Hd * op.Wd * op.cout;
   a.src_plane = src_plane;
@@ -560,8 +612,8 @@ int tap_prepare(const cpb200_op &op, Prepared **out) {
     // a channel slice of a wider tensor: op.src[s] already points at the slice
     const cuuint32_t box[4] = {(cuuint32_t)bk, (cuuint32_t)(a.TW * op.stride), (cuuint32_t)(a.TH * op.stride), 1};
     const cuuint32_t estr[4] = {1, (cuuint32_t)op.stride, (cuuint32_t)op.stride, 1};
-    if (int rc = encode_act_map(&a.amap[s], op.src[s], op.cin[s], op.src_pitch[s] > 0 ? op.src_pitch[s] : op.cin[s], op.W, op.H,
-                                op.B, P, pr.fmt, sl.swizzle, box, estr, "tc"))
+    if (int rc = encode_act_map(&a.amap[s], op.src[s], op.cin[s], op.src_pitch[s] > 0 ? op.src_pitch[s] : op.cin[s], map_w, map_h,
+                                a.B, P, pr.fmt, sl.swizzle, box, estr, "tc"))
       return rc;
   }
   if (int rc = encode_weight_map(&a.bmap, op.weight, pr.fmt, bk, (op.cout + 15) / 16 * 16, BN, (long long)P * a.wplane, sl.swizzle, "tc"))
@@ -576,6 +628,8 @@ int tap_run(const Prepared &p, const cpb200_op &op, cudaStream_t st) {
   TcArgs args = t.args;
   args.dst = op.dst; args.res = op.res; args.bias = op.bias;
   args.dcn_om = static_cast<const float *>(op.aux);
+  if (args.vec8 && ((reinterpret_cast<uintptr_t>(op.dst) | reinterpret_cast<uintptr_t>(op.res)) & 15))
+    return fail(CPB200_ERR_ARG, "tc: a pointwise conv's dst and res must be 16-byte aligned (16-byte epilogue stores)");
 #define TC_CASE(N, D)                                                                                  \
   case N: return t.P == 2 ? launch_tc<N, D, 2>(t, args, st) : launch_tc<N, D, 1>(t, args, st);
   if (t.dcn) {

@@ -252,6 +252,78 @@ __device__ __forceinline__ void epilogue_pair(const float *acc, const float *acc
   }
 }
 
+// Row-vector form of the fragment, for 16-byte epilogue accesses.  Over a 16-column group (registers 8g .. 8g + 7) the four
+// lanes of a quad hold two rows x two 8-column blocks; lane q holds, as v[u], columns (2q, 2q + 1) of unit u = (row
+// r0 + 8 (u & 1), block u >> 1).  A 4 x 4 transpose within the quad (two butterfly steps, four shuffles each) leaves
+// lane q with unit q: v[s] = columns (2s, 2s + 1) of that block, 8 consecutive channels of one pixel.  Values move, none
+// is computed.
+__device__ __forceinline__ void quad_rows8(float2 (&v)[4], int q) {
+#pragma unroll
+  for (int m = 1; m <= 2; m <<= 1) {
+    const bool hi = q & m;
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      // the two slots whose bit m differs from the lane's: sent to and refilled from lane q ^ m
+      const int i0 = m == 1 ? 2 * k : k, i1 = i0 + m;
+      float2 s = hi ? v[i0] : v[i1];
+      s.x = __shfl_xor_sync(0xffffffffu, s.x, m);
+      s.y = __shfl_xor_sync(0xffffffffu, s.y, m);
+      if (hi) v[i0] = s; else v[i1] = s;
+    }
+  }
+}
+
+// epilogue_pair for 8 consecutive channels of one output pixel (element e of dst, 16-byte aligned), after bias and
+// acc_scale (quad_rows8's v): the same residual, activation and rounding per element, in 16-byte loads and stores per
+// plane.  NHWC forms only: 16-bit (P = 2: hi and lo planes `plane` elements apart) and fp32.
+template <int P>
+__device__ __forceinline__ void epilogue_vec8(const float2 (&v)[4], uint32_t act, int form, void *dst, const void *res, size_t e,
+                                              long long plane, uint32_t fmt) {
+  float f[8];
+#pragma unroll
+  for (int s = 0; s < 4; ++s) { f[2 * s] = v[s].x; f[2 * s + 1] = v[s].y; }
+  if (form == OUT_F32) {
+    float4 *o = reinterpret_cast<float4 *>(static_cast<float *>(dst) + e);
+    o[0] = make_float4(cpb::act_fast(f[0], act), cpb::act_fast(f[1], act), cpb::act_fast(f[2], act), cpb::act_fast(f[3], act));
+    o[1] = make_float4(cpb::act_fast(f[4], act), cpb::act_fast(f[5], act), cpb::act_fast(f[6], act), cpb::act_fast(f[7], act));
+  } else if constexpr (P == 2) {
+    uint16_t *o = static_cast<uint16_t *>(dst) + e;
+    if (res) {
+      const uint16_t *r = static_cast<const uint16_t *>(res) + e;
+      const uint4 h = __ldg(reinterpret_cast<const uint4 *>(r)), l = __ldg(reinterpret_cast<const uint4 *>(r + plane));
+      const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        const float2 x = join2(hw[s], lw[s], fmt);
+        f[2 * s] += x.x; f[2 * s + 1] += x.y;
+      }
+    }
+    uint32_t hi[4], lo[4];
+#pragma unroll
+    for (int s = 0; s < 4; ++s) split2(cpb::act_fast(f[2 * s], act), cpb::act_fast(f[2 * s + 1], act), fmt, hi[s], lo[s]);
+    *reinterpret_cast<uint4 *>(o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    *reinterpret_cast<uint4 *>(o + plane) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+  } else {
+    __nv_bfloat16 *o = static_cast<__nv_bfloat16 *>(dst) + e;
+    if (res) {
+      const uint4 h = __ldg(reinterpret_cast<const uint4 *>(static_cast<const __nv_bfloat16 *>(res) + e));
+      const uint32_t hw[4] = {h.x, h.y, h.z, h.w};
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        const float2 x = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&hw[s]));
+        f[2 * s] += x.x; f[2 * s + 1] += x.y;
+      }
+    }
+    uint32_t w[4];
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const __nv_bfloat162 b = __floats2bfloat162_rn(cpb::act_fast(f[2 * s], act), cpb::act_fast(f[2 * s + 1], act));
+      w[s] = *reinterpret_cast<const uint32_t *>(&b);
+    }
+    *reinterpret_cast<uint4 *>(o) = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
