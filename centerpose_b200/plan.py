@@ -615,6 +615,9 @@ class Plan:
             raise RuntimeError("cpb200_op layout mismatch between Python binding and library")
         self.n = n
         self._prepared = False
+        self._done = None           # event recorded after the last run, on _last_stream (see run)
+        self._last_stream = None
+        self._streams = set()       # the streams the plan's memory is recorded on
 
     @staticmethod
     def _root(s: Sym) -> Sym:
@@ -768,15 +771,37 @@ class Plan:
 
     def run(self, stream: Optional[int] = None):
         """Enqueue the program on the current stream of the plan's device, or on ``stream`` (a raw ``cudaStream_t``
-        handle of the current device) for callers that hold one."""
+        handle of the current device) for callers that hold one.
+
+        Every run reads and writes the plan's one set of activation buffers, so runs are ordered across streams: a run
+        on another stream than the previous run's first waits for that run to end.  The first run on a stream also
+        records the plan's buffers and weights on it, so when the plan is dropped the allocator does not hand their
+        memory out before the work enqueued there has finished."""
         L = _lib.lib()
         if not self._prepared:
             _lib.check(L.cpb200_prepare_ops(self.ops, self.n), "cpb200_prepare_ops")
             self._prepared = True
+        s = torch.cuda.current_stream(self.device) if stream is None else \
+            torch.cuda.ExternalStream(stream, device=self.device)
+        self._order(s)
         if stream is None:
             _lib.launch("run_ops", self.device, self.ops, self.n)
         else:
             _lib.check(L.cpb200_run_ops(self.ops, self.n, stream), "cpb200_run_ops")
+        self._done.record(s)
+
+    def _order(self, s):
+        """Make stream ``s`` wait for the previous run when that ran on another stream, and record the plan's device
+        memory on ``s`` the first time a run uses it."""
+        if self._done is None:
+            self._done = torch.cuda.Event()
+        elif self._last_stream != s.cuda_stream:
+            s.wait_event(self._done)
+        if s.cuda_stream not in self._streams:
+            self._streams.add(s.cuda_stream)
+            for t in {id(t): t for t in (*self.buffers, *self.pb.keep) if t.is_cuda}.values():
+                t.record_stream(s)
+        self._last_stream = s.cuda_stream
 
     def profile_ops(self, stream: int, reps: int = 3):
         """CUDA-event time of every op launched ON ITS OWN (ms, best of ``reps``), after one full run has filled the buffers.

@@ -96,7 +96,7 @@ def targets(ev, image_ids, shapes, cfg):
     out = {name: torch.empty((B,) + shape(R), dtype=dt, device=ev.device) for name, dt, shape in TARGETS}
     if B == 0:
         return out
-    up = torch.from_numpy(table.view(np.uint8).reshape(-1).copy()).to(ev.device)
+    up = torch.from_numpy(table.view(np.uint8).reshape(-1).copy()).pin_memory().to(ev.device, non_blocking=True)
     _lib.launch("multi_pose_targets_batch", ev.device, up, B, ev.gts, R, targets_struct(out))
     return out
 
