@@ -431,15 +431,22 @@ __global__ void dcn_wgrad_reduce_kernel(const float *__restrict__ part, float *_
   }
 }
 
-// grad_bias[o] = sum over (b, p) of gout[b, o, p]: thread-strided partial sums, then a fixed shared-memory tree
+// grad_bias[o] = sum over (b, p) of gout[b, o, p]: thread-strided partial sums, then a fixed shared-memory tree.
+// Each thread adds B*HW/256 values in sequence (4 096 at B = 64 on 128x128); a plain running sum drifts by some 1e-6
+// relative there, so the partial sums are compensated (Kahan): each carries its rounding error into the next add.
 __global__ void __launch_bounds__(NT) dcn_bgrad_kernel(const float *__restrict__ gout, float *__restrict__ gbias, int B,
                                                        int Co, int HW) {
   __shared__ float red[NT];
   const int o = blockIdx.x;
-  float s = 0.f;
+  float s = 0.f, c = 0.f;
   for (int b = 0; b < B; ++b) {
     const float *row = gout + ((size_t)b * Co + o) * HW;
-    for (int p = threadIdx.x; p < HW; p += NT) s += row[p];
+    for (int p = threadIdx.x; p < HW; p += NT) {
+      const float y = __fsub_rn(row[p], c);
+      const float t = __fadd_rn(s, y);
+      c = __fsub_rn(__fsub_rn(t, s), y);
+      s = t;
+    }
   }
   red[threadIdx.x] = s;
   __syncthreads();

@@ -126,6 +126,25 @@ def test_refusals_before_the_device(monkeypatch):
         dcn.dcn_v2_forward(*x, *CFG, precision="bf16")
 
 
+def test_split_rule_matches_library_and_cases_reach_every_regime():
+    """The weight gradient's split K restated in tests/dcn_train_cases.py gives the library's split count (its
+    workspace holds one Co x C*9 fp32 partial per split) on every accuracy case, and the cases reach every regime of
+    the rule, from one K step per split to single splits of several steps and splits of hundreds of steps."""
+    from centerpose_b200 import _lib
+    from tests import dcn_train_cases as dc
+    L = _lib.lib()
+    reached = set()
+    for B, C, Co, H, W in dc.ACCURACY:
+        splits, steps = dc.wgrad_split(B, C, H, W, Co)
+        assert L.cpb200_dcn_train_workspace_bytes(B, C, H, W, Co) == splits * Co * C * 9 * 4, (B, C, Co, H, W)
+        assert (splits - 1) * steps < -(-B * H * W // dc.BK) <= splits * steps, (B, C, Co, H, W)
+        reached |= dc.split_regimes(B, C, H, W, Co)
+    assert reached == set(dc.REGIMES), set(dc.REGIMES) - reached
+    assert dc.split_regimes(32, 64, 128, 128, 64) >= {"over 400 steps per split", "short last split",
+                                                      "split boundary inside an image"}
+    assert dc.wgrad_split(32, 64, 128, 128, 64) == (53, 619)
+
+
 def test_modules_match_reference_layout():
     torch.manual_seed(3)
     m = dcn.DCN(40, 24, kernel_size=(3, 3), stride=1, padding=1, dilation=1, deformable_groups=1)

@@ -3,8 +3,9 @@ restatement (oracle/dcn_ref.py, oracle/dcn_train_ref.py) on the device, and agai
 
 Accuracy: for the output and each of the five gradients, max|dev - f64| / max|f64| and the relative L2 error must be
 at most max(4 * e32, 1e-6), where e32 is the same statistic of torch's fp32 autograd through the same restatement.
+The restatement runs image-chunk by image-chunk (tests/dcn_train_cases.restated), so the float64 reference fits at the
+training batches; e32 sums the same chunks' weight and bias gradients in fp32.
 """
-import math
 import os
 
 import numpy as np
@@ -13,75 +14,41 @@ import torch
 from torch import nn
 
 from centerpose_b200 import dcn
-from oracle import dcn_ref, dcn_train_ref
+from oracle import dcn_ref
+from tests.dcn_train_cases import (ACCURACY, CFG, DEV, NAMES, PRECISIONS, case_id, check_accuracy, device,
+                                   make_inputs, restated)
 
 pytestmark = pytest.mark.gpu
 
-DEV = torch.device("cuda:0")
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "dcn_train.npz")
-NAMES = ("out", "grad_input", "grad_offset", "grad_mask", "grad_weight", "grad_bias")
-PRECISIONS = ("default", "fp32")
-
-# (C, Co, H, W): every DCN of DLA-34 and MobileNetV3 at its map size for a 512x512 input, then odd shapes
-DLA34 = [(512, 256, 16, 16), (256, 256, 32, 32), (256, 128, 32, 32), (128, 128, 64, 64), (128, 64, 64, 64),
-         (256, 64, 32, 32), (64, 64, 128, 128)]
-MOBILENETV3 = [(40, 24, 64, 64), (160, 24, 32, 32), (960, 24, 16, 16), (24, 24, 128, 128), (24, 24, 64, 64),
-               (24, 24, 32, 32)]
-ODD = [(8, 8, 7, 13), (8, 8, 1, 1), (64, 8, 7, 13), (8, 64, 13, 7), (3, 5, 2, 3), (24, 24, 1, 9)]
-CFG = (3, 3, 1, 1, 1, 1, 1, 1, 1)
 
 
-def make_inputs(B, C, Co, H, W, seed):
-    g = torch.Generator(device="cpu").manual_seed(seed)
-    stdv = 1.0 / math.sqrt(9 * C)
-    t = dict(input=torch.randn(B, C, H, W, generator=g), weight=(torch.rand(Co, C, 3, 3, generator=g) * 2 - 1) * stdv,
-             bias=torch.randn(Co, generator=g) * 0.1, offset=torch.randn(B, 18, H, W, generator=g) * 2,
-             mask=torch.rand(B, 9, H, W, generator=g), grad_out=torch.randn(B, Co, H, W, generator=g))
-    return {k: v.to(DEV) for k, v in t.items()}
-
-
-def restated(t, dtype):
-    c = {k: v.to(dtype) for k, v in t.items()}
-    out = dcn_ref.dcn_v2_forward(c["input"], c["weight"], c["bias"], c["offset"], c["mask"])
-    grads = dcn_train_ref.dcn_v2_backward(c["input"], c["weight"], c["bias"], c["offset"], c["mask"], c["grad_out"])
-    return [out.detach()] + [g.detach() for g in grads]
-
-
-def device(t, precision):
-    out = dcn.dcn_v2_forward(t["input"], t["weight"], t["bias"], t["offset"], t["mask"], *CFG, precision=precision)
-    grads = dcn.dcn_v2_backward(t["input"], t["weight"], t["bias"], t["offset"], t["mask"], t["grad_out"], *CFG,
-                                precision=precision)
-    return [out] + list(grads)
-
-
-def stats(got, want):
-    d = (got.double() - want).abs()
-    mx = want.abs().max().item()
-    l2 = want.norm().item()
-    return (d.max().item() / mx if mx > 0 else d.max().item(),
-            (d.norm().item() / l2) if l2 > 0 else d.norm().item())
-
-
-def check_accuracy(got, ref64, ref32, label):
-    bad = []
-    for name, g, r, r32 in zip(NAMES, got, ref64, ref32):
-        assert g.shape == r.shape and g.dtype == torch.float32, name
-        assert torch.isfinite(g).all(), "%s %s: not finite" % (label, name)
-        e_dev, e32 = stats(g, r), stats(r32, r)
-        for what, a, b in zip(("max", "l2"), e_dev, e32):
-            if a > max(4 * b, 1e-6):
-                bad.append("%s %s %s: %.3g > max(4 * %.3g, 1e-6)" % (label, name, what, a, b))
-    assert not bad, "\n".join(bad)
-
-
-@pytest.mark.parametrize("shape", DLA34 + MOBILENETV3 + ODD, ids=lambda s: "%dx%d_%dx%d" % s)
-def test_accuracy(shape):
-    C, Co, H, W = shape
-    t = make_inputs(2, C, Co, H, W, seed=C * 7919 + Co * 31 + H)
+def _accuracy(t, label):
     ref64 = restated(t, torch.float64)
     ref32 = restated(t, torch.float32)
-    for p in PRECISIONS:
-        check_accuracy(device(t, p), ref64, ref32, "%s %s" % (shape, p))
+    report = {}
+    try:
+        for p in PRECISIONS:
+            check_accuracy(device(t, p), ref64, ref32, "%s %s" % (label, p), report)
+    finally:
+        for (lab, name), (e_dev, e32) in report.items():
+            print("%s %s: max %.3g (e32 %.3g), l2 %.3g (e32 %.3g)" % (lab, name, e_dev[0], e32[0], e_dev[1], e32[1]))
+
+
+@pytest.mark.parametrize("case", ACCURACY, ids=case_id)
+def test_accuracy(case):
+    """Every DCN of DLA-34 and MobileNetV3 at B = 2 and at its training batch, the odd shapes, and a case of one
+    weight-gradient split of several K steps (tests/dcn_train_cases.py: every regime of the split rule)."""
+    B, C, Co, H, W = case
+    seed = C * 7919 + Co * 31 + H + (0 if B == 2 else 104729 * B)
+    _accuracy(make_inputs(B, C, Co, H, W, seed=seed), case_id(case))
+
+
+@pytest.mark.parametrize("stats", ("same_sign", "sparse"))
+def test_accuracy_training_statistics(stats):
+    """At B = 32, 64 -> 64 on 128x128: post-ReLU inputs, 0.5 px offsets, saturated masks, and a same-sign or sparse
+    grad_output (tests/dcn_train_cases.make_inputs)."""
+    _accuracy(make_inputs(32, 64, 64, 128, 128, seed=11, stats=stats), "b32_64x64_128x128 " + stats)
 
 
 @pytest.mark.parametrize("case", ("edges", "pile", "one", "random"))
@@ -95,9 +62,19 @@ def test_golden(case):
         check_accuracy(device(t, p), ref64, ref32, "%s %s" % (case, p))
 
 
-@pytest.mark.parametrize("precision", PRECISIONS)
-def test_scaling_is_exact(precision):
-    t = make_inputs(2, 64, 64, 24, 20, seed=5)
+TRAINING_SHAPE = (32, 64, 64, 128, 128)      # DLA-34's widest DCN at its training batch: 53 splits of 619 K steps
+
+
+def _bit_cases(small):
+    """(precision, shape) over both precisions at ``small`` (id: the precision) and at TRAINING_SHAPE."""
+    return [pytest.param(p, small, id=p) for p in PRECISIONS] + \
+        [pytest.param(p, TRAINING_SHAPE, id="%s-%s" % (p, case_id(TRAINING_SHAPE))) for p in PRECISIONS]
+
+
+@pytest.mark.parametrize("precision,shape", _bit_cases((2, 64, 64, 24, 20)))
+def test_scaling_is_exact(precision, shape):
+    B, C, Co, H, W = shape
+    t = make_inputs(B, C, Co, H, W, seed=5)
     base = device(t, precision)
     for k in (-30, -10, 10):
         s = 2.0 ** k
@@ -122,9 +99,10 @@ def test_small_magnitudes_keep_their_precision():
     check_accuracy(device(t, "default"), ref64, ref32, "grad_output 1e-9")
 
 
-@pytest.mark.parametrize("precision", PRECISIONS)
-def test_deterministic(precision):
-    t = make_inputs(2, 128, 64, 33, 29, seed=3)
+@pytest.mark.parametrize("precision,shape", _bit_cases((2, 128, 64, 33, 29)))
+def test_deterministic(precision, shape):
+    B, C, Co, H, W = shape
+    t = make_inputs(B, C, Co, H, W, seed=3)
     a, b = device(t, precision), device(t, precision)
     for name, x, y in zip(NAMES, a, b):
         if name != "grad_input":

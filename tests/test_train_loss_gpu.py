@@ -14,18 +14,16 @@ Bounds:
 """
 import copy
 import os
-import random
 
-import cv2
 import numpy as np
 import pytest
 import torch
 
-from centerpose_b200 import train_data, train_loss
+from centerpose_b200 import train_loss
 from centerpose_b200.config import default_cfg
 from oracle import train_loss_ref
 from tests import train_loss_cases as tc
-from tests.train_cases import case_cfg, seeded_case
+from tests.train_cases import seeded_jpeg_batch
 
 pytestmark = pytest.mark.gpu
 
@@ -147,24 +145,9 @@ def test_clamp_edges_reach_both_sides(gold):
             assert g[i, 0, row, 0] != 0 and g[i, 0, row, 1] == 0 and g[i, 0, row, 2] != 0 and g[i, 0, row, 3] == 0
 
 
-def _jpeg_batch(tmp_path, B=32, res=512, seed=0, settings=None):
-    from oracle.make_golden_val import image
-    cfg = case_cfg(default_cfg("dla_34"), settings or {"AUG_ROT": 0.3, "ROTATE": 30., "FLIP": 0.5}, res)
-    ds = seeded_case(700 + seed, B, lo=200, hi=700, people=(1, 12))
-    paths = []
-    for im in ds["images"]:
-        p = str(tmp_path / ("%d_%d.jpg" % (seed, im["id"])))
-        cv2.imwrite(p, image(9000 + 100 * seed + im["id"], im["height"], im["width"]), [cv2.IMWRITE_JPEG_QUALITY, 90])
-        paths.append(p)
-    np.random.seed(60 + seed)
-    random.seed(70 + seed)
-    batch = train_data.TrainData(cfg, ds).batch(paths, [im["id"] for im in ds["images"]])
-    return cfg, batch
-
-
 @pytest.fixture(scope="module")
 def jpeg_batch(tmp_path_factory):
-    return _jpeg_batch(tmp_path_factory.mktemp("train_loss"))
+    return seeded_jpeg_batch(tmp_path_factory.mktemp("train_loss"))
 
 
 def test_train_batches_match_restatement(jpeg_batch):
@@ -263,7 +246,7 @@ class Tiny(torch.nn.Module):
 def test_short_training_loop(tmp_path):
     """Five Adam steps on the same five TrainData batches, with the device loss and with the restatement: the
     parameters agree within 1e-4 (1 % of one step at lr 1e-2), and the loss on the first batch falls in both."""
-    batches = [_jpeg_batch(tmp_path, B=8, res=128, seed=s) for s in range(5)]
+    batches = [seeded_jpeg_batch(tmp_path, B=8, res=128, seed=s) for s in range(5)]
     cfg = batches[0][0]
     runs = []
     for use_device in (True, False):

@@ -64,6 +64,30 @@ def dataset(name):
     return seeded_case(1, 2, lo=300, hi=700, people=(3, 8))
 
 
+def seeded_jpeg_batch(tmp_path, B=32, res=512, seed=0, settings=None):
+    """``(cfg, batch)``: a TrainData batch on the device from B seeded JPEG files written under ``tmp_path`` (images of
+    200 to 700 pixels a side, 1 to 11 people each), at input resolution ``res``, with DLA-34's config and the DATASET
+    ``settings`` (default: rotation and flips)."""
+    import random
+
+    import cv2
+
+    from centerpose_b200 import train_data
+    from centerpose_b200.config import default_cfg
+    from oracle.make_golden_val import image
+    cfg = case_cfg(default_cfg("dla_34"), settings or {"AUG_ROT": 0.3, "ROTATE": 30., "FLIP": 0.5}, res)
+    ds = seeded_case(700 + seed, B, lo=200, hi=700, people=(1, 12))
+    paths = []
+    for im in ds["images"]:
+        p = str(tmp_path / ("%d_%d.jpg" % (seed, im["id"])))
+        cv2.imwrite(p, image(9000 + 100 * seed + im["id"], im["height"], im["width"]), [cv2.IMWRITE_JPEG_QUALITY, 90])
+        paths.append(p)
+    np.random.seed(60 + seed)
+    random.seed(70 + seed)
+    batch = train_data.TrainData(cfg, ds).batch(paths, [im["id"] for im in ds["images"]])
+    return cfg, batch
+
+
 def case_cfg(base, settings, res):
     """``base`` with the DATASET ``settings`` and the input resolution ``res`` (output res / 4)."""
     cfg = copy.deepcopy(base)
