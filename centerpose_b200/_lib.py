@@ -1,7 +1,7 @@
-"""ctypes binding of the C ABI declared in ``include/centerpose_b200.h``.
+"""ctypes binding of the C ABI declared in ``include/centerpose_b200.h`` and ``include/centerpose_b200_heads_train.h``.
 
-The header is the only statement of the ABI: ``lib()`` binds ``restype`` and ``argtypes`` of every ``cpb200_*``
-prototype from it when the library loads, and a type the binding does not know fails the load.  ``launch`` makes
+The headers are the only statement of the ABI: ``lib()`` binds ``restype`` and ``argtypes`` of every ``cpb200_*``
+prototype of each of them (``HEADERS``) when the library loads, and a type the binding does not know fails the load.  ``launch`` makes
 every call that enqueues work on a stream; the queries that take none (``*_workspace_bytes``, ``launch_count``,
 ``sizeof_op``, ``prepare_ops``, ``release_ops``) are plain calls on ``lib()``.
 
@@ -19,6 +19,9 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIBPATH = os.path.join(_HERE, "lib", "libcenterpose_b200.so")
 HEADER = os.path.join(_HERE, "..", "include", "centerpose_b200.h")
+# the library's other public headers, each declaring its own entry points with HEADER's conventions and types
+HEADS_TRAIN_HEADER = os.path.join(_HERE, "..", "include", "centerpose_b200_heads_train.h")
+HEADERS = (HEADER, HEADS_TRAIN_HEADER)
 
 _lib = None
 
@@ -64,7 +67,7 @@ def _ctype(fn: str, decl: str, ret: bool):
 
 
 def signatures(text: str | None = None) -> dict:
-    """``{name: (restype, argtypes)}`` of every ``cpb200_*`` prototype of ``text`` (default: the header).  Reads no
+    """``{name: (restype, argtypes)}`` of every ``cpb200_*`` prototype of ``text`` (default: ``HEADER``).  Reads no
     library, so it also works where the library is not built."""
     if text is None:
         with open(HEADER) as f:
@@ -90,9 +93,11 @@ def lib() -> ctypes.CDLL:
             f"centerpose_b200: CUDA library not built ({LIBPATH} missing). Run "
             "`python -m centerpose_b200.build` (needs nvcc); there is no CPU fallback.")
     L = ctypes.CDLL(LIBPATH)
-    for name, (restype, argtypes) in signatures().items():
-        fn = getattr(L, name)
-        fn.restype, fn.argtypes = restype, argtypes
+    for path in HEADERS:
+        with open(path) as f:
+            for name, (restype, argtypes) in signatures(f.read()).items():
+                fn = getattr(L, name)
+                fn.restype, fn.argtypes = restype, argtypes
     _lib = L
     return L
 

@@ -46,7 +46,7 @@ def _sources():
 def _digest() -> str:
     h = hashlib.sha256()
     for p in _sources() + sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + \
-            [os.path.join(HERE, "..", "include", "centerpose_b200.h")]:
+            sorted(glob.glob(os.path.join(HERE, "..", "include", "*.h"))):
         with open(p, "rb") as f:
             h.update(p.encode()); h.update(f.read())
     h.update(" ".join(NVCC_FLAGS).encode()); h.update(repr(sorted(FILE_FLAGS.items())).encode())

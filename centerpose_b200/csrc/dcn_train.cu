@@ -11,135 +11,21 @@
 //                    then col2im / col2im_coord on the tile, from shared memory
 //   weight backward  gW[o, r]    = sum_p gout[o, p] col[r, p]               tile Co x (c, tap), K = B*H*W, split K
 //
-// Two inner products share every kernel, tile and accumulator layout (DcnPrec):
-//   DCN_TF32X3  tensor cores, mma.sync m16n8k8 tf32 with each fp32 operand split as big + small (both tf32, rounded to
-//               nearest), summed as small*big + big*small + big*big in fp32.  tf32 keeps fp32's 8-bit exponent, so the
-//               split is scale-free: 2^k x splits to 2^k big + 2^k small over fp32's whole normal range, and every
-//               product and sum scales with it.
-//   DCN_FP32    CUDA-core fp32 FMAs over the same shared-memory tiles, for reference-precision parity.
+// Two inner products share every kernel, tile and accumulator layout: train_mma.cuh's 3xTF32 tensor-core split
+// (TRAIN_TF32X3) and CUDA-core fp32 (TRAIN_FP32).
 //
 // Determinism: the forward, grad_offset, grad_mask, grad_weight and grad_bias are sums in a fixed order (no atomics);
 // grad_input is scattered with fp32 atomics, as the reference and torchvision do.
 #include "common.cuh"
+#include "train_mma.cuh"
 
 namespace cpb {
 namespace {
 
-constexpr int NT = 256;                 // 8 warps: 2 along M x 4 along N, a 32 x 32 warp tile each
-constexpr int BM = 64, BN = 128, BK = 16;
-constexpr int AP = BK + 4;              // As[m][k] row pitch: fragment loads hit 32 distinct banks
-constexpr int BP = BN + 8;              // Bs[k][n] row pitch, likewise
+using namespace train;
 constexpr int TAPS = 9;
 constexpr int WG_TARGET_CTAS = 264;     // weight-backward split-K aims at two CTAs per SM of a 132-SM H100
 constexpr size_t WG_WS_CAP = size_t(16) << 20;  // and keeps its per-split partials under 16 MiB
-
-enum DcnPrec { DCN_TF32X3 = 0, DCN_FP32 = 1 };
-
-__device__ __forceinline__ uint32_t tf32_rna(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return r;
-}
-
-__device__ __forceinline__ void split_tf32(float x, uint32_t &big, uint32_t &small) {
-  big = tf32_rna(x);
-  small = tf32_rna(__fsub_rn(x, __uint_as_float(big)));
-}
-
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// acc += As (BM x BK) * Bs (BK x BN) for this warp's 32 x 32 tile.  Thread (gid = lane / 4, tig = lane % 4) holds the
-// m16n8 accumulator fragment: acc[mt][nt][0..3] at rows wm*32 + mt*16 + gid (+8 for [2], [3]) and columns
-// wn*32 + nt*8 + 2*tig (+1 for [1], [3]) -- the same positions in both precisions.
-// The BK-deep product goes to a fresh partial that is added to acc with one rounded fp32 add.  The tensor cores'
-// accumulation truncates, so chaining every MMA of a K = 4608 reduction into one accumulator drifts by some 1e-5
-// relative; a partial per slab bounds the truncated chain at 6 MMAs and the long sum is rounded to nearest.  The CUDA-
-// core path blocks its sum the same way.
-template <int P>
-__device__ __forceinline__ void tile_mma(const float (*As)[AP], const float (*Bs)[BP], int wm, int wn, int lane,
-                                         float (&acc)[2][4][4]) {
-  const int gid = lane >> 2, tig = lane & 3;
-  float part[2][4][4];
-#pragma unroll
-  for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) part[mt][nt][i] = 0.f;
-  if constexpr (P == DCN_TF32X3) {
-#pragma unroll
-    for (int kk = 0; kk < BK; kk += 8) {
-      uint32_t ab[2][4], as[2][4], bb[4][2], bs[4][2];
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        const int m = wm * 32 + mt * 16 + gid;
-        split_tf32(As[m][kk + tig], ab[mt][0], as[mt][0]);
-        split_tf32(As[m + 8][kk + tig], ab[mt][1], as[mt][1]);
-        split_tf32(As[m][kk + tig + 4], ab[mt][2], as[mt][2]);
-        split_tf32(As[m + 8][kk + tig + 4], ab[mt][3], as[mt][3]);
-      }
-#pragma unroll
-      for (int nt = 0; nt < 4; ++nt) {
-        const int n = wn * 32 + nt * 8 + gid;
-        split_tf32(Bs[kk + tig][n], bb[nt][0], bs[nt][0]);
-        split_tf32(Bs[kk + tig + 4][n], bb[nt][1], bs[nt][1]);
-      }
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-          mma_tf32(part[mt][nt], as[mt], bb[nt][0], bb[nt][1]);
-          mma_tf32(part[mt][nt], ab[mt], bs[nt][0], bs[nt][1]);
-          mma_tf32(part[mt][nt], ab[mt], bb[nt][0], bb[nt][1]);
-        }
-    }
-  } else {
-#pragma unroll 4
-    for (int k = 0; k < BK; ++k) {
-      float a[2][2], b[4][2];
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        a[mt][0] = As[wm * 32 + mt * 16 + gid][k];
-        a[mt][1] = As[wm * 32 + mt * 16 + gid + 8][k];
-      }
-#pragma unroll
-      for (int nt = 0; nt < 4; ++nt) {
-        const float2 v = *reinterpret_cast<const float2 *>(&Bs[k][wn * 32 + nt * 8 + 2 * tig]);
-        b[nt][0] = v.x;
-        b[nt][1] = v.y;
-      }
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-          part[mt][nt][0] = fmaf(a[mt][0], b[nt][0], part[mt][nt][0]);
-          part[mt][nt][1] = fmaf(a[mt][0], b[nt][1], part[mt][nt][1]);
-          part[mt][nt][2] = fmaf(a[mt][1], b[nt][0], part[mt][nt][2]);
-          part[mt][nt][3] = fmaf(a[mt][1], b[nt][1], part[mt][nt][3]);
-        }
-    }
-  }
-#pragma unroll
-  for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) acc[mt][nt][i] = __fadd_rn(acc[mt][nt][i], part[mt][nt][i]);
-}
-
-__device__ __forceinline__ void zero_acc(float (&acc)[2][4][4]) {
-#pragma unroll
-  for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) acc[mt][nt][i] = 0.f;
-}
 
 // One bilinear sample of tap `tap` at output pixel (ho, wo): dmcn_im2col_bilinear's corners and weights
 // (dcn_v2_im2col_cuda.cu:25-54) behind the `> -1 / < H` test of :180.  bits 0..3 = corners v1..v4 in bounds; all clear
@@ -481,7 +367,7 @@ int check_shape(const char *what, int B, int C, int H, int W, int Co, int precis
   if ((long long)B * C * H * W >= (1ll << 31) || (long long)B * 2 * TAPS * H * W >= (1ll << 31) ||
       (long long)B * Co * H * W >= (1ll << 31) || (long long)C * TAPS * Co >= (1ll << 31))
     return fail(CPB200_ERR_ARG, "%s: tensors over 2^31 elements", what);
-  if (precision != DCN_TF32X3 && precision != DCN_FP32)
+  if (precision != TRAIN_TF32X3 && precision != TRAIN_FP32)
     return fail(CPB200_ERR_ARG, "%s: unknown precision %d", what, precision);
   return CPB200_OK;
 }
@@ -507,12 +393,12 @@ extern "C" int cpb200_dcn_train_forward(const float *input, const float *weight,
     return fail(CPB200_ERR_ARG, "dcn_train_forward: null pointer");
   cudaStream_t s = (cudaStream_t)stream;
   const dim3 grid(ceil_div(H * W, BN), ceil_div(Co, BM), B);
-  if (precision == DCN_TF32X3) {
-    dcn_fwd_kernel<DCN_TF32X3><<<grid, NT, 0, s>>>(input, weight, bias, offset, mask, output, C, H, W, Co);
-    return check_launch("dcn_fwd_kernel<tf32x3>", dcn_fwd_kernel<DCN_TF32X3>);
+  if (precision == TRAIN_TF32X3) {
+    dcn_fwd_kernel<TRAIN_TF32X3><<<grid, NT, 0, s>>>(input, weight, bias, offset, mask, output, C, H, W, Co);
+    return check_launch("dcn_fwd_kernel<tf32x3>", dcn_fwd_kernel<TRAIN_TF32X3>);
   }
-  dcn_fwd_kernel<DCN_FP32><<<grid, NT, 0, s>>>(input, weight, bias, offset, mask, output, C, H, W, Co);
-  return check_launch("dcn_fwd_kernel<fp32>", dcn_fwd_kernel<DCN_FP32>);
+  dcn_fwd_kernel<TRAIN_FP32><<<grid, NT, 0, s>>>(input, weight, bias, offset, mask, output, C, H, W, Co);
+  return check_launch("dcn_fwd_kernel<fp32>", dcn_fwd_kernel<TRAIN_FP32>);
 }
 
 template <int P>
@@ -553,9 +439,9 @@ extern "C" int cpb200_dcn_train_backward(const float *input, const float *weight
     return fail(CPB200_ERR_ARG, "dcn_train_backward: workspace of %zu bytes, %zu needed", workspace_bytes, need);
   cudaStream_t s = (cudaStream_t)stream;
   float *part = static_cast<float *>(workspace);
-  if (precision == DCN_TF32X3)
-    return dcn_backward_impl<DCN_TF32X3>(input, weight, offset, mask, grad_output, grad_input, grad_offset, grad_mask,
+  if (precision == TRAIN_TF32X3)
+    return dcn_backward_impl<TRAIN_TF32X3>(input, weight, offset, mask, grad_output, grad_input, grad_offset, grad_mask,
                                          grad_weight, grad_bias, B, C, H, W, Co, part, ws, s);
-  return dcn_backward_impl<DCN_FP32>(input, weight, offset, mask, grad_output, grad_input, grad_offset, grad_mask,
+  return dcn_backward_impl<TRAIN_FP32>(input, weight, offset, mask, grad_output, grad_input, grad_offset, grad_mask,
                                      grad_weight, grad_bias, B, C, H, W, Co, part, ws, s);
 }
