@@ -211,6 +211,11 @@ class PlanBuilder:
 
     # ---- symbolic tensors -------------------------------------------------------------
     def _sym(self, C, H, W, kind="act", name=""):
+        # An input too small for the network's deepest stride (HarDNet at 32 pixels: its sixth halving leaves 0 rows)
+        # would lower to ops of zero extent; refuse it here, before anything is launched, as the reference's pool raises.
+        if C <= 0 or H <= 0 or W <= 0:
+            raise ValueError(f"centerpose_b200: a {self.H}x{self.W} input is too small for this network "
+                             f"(an intermediate map would be {C}x{H}x{W})")
         s = Sym(C, H, W, kind, name)
         self.syms.append(s)
         return s

@@ -122,8 +122,9 @@ def keypoint_head(sd, feat, p="head_model"):
 
 @torch.no_grad()
 def forward(sd, x, arch="dla_34"):
-    """state_dict + (B,3,H,W) fp32 -> [hm, wh, hps, reg, hm_hp, hp_offset] logits (NCHW)."""
-    sd = {k: v.float() for k, v in sd.items() if v.dtype.is_floating_point}
+    """state_dict + (B,3,H,W) -> [hm, wh, hps, reg, hm_hp, hp_offset] logits (NCHW), evaluated in the dtype and on the
+    device of ``x`` (fp32 on the CPU pins the reference; float64 on the GPU is the network tests' oracle)."""
+    sd = {k: v.to(x.device, x.dtype) for k, v in sd.items() if v.dtype.is_floating_point}
     if arch == "dla_34":
         feat = dla34_backbone(sd, x)
     elif arch == "res_50":

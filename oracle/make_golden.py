@@ -26,7 +26,8 @@ warnings.filterwarnings("ignore")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from oracle import decode_ref, dcn_ref, dla_ref, post_process_ref  # noqa: E402
+from oracle import (decode_ref, dcn_ref, dla_ref, ghostnet_ref, hardnet_ref, mobilenetv2_ref,  # noqa: E402
+                    post_process_ref)
 from oracle.init_recipe import conditioned_state_dict, synth_images  # noqa: E402
 from oracle.ref_harness import load_reference, ref_create_model  # noqa: E402
 
@@ -206,6 +207,44 @@ def gen_mbv3(ns):
         print(f"mobilenetv3 {tag}: oracle max abs err {err:.2e} (scale {scale:.1f})")
 
 
+# One extreme-aspect input per configuration: the network input a 96x640 strip of an image becomes with TEST.FIX_RES
+# false.  Its deep maps are 3x20 (1/32) and 1x10 (HarDNet's 1/64), so the product runs tensor-core tiles with fewer than
+# 8 rows and maps one pixel high.  The head maps are stored every AR_STRIDE pixels (GhostNet's always-128x128 ones every 4).
+AR_H, AR_W, AR_STRIDE = 96, 640, 2
+AR_CASES = [
+    # file tag, experiments yaml, oracle forward
+    ("dla34", "dla_34_512x512", lambda sd, x: dla_ref.forward(sd, x, arch="dla_34")),
+    ("res50", "res_50_512x512", lambda sd, x: dla_ref.forward(sd, x, arch="res_50")),
+    ("hrnet32", "hrnet_w32_512", lambda sd, x: dla_ref.forward(sd, x, arch="hrnet")),
+    ("hrnet48", "hrnet_w48_512", lambda sd, x: dla_ref.forward(sd, x, arch="hrnet")),
+    ("mbv3", "mobilenetv3_512x512", lambda sd, x: dla_ref.forward(sd, x, arch="mobilenetv3")),
+    ("hardnet", "hardnet_512x512", lambda sd, x: hardnet_ref.forward(sd, x)),
+    ("mbv2", "mobilenetv2_512x512", lambda sd, x: mobilenetv2_ref.forward(sd, x)),
+    ("ghostnet", "ghost_net", lambda sd, x: ghostnet_ref.forward(sd, x)),
+]
+
+
+def gen_aspect(ns):
+    for name, yaml, oracle in AR_CASES:
+        model, cfg = ref_create_model(yaml)
+        sd = conditioned_state_dict(model.state_dict(), 317)
+        model.load_state_dict(sd)
+        sd_sha = sha(*[sd[k].numpy() for k in sorted(sd) if sd[k].is_floating_point()])
+        x = synth_images(1, AR_H, AR_W, seed=317)
+        with torch.no_grad():
+            ref = model(x)
+            mine = oracle(sd, x)
+        err = max(float((a - b).abs().max()) for a, b in zip(ref, mine))
+        scale = max(float(a.abs().max()) for a in ref)
+        assert err <= 1e-4 * scale, f"{name} {AR_H}x{AR_W}: oracle != reference ({err})"
+        st = 4 if ref[0].shape[2] == 128 else AR_STRIDE
+        maps = torch.cat(ref, dim=1).numpy()[:, :, ::st, ::st]
+        tag = f"{name}_{AR_H}x{AR_W}"
+        np.savez_compressed(os.path.join(GOLD, f"{tag}.npz"), maps=maps.astype(np.float32), stride=np.array(st),
+                            shape=np.array([1, AR_H, AR_W]), sd_sha=np.array(sd_sha), x_sha=np.array(sha(x.numpy())))
+        print(f"{tag}: oracle max abs err {err:.2e} (scale {scale:.1f}), maps {tuple(ref[0].shape[2:])}")
+
+
 def gen_soft_nms(ns=None):
     """Golden vectors of the reference's own Cython ``soft_nms_39`` compiled here (oracle/build_ref.py)."""
     from oracle.build_ref import load
@@ -302,6 +341,7 @@ def main():
     gen_res50(ns)
     gen_hrnet(ns)
     gen_mbv3(ns)
+    gen_aspect(ns)
     gen_soft_nms(ns)
     gen_soft_nms_cases(ns)
     print("golden fixtures written to", GOLD)

@@ -71,6 +71,6 @@ def mobilenetv2_backbone(sd, x, p="backbone_model"):
 
 @torch.no_grad()
 def forward(sd, x):
-    """state_dict + (B,3,H,W) fp32 -> [hm, wh, hps, reg, hm_hp, hp_offset] logits (NCHW), as ``dla_ref.forward``."""
-    sd = {k: v.float() for k, v in sd.items() if v.dtype.is_floating_point}
+    """state_dict + (B,3,H,W) -> [hm, wh, hps, reg, hm_hp, hp_offset] logits (NCHW), as ``dla_ref.forward``."""
+    sd = {k: v.to(x.device, x.dtype) for k, v in sd.items() if v.dtype.is_floating_point}
     return keypoint_head(sd, mobilenetv2_backbone(sd, x))

@@ -157,3 +157,34 @@ def test_mobilenetv3_oracle_matches_golden():
     x = synth_images(B, H, W, seed=317)
     maps = torch.cat(dla_ref.forward(sd, x, arch="mobilenetv3"), dim=1).numpy()
     assert np.abs(maps - g["maps"]).max() <= 1e-4 * np.abs(g["maps"]).max()
+
+
+AR_TAGS = {"dla34": ("dla_34", "dla_34"), "res50": ("res_50", "res_50"), "hrnet32": ("hrnet", "hrnet"),
+           "hrnet48": ("hrnet_w48", "hrnet"), "mbv3": ("mobilenetv3", "mobilenetv3"), "hardnet": ("hardnet", None),
+           "mbv2": ("mobilenetv2", None), "ghostnet": ("ghostnet", None)}
+
+
+@pytest.mark.parametrize("name", sorted(AR_TAGS))
+def test_oracle_matches_extreme_aspect_golden(name):
+    """Every configuration at the 96x640 input of tests/golden/<name>_96x640.npz (oracle/make_golden.py: gen_aspect):
+    deep maps 3x20 and 1x10.  Also pins that the product's parameter tree of each configuration (HRNet-W48 included)
+    draws the reference's weights."""
+    from centerpose_b200.model import create_model
+    from oracle import ghostnet_ref, hardnet_ref, mobilenetv2_ref
+    from tests.util import config
+    arch, oracle_arch = AR_TAGS[name]
+    g = np.load(os.path.join(GOLD, f"{name}_96x640.npz"))
+    B, H, W = [int(v) for v in g["shape"]]
+    st = int(g["stride"])
+    cfg = config(arch)
+    sd = conditioned_state_dict(create_model(cfg.MODEL.NAME, cfg.MODEL.HEAD_CONV, cfg).state_dict(), 317)
+    assert _sha(*[sd[k].numpy() for k in sorted(sd) if sd[k].is_floating_point()]) == str(g["sd_sha"])
+    x = synth_images(B, H, W, seed=317)
+    assert _sha(x.numpy()) == str(g["x_sha"])
+    if oracle_arch is not None:
+        out = dla_ref.forward(sd, x, arch=oracle_arch)
+    else:
+        out = {"hardnet": hardnet_ref, "mobilenetv2": mobilenetv2_ref, "ghostnet": ghostnet_ref}[arch].forward(sd, x)
+    maps = torch.cat(out, dim=1).numpy()[:, :, ::st, ::st]
+    assert maps.shape == g["maps"].shape
+    assert np.abs(maps - g["maps"]).max() <= 1e-4 * np.abs(g["maps"]).max()

@@ -157,9 +157,16 @@ def _assert_like_run(got, want, what):
     assert err <= 2e-3 * max(1.0, float(np.abs(want).max())), (what, err, match_rows(got, want, tol=2e-3, box_tol=5e-2))
 
 
-@pytest.mark.parametrize("case", ["dla34_test_section", "scales_1_075_flip", "fix_res_no_flip_no_nms"])
+@pytest.mark.parametrize("case", ["dla34_test_section", "scales_1_075_flip", "fix_res_no_flip_no_nms",
+                                  "extreme_aspect_scales_05_1_15_flip"])
 def test_run_images_matches_run(case):
-    if case == "dla34_test_section":
+    if case == "extreme_aspect_scales_05_1_15_flip":
+        # strips and a small image at three scales: network inputs 32x320, 64x608, 64x928, their transposes, 32x32,
+        # 64x64 and 96x96 (deep maps one pixel high or wide).  The 32x32 input has an 8x8 head map, fewer cells than the
+        # default K = 100 (the reference's topk raises there too), so K is 64 for this case.
+        det = _detector("fp16x2", flip=True, nms=True, fix_res=False, scales=(0.5, 1, 1.5))
+        shapes = [(40, 600), (600, 40), (60, 60)]
+    elif case == "dla34_test_section":
         det = _detector("fp16x2", flip=True, nms=True, fix_res=False)
         shapes = [(240, 320), (300, 200), (250, 330), (427, 640), (225, 340)]     # 256x352 x3, 320x224, 448x672
     elif case == "scales_1_075_flip":
@@ -171,11 +178,16 @@ def test_run_images_matches_run(case):
     images = _images(shapes, 31)
     if case == "dla34_test_section":
         assert len({det._pre_process_geometry(h, w, 1)[2:4] for h, w in shapes}) == 3
-    got = det.run_images(images)
-    assert len(got) == len(images)
-    for n, im in enumerate(images):
-        want = np.asarray(det.run(im)["results"][1], dtype=np.float32)
-        _assert_like_run(got[n], want, (case, n))
+    topk = det.cfg.TEST.TOPK
+    det.cfg.TEST.TOPK = 64 if case == "extreme_aspect_scales_05_1_15_flip" else topk
+    try:
+        got = det.run_images(images)
+        assert len(got) == len(images)
+        for n, im in enumerate(images):
+            want = np.asarray(det.run(im)["results"][1], dtype=np.float32)
+            _assert_like_run(got[n], want, (case, n))
+    finally:
+        det.cfg.TEST.TOPK = topk
 
 
 def test_run_images_batch_size_does_not_change_rows(tmp_path):

@@ -15,13 +15,45 @@ DEV = "cuda:0"
 OP_TOL = {"fp32": 2e-4, "bf16": 1e-2, "fp16x2": 1e-5, "bf16x2": 3e-4}
 
 
-def model(arch, precision, tc=None):
-    """The arch's default config with the conditioned seed-317 weights (oracle/init_recipe.py), on cuda:0 in
-    ``precision``.  Returns (model, state_dict)."""
+# MODEL.EXTRA of experiments/hrnet_w48_512.yaml (HRNet-W48; its INTERMEDIATE_CHANNEL is 48, HEAD_CONV 64 as W32's)
+HRNET_W48_EXTRA = {
+    "STAGE2": {"NUM_MODULES": 1, "NUM_BRANCHES": 2, "BLOCK": "BASIC", "NUM_BLOCKS": [4, 4], "NUM_CHANNELS": [48, 96]},
+    "STAGE3": {"NUM_MODULES": 4, "NUM_BRANCHES": 3, "BLOCK": "BASIC", "NUM_BLOCKS": [4, 4, 4],
+               "NUM_CHANNELS": [48, 96, 192]},
+    "STAGE4": {"NUM_MODULES": 3, "NUM_BRANCHES": 4, "BLOCK": "BASIC", "NUM_BLOCKS": [4, 4, 4, 4],
+               "NUM_CHANNELS": [48, 96, 192, 384]},
+}
+
+# The eight configurations the network tests run: the seven archs' defaults and HRNet-W48 ("hrnet_w48").
+ARCHS = ["dla_34", "res_50", "hrnet", "hrnet_w48", "mobilenetv3", "hardnet", "mobilenetv2", "ghostnet"]
+
+# Network inputs the detector builds at deployment (TEST.FIX_RES false pads an image of h x w at a test scale to
+# (h | 31) + 1 by (w | 31) + 1): a small image at scale 0.5 (32x32, 64x64), extreme strips (32x640, 640x32: deep maps of
+# one pixel), COCO's 640x213 / 213x640 (224x640, 640x224), 427x640 (448x640) and 480x640 at scale 1.5 (736x960).  B = 1.
+DEPLOY_SHAPES = [(32, 32), (64, 64), (32, 640), (640, 32), (224, 640), (640, 224), (448, 640), (736, 960)]
+# (arch, H, W) the reference cannot run, with the reason; the product refuses them when it builds the plan
+_NO_POOL = "HarDNet's %s deepest map has no 2x2 average pool (the reference's AvgPool2d raises)"
+TOO_SMALL = {("hardnet", 32, 32): _NO_POOL % "1x1", ("hardnet", 32, 640): _NO_POOL % "1x20",
+             ("hardnet", 640, 32): _NO_POOL % "20x1"}
+
+
+def config(arch):
+    """the default config of ``arch``, one of ARCHS ("hrnet_w48": the 'hrnet' arch with HRNET_W48_EXTRA)"""
     from centerpose_b200.config import default_cfg
+    if arch != "hrnet_w48":
+        return default_cfg(arch)
+    cfg = default_cfg("hrnet")
+    cfg.MODEL.EXTRA = HRNET_W48_EXTRA
+    cfg.MODEL.INTERMEDIATE_CHANNEL = 48
+    return cfg
+
+
+def model(arch, precision, tc=None):
+    """``config(arch)`` with the conditioned seed-317 weights (oracle/init_recipe.py), on cuda:0 in ``precision``.
+    Returns (model, state_dict)."""
     from centerpose_b200.model import create_model
     from oracle.init_recipe import conditioned_state_dict
-    cfg = default_cfg(arch)
+    cfg = config(arch)
     m = create_model(cfg.MODEL.NAME, cfg.MODEL.HEAD_CONV, cfg)
     sd = conditioned_state_dict(m.state_dict(), 317)
     m.load_state_dict(sd)
