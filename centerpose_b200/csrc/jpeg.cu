@@ -5,10 +5,11 @@
 //   jpeg_progressive_kernel  progressive images: one CTA per image runs the scans in file order into the same blocks,
 //                        one thread per segment of a scan,
 //   jpeg_idct_kernel     dequantise + libjpeg's ISLOW integer IDCT (jidctint.c), 8 threads per block, into 8-bit
-//                        component planes padded to whole MCUs,
+//                        component planes padded to whole MCUs; status 1 for a block outside the 16-bit range,
 //   jpeg_color_kernel    one thread per output pixel: libjpeg-turbo's fancy upsampling (jdsample.c), integer
 //                        YCbCr->BGR (jdcolor.c), and OpenCV's EXIF orientation as an index mapping.
 // The host side (centerpose_b200/jpeg.py) parses and checks the headers and builds the table; the kernels trust it.
+// An entry with missing_eoi gets status 1 and is not decoded: cv2.imread reads or refuses such files.
 #include "common.cuh"
 
 namespace {
@@ -120,6 +121,10 @@ __global__ void __launch_bounds__(32) jpeg_entropy_kernel(const unsigned char *_
   const Geo g = geometry(e);
   if (!fits(e, g, ws_bytes)) {
     if (threadIdx.x == 0) status[blockIdx.x] = 2;
+    return;
+  }
+  if (e.missing_eoi) {                                      // cv2.imread decides these files
+    if (threadIdx.x == 0) status[blockIdx.x] = 1;
     return;
   }
   if (threadIdx.x == 0) status[blockIdx.x] = 0;
@@ -287,6 +292,10 @@ __global__ void __launch_bounds__(32, 1) jpeg_progressive_kernel(const unsigned 
     if (threadIdx.x == 0) status[blockIdx.x] = 2;
     return;
   }
+  if (e.missing_eoi) {                                      // cv2.imread decides these files
+    if (threadIdx.x == 0) status[blockIdx.x] = 1;
+    return;
+  }
   if (threadIdx.x == 0) {
     status[blockIdx.x] = 0;
     failed = 0;
@@ -339,14 +348,21 @@ __device__ __forceinline__ void idct8(const int (&x)[8], int (&o)[8], int shift)
   o[3] = (t13 + a0 + rnd) >> shift; o[4] = (t13 - a0 + rnd) >> shift;
 }
 
+// a dequantised coefficient or pass-1 output beyond this is flagged (jpeg.IDCT_RANGE): below it every sum and product
+// of libjpeg-turbo's 16-bit SIMD IDCT fits int16, so its saturating and wrapping arithmetic agrees with these 32-bit
+// passes; no encoder writes such blocks, corrupt or hostile files can
+constexpr int kIdctRange = 16383;
+
 // grid (block groups, image) x 256 threads: 8 lanes per 8x8 block, lane r takes column r (pass 1, through shared
-// memory) then row r (pass 2); the warps of an image stride over all its blocks, 4 per warp at a time
+// memory) then row r (pass 2); the warps of an image stride over all its blocks, 4 per warp at a time.  A block with a
+// value outside +-kIdctRange sets the image's status to 1 (the caller decodes it on the host)
 __global__ void __launch_bounds__(256) jpeg_idct_kernel(const cpb200_jpeg_image *__restrict__ table,
-                                                        unsigned char *__restrict__ ws, size_t ws_bytes) {
+                                                        unsigned char *__restrict__ ws, size_t ws_bytes,
+                                                        int *__restrict__ status) {
   __shared__ int sh[8][4][64];
   const cpb200_jpeg_image &e = table[blockIdx.y];
   const Geo g = geometry(e);
-  if (!fits(e, g, ws_bytes)) return;
+  if (!fits(e, g, ws_bytes) || e.missing_eoi) return;
   const short *coef = reinterpret_cast<const short *>(ws + e.coef_offset);
   unsigned char *planes = ws + e.plane_offset;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, grp = lane >> 3, r = lane & 7;
@@ -358,12 +374,20 @@ __global__ void __launch_bounds__(256) jpeg_idct_kernel(const cpb200_jpeg_image 
     if (active) {
       c = blk >= g.base[2] && e.ncomp == 3 ? 2 : blk >= g.base[1] && e.ncomp == 3 ? 1 : 0;
       int x[8], o[8];
+      bool out = false;
 #pragma unroll
-      for (int k = 0; k < 8; ++k)   // dequantise as libjpeg-turbo's SIMD code does: the 16-bit product
-        x[k] = (short)(coef[blk * 64 + k * 8 + r] * e.qt[c][k * 8 + r]);
+      for (int k = 0; k < 8; ++k) {   // flagged blocks go on with the 16-bit product, so no 32-bit sum overflows
+        const int p = coef[blk * 64 + k * 8 + r] * e.qt[c][k * 8 + r];
+        out |= abs(p) > kIdctRange;
+        x[k] = (short)p;
+      }
       idct8(x, o, 11);                                        // CONST_BITS - PASS1_BITS
 #pragma unroll
-      for (int k = 0; k < 8; ++k) sh[warp][grp][k * 8 + r] = o[k];
+      for (int k = 0; k < 8; ++k) {
+        sh[warp][grp][k * 8 + r] = o[k];
+        out |= abs(o[k]) > kIdctRange;
+      }
+      if (out) status[blockIdx.y] = 1;
     }
     __syncwarp();
     if (active) {
@@ -412,7 +436,7 @@ __global__ void __launch_bounds__(256) jpeg_color_kernel(const cpb200_jpeg_image
                                                          unsigned char *__restrict__ dst) {
   const cpb200_jpeg_image &e = table[blockIdx.y];
   const Geo g = geometry(e);
-  if (!fits(e, g, ws_bytes)) return;
+  if (!fits(e, g, ws_bytes) || e.missing_eoi) return;
   const int h = e.h, w = e.w, o = e.orientation;
   const int ow = o >= 5 ? h : w;
   const int64_t total = (int64_t)h * w;
@@ -468,7 +492,7 @@ extern "C" int cpb200_jpeg_decode_batch(const unsigned char *src, const cpb200_j
   if (rc) return rc;
   // the sizes live on the device: enough blocks per image to fill the GPU for one large image, fewer as B grows
   const dim3 grid((unsigned)std::max(1, 132 * 8 / B), (unsigned)B);
-  jpeg_idct_kernel<<<grid, 256, 0, st>>>(table, ws, workspace_bytes);
+  jpeg_idct_kernel<<<grid, 256, 0, st>>>(table, ws, workspace_bytes, status);
   rc = cpb::check_launch("jpeg_idct_kernel");
   if (rc) return rc;
   jpeg_color_kernel<<<grid, 256, 0, st>>>(table, ws, workspace_bytes, dst);

@@ -18,7 +18,16 @@ The device decodes 8-bit grayscale or YCbCr files with chroma sampled (1, 1) and
 
 Everything else has ``eligible == False`` and ``progressive is None``, ``reason`` says why, and the file stays with
 ``cv2.imread``.  The kernels trust the table, so everything read from the file that sizes or indexes it is checked
-here; a file the parser cannot read raises ``ValueError`` naming the image.
+here; a file the parser cannot read raises ``ValueError`` naming the image.  That includes a Huffman table with an
+all-ones code, which libjpeg refuses.
+
+The device sets status 1 for a file it takes, which then goes to ``cv2.imread``, when:
+
+- its last scan is not ended by EOI (``info.eoi`` False, the table's ``missing_eoi``).  libjpeg refuses some such
+  files and reads others, by more than their headers say, so the kernels do not decode them.
+- its entropy data ends early or holds an undefined code.
+- a block's dequantised coefficients or IDCT pass-1 outputs leave +-``IDCT_RANGE``.  There libjpeg-turbo's 16-bit SIMD
+  arithmetic saturates or wraps, and no real encoder goes.
 """
 from __future__ import annotations
 
@@ -31,6 +40,9 @@ ZIGZAG = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 1
                    6, 7, 14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38,
                    31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63], np.int64)
 LUT_BITS = 9
+# jpeg_idct_kernel sets status 1 for a block with a dequantised coefficient or a pass-1 output beyond +-IDCT_RANGE:
+# below it every sum and product libjpeg-turbo's 16-bit SIMD IDCT forms fits int16 (see DESIGN.md)
+IDCT_RANGE = 16383
 # libjpeg refuses dimensions above JPEG_MAX_DIMENSION, so cv2.imread returns nothing for them: they stay on the host
 MAX_DIMENSION = 65500
 
@@ -44,7 +56,7 @@ JPEG_IMAGE = np.dtype([("seg_offset", "<i8"), ("huff_offset", "<i8"), ("coef_off
                        ("dst_offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("ncomp", "<i4"), ("hs", "<i4"), ("vs", "<i4"),
                        ("orientation", "<i4"), ("restart_interval", "<i4"), ("nseg", "<i4"), ("dc_tbl", "u1", (4,)),
                        ("ac_tbl", "u1", (4,)), ("qt", "<u2", (3, 64)), ("scan_offset", "<i8"), ("nscan", "<i4"),
-                       ("pad", "<i4")])
+                       ("missing_eoi", "<i4")])
 assert JPEG_IMAGE.itemsize == 480
 # struct cpb200_jpeg_scan (include/centerpose_b200.h): one scan of a progressive image
 SCAN = np.dtype([("seg_offset", "<i8"), ("nseg", "<i4"), ("restart_interval", "<i4"), ("ncomp", "<i4"),
@@ -63,7 +75,7 @@ class JpegInfo:
     ``restart_interval`` and ``segments``, the (start, end) byte range of each entropy-coded segment.  For progressive
     files the device takes, ``progressive`` is the list of scans (``JpegScan``) and ``tables`` the ``HUFF`` tables
     they bind, in the order of their first use; ``qt`` is set, and ``dc``, ``ac``, ``restart_interval`` and
-    ``segments`` are per scan."""
+    ``segments`` are per scan.  ``eoi`` says whether EOI ends the last scan (the device flags the file otherwise)."""
 
     def __init__(self):
         self.eligible = False
@@ -71,6 +83,7 @@ class JpegInfo:
         self.reason = ""
         self.orientation = 1
         self.restart_interval = 0
+        self.eoi = True
 
     def size_after_orientation(self):
         return oriented_size(self.h, self.w, self.orientation)
@@ -156,7 +169,8 @@ def tiff_orientation(t):
 
 def build_huff(bits, vals, name, dc):
     """One ``HUFF`` table from the DHT code-length counts ``bits[1..16]`` and symbols; rejects counts that do not form
-    a prefix code (T.81 C.2) and, for DC tables, symbols above 15 (libjpeg refuses both)."""
+    a prefix code without an all-ones code (T.81 C.2, Annex C: no code may consist of 1-bits only) and, for DC tables,
+    symbols above 15 (libjpeg refuses all of these)."""
     if sum(bits) > 256 or sum(bits) > len(vals):
         raise ValueError("%s: bad Huffman table (%d codes)" % (name, sum(bits)))
     if dc and any(v > 15 for v in vals):
@@ -177,8 +191,8 @@ def build_huff(bits, vals, name, dc):
                 code += 1
                 k += 1
             t["maxcode"][ln] = code - 1
-        if code > (1 << ln):
-            raise ValueError("%s: Huffman code lengths do not form a prefix code" % name)
+        if code >= (1 << ln):                    # the next code of this length would be all ones, or no code fits
+            raise ValueError("%s: Huffman code lengths do not form a prefix code without an all-ones code" % name)
         code <<= 1
     return t
 
@@ -359,10 +373,11 @@ def parse(data, name="image"):
         info.ac.append(ta)
     info.huff = huff
     mx, my = info.mcu
-    info.segments, _, why = _segments(_markers(d, pos), pos, n, mx * my, info.restart_interval)
+    info.segments, end, why = _segments(_markers(d, pos), pos, n, mx * my, info.restart_interval)
     if why:
         info.reason = why
         return info
+    info.eoi = end + 1 < n and d[end + 1] == 0xD9
     info.eligible = True
     return info
 
@@ -420,7 +435,8 @@ def _progressive_scans(d, pos, seg, info, comps, huff, name):
             return None, None, "scan %d: %s" % (k, why)
         scans.append(scan)
         if end >= n:
-            break                                # cut inside this scan's data: the device flags what is missing
+            info.eoi = False                     # cut inside this scan's data, or no EOI after it: the device flags it
+            break
         # the markers up to the next scan: tables and restart intervals may change, nothing else may
         pos, m = end, 0
         while m != 0xDA:
@@ -496,6 +512,7 @@ def pack(infos, datas, dst_offsets, alloc=lambda n: np.empty(n, np.uint8)):
         e["dst_offset"] = dst_offsets[n]
         e["h"], e["w"], e["ncomp"], e["hs"], e["vs"] = info.h, info.w, info.ncomp, info.hs, info.vs
         e["orientation"] = info.orientation
+        e["missing_eoi"] = not info.eoi
         for c in range(info.ncomp):
             e["qt"][c] = info.qt[c]
     if pos >= 2 ** 62:

@@ -194,7 +194,8 @@ typedef struct cpb200_jpeg_image {
   int32_t nscan;             /* 0: sequential, every field above as described.  > 0: progressive, decoded scan by
                                 scan; seg_offset, restart_interval, nseg, dc_tbl and ac_tbl are unused, the scans
                                 carry them */
-  int32_t pad;
+  int32_t missing_eoi;       /* 1: the last scan is not ended by EOI; status 1 without decoding (libjpeg reads some
+                                such files and refuses others) */
 } cpb200_jpeg_image;
 
 /* cv2.imread(path, IMREAD_COLOR) of sequential- and progressive-Huffman JPEG files, byte for byte (libjpeg-turbo's
@@ -208,8 +209,10 @@ typedef struct cpb200_jpeg_image {
  * (every coefficient coded down to bit 0), since libjpeg smooths blocks otherwise.  IDCT, upsampling and colour
  * conversion then run over the whole launch.  status[b] (DEVICE int array) is 0 when image b decoded, non-zero when
  * its entropy data was bad (a code longer than 16 bits, a run past the scan's last coefficient, a refinement symbol
- * of size other than 0 or 1, or data ending before a segment's last unit); the image's pixels are then undefined,
- * other images are unaffected.  1 <= B <= 65535. */
+ * of size other than 0 or 1, or data ending before a segment's last unit), when a block's dequantised coefficients or
+ * IDCT pass-1 outputs leave +-16383 (libjpeg-turbo's 16-bit SIMD IDCT saturates or wraps there), or when the entry's
+ * missing_eoi is set (then it is not decoded at all); the image's pixels are then undefined, other images are
+ * unaffected.  1 <= B <= 65535. */
 int cpb200_jpeg_decode_batch(const unsigned char *src, const cpb200_jpeg_image *table, int B, void *workspace,
                              size_t workspace_bytes, unsigned char *dst, int *status, void *stream);
 
