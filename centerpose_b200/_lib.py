@@ -1,4 +1,5 @@
-"""ctypes binding of the C ABI declared in ``include/centerpose_b200.h`` and ``include/centerpose_b200_heads_train.h``.
+"""ctypes binding of the C ABI declared in ``include/centerpose_b200.h``, ``include/centerpose_b200_heads_train.h`` and
+``include/centerpose_b200_video.h``.
 
 The headers are the only statement of the ABI: ``lib()`` binds ``restype`` and ``argtypes`` of every ``cpb200_*``
 prototype of each of them (``HEADERS``) when the library loads, and a type the binding does not know fails the load.  ``launch`` makes
@@ -21,7 +22,8 @@ LIBPATH = os.path.join(_HERE, "lib", "libcenterpose_b200.so")
 HEADER = os.path.join(_HERE, "..", "include", "centerpose_b200.h")
 # the library's other public headers, each declaring its own entry points with HEADER's conventions and types
 HEADS_TRAIN_HEADER = os.path.join(_HERE, "..", "include", "centerpose_b200_heads_train.h")
-HEADERS = (HEADER, HEADS_TRAIN_HEADER)
+VIDEO_HEADER = os.path.join(_HERE, "..", "include", "centerpose_b200_video.h")
+HEADERS = (HEADER, HEADS_TRAIN_HEADER, VIDEO_HEADER)
 
 _lib = None
 

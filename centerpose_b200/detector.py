@@ -12,6 +12,8 @@ Differences that are additive only:
   * ``run_batch`` (new): many pre-processed images per call — the reference API is single-image;
   * ``run_images`` (new): ``run()`` for a list of raw images, batched on the device, with the reference's
     test-time flip / multi-scale / soft-NMS settings, and optionally the drawn images and the heat-map views;
+  * ``run_video`` (new): tools/demo.py's video and webcam loop as a generator of per-frame rows (and drawn frames),
+    frames read on a background thread (``video.FrameReader``) and batched through ``run_images``' kernels;
   * ``show_results`` / ``render_poses`` draw the detections on the device (csrc/render.cu), and ``debug()`` (DEBUG >= 2)
     blends the predicted heat maps onto the network input on the device (csrc/heatmaps.cu), byte for byte as the
     reference's Debugger.  ``debug()`` reads ``output[0]`` / ``output[4]`` and ``cfg.LOSS.HM_HP`` where the
@@ -799,23 +801,12 @@ class MultiPoseDetector(BaseDetector):
             inp = torch.empty((2 * B if flip else B, 3, inp_h, inp_w), dtype=torch.float32, device=dev)
             _lib.launch("pre_process_batch", dev, pixels, buf, B, inp, inp_h, inp_w, mean, std, 1 if flip else 0)
             outputs = self.model(inp)
-            if flip:
-                # process()'s gating (multi_pose.py:35-53) on B [image, mirror] pairs
-                hm, wh, hps, reg, hm_hp, hp_offset = outputs
-                sigmoid_(hm)
-                if cfg.LOSS.HM_HP and not cfg.LOSS.MSE_LOSS:
-                    sigmoid_(hm_hp)
-                hm, wh, hps, hm_hp = flip_merge(hm, wh, hps, hm_hp if cfg.LOSS.HM_HP else None, self.flip_idx)
-                reg = reg[0::2].contiguous() if cfg.LOSS.REG_OFFSET else None
-                hp_offset = hp_offset[0::2].contiguous() if cfg.LOSS.REG_HP_OFFSET else None
-                dets = multi_pose_decode(hm, wh, hps, reg=reg, hm_hp=hm_hp, hp_offset=hp_offset, K=K, affine=aff)
-            else:
-                dets = self._decode_heads(outputs, affine=aff)
-                if return_heatmaps and si == S - 1:
-                    # the decode read the logits; the views take the maps as process() leaves them
-                    sigmoid_(outputs[0])
-                    if not cfg.LOSS.MSE_LOSS:
-                        sigmoid_(outputs[4])
+            dets = self._decode_outputs(outputs, aff)
+            if not flip and return_heatmaps and si == S - 1:
+                # the decode read the logits; the views take the maps as process() leaves them
+                sigmoid_(outputs[0])
+                if not cfg.LOSS.MSE_LOSS:
+                    sigmoid_(outputs[4])
             rows[dst, si * K:(si + 1) * K] = dets
             if return_heatmaps and si == S - 1:
                 step = 2 if flip else 1
@@ -862,6 +853,235 @@ class MultiPoseDetector(BaseDetector):
             if return_heatmaps:
                 res += ([dict(zip(heatmaps.VIEWS, files[2 * i:2 * i + 2])) for i in range(len(loaded))],)
         return res
+
+    # -- additive: video and webcam streams (tools/demo.py's video branch) --------------------------
+    def run_video(self, source, max_batch=None, return_images=False, encode_png=False):
+        """Additive: tools/demo.py's video and webcam loop (``detector.run(img)`` per ``cv2.VideoCapture`` frame) as a
+        generator.  ``source`` is a video path, ``"webcam"``, a camera index or an iterable of BGR uint8 (H, W, 3)
+        arrays (``video.FrameReader``).  Yields ``(frame_index, rows)`` in frame order, ``rows`` the float32 (N, 56)
+        array ``run_images([frame])[0]`` returns, bit for bit, under the same test settings (``FLIP_TEST``,
+        ``TEST_SCALES``, ``FIX_RES``, ``NMS``); like those, they match ``run(frame)['results'][1]`` up to ``run()``'s
+        host back-projection.  With ``return_images=True`` it yields ``(frame_index, rows, drawn)``, ``drawn`` what
+        ``render_poses([frame], [rows])`` draws, byte for byte, or with ``encode_png=True`` its PNG file as
+        ``run_images`` encodes it.  The drawing tables are built on the device from the rows
+        (``render.DevicePlan``, ``cpb200_render_plan_batch``); that needs ``TEST.VIS_THRESH >= 0``.
+
+        Frames are batched, at most ``max_batch`` per forward (default 32; 1 for a camera, which would otherwise wait
+        for frames that have not happened yet).  A batch holds frames of one shape; the resize and pre-process tables,
+        the back-projections and the network plan are made once per shape.  Per batch the frames go up on a copy
+        stream into one of two device buffers while the previous batch computes, the same kernels as ``run_images``
+        run (``cpb200_resize_linear_u8_batch``, ``cpb200_pre_process_batch``, the forward, ``cpb200_flip_merge``, the
+        decode with the back-projection, ``cpb200_soft_nms_39_batch``), and the rows come back into pinned memory
+        without a wait; the generator waits for them one batch later.  With drawing, batch n's frames are drawn in
+        their device buffer once batch n + 1 is enqueued and copied back into pinned memory without a wait
+        (``encode_png`` waits for the files), and yielded one batch later still.  The work goes to the stream that
+        is current when ``run_video`` is called.  A path that does not open raises
+        ``FileNotFoundError`` here, before the first frame."""
+        from .video import FrameReader, is_live
+        if encode_png and not return_images:
+            raise ValueError("run_video: encode_png=True needs return_images=True")
+        if max_batch is None:
+            max_batch = 1 if is_live(source) else 32
+        if int(max_batch) < 1:
+            raise ValueError("run_video: max_batch must be >= 1, got %r" % (max_batch,))
+        if return_images and not float(self.cfg.TEST.VIS_THRESH) >= 0:
+            raise ValueError("run_video: drawing on the device needs TEST.VIS_THRESH >= 0, got %r"
+                             % (self.cfg.TEST.VIS_THRESH,))
+        reader = FrameReader(source, slots=2 * int(max_batch) + 2)
+        return self._video_frames(reader, int(max_batch), bool(return_images), bool(encode_png),
+                                  torch.cuda.current_stream(torch.device("cuda")))
+
+    def _video_shape(self, h, w, max_batch):
+        """What every batch of (h, w) frames shares: per test scale the ``pack_group`` tables of ``max_batch`` frames
+        lying back to back in a pixel buffer, uploaded once, with the back-projections, and the resize scratch."""
+        dev = torch.device("cuda")
+        scales = []
+        frame = np.broadcast_to(np.uint8(0), (h, w, 3))
+        for scale in self.scales:
+            new_h, new_w, inp_h, inp_w, trans_input, meta = self._pre_process_geometry(h, w, scale)
+            aff = affine_for_meta([meta], scale).numpy()
+            host, at = pack_group([frame] * max_batch, [(new_h, new_w)] * max_batch, [trans_input] * max_batch,
+                                  np.repeat(aff, max_batch, 0), list(range(max_batch)),
+                                  alloc=lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True),
+                                  src_offsets=[b * h * w * 3 for b in range(max_batch)])
+            tables = host.to(dev)
+            scales.append({"tables": tables, "at": at, "inp": (inp_h, inp_w),
+                           "aff": tables[at["o_aff"]:at["o_aff"] + max_batch * 24].view(torch.float32).view(-1, 6),
+                           "scratch": torch.empty(at["scratch"], dtype=torch.uint8, device=dev)
+                           if at["o_rsz"] is not None else None})
+        return {"hw": (h, w), "scales": scales,
+                "pixels": [torch.empty(max_batch * h * w * 3, dtype=torch.uint8, device=dev) for _ in range(2)]}
+
+    def _decode_outputs(self, outputs, aff):
+        """The decode, with the back-projections ``aff``, of one forward of B images (B [image, mirror] pairs with
+        ``FLIP_TEST``) for ``run_images`` and ``run_video``: ``process()``'s gating (multi_pose.py:35-53)."""
+        cfg = self.cfg
+        if not cfg.TEST.FLIP_TEST:
+            return self._decode_heads(outputs, affine=aff)
+        hm, wh, hps, reg, hm_hp, hp_offset = outputs
+        sigmoid_(hm)
+        if cfg.LOSS.HM_HP and not cfg.LOSS.MSE_LOSS:
+            sigmoid_(hm_hp)
+        hm, wh, hps, hm_hp = flip_merge(hm, wh, hps, hm_hp if cfg.LOSS.HM_HP else None, self.flip_idx)
+        reg = reg[0::2].contiguous() if cfg.LOSS.REG_OFFSET else None
+        hp_offset = hp_offset[0::2].contiguous() if cfg.LOSS.REG_HP_OFFSET else None
+        return multi_pose_decode(hm, wh, hps, reg=reg, hm_hp=hm_hp, hp_offset=hp_offset, K=int(cfg.TEST.TOPK),
+                                 affine=aff)
+
+    def _video_batch(self, shape, pix, B):
+        """Enqueues one batch of B frames lying in ``pix`` on the current stream; returns its (B, S * K, 56) rows."""
+        import ctypes
+        from . import _lib
+        from .soft_nms import soft_nms_39_cuda_batch
+        cfg, dev = self.cfg, torch.device("cuda")
+        flip = bool(cfg.TEST.FLIP_TEST)
+        K, S = int(cfg.TEST.TOPK), len(self.scales)
+        mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
+        std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
+        rows = torch.empty((B, S * K, 56), dtype=torch.float32, device=dev)
+        for si, st in enumerate(shape["scales"]):
+            at, tables = st["at"], st["tables"]
+            pixels = pix.data_ptr()
+            if st["scratch"] is not None:
+                _lib.launch("resize_linear_u8_batch", dev, pixels, tables.data_ptr() + at["o_rsz"], B, st["scratch"])
+                pixels = st["scratch"].data_ptr()
+            inp_h, inp_w = st["inp"]
+            inp = torch.empty((2 * B if flip else B, 3, inp_h, inp_w), dtype=torch.float32, device=dev)
+            _lib.launch("pre_process_batch", dev, pixels, tables, B, inp, inp_h, inp_w, mean, std, 1 if flip else 0)
+            rows[:, si * K:(si + 1) * K] = self._decode_outputs(self.model(inp), st["aff"][:B])
+        if cfg.TEST.NMS or S > 1:
+            soft_nms_39_cuda_batch(rows, Nt=0.5, method=2)
+        return rows
+
+    def _video_frames(self, reader, max_batch, return_images, encode_png, compute):
+        """The generator of ``run_video``.  All its device work goes to ``compute`` (the caller's stream when
+        ``run_video`` was called) and to its own copy stream, whatever stream is current when it resumes.  Batch n's
+        upload and compute are enqueued before batch n - 1 is finished; with drawing, batch n - 1's drawing is
+        enqueued then too, and its frames are yielded once batch n's is enqueued, so each wait is for work enqueued
+        one batch earlier."""
+        from . import render
+        dev = torch.device("cuda")
+        copy = torch.cuda.Stream(dev)
+        plan = render.DevicePlan(self.cfg.TEST.VIS_THRESH, self.cfg.DEBUG_THEME, dev) if return_images else None
+        shape = None                   # the state of the current frame shape; a new shape replaces it
+        host_rows = [None, None]
+        n_batch = 0
+        computed = drawn = None        # the batch whose rows are on their way back; the batch being drawn
+
+        def batches():
+            batch = []
+            for fr in reader:
+                if batch and (fr.image.shape != batch[0].image.shape or len(batch) == max_batch):
+                    yield batch
+                    batch = []
+                batch.append(fr)
+                if len(batch) == max_batch or reader.live:
+                    yield batch
+                    batch = []
+            if batch:
+                yield batch
+
+        def rows_of(p):
+            """Waits for batch p's rows, copies them out and hands its frames back to the reader."""
+            p["ready"].synchronize()
+            rows = p["host"][:p["B"]].numpy()
+            p["out"] = [(fr.index, rows[b].copy()) for b, fr in enumerate(p["frames"])]
+            for fr in p["frames"]:
+                fr.release()
+            return p["out"]
+
+        def draw(p):
+            """Enqueues batch p's drawing in place in its pixel buffer and the copy of the drawn frames."""
+            rows_of(p)
+            h, w = p["shape"]["hw"]
+            B, hw3 = p["B"], h * w * 3
+            plan.draw(p["plan"], p["pix"])
+            if encode_png:
+                from . import png
+                p["drawn"] = png.encode_at([p["pix"].data_ptr() + b * hw3 for b in range(B)], [(h, w)] * B,
+                                           [3 * w] * B, dev)
+            else:
+                host = p["shape"]["drawn"][p["k"]]
+                host[:B * hw3].copy_(p["pix"][:B * hw3], non_blocking=True)
+                p["drawn_ready"] = torch.cuda.Event()
+                p["drawn_ready"].record(compute)
+            p["free"].record(compute)
+
+        def drawn_of(p):
+            h, w = p["shape"]["hw"]
+            if encode_png:
+                drawn = p["drawn"]
+            else:
+                p["drawn_ready"].synchronize()
+                hv = p["shape"]["drawn"][p["k"]].numpy()
+                drawn = [hv[b * h * w * 3:(b + 1) * h * w * 3].reshape(h, w, 3).copy() for b in range(p["B"])]
+            return [(i, r, d) for (i, r), d in zip(p["out"], drawn)]
+
+        try:
+            with torch.no_grad():
+                for frames in batches():
+                    with torch.cuda.stream(compute):
+                        B = len(frames)
+                        h, w = frames[0].image.shape[:2]
+                        if shape is None or shape["hw"] != (h, w):
+                            shape = self._video_shape(h, w, max_batch)
+                            shape["free"] = [torch.cuda.Event(), torch.cuda.Event()]
+                            shape["next"] = 0
+                            for t in shape["pixels"]:
+                                t.record_stream(copy)
+                            if return_images and not encode_png:
+                                shape["drawn"] = [torch.empty(max_batch * h * w * 3, dtype=torch.uint8,
+                                                              pin_memory=True) for _ in range(2)]
+                        k = shape["next"]
+                        shape["next"] = 1 - k
+                        pix, hw3 = shape["pixels"][k], h * w * 3
+                        # the upload waits until the batch before last (the last user of this buffer) is done with it
+                        copy.wait_event(shape["free"][k])
+                        with torch.cuda.stream(copy):
+                            for b, fr in enumerate(frames):
+                                pix[b * hw3:(b + 1) * hw3].copy_(fr.slot, non_blocking=True)
+                            uploaded = torch.cuda.Event()
+                            uploaded.record(copy)
+                        compute.wait_event(uploaded)
+                        rows = self._video_batch(shape, pix, B)
+                        batch = {"frames": frames, "B": B, "shape": shape, "pix": pix, "k": k, "free": shape["free"][k]}
+                        if return_images:
+                            batch["plan"] = plan.plan(rows, h, w)
+                        j = n_batch % 2
+                        n_batch += 1
+                        if host_rows[j] is None:
+                            host_rows[j] = torch.empty((max_batch,) + tuple(rows.shape[1:]), dtype=torch.float32,
+                                                       pin_memory=True)
+                        host_rows[j][:B].copy_(rows, non_blocking=True)
+                        batch["host"] = host_rows[j]
+                        batch["ready"] = torch.cuda.Event()
+                        batch["ready"].record(compute)
+                        if not return_images:
+                            batch["free"].record(compute)
+                            out = rows_of(computed) if computed is not None else []
+                        else:
+                            out = drawn_of(drawn) if drawn is not None else []
+                            drawn = None
+                            if computed is not None:
+                                draw(computed)
+                                drawn = computed
+                        computed = batch
+                    yield from out
+                with torch.cuda.stream(compute):
+                    out = []
+                    if return_images:
+                        if drawn is not None:
+                            out += drawn_of(drawn)
+                        if computed is not None:
+                            draw(computed)
+                            out += drawn_of(computed)
+                    elif computed is not None:
+                        out = rows_of(computed)
+                    computed = drawn = None
+                yield from out
+        finally:
+            reader.close()
+            compute.wait_stream(copy)
 
 
 detector_factory = {"multi_pose": MultiPoseDetector}     # detector_factory.py:5-7

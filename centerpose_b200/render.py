@@ -230,3 +230,143 @@ def download(pixels, offsets, shapes):
     end = max((o + h * w * 3 for o, (h, w) in zip(offsets, shapes)), default=0)
     host = pixels[:end].cpu().numpy()
     return [host[o:o + h * w * 3].reshape(h, w, 3) for o, (h, w) in zip(offsets, shapes)]
+
+
+# -- the drawing plan built on the device (csrc/render_plan.cu, include/centerpose_b200_video.h) ------------------
+LABEL = np.dtype([(n, "<i4") for n in ("tw", "th", "x0", "x1", "y0", "y1")])
+KEY = np.dtype([(n, "<i4") for n in ("label", "ax", "bx", "ay", "by", "valid")])
+assert (LABEL.itemsize, KEY.itemsize) == (24, 24)
+LABELS = 11                                  # p0.0 .. p1.0, every score a sigmoid and the soft-NMS decay can give
+_PERSON_TEXT = PERSON.fields["text_begin"][1] // 4      # text_begin, text_count: int32 words 10 and 11
+
+
+def label_string(k):
+    """The label of label index k >= 0: ``label_text(score)`` for every score with round(10 * score) == k."""
+    return "p%d.%d" % (k // 10, k % 10)
+
+
+def label_table(n):
+    """The ``cpb200_render_label`` metrics of label indices 0 .. n - 1."""
+    t = np.zeros(n, LABEL)
+    for k in range(n):
+        txt = label_string(k)
+        (tw, th), _ = cv2.getTextSize(txt, FONT, 0.5, 2)
+        t[k] = (tw, th) + _text_extent(txt)
+    return t
+
+
+class DevicePlan:
+    """Draws detection rows that are on the device with no host loop over persons or limbs.
+    ``cpb200_render_plan_batch`` builds ``build()``'s person, limb and vertex tables from the rows and lists each
+    person's label key (label string, border cut).  One small copy brings the keys back; the text tables of keys not
+    seen before are captured from ``cv2.putText`` (``text_table``) and added to a device cache, and each person's
+    text_begin / text_count is pointed at its key's entry.  ``cpb200_render_poses_batch`` then draws, byte for byte as
+    ``build()`` + ``launch()``.  Everything is enqueued on the current stream."""
+
+    def __init__(self, vis_thresh, theme, device):
+        vis_thresh = float(vis_thresh)
+        if not vis_thresh >= 0:
+            raise ValueError("render: the device drawing plan needs TEST.VIS_THRESH >= 0, got %r" % vis_thresh)
+        self.vis_thresh, self.device = vis_thresh, device
+        b, g, r = theme_color(theme)
+        self.color = b | g << 8 | r << 16
+        self._set_labels(LABELS)
+        self.verts_per_image, self.rows_per_image = 1 << 14, 1 << 20
+        self._keys = {}                          # key -> (text_begin, text_count) in the cache
+        self._text_px, self._luts = [np.zeros(0, TEXT_PX)], [np.zeros(0, np.uint8)]
+        self._n_px = self._n_lut = 0
+        self._cache = None
+
+    def _set_labels(self, n):
+        self.n_labels = n
+        self._labels = torch.from_numpy(label_table(n).view(np.uint8)).to(self.device)
+
+    def plan(self, rows, h, w):
+        """Enqueues the plan of the (B, N, 56) float32 CUDA ``rows`` of B (h, w) images, and the copy of its keys to
+        pinned memory.  Returns the handle ``draw`` takes."""
+        from . import _lib
+        B, N = int(rows.shape[0]), int(rows.shape[1])
+        dev = self.device
+        sizes = [B * IMAGE.itemsize, B * N * PERSON.itemsize, B * N * 18 * LIMB.itemsize,
+                 B * self.verts_per_image * 8, B * N * KEY.itemsize, B * 16]
+        at = np.cumsum([0] + [(s + 15) // 16 * 16 for s in sizes]).tolist()
+        buf = torch.empty(max(at[-1], 16), dtype=torch.uint8, device=dev)
+        base = buf.data_ptr()
+        _lib.launch("render_plan_batch", dev, rows, B, N, h, w, self.vis_thresh, self.color, self._labels,
+                    self.n_labels, self.verts_per_image, self.rows_per_image, base + at[0], base + at[1],
+                    base + at[2], base + at[3], base + at[4], base + at[5])
+        host = torch.empty(at[6] - at[4], dtype=torch.uint8, pin_memory=True)
+        host.copy_(buf[at[4]:at[6]], non_blocking=True)
+        done = torch.cuda.Event()
+        done.record(torch.cuda.current_stream(dev))
+        return {"rows": rows, "B": B, "N": N, "hw": (h, w), "buf": buf, "at": at, "host": host, "done": done,
+                "verts_per_image": self.verts_per_image, "rows_per_image": self.rows_per_image}
+
+    def _text(self, key):
+        """The cache entry (text_begin, text_count) of ``key`` = (label, ax, bx, ay, by), captured when new."""
+        hit = self._keys.get(key)
+        if hit is None:
+            k, ax, bx, ay, by = key
+            dx, dy, tl = text_table(label_string(k), ax, bx, ay, by)
+            t = np.zeros(len(dx), TEXT_PX)
+            t["dx"], t["dy"], t["lut"] = dx, dy, self._n_lut + 256 * np.arange(len(dx))
+            self._text_px.append(t)
+            self._luts.append(np.ascontiguousarray(tl).reshape(-1))
+            hit = self._keys[key] = (self._n_px, len(dx))
+            self._n_px += len(dx)
+            self._n_lut += tl.size
+            self._cache = None
+        return hit
+
+    def draw(self, p, pixels):
+        """Waits for ``p``'s keys, then enqueues the drawing of its B images, which lie back to back in the uint8 CUDA
+        tensor ``pixels``, in place."""
+        from . import _lib
+        p["done"].synchronize()
+        B, N = p["B"], p["N"]
+        at = p["at"]
+        hv = p["host"].numpy()
+        keys = hv[:B * N * KEY.itemsize].view(KEY).reshape(B, N)
+        counts = hv[at[5] - at[4]:at[5] - at[4] + B * 16].view(np.int32).reshape(B, 4)
+        status = counts[:, 3]
+        if (status == 3).any():
+            raise ValueError("render: a limb's squared length overflows int32 (the reference's numpy length is NaN)")
+        if (status == 2).any():
+            labels = [int(keys[b, i]["label"]) for b in np.flatnonzero(status == 2) for i in range(N)]
+            if min(labels) < 0 or not np.isfinite(p["rows"][..., 4].float().cpu().numpy()).all():
+                raise ValueError("render: a drawn row's score is not finite")
+        if (status != 0).any():
+            # a vertex or span-row share, or the label table, was too small: plan again with enough of each
+            need_v, need_r = int(counts[:, 1].max()), int(counts[:, 2].max())
+            self.verts_per_image = max(self.verts_per_image, 1 << max(need_v - 1, 1).bit_length())
+            self.rows_per_image = max(self.rows_per_image, 1 << max(need_r - 1, 1).bit_length())
+            if (status == 2).any():
+                scores = p["rows"][..., 4].double().cpu().numpy()
+                scores = scores[scores > self.vis_thresh]
+                self._set_labels(max(self.n_labels, int(np.floor(scores.max() * 10 + 1)) + 2))
+            return self.draw(self.plan(p["rows"], *p["hw"]), pixels)
+        n = counts[:, 0]
+        text = np.zeros((B, N, 2), np.int32)
+        for b in range(B):
+            kb = keys[b, :n[b]]
+            valid = kb["valid"] != 0
+            if not valid.any():
+                continue
+            k5 = np.stack([kb[f] for f in ("label", "ax", "bx", "ay", "by")], 1)[valid]
+            uniq, inv = np.unique(k5, axis=0, return_inverse=True)
+            entries = np.array([self._text(tuple(int(v) for v in u)) for u in uniq], np.int32).reshape(-1, 2)
+            text[b, np.flatnonzero(valid)] = entries[inv.reshape(-1)]
+        dev = self.device
+        if self._cache is None:
+            px = np.concatenate(self._text_px)
+            luts = np.concatenate(self._luts)
+            self._cache = (torch.from_numpy(np.concatenate([px.view(np.uint8), np.zeros(16, np.uint8)])).to(dev),
+                           torch.from_numpy(np.concatenate([luts, np.zeros(16, np.uint8)])).to(dev))
+        buf = p["buf"]
+        persons = buf[at[1]:at[1] + B * N * PERSON.itemsize].view(torch.int32).view(B * N, PERSON.itemsize // 4)
+        persons[:, _PERSON_TEXT:_PERSON_TEXT + 2] = torch.from_numpy(text.reshape(-1, 2)).to(dev)
+        h, w = p["hw"]
+        ws = torch.empty(max(B * ((h * w + 7) // 8 * 8 + p["rows_per_image"]), 8), dtype=torch.uint8, device=dev)
+        base = buf.data_ptr()
+        _lib.launch("render_poses_batch", dev, pixels, base + at[0], B, base + at[1], base + at[2], base + at[3],
+                    self._cache[0], self._cache[1], ws)
