@@ -21,6 +21,7 @@ Differences that are additive only:
 """
 from __future__ import annotations
 
+import ctypes
 import time
 
 import cv2
@@ -88,12 +89,10 @@ class BaseDetector(object):
         new_height, new_width, inp_height, inp_width, trans_input, meta = self._pre_process_geometry(height, width, scale)
         if self.device_preprocess and image.dtype == np.uint8 and image.ndim == 3 and image.shape[2] == 3:
             # resize, then warp + normalise + HWC->CHW (+ mirrored copy), as CUDA kernels bit-exact with the cv2 / numpy
-            # lines below (csrc/post.cu)
-            if (new_width, new_height) == (width, height):
-                src = torch.from_numpy(np.ascontiguousarray(image)).to(torch.device("cuda"), non_blocking=True)
-            else:
-                src = self._resize_device(image, new_height, new_width)
-            return self._pre_process_device(src, trans_input, inp_height, inp_width), meta
+            # lines below (csrc/post.cu), on a group of one image
+            group = DeviceGroup([image], [(new_height, new_width)], [trans_input], np.zeros((1, 6), np.float32), [0])
+            return group.pre_process(None, 1, (inp_height, inp_width), *self._mean_std(),
+                                     bool(self.cfg.TEST.FLIP_TEST)), meta
         resized = cv2.resize(image, (new_width, new_height))
         inp = cv2.warpAffine(resized, trans_input, (inp_width, inp_height), flags=cv2.INTER_LINEAR)
         inp = ((inp / 255. - self.mean) / self.std).astype(np.float32)
@@ -103,34 +102,9 @@ class BaseDetector(object):
         images = torch.from_numpy(np.ascontiguousarray(images))
         return images, meta
 
-    def _resize_device(self, image_u8, new_height, new_width):
-        """``cv2.resize(image_u8, (new_width, new_height))`` on the device: one upload of the image behind its
-        one-entry table, one ``cpb200_resize_linear_u8_batch``.  Returns the (new_height, new_width, 3) uint8 CUDA
-        tensor."""
-        from . import _lib
-        dev = torch.device("cuda")
-        table = resize_table([image_u8.shape[0:2]], [(new_height, new_width)])
-        host = np.empty(table.nbytes + image_u8.nbytes, np.uint8)
-        host[:table.nbytes] = table.view(np.uint8)
-        host[table.nbytes:] = np.ascontiguousarray(image_u8).reshape(-1)
-        buf = torch.from_numpy(host).to(dev)
-        out = torch.empty((new_height, new_width, 3), dtype=torch.uint8, device=dev)
-        _lib.launch("resize_linear_u8_batch", dev, buf.data_ptr() + table.nbytes, buf, 1, out)
-        return out
-
-    def _pre_process_device(self, src, trans_input, inp_height, inp_width):
-        """``src``: the (h, w, 3) uint8 image as a CUDA tensor."""
-        import ctypes
-        from . import _lib
-        dev = torch.device("cuda")
-        flip = bool(self.cfg.TEST.FLIP_TEST)
-        out = torch.empty((2 if flip else 1, 3, inp_height, inp_width), dtype=torch.float32, device=dev)
-        M = (ctypes.c_double * 6)(*np.asarray(trans_input, np.float64).reshape(-1))
-        mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
-        std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
-        _lib.launch("pre_process", dev, src, src.shape[0], src.shape[1], M, out, inp_height, inp_width, mean, std,
-                    1 if flip else 0)
-        return out
+    def _mean_std(self):
+        """``self.mean`` and ``self.std`` as the float[3] arrays the pre-process kernels take."""
+        return tuple((ctypes.c_float * 3)(*np.asarray(v, np.float32).reshape(-1)) for v in (self.mean, self.std))
 
     def process(self, images, return_time=False):
         raise NotImplementedError
@@ -282,6 +256,46 @@ def pack_group(images, new_shapes, trans_inputs, affine, dst_index, alloc=lambda
         pos += im.nbytes
     scratch = sum(h * w * 3 for h, w in new_shapes) if resize else 0
     return buf, {"o_rsz": o_rsz, "o_aff": o_aff, "o_idx": o_idx, "o_img": o_img, "scratch": scratch}
+
+
+class DeviceGroup:
+    """A ``pack_group`` upload on the device and the launches that read it; it takes what ``pack_group`` takes.  The
+    pinned buffer goes up without a wait on the current stream.  ``aff`` (B x 6 float32) and ``dst`` (B int64) are the
+    back-projections and destination indices, views into the upload; ``scratch`` is the device buffer the resized
+    images go to when a size changes, else None."""
+
+    def __init__(self, images, new_shapes, trans_inputs, affine, dst_index, src_offsets=None):
+        dev = torch.device("cuda")
+        host, at = pack_group(images, new_shapes, trans_inputs, affine, dst_index,
+                              alloc=lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True),
+                              src_offsets=src_offsets)
+        B = len(images)
+        self.buf = host.to(dev, non_blocking=True)
+        self.aff = self.buf[at["o_aff"]:at["o_aff"] + B * 24].view(torch.float32).view(B, 6)
+        self.dst = self.buf[at["o_idx"]:at["o_idx"] + B * 8].view(torch.int64)
+        self.o_rsz, self.o_img = at["o_rsz"], at["o_img"]
+        self.scratch = torch.empty(at["scratch"], dtype=torch.uint8, device=dev) if at["o_rsz"] is not None else None
+
+    def pre_process(self, pixels, B, size, mean, std, flip, f32=False):
+        """Enqueues, for the group's first ``B`` images, ``cpb200_resize_linear_u8_batch`` into ``scratch`` when there
+        is a resize table, then ``cpb200_pre_process_batch`` into the network input, which it returns: (B, 3, H, W)
+        float32 for ``size`` (H, W), or (2B, ...) with each image's mirrored copy after it with ``flip``.  ``pixels`` is
+        the device buffer ``src_offsets`` point into, or None for the pixels packed into the upload; ``mean`` and
+        ``std`` are float[3].  ``f32`` normalises as the training dataset does (``cpb200_pre_process_batch_f32``,
+        which makes no mirrored copy: ``flip`` must be off)."""
+        from . import _lib
+        dev = self.buf.device
+        if pixels is None:
+            pixels = self.buf.data_ptr() + self.o_img
+        if self.scratch is not None:
+            _lib.launch("resize_linear_u8_batch", dev, pixels, self.buf.data_ptr() + self.o_rsz, B, self.scratch)
+            pixels = self.scratch
+        inp = torch.empty((2 * B if flip else B, 3) + tuple(size), dtype=torch.float32, device=dev)
+        if f32:
+            _lib.launch("pre_process_batch_f32", dev, pixels, self.buf, B, inp, *size, mean, std)
+        else:
+            _lib.launch("pre_process_batch", dev, pixels, self.buf, B, inp, *size, mean, std, 1 if flip else 0)
+        return inp
 
 
 # run_images decodes JPEG, PNG and WebP files on the device in launches of at most this many images, whose workspace
@@ -643,8 +657,7 @@ class MultiPoseDetector(BaseDetector):
         decode with the back-projection fused; one copy of the stats and rows at the end.  ``KeypointEval.cat_img_ids``
         lists the images the reference's val split holds.  Raises ``NotImplementedError`` for the settings
         ``val.check_cfg`` refuses."""
-        import ctypes
-        from . import _lib, val
+        from . import val
         from .coco_eval import KeypointEval
         t_start = time.time()
         cfg = self.cfg
@@ -665,8 +678,7 @@ class MultiPoseDetector(BaseDetector):
         loaded, offsets, pixels = load_images_device(images)
         dev = torch.device("cuda")
         res, R, K = int(cfg.MODEL.INPUT_RES), int(cfg.MODEL.OUTPUT_RES), int(cfg.TEST.TOPK)
-        mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
-        std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
+        mean, std = self._mean_std()
         stats = torch.empty((n, len(val.STATS)), dtype=torch.float32, device=dev)
         rows = torch.empty((n, K, 56), dtype=torch.float32, device=dev)
         for a in range(0, n, int(max_batch)):
@@ -678,17 +690,12 @@ class MultiPoseDetector(BaseDetector):
                 c, s = val.center_scale(h, w)
                 trans.append(get_affine_transform(c, s, 0, [res, res]))
                 metas.append({"c": c, "s": s, "out_height": R, "out_width": R})
-            host, at = pack_group([loaded[i] for i in idx], shapes, trans, affine_for_meta(metas).numpy(), idx,
-                                  alloc=lambda nb: torch.empty(nb, dtype=torch.uint8, pin_memory=True),
-                                  src_offsets=[offsets[i] for i in idx])
-            buf = host.to(dev, non_blocking=True)
-            aff = buf[at["o_aff"]:at["o_aff"] + B * 24].view(torch.float32).view(B, 6)
-            inp = torch.empty((B, 3, res, res), dtype=torch.float32, device=dev)
-            _lib.launch("pre_process_batch_f32", dev, pixels, buf, B, inp, res, res, mean, std)
-            outputs = self.model(inp)
+            group = DeviceGroup([loaded[i] for i in idx], shapes, trans, affine_for_meta(metas).numpy(), idx,
+                                src_offsets=[offsets[i] for i in idx])
+            outputs = self.model(group.pre_process(pixels, B, (res, res), mean, std, False, f32=True))
             tg = val.targets(ev, [image_ids[i] for i in idx], shapes, cfg)
             stats[a:a + B] = val.loss(outputs, tg, cfg)
-            rows[a:a + B] = self._decode_heads(outputs, affine=aff)
+            rows[a:a + B] = self._decode_heads(outputs, affine=group.aff)
         host_stats, host_rows = stats.cpu().numpy(), rows.cpu().numpy()
         log = {}
         for j, k in enumerate(val.STATS):
@@ -708,9 +715,10 @@ class MultiPoseDetector(BaseDetector):
         ``run(image)['results'][1]``: all rows, suppressed ones at the tail, as the reference's ``merge_outputs``.
 
         Per test scale every image gets ``pre_process``'s geometry.  Images with the same (scale, input size) are
-        batched, at most ``max_batch`` per forward (2x that many network images with ``FLIP_TEST``): one pinned upload
-        of the raw images, at a scale != 1 one ``cpb200_resize_linear_u8_batch`` (``cv2.resize`` on the device, bit for
-        bit), one ``cpb200_pre_process_batch``, the forward, the flip merge and the decode with the back-projection
+        batched, at most ``max_batch`` per forward (2x that many network images with ``FLIP_TEST``).  Each batch is one
+        ``DeviceGroup``: one pinned upload of its tables and raw images, at a scale != 1 one
+        ``cpb200_resize_linear_u8_batch`` (``cv2.resize`` on the device, bit for bit) and one
+        ``cpb200_pre_process_batch``; then the forward, the flip merge and the decode with the back-projection
         fused.  The per-scale rows are then concatenated per image
         and, with ``TEST.NMS`` or several scales, go through one ``cpb200_soft_nms_39_batch`` for all images.  The
         only host wait is the final device-to-host copy.
@@ -746,12 +754,10 @@ class MultiPoseDetector(BaseDetector):
         back in place of the images.  It needs ``return_images`` or ``return_heatmaps``."""
         if encode_png and not (return_images or return_heatmaps):
             raise ValueError("run_images: encode_png=True needs return_images=True or return_heatmaps=True")
-        import ctypes
-        from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch
         if int(max_batch) < 1:
             raise ValueError("run_images: max_batch must be >= 1, got %r" % (max_batch,))
-        offsets = None
+        offsets = pixels_dev = None
         if self.device_preprocess and any(isinstance(src, str) for src in images):
             loaded, offsets, pixels_dev = load_images_device(images)
         elif return_images:
@@ -766,8 +772,7 @@ class MultiPoseDetector(BaseDetector):
         dev = torch.device("cuda")
         flip = bool(cfg.TEST.FLIP_TEST)
         K, S = int(cfg.TEST.TOPK), len(self.scales)
-        mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
-        std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
+        mean, std = self._mean_std()
         items, keys = [], []                     # one item per (image, scale)
         for i, image in enumerate(loaded):
             height, width = image.shape[0:2]
@@ -782,36 +787,23 @@ class MultiPoseDetector(BaseDetector):
             view_at = np.cumsum([0] + [heatmaps.view_bytes(H, W) for H, W in view_shapes]).tolist()
             views_dev = torch.empty(max(view_at[-1], 1), dtype=torch.uint8, device=dev)
         for (si, inp_h, inp_w), idx in group_by_shape(keys, max_batch):
-            B = len(idx)
-            # one pinned buffer, one upload of the raw images with their tables (pack_group)
-            host, at = pack_group([loaded[items[j][0]] for j in idx], [items[j][1] for j in idx], [items[j][2] for j in idx],
-                                  affine_for_meta([items[j][3] for j in idx], self.scales[si]).numpy(),
-                                  [items[j][0] for j in idx],
-                                  alloc=lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True),
-                                  src_offsets=None if offsets is None else [offsets[items[j][0]] for j in idx])
-            buf = host.to(dev, non_blocking=True)
-            aff = buf[at["o_aff"]:at["o_aff"] + B * 24].view(torch.float32).view(B, 6)
-            dst = buf[at["o_idx"]:at["o_idx"] + B * 8].view(torch.int64)
-            pixels = buf.data_ptr() + at["o_img"] if offsets is None else pixels_dev.data_ptr()
-            if at["o_rsz"] is not None:
-                # the scaled images go into a device scratch buffer, where the pre-process table points
-                scratch = torch.empty(at["scratch"], dtype=torch.uint8, device=dev)
-                _lib.launch("resize_linear_u8_batch", dev, pixels, buf.data_ptr() + at["o_rsz"], B, scratch)
-                pixels = scratch.data_ptr()
-            inp = torch.empty((2 * B if flip else B, 3, inp_h, inp_w), dtype=torch.float32, device=dev)
-            _lib.launch("pre_process_batch", dev, pixels, buf, B, inp, inp_h, inp_w, mean, std, 1 if flip else 0)
+            B, n_img = len(idx), [items[j][0] for j in idx]
+            # one upload of the group's tables, with the raw images unless they are on the device already
+            group = DeviceGroup([loaded[i] for i in n_img], [items[j][1] for j in idx], [items[j][2] for j in idx],
+                                affine_for_meta([items[j][3] for j in idx], self.scales[si]).numpy(), n_img,
+                                src_offsets=None if offsets is None else [offsets[i] for i in n_img])
+            inp = group.pre_process(pixels_dev, B, (inp_h, inp_w), mean, std, flip)
             outputs = self.model(inp)
-            dets = self._decode_outputs(outputs, aff)
+            dets = self._decode_outputs(outputs, group.aff)
             if not flip and return_heatmaps and si == S - 1:
                 # the decode read the logits; the views take the maps as process() leaves them
                 sigmoid_(outputs[0])
                 if not cfg.LOSS.MSE_LOSS:
                     sigmoid_(outputs[4])
-            rows[dst, si * K:(si + 1) * K] = dets
+            rows[group.dst, si * K:(si + 1) * K] = dets
             if return_heatmaps and si == S - 1:
                 step = 2 if flip else 1
                 hm, hm_hp = outputs[0], outputs[4]
-                n_img = [items[j][0] for j in idx]
                 heatmaps.check([inp[b * step] for b in range(B)], [hm[b * step] for b in range(B)],
                                [hm_hp[b * step] for b in range(B)], cfg.MODEL.DOWN_RATIO)
                 table, _, ws = heatmaps.layout(
@@ -867,11 +859,12 @@ class MultiPoseDetector(BaseDetector):
         (``render.DevicePlan``, ``cpb200_render_plan_batch``); that needs ``TEST.VIS_THRESH >= 0``.
 
         Frames are batched, at most ``max_batch`` per forward (default 32; 1 for a camera, which would otherwise wait
-        for frames that have not happened yet).  A batch holds frames of one shape; the resize and pre-process tables,
-        the back-projections and the network plan are made once per shape.  Per batch the frames go up on a copy
-        stream into one of two device buffers while the previous batch computes, the same kernels as ``run_images``
-        run (``cpb200_resize_linear_u8_batch``, ``cpb200_pre_process_batch``, the forward, ``cpb200_flip_merge``, the
-        decode with the back-projection, ``cpb200_soft_nms_39_batch``), and the rows come back into pinned memory
+        for frames that have not happened yet).  A batch holds frames of one shape; one ``DeviceGroup`` per test scale
+        (the resize and pre-process tables and the back-projections) and the network plan are made once per shape.
+        Per batch the frames go up on a copy stream into one of two device buffers while the previous batch computes,
+        each scale's group runs its resize and pre-process on them as ``run_images``' groups do, then come the forward,
+        ``cpb200_flip_merge``, the decode with the back-projection and ``cpb200_soft_nms_39_batch`` as in
+        ``run_images``, and the rows come back into pinned memory
         without a wait; the generator waits for them one batch later.  With drawing, batch n's frames are drawn in
         their device buffer once batch n + 1 is enqueued and copied back into pinned memory without a wait
         (``encode_png`` waits for the files), and yielded one batch later still.  The work goes to the stream that
@@ -892,23 +885,18 @@ class MultiPoseDetector(BaseDetector):
                                   torch.cuda.current_stream(torch.device("cuda")))
 
     def _video_shape(self, h, w, max_batch):
-        """What every batch of (h, w) frames shares: per test scale the ``pack_group`` tables of ``max_batch`` frames
-        lying back to back in a pixel buffer, uploaded once, with the back-projections, and the resize scratch."""
+        """What every batch of (h, w) frames shares: per test scale the ``DeviceGroup`` of ``max_batch`` frames lying
+        back to back in a pixel buffer and its network input size, and two such pixel buffers."""
         dev = torch.device("cuda")
         scales = []
         frame = np.broadcast_to(np.uint8(0), (h, w, 3))
         for scale in self.scales:
             new_h, new_w, inp_h, inp_w, trans_input, meta = self._pre_process_geometry(h, w, scale)
             aff = affine_for_meta([meta], scale).numpy()
-            host, at = pack_group([frame] * max_batch, [(new_h, new_w)] * max_batch, [trans_input] * max_batch,
-                                  np.repeat(aff, max_batch, 0), list(range(max_batch)),
-                                  alloc=lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True),
-                                  src_offsets=[b * h * w * 3 for b in range(max_batch)])
-            tables = host.to(dev)
-            scales.append({"tables": tables, "at": at, "inp": (inp_h, inp_w),
-                           "aff": tables[at["o_aff"]:at["o_aff"] + max_batch * 24].view(torch.float32).view(-1, 6),
-                           "scratch": torch.empty(at["scratch"], dtype=torch.uint8, device=dev)
-                           if at["o_rsz"] is not None else None})
+            group = DeviceGroup([frame] * max_batch, [(new_h, new_w)] * max_batch, [trans_input] * max_batch,
+                                np.repeat(aff, max_batch, 0), list(range(max_batch)),
+                                src_offsets=[b * h * w * 3 for b in range(max_batch)])
+            scales.append((group, (inp_h, inp_w)))
         return {"hw": (h, w), "scales": scales,
                 "pixels": [torch.empty(max_batch * h * w * 3, dtype=torch.uint8, device=dev) for _ in range(2)]}
 
@@ -930,25 +918,14 @@ class MultiPoseDetector(BaseDetector):
 
     def _video_batch(self, shape, pix, B):
         """Enqueues one batch of B frames lying in ``pix`` on the current stream; returns its (B, S * K, 56) rows."""
-        import ctypes
-        from . import _lib
         from .soft_nms import soft_nms_39_cuda_batch
-        cfg, dev = self.cfg, torch.device("cuda")
-        flip = bool(cfg.TEST.FLIP_TEST)
+        cfg = self.cfg
         K, S = int(cfg.TEST.TOPK), len(self.scales)
-        mean = (ctypes.c_float * 3)(*np.asarray(self.mean, np.float32).reshape(-1))
-        std = (ctypes.c_float * 3)(*np.asarray(self.std, np.float32).reshape(-1))
-        rows = torch.empty((B, S * K, 56), dtype=torch.float32, device=dev)
-        for si, st in enumerate(shape["scales"]):
-            at, tables = st["at"], st["tables"]
-            pixels = pix.data_ptr()
-            if st["scratch"] is not None:
-                _lib.launch("resize_linear_u8_batch", dev, pixels, tables.data_ptr() + at["o_rsz"], B, st["scratch"])
-                pixels = st["scratch"].data_ptr()
-            inp_h, inp_w = st["inp"]
-            inp = torch.empty((2 * B if flip else B, 3, inp_h, inp_w), dtype=torch.float32, device=dev)
-            _lib.launch("pre_process_batch", dev, pixels, tables, B, inp, inp_h, inp_w, mean, std, 1 if flip else 0)
-            rows[:, si * K:(si + 1) * K] = self._decode_outputs(self.model(inp), st["aff"][:B])
+        mean, std = self._mean_std()
+        rows = torch.empty((B, S * K, 56), dtype=torch.float32, device=pix.device)
+        for si, (group, size) in enumerate(shape["scales"]):
+            inp = group.pre_process(pix, B, size, mean, std, bool(cfg.TEST.FLIP_TEST))
+            rows[:, si * K:(si + 1) * K] = self._decode_outputs(self.model(inp), group.aff[:B])
         if cfg.TEST.NMS or S > 1:
             soft_nms_39_cuda_batch(rows, Nt=0.5, method=2)
         return rows
@@ -1029,6 +1006,9 @@ class MultiPoseDetector(BaseDetector):
                             shape["next"] = 0
                             for t in shape["pixels"]:
                                 t.record_stream(copy)
+                            # the new pixel buffers can reuse memory that work already enqueued on the compute
+                            # stream still uses, so the copy stream writes into them only after that work
+                            copy.wait_stream(compute)
                             if return_images and not encode_png:
                                 shape["drawn"] = [torch.empty(max_batch * h * w * 3, dtype=torch.uint8,
                                                               pin_memory=True) for _ in range(2)]

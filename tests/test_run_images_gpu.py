@@ -55,11 +55,24 @@ def _pre_process_batch(det, images, trans, inp_h, inp_w, flip):
     return out
 
 
+def _pre_process_one(det, image, trans, inp_h, inp_w, flip):
+    """cpb200_pre_process, the single-image entry point, on one image."""
+    from centerpose_b200 import _lib
+    src = torch.from_numpy(np.ascontiguousarray(image)).cuda()
+    out = torch.full(((2 if flip else 1), 3, inp_h, inp_w), float("nan"), device="cuda")
+    M = (ctypes.c_double * 6)(*np.asarray(trans, np.float64).reshape(-1))
+    mean = (ctypes.c_float * 3)(*det.mean.reshape(-1)); std = (ctypes.c_float * 3)(*det.std.reshape(-1))
+    _lib.launch("pre_process", out.device, src, image.shape[0], image.shape[1], M, out, inp_h, inp_w, mean, std,
+                1 if flip else 0)
+    return out
+
+
 @pytest.mark.parametrize("fix_res", [True, False])
 @pytest.mark.parametrize("flip", [False, True])
 def test_pre_process_batch_equals_per_image_kernel(fix_res, flip):
     """Every image of one batched launch == cpb200_pre_process on that image alone (torch.equal), mixed image sizes
-    sharing one input size, at scale 1 and 0.75 (host cv2.resize first)."""
+    sharing one input size, at scale 1 and 0.75 (host cv2.resize first); and pre_process, which resizes on the device,
+    == cpb200_pre_process on the host-resized image."""
     det = _detector("fp32", flip=flip, fix_res=fix_res)
     shapes = [(480, 640), (333, 500), (720, 405), (512, 512)] if fix_res else [(240, 320), (250, 330), (225, 340)]
     images = _images(shapes, 21)
@@ -77,9 +90,11 @@ def test_pre_process_batch_equals_per_image_kernel(fix_res, flip):
                    for im, g in zip(images_s, geo)]
         out = _pre_process_batch(det, resized, [g[4] for g in geo], geo[0][2], geo[0][3], flip)
         per = 2 if flip else 1
-        for n, im in enumerate(images_s):
-            want, _ = det.pre_process(im, scale)
+        for n, (im, r, g) in enumerate(zip(images_s, resized, geo)):
+            want = _pre_process_one(det, r, g[4], g[2], g[3], flip)
             assert torch.equal(out[per * n:per * (n + 1)], want), (scale, n)
+            got, _ = det.pre_process(im, scale)
+            assert torch.equal(got, want), (scale, n)
     # and against the host cv2.warpAffine / numpy branch of pre_process (base_detector.py:44-55)
     geo = [det._pre_process_geometry(h, w, 1.0) for h, w in shapes]
     got = _pre_process_batch(det, images, [g[4] for g in geo], geo[0][2], geo[0][3], flip).cpu()
