@@ -25,7 +25,13 @@ Tolerances (floating point; this docstring is the one statement of the network b
                    >= 97 % of the values; fp16x2 >= 99 % / 99 %, all rows and all values for MobileNetV2 and GhostNet,
                    all rows and >= 99.9 % of the values for HarDNet (a near-tie, see ROWS); bf16x2 >= 90 % / 95 %;
                    bf16 DLA-34 >= 20 % of the rows within half an output pixel, the other bf16 statistics reported
-  batch consistency (BATCH): bit for bit
+  batch consistency (BATCH): bit for bit, every image of the batch against the same image run alone at B = 1.  The
+                   benchmarked batches at 512x512 (BENCH_BATCH): DLA-34 B = 32 in all four precisions; ResNet-50 and
+                   HRNet-W32 B = 16, MobileNetV3, HarDNet, MobileNetV2 and GhostNet B = 64, in fp16x2 and bf16.  The
+                   golden's input at slots 0 and B - 1 is held to MAPS and ROWS, slot B // 2 to ORACLE.  run_images'
+                   network batch, DLA-34 fp16x2 B = 64 at 512x672: slots 0, B // 2 and B - 1 held to ORACLE.  Smaller:
+                   bf16 at the same batch sizes on 128x160, DLA-34 fp16x2 B = 3 at 128x160 and 640x224, HRNet bf16 B = 3
+                   at 640x224
 """
 import os
 
@@ -77,22 +83,31 @@ ROWS = {**{(t, "fp32"): (0.9, 0.97, 2e-2) for t in ("dla34_512", "res50_512", "h
 NO_CONVERT = {("hardnet_512", "fp16x2")}
 
 
-@pytest.mark.parametrize("tag,precision,max_tol,rel_tol", MAPS, ids=[f"{t}-{p}" for t, p, _, _ in MAPS])
-def test_head_maps_match_golden(tag, precision, max_tol, rel_tol):
+MAP_BOUND = {(t, p): (mx, rel) for t, p, mx, rel in MAPS}
+
+
+def _assert_golden(tag, precision, mx, rel, rows, what=""):
+    """(tag, precision)'s MAPS bound on the head maps and, where it has them, its ROWS thresholds on the decoded rows"""
+    max_tol, rel_tol = MAP_BOUND[(tag, precision)]
+    print(f"{what}{tag} {precision}: max/max {mx:.3e} relL2 {rel:.3e}")
+    assert max_tol is None or mx <= max_tol, (what, mx, rel)
+    assert rel_tol is None or rel <= rel_tol, (what, mx, rel)
+    if (tag, precision) in ROWS:
+        min_rows, min_elems, box_tol = ROWS[(tag, precision)]
+        r, e = match_rows(*rows, tol=1e-3, box_tol=box_tol)
+        print(f"{what}{tag} {precision}: rows matched within {box_tol} {r:.3f}, elements within 1e-3 {e:.4f}")
+        assert min_rows is None or r >= min_rows, (what, r, e)
+        assert min_elems is None or e >= min_elems, (what, r, e)
+
+
+@pytest.mark.parametrize("tag,precision", [(t, p) for t, p, _, _ in MAPS], ids=[f"{t}-{p}" for t, p, _, _ in MAPS])
+def test_head_maps_match_golden(tag, precision):
     """Whole network against the unmodified reference's head maps; at 512x512 the decoded rows too.  Small inputs also
     exercise the fp32 islands of the split precisions (maps < 8 pixels wide, HRNet's upsample-add, MobileNetV3's
     depthwise / SE ops, HarDNet's 2x2 deepest map and odd pools, the stride-2 stem)."""
     m, _ = model(ARCH[tag.rsplit("_", 1)[0]], precision)
     _, mx, rel, rows = golden_check(m, tag)
-    print(f"{tag} {precision}: max/max {mx:.3e} relL2 {rel:.3e}")
-    assert max_tol is None or mx <= max_tol, (mx, rel)
-    assert rel_tol is None or rel <= rel_tol, (mx, rel)
-    if (tag, precision) in ROWS:
-        min_rows, min_elems, box_tol = ROWS[(tag, precision)]
-        r, e = match_rows(*rows, tol=1e-3, box_tol=box_tol)
-        print(f"{tag} {precision}: rows matched within {box_tol} {r:.3f}, elements within 1e-3 {e:.4f}")
-        assert min_rows is None or r >= min_rows, (r, e)
-        assert min_elems is None or e >= min_elems, (r, e)
+    _assert_golden(tag, precision, mx, rel, rows)
     if (tag, precision) in NO_CONVERT:
         from centerpose_b200.plan import OP_CONVERT
         plan = next(iter(m._plans.values()))
@@ -132,10 +147,17 @@ _MODEL = {}                                        # the last arch's model
 _ORACLE = {}                                       # the last (arch, input)'s input and float64 maps
 
 
+def _oracle_forward(arch, sd, x):
+    """The float64 oracle's six head maps of the device batch ``x`` on the weights ``sd``"""
+    from oracle import dla_ref, ghostnet_ref, hardnet_ref, mobilenetv2_ref
+    fwd = {"hardnet": hardnet_ref.forward, "mobilenetv2": mobilenetv2_ref.forward,
+           "ghostnet": ghostnet_ref.forward}.get(arch)
+    return fwd(sd, x.double()) if fwd else dla_ref.forward(sd, x.double(), arch=arch.split("_w")[0])
+
+
 def _oracle_case(arch, inp):
     """(model, input on the device, float64 oracle maps on the device); the maps are computed once per (arch, input):
     the rows of one input run one after the other"""
-    from oracle import dla_ref, ghostnet_ref, hardnet_ref, mobilenetv2_ref
     from oracle.init_recipe import synth_images
     if arch not in _MODEL:
         _MODEL.clear()
@@ -147,11 +169,34 @@ def _oracle_case(arch, inp):
         x = synth_images(2, 128, 160, seed=5) if inp is None else golden_input(inp) if isinstance(inp, str) else \
             synth_images(1, *inp, 317)
         x = x.to(DEV)
-        fwd = {"hardnet": hardnet_ref.forward, "mobilenetv2": mobilenetv2_ref.forward,
-               "ghostnet": ghostnet_ref.forward}.get(arch)
-        ref = fwd(sd, x.double()) if fwd else dla_ref.forward(sd, x.double(), arch=arch.split("_w")[0])
-        _ORACLE[(arch, inp)] = (x, ref)
+        _ORACLE[(arch, inp)] = (x, _oracle_forward(arch, sd, x))
     return (m, *_ORACLE[(arch, inp)])
+
+
+def _assert_oracle(arch, inp, precision, outs, ref, what):
+    """``outs`` against the oracle's maps ``ref`` under _oracle_bound; in fp32 and fp16x2, where the head map has at
+    least K = 100 cells, image 0's decoded rows against the oracle's under ROWS' 512x512 thresholds"""
+    from centerpose_b200 import multi_pose_decode
+    from oracle import decode_ref
+    max_tol, rel_tol = _oracle_bound(arch, inp, precision)
+    got = torch.cat(outs, dim=1).double()
+    r = torch.cat(ref, dim=1)
+    mx = ((got - r).abs().max() / r.abs().max()).item()
+    rel = ((got - r).norm() / r.norm()).item()
+    print(f"{what} {precision}: max/max {mx:.3e} relL2 {rel:.3e}")
+    assert max_tol is None or mx <= max_tol, (what, mx, rel)
+    assert rel_tol is None or rel <= rel_tol, (what, mx, rel)
+    H, W = outs[0].shape[2:]
+    if precision in ("fp32", "fp16x2") and H * W >= 100:
+        min_rows, min_elems, box_tol = {"fp32": (0.9, 0.97, 2e-2), "fp16x2": (0.99, 0.99, 2e-2)}[precision]
+        hm, wh, hps, reg, hm_hp, hp_off = outs
+        dets = multi_pose_decode(hm, wh, hps, reg=reg, hm_hp=hm_hp, hp_offset=hp_off, K=100, apply_sigmoid=True)
+        o = [t[:1].cpu().numpy() for t in ref]
+        sig = lambda a: 1.0 / (1.0 + np.exp(-a))
+        want = decode_ref.multi_pose_decode(sig(o[0]), o[1], o[2], o[3], sig(o[4]), o[5], K=100)
+        rows, elems = match_rows(dets[0].cpu().numpy(), want[0], tol=1e-3, box_tol=box_tol)
+        print(f"{what} {precision}: rows matched within {box_tol} {rows:.3f}, elements within 1e-3 {elems:.4f}")
+        assert rows >= min_rows and elems >= min_elems, (what, rows, elems)
 
 
 @pytest.mark.parametrize("arch,inp,precision", ORACLE, ids=[f"{a}-{_input_id(i)}-{p}" for a, i, p in ORACLE])
@@ -162,55 +207,54 @@ def test_forward_matches_oracle(arch, inp, precision):
     tensor-core tiles with fewer than 8 rows, fp32 islands with their CONVERT ops, CUDA-core DCNs between tensor-core
     ones, the fused heads on 8 x N maps, deep maps one pixel high or wide, and maps larger than at 512x512.  Where the
     head map has at least K = 100 cells, fp32 and fp16x2 also hold the decoded rows to ROWS' 512x512 thresholds."""
-    from centerpose_b200 import multi_pose_decode
-    from oracle import decode_ref
     m, x, ref = _oracle_case(arch, inp)
-    max_tol, rel_tol = _oracle_bound(arch, inp, precision)
     if precision == "bf16-simt":
         m.set_precision("bf16", tc=False)
     else:
         m.set_precision(precision)
-    outs = m(x)
-    got = torch.cat(outs, dim=1).double()
-    r = torch.cat(ref, dim=1)
-    mx = ((got - r).abs().max() / r.abs().max()).item()
-    rel = ((got - r).norm() / r.norm()).item()
-    print(f"{arch} {_input_id(inp)} {precision}: max/max {mx:.3e} relL2 {rel:.3e}")
-    assert max_tol is None or mx <= max_tol, (mx, rel)
-    assert rel_tol is None or rel <= rel_tol, (mx, rel)
-    H, W = outs[0].shape[2:]
-    if precision in ("fp32", "fp16x2") and H * W >= 100:
-        min_rows, min_elems, box_tol = {"fp32": (0.9, 0.97, 2e-2), "fp16x2": (0.99, 0.99, 2e-2)}[precision]
-        hm, wh, hps, reg, hm_hp, hp_off = outs
-        dets = multi_pose_decode(hm, wh, hps, reg=reg, hm_hp=hm_hp, hp_offset=hp_off, K=100, apply_sigmoid=True)
-        o = [t[:1].cpu().numpy() for t in ref]
-        sig = lambda a: 1.0 / (1.0 + np.exp(-a))
-        want = decode_ref.multi_pose_decode(sig(o[0]), o[1], o[2], o[3], sig(o[4]), o[5], K=100)
-        rows, elems = match_rows(dets[0].cpu().numpy(), want[0], tol=1e-3, box_tol=box_tol)
-        print(f"{arch} {_input_id(inp)} {precision}: rows matched within {box_tol} {rows:.3f}, "
-              f"elements within 1e-3 {elems:.4f}")
-        assert rows >= min_rows and elems >= min_elems, (rows, elems)
+    _assert_oracle(arch, inp, precision, m(x), ref, f"{arch} {_input_id(inp)}")
 
 
-# (arch, precision, batch, input shape): the bf16 batches are the benchmark's per-backbone sizes; 640x224 is a COCO
-# 213x640 image at TEST.FIX_RES false (fp32 islands, CUDA-core DCNs).  The DLA-34 640x224 row also cycles the model
-# through more shapes than its plan cache keeps (model.py) and back.
+# (arch, precision, batch, input shape): the bf16 batches at 128x160 are the benchmark's per-backbone sizes on small
+# maps; 640x224 is a COCO 213x640 image at TEST.FIX_RES false (fp32 islands, CUDA-core DCNs).  The DLA-34 640x224 row
+# also cycles the model through more shapes than its plan cache keeps (model.py) and back.
 BATCH = [("dla_34", "bf16", 32, (128, 160)), ("res_50", "bf16", 16, (128, 160)), ("hrnet", "bf16", 16, (128, 160)),
          ("mobilenetv3", "bf16", 64, (128, 160)), ("hardnet", "bf16", 64, (128, 160)),
          ("dla_34", "fp16x2", 3, (128, 160)), ("dla_34", "fp16x2", 3, (640, 224)), ("hrnet", "bf16", 3, (640, 224))]
 CYCLE = {("dla_34", "fp16x2", 3, (640, 224))}
+# The batches the benchmarks time (bench.py: DLA-34 B = 32; tools/final_check.sh and tools/bench_backbones.py: the other
+# backbones), where the persistent wgmma kernels loop hundreds of times per CTA and image indices reach 63, and
+# run_images' network batch at its default max_batch = 32: 32 COCO 480x640 images with the dla_34 test section's flip
+# test are one B = 64 batch at 512x672.
+BENCH_BATCH = ([("dla_34", p, 32, (512, 512)) for p in ("fp16x2", "bf16x2", "bf16", "fp32")]
+               + [(a, p, b, (512, 512)) for a, b in (("res_50", 16), ("hrnet", 16), ("mobilenetv3", 64), ("hardnet", 64),
+                                                     ("mobilenetv2", 64), ("ghostnet", 64)) for p in ("fp16x2", "bf16")]
+               + [("dla_34", "fp16x2", 64, (512, 672))])
+BATCH += BENCH_BATCH
+GOLDEN_PREFIX = {a: t for t, a in ARCH.items()}          # arch -> its goldens' tag prefix
 
 
 @pytest.mark.parametrize("arch,precision,B,shape", BATCH, ids=[f"{a}-{p}-{b}-{h}x{w}" for a, p, b, (h, w) in BATCH])
 def test_batch_consistency_and_output_rebinding(arch, precision, B, shape):
-    """(1) Image i of a batch equals the same image run alone, bit for bit (tiles never mix images).  (2) The
+    """(1) Every image of a batch equals the same image run alone, bit for bit (tiles never mix images).  (2) The
     tensor-core ops read dst / res / bias from the live op at every launch: a second forward on the SAME plan while the
     first call's outputs are still held must return independent, correct tensors (an earlier bug: `Plan.bind`
     re-pointed ops[i].dst after the one-time prepare had cached it).  (3) CYCLE rows: after the model has run more
-    shapes than its plan cache holds, which evicts this shape's plan, the rebuilt plan gives the same bits."""
+    shapes than its plan cache holds, which evicts this shape's plan, the rebuilt plan gives the same bits.
+    (4) BENCH_BATCH rows: at 512x512 the golden's input sits at slots 0 and B - 1 and both are held to its MAPS bound
+    and ROWS thresholds; slot B // 2 (without a golden, slots 0, B // 2 and B - 1) is held to the float64 oracle's
+    forward of that image under _oracle_bound, and in fp32 / fp16x2 its decoded rows to the oracle's."""
+    import time
     from oracle.init_recipe import synth_images
-    m, _ = model(arch, precision)
+    torch.cuda.empty_cache()
+    torch.cuda.reset_peak_memory_stats()
+    t0 = time.perf_counter()
+    bench = (arch, precision, B, shape) in BENCH_BATCH
+    tag = f"{GOLDEN_PREFIX[arch]}_512" if bench and shape == (512, 512) else None
+    m, sd = model(arch, precision)
     x1 = synth_images(B, *shape, seed=21).to(DEV)
+    if tag:
+        x1[0] = x1[B - 1] = golden_input(tag)[0].to(DEV)
     x2 = synth_images(B, *shape, seed=22).to(DEV)
     ref1 = [t.clone() for t in m(x1)]
     m.invalidate()
@@ -226,7 +270,8 @@ def test_batch_consistency_and_output_rebinding(arch, precision, B, shape):
     for a, b in zip(o3, ref1):
         assert torch.equal(a, b)
     assert len({t.data_ptr() for t in o1 + o2 + o3}) == 18
-    for i in (0, B // 2, B - 1):
+    del x2, ref2, o1, o2, o3
+    for i in range(B):               # one B = 1 plan, run per slot
         alone = m(x1[i:i + 1])
         for a, b in zip(ref1, alone):
             assert torch.equal(a[i:i + 1], b), (arch, i)
@@ -237,6 +282,17 @@ def test_batch_consistency_and_output_rebinding(arch, precision, B, shape):
         assert not any(k[:3] == (B, *shape) for k in m._plans), "the plan cache kept every shape"
         for a, b in zip(m(x1), ref1):
             assert torch.equal(a, b)
+    if bench:
+        m.invalidate()
+        for i in ((0, B - 1) if tag else ()):
+            _, mx, rel, rows = golden_check(m, tag, [t[i:i + 1] for t in ref1])
+            _assert_golden(tag, precision, mx, rel, rows, f"slot {i} of B = {B}: ")
+        for i in ((B // 2,) if tag else (0, B // 2, B - 1)):
+            _assert_oracle(arch, shape, precision, [t[i:i + 1] for t in ref1],
+                           _oracle_forward(arch, sd, x1[i:i + 1]), f"{arch} {_input_id(shape)} slot {i} of B = {B}")
+    print(f"{arch} {precision} B = {B} {_input_id(shape)}: peak {torch.cuda.max_memory_allocated() / 2**30:.2f} GiB "
+          f"allocated, {time.perf_counter() - t0:.1f} s")
+    m.invalidate()
 
 
 def test_forward_rejects_cpu_and_training():

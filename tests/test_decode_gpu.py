@@ -206,3 +206,54 @@ def test_soft_nms_cuda_matches_compiled_reference_golden():
     dev = torch.from_numpy(rows.copy()).to(DEV); kd = soft_nms_39_cuda(dev, Nt=0.5, method=2)
     assert kd == kh and np.abs(dev.cpu().numpy() - host).max() <= 2e-7
     assert soft_nms_39_cuda(torch.zeros(0, 56, device=DEV), Nt=0.5, method=2) == 0
+
+
+def _bench_maps(B):
+    """bench.py's synthetic head maps of its large-batch decode timings, drawn as it draws them: one seed-317 device
+    generator for B = 256, then B = 1024."""
+    dev = torch.device(DEV)
+    g = torch.Generator(device=dev).manual_seed(317)
+    for Bd in (256, 1024):
+        maps = (torch.randn(Bd, 1, 128, 128, device=dev, generator=g) * 2 - 2.19,
+                torch.rand(Bd, 2, 128, 128, device=dev, generator=g) * 40,
+                torch.randn(Bd, 34, 128, 128, device=dev, generator=g) * 10,
+                torch.rand(Bd, 2, 128, 128, device=dev, generator=g),
+                torch.randn(Bd, 17, 128, 128, device=dev, generator=g) * 2 - 2.19,
+                torch.rand(Bd, 2, 128, 128, device=dev, generator=g))
+        if Bd == B:
+            return maps
+        del maps
+
+
+@pytest.mark.parametrize("B", [256, 1024])
+def test_decode_at_bench_batches(B):
+    """bench.py's decode call (apply_sigmoid=True, K = 100) at B = 256 and 1024, B * 18 CTAs grouping keypoints through
+    one release/acquire flag per (image, joint): every image's rows equal a B = 1 call on that image, bit for bit.  On
+    maps torch turned into sigmoids (apply_sigmoid=False: the fused logistic uses ex2.approx), slots 0, 1, B // 2, B - 1
+    and every multiple of 128 equal the oracle's rows bit for bit.  After every call the workspace's pair counters are
+    back at zero."""
+    from centerpose_b200 import multi_pose_decode
+    from centerpose_b200.decode import _workspace
+    K, J = 100, 17
+    hm, wh, hps, reg, hm_hp, hpo = _bench_maps(B)
+
+    def decode(b0, b1, heat, joints, sig):
+        out = multi_pose_decode(heat[b0:b1], wh[b0:b1], hps[b0:b1], reg=reg[b0:b1], hm_hp=joints[b0:b1],
+                                hp_offset=hpo[b0:b1], K=K, apply_sigmoid=sig)
+        _, ws = _workspace(hm.device, b1 - b0, J, K)
+        n = (b1 - b0) * (1 + J) * K
+        counters = ws[2 * (-(-n * 4 // 16) * 16):].view(torch.int32)[:(b1 - b0) * J]
+        assert not counters.any(), f"B = {b1 - b0}: {int(counters.count_nonzero())} pair counters left non-zero"
+        return out
+
+    got = decode(0, B, hm, hm_hp, True)
+    for b in range(B):
+        assert torch.equal(got[b:b + 1], decode(b, b + 1, hm, hm_hp, True)), b
+    hm_s, hm_hp_s = hm.sigmoid(), hm_hp.sigmoid()
+    got = decode(0, B, hm_s, hm_hp_s, False).cpu().numpy()
+    for b in sorted({0, 1, B // 2, B - 1, *range(128, B, 128)}):
+        inp = {k: t[b:b + 1].cpu().numpy() for k, t in
+               (("heat", hm_s), ("wh", wh), ("kps", hps), ("reg", reg), ("hm_hp", hm_hp_s), ("hp_offset", hpo))}
+        want = _oracle(inp, K)
+        _assert_same(got[b:b + 1], want)
+        assert np.array_equal(got[b:b + 1], want), b

@@ -217,6 +217,14 @@ def test_run_images_batch_size_does_not_change_rows(tmp_path):
     for n in range(len(images)):
         assert np.array_equal(a[n], b[n]), n
         assert np.array_equal(a[n], c[n]), n
+    # the dla_34 test section at the default max_batch = 32 on COCO-sized images: 34 at 480x640 make network batches
+    # of 64 and 4 at 512x672, the 6 at 427x640 one of 12 at 448x672
+    det = _detector("fp16x2", flip=True, nms=True, fix_res=False)
+    images = _images([(427, 640) if n % 7 == 3 else (480, 640) for n in range(40)], 43)
+    a = det.run_images(images)
+    b = det.run_images(images, max_batch=1)
+    for n in range(len(images)):
+        assert np.array_equal(a[n], b[n]), ("dla34_test_section", n)
 
 
 @pytest.mark.parametrize("precision", ["fp32", "fp16x2"])

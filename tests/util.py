@@ -67,14 +67,16 @@ def golden_input(tag):
     return synth_images(B, H, W, 317)
 
 
-def golden_check(model, tag):
+def golden_check(model, tag, outs=None):
     """Run ``model`` on the input of tests/golden/<tag>.npz and compare its head maps, subsampled by the golden's
     ``stride``, with the golden's.  Returns (outputs, max|err| / max|ref|, relative L2, rows); for a golden that holds
-    ``dets``, rows is (decoded rows of image 0, the golden's rows of image 0), else None."""
+    ``dets``, rows is (decoded rows of image 0, the golden's rows of image 0), else None.  ``outs``: compare these
+    six head maps (the model's outputs on that input, e.g. one image's slice of a batch) instead of running it."""
     from centerpose_b200 import multi_pose_decode
     g = np.load(os.path.join(GOLD, tag + ".npz"))
     st = int(g["stride"]) if "stride" in g.files else 1
-    outs = model(golden_input(tag).to(DEV))
+    if outs is None:
+        outs = model(golden_input(tag).to(DEV))
     maps = torch.cat(outs, dim=1).cpu().numpy()[:, :, ::st, ::st].astype(np.float64)
     ref = g["maps"].astype(np.float64)
     assert maps.shape == ref.shape, (maps.shape, ref.shape)
